@@ -4,7 +4,7 @@
 12-step windows, hidden 32).
 
 A "step" = one pass of the hot path over one batch of `--windows` windows per GPU (one launch of the
-fused sm_100a kernel).  One graph-snapshot = one (207 x 2 x 12) window pushed through 12 chained DCRNN
+fused sm_90a kernel).  One graph-snapshot = one (207 x 2 x 12) window pushed through 12 chained DCRNN
 cell steps, all 12 hidden states emitted (SURVEY.md section 8d).
 
   python bench.py [--gpus N --steps K --warmup W]      our arm (N>1 under torchrun, one rank per GPU)
@@ -40,7 +40,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": float(d["hbm_gbs"]), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "source": "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"}
 
 
 class ClockSampler:
@@ -326,7 +326,7 @@ def run_ours(args):
     model = make_model().to(dev)
 
     # Rotating device-resident input batches: R x (B x 19 872 B); together with the 318 KB/window output
-    # (B x 317 952 B written per step) each step's traffic exceeds the 126 MB L2.
+    # (B x 317 952 B written per step) each step's traffic exceeds the 50 MB L2.
     n_rot = 8
     g = torch.Generator().manual_seed(1234 + rank)
     starts = [torch.randint(0, series.size(0) - HORIZON, (B,), generator=g) for _ in range(n_rot)]
@@ -359,6 +359,8 @@ def run_ours(args):
     barrier()
     launches = _lib.launch_count() - l0
     ms_total = e0.elapsed_time(e1)
+    if getattr(args, "dump_outputs", None) and rank == 0:
+        dump_outputs(args.dump_outputs, hidden_states=out)
     clocks = sampler.stop() if rank == 0 else None
     t = torch.tensor([ms_total], device=dev)
     if world > 1:
@@ -406,6 +408,7 @@ def run_ours(args):
         if prev is not None:
             pred_done[prev].synchronize()
             last = float(pred_host[prev][0, 0]) + float(pred_host[prev][-1, -1])
+        run_e2e.last_pred = pred_host[prev] if prev is not None else None
         return last
 
     roofline = cpu_note = None
@@ -423,6 +426,8 @@ def run_ours(args):
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         e2e["value"] = world * B * args.steps / (float(t.item()) * 1e-3)
+        if getattr(args, "dump_outputs", None) and rank == 0:
+            dump_outputs(args.dump_outputs, e2e_prediction=run_e2e.last_pred)
     except Exception as e:  # noqa: the device-timed headline above must survive a failure here
         if world > 1:
             raise                                   # ranks must stay in lock step around collectives: fail loudly under torchrun
@@ -437,10 +442,10 @@ def run_ours(args):
             traffic = json.load(open(tp)).get("dram_bytes_per_launch")
         except Exception:
             traffic = None
-    roofline = {"kernel": "k_dcrnn_seq_tc (tcgen05)", "bound": "hbm", "achieved": achieved_gbs, "peak": pk["hbm_gbs"], "unit": "GB/s",
+    roofline = {"kernel": "k_dcrnn_seq_tc (wgmma)", "bound": "hbm", "achieved": achieved_gbs, "peak": pk["hbm_gbs"], "unit": "GB/s",
                 "frac": achieved_gbs / pk["hbm_gbs"], "traffic": traffic, "peak_source": pk["source"],
                 "algorithmic_bytes_per_launch": B * BYTES_PER_SNAPSHOT,
-                "note": "fused kernel is shared-memory-bandwidth bound (gather/scatter of the diffusion); contraction on tcgen05; HBM fraction reported as north_star asks",
+                "note": "fused kernel is shared-memory-bandwidth bound (gather/scatter of the diffusion); contraction on wgmma; HBM fraction reported as north_star asks",
                 "fp32_tflops_achieved": B * FLOPS_PER_SNAPSHOT / (ms_step * 1e-3) / 1e12}
     line = {
         "metric": "graph-snapshots/sec", "value": value, "unit": "snapshots/s", "n_gpus": world, "steps": args.steps,
@@ -448,7 +453,7 @@ def run_ours(args):
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": "DCRNN K=2 METR-LA-shape (207 nodes, 1722 edges, 2 feats, 12-step window, hidden 32), forward (BatchedDCRNN.forward), all 12 H_t written",
                    "windows_per_step_per_gpu": B, "parallelism": f"dp{world} (independent windows, no data-path collective)",
-                   "l2_policy": "8 rotating input batches + 318 KB/window output: per-step traffic > 126 MB L2"},
+                   "l2_policy": "8 rotating input batches + 318 KB/window output: per-step traffic > 50 MB L2"},
         "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline,
         "path_counters": {k: v for k, v in _lib.path_counters().items() if v},
         "spmm": None, "train": None, "cpu_baseline": None, "reference_gpu": None, "e2e_host_windows": None,
@@ -496,8 +501,23 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+DUMP_WINDOWS = 48      # windows of a batch written by --dump-outputs: 48 x 318 KB of hidden states stays far below 64 MB
+
+
+def dump_outputs(directory, **arrays):
+    """Writes each (B, ...) output as directory/<name>.npy in float32: the rows of DUMP_WINDOWS windows drawn with a fixed seed, so that
+    two builds run with the same arguments can be compared output for output."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.detach()
+        g = torch.Generator().manual_seed(2024)
+        idx = torch.randperm(a.size(0), generator=g)[:DUMP_WINDOWS].sort().values
+        np.save(os.path.join(directory, name + ".npy"), a[idx.to(a.device)].float().cpu().numpy())
+
+
 def reference_gpu_probe(dev, ei_d, ew_d, series, windows, iters=5):
-    """The "reference-on-B200" comparator (SURVEY 8d, GPU timing): the reference's op-for-op sequence -- index_select ->
+    """The "reference-on-GPU" comparator (SURVEY 8d, GPU timing): the reference's op-for-op sequence -- index_select ->
     norm * x_j -> scatter_add_ -> matmul per gate per step, block-diagonal batch graph -- with every tensor on the GPU
     (oracle port, device-agnostic), eager and replayed from a CUDA graph.  Same windows per step as our arm."""
     from oracle import recurrent as R
@@ -645,7 +665,9 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--windows", type=int, default=1184, help="windows per step per GPU (8 per SM)")
+    ap.add_argument("--windows", type=int, default=1056, help="windows per step per GPU (8 per SM of an H100)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (fixed window sample)")
     ap.add_argument("--no-spmm", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-train", action="store_true")

@@ -1,5 +1,5 @@
 /*
- * stmp.h -- C ABI of libstmp.so, the sm_100a spatiotemporal message-passing engine.
+ * stmp.h -- C ABI of libstmp.so, the sm_90a (H100) spatiotemporal message-passing engine.
  *
  * The reference (benedekrozemberczki/pytorch_geometric_temporal @ adefe44) is pure Python and has no
  * FFI layer: its hot path is `torch.nn.Module.forward` -> torch_geometric `MessagePassing.propagate`
@@ -141,7 +141,7 @@ int stmp_dcrnn_seq_fwd(const stmp_plan* plan, int64_t B, int64_t T, int64_t cin,
 /* 1 if stmp_dcrnn_seq_fwd can take this configuration on the current device, else 0. */
 int stmp_dcrnn_seq_supported(const stmp_plan* plan, int64_t cin, int64_t cout, int64_t K);
 
-/* Generic fused graph-GRU recurrence on the tensor cores (tcgen05, fp16 hi/lo operand split = fp32-class accuracy):
+/* Generic fused graph-GRU recurrence on the tensor cores (wgmma, fp16 hi/lo operand split = fp32-class accuracy):
  *   pre_g = [H' | Op0 H' | Op1 H' | X | Op0 X | Op1 X] @ wcat_g^T + bcat_g      g in {z, r, h};  H' = H (z, r) or H*R (h)
  *   Z = sigmoid(pre_z); R = sigmoid(pre_r); Ht = tanh(pre_h); H_t = Z*H + (1-Z)*Ht
  * with the first `n_ops` (0..2) operators of `plan` (any flavor).  This one kernel serves DCRNN K=2 (DConv plan, 2 ops),
@@ -154,15 +154,15 @@ int stmp_gru_seq_fwd(const stmp_plan* plan, int n_ops, int64_t B, int64_t T, int
                      const int64_t* win_start, int64_t x_bstride, int64_t x_tstride, const float* wcat,
                      const float* bcat, const float* h0, int64_t h0_bstride, float* out, float* stash,
                      const void* wimage, void* workspace, void* stream);
-/* Optional weight image for the tcgen05 kernel: the B operand (fp16 hi/lo halves, SWIZZLE_128B, + biases) exactly as the kernel
+/* Optional weight image for the wgmma kernel: the B operand (fp16 hi/lo halves, SWIZZLE_128B, + biases) exactly as the kernel
  * holds it in shared memory, so every CTA fetches it with one TMA bulk copy instead of converting the fp32 weights itself.
  * Build it once per weight update into a device buffer of stmp_gru_weight_image_bytes() bytes and pass it as `wimage`
  * (NULL => the kernel converts in place).  The plan carries the analogous graph image. */
 int64_t stmp_gru_weight_image_bytes(void);
-/* Optional workspace of the tcgen05 kernel (both entries): stmp_seq_workspace_bytes(plan, T, cin) bytes of device memory, reusable across
+/* Optional workspace of the wgmma kernel (both entries): stmp_seq_workspace_bytes(plan, T, cin) bytes of device memory, reusable across
  * calls on one stream.  The window prologue parks P_o X_t / P_i X_t of all steps there (per-CTA rows, rewritten every window => L2-resident,
  * full-sector stores).  NULL => they are parked in the window's own not-yet-written output rows instead (same results; partial-sector
- * writes cost extra DRAM traffic: 1.7x the algorithmic bytes measured). */
+ * writes cost extra DRAM traffic). */
 int64_t stmp_seq_workspace_bytes(const stmp_plan* plan, int64_t T, int64_t cin);
 int stmp_dcrnn_pack_weights(int64_t cin, int64_t cout, int64_t K, const float* w_z, const float* w_r, const float* w_h,
                             const float* b_z, const float* b_r, const float* b_h, void* image, void* stream);
@@ -239,7 +239,7 @@ int stmp_tgcn_attn_bwd(const stmp_plan* plan, int64_t B, int64_t fin, int64_t pe
  * `+ bias` of dcrnn.py:86-111 across steps, gates and hops): S1 / S2 (rows, ld) are stmp_dcrnn_bwd_basis' bases (ld = 3(cin+cout) rounded
  * up to 8), dpzr (rows, 2cout) / dph (rows, cout) stmp_dcrnn_bwd_seq's d pre-activations.  Writes gz / gr / gh in the module's
  * (2, K, cin+cout, cout) layout and the bias gradients (nullable).  Two launches (per-CTA partials, fixed-order reduction: deterministic);
- * the contraction runs on tcgen05 (kind::tf32, MN-major operands, TF32 hi/lo split; stmp_set_option("dcrnn_wgrad_tc", 0) selects the
+ * the contraction runs on wgmma (TF32, K-major operands transposed as they are staged, TF32 hi/lo split; stmp_set_option("dcrnn_wgrad_tc", 0) selects the
  * fp32 FFMA kernel).  Workspace of stmp_dcrnn_bwd_wgrad_workspace_bytes(cin) bytes.  K = 2, cout = 32, cin <= 4. */
 int64_t stmp_dcrnn_bwd_wgrad_workspace_bytes(int64_t cin);
 int stmp_dcrnn_bwd_wgrad(int64_t cin, int64_t cout, int64_t K, int64_t rows, int64_t ld, const float* S1, const float* S2,
@@ -286,10 +286,10 @@ int stmp_gru_bwd_zr(int64_t B, int64_t N, int64_t cin, int64_t cout, int64_t du_
                     int64_t hprev_bstride, const float* z, const float* r, const float* ht, int64_t stash_bstride,
                     const float* du2, float* dpzr, void* stream);
 
-/* ---- K4: dense node-feature x weight contraction on the tensor cores (tcgen05), fp32 in / fp32 out ------------------
+/* ---- K4: dense node-feature x weight contraction on the tensor cores (wgmma), fp32 in / fp32 out ------------------
  * C[M,N] = A[M,K] @ W[K,N] + bias.  Replaces `torch.matmul(Tx_k, weight[..][k])` / ChebConv `lins[k](Tx_k)` / GCNConv
  * `lin(x)` (dcrnn.py:81-105; PyG) for the large-graph (tiled) path.  fp32-class accuracy: operands are split into fp16
- * hi/lo halves and multiplied in three tcgen05.mma passes with an fp32 TMEM accumulator.
+ * hi/lo halves and multiplied in three wgmma passes with fp32 register accumulators.
  *   stmp_gemm_packed_elems(K,N): number of fp16 elements of the packed weight buffer
  *   stmp_gemm_prepack: W [K,N] row-major (row stride ldw) -> packed (hi/lo, K-major, K padded to 64); once per weight update
  *   stmp_gemm_f32: A row-major (row stride lda), C row-major (ldc); needs N <= 256, N % 32 == 0, K % 4 == 0, 16-byte aligned
@@ -306,7 +306,7 @@ int stmp_gemm_lstm_f32(const float* A, int64_t lda, int64_t M, int64_t K, int64_
                        const float* bi, const float* bf, const float* bc, const float* bo, float* h_out, float* c_out,
                        void* stream);
 
-/* ---- ASTGCN block (nn/attention/astgcn.py:408-481): the dense products on tcgen05 with their operand gathers and pointwise tails fused
+/* ---- ASTGCN block (nn/attention/astgcn.py:408-481): the dense products on wgmma with their operand gathers and pointwise tails fused
  * stmp_gemm_blocks_f32:  C[m, 0:ncols] = epilogue( sum_i A_i[m + shift_i, 0:width_i] @ W_i + bias )
  *   the A operand is a list of nblk (<= 12) K-blocks of <= 64 columns: blk_ptr[i] (device pointer, HOST array), row stride blk_ld[i],
  *   valid columns blk_width[i], row shift blk_shift[i] inside sequences of `seq` consecutive rows (rows shifted out of their sequence read
@@ -345,20 +345,20 @@ int stmp_gemm_blocks_image(const void* packed, int64_t N, int64_t nblk, void* im
 int stmp_window_gather(const float* series, int64_t t_total, int64_t row_elems, const int64_t* start,
                        int64_t B, int64_t horizon, float* x, float* y, void* stream);
 
-/* Run-time switches for tests: "dcrnn_tc" = 1 (tcgen05 kernel, default) / 0 (FFMA kernel) behind stmp_dcrnn_seq_fwd; "spmm_variant" = 0
+/* Run-time switches for tests: "dcrnn_tc" = 1 (wgmma kernel, default) / 0 (FFMA kernel) behind stmp_dcrnn_seq_fwd; "spmm_variant" = 0
  * (register gather, default) / 1, 2 (TMA-staged rows, 8 / 16 per warp); "dcrnn_bwd_all_cin" = 1 (default) / 0 (persistent backward only for cin == 2); "dcrnn_bwd_split" = 1 (default: a 2-CTA cluster per window
  * when 2 B <= SM count) / 0 (one CTA per window); "dcrnn_fwd_split" = 1 (default: the fused forward also runs on a 2-CTA cluster per window when 2 B <= SM count and N > 128) / 0;
- * "dcrnn_wgrad_tc" = 1 (default, tcgen05) / 0 (FFMA); "spmm_rows_per_group" (default 8) and
+ * "dcrnn_wgrad_tc" = 1 (default, wgmma) / 0 (FFMA); "spmm_rows_per_group" (default 8) and
  * "spmm_block" (256 / 1024): the SpMM's row blocking. */
 int stmp_set_option(const char* name, int value);
 
 /* ---- misc ---------------------------------------------------------------------------------------- */
 const char* stmp_last_error(void);
-/* "stmp <version> sm_100a" */
+/* "stmp <version> sm_90a" */
 const char* stmp_version(void);
 /* Number of kernels this library has launched in the calling process (bench.py's gpu_launches). */
 int64_t stmp_launch_count(void);
-/* Which kernels served the calls so far ("did the fused tcgen05 path run, or the tiled one?" -- the dispatchers fall back
+/* Which kernels served the calls so far ("did the fused wgmma path run, or the tiled one?" -- the dispatchers fall back
  * silently on STMP_EUNSUPPORTED, e.g. dcrnn.py:429-475 at N > 207).  Fills up to max_entries (kernel name, launches) pairs,
  * names are static strings such as "k_dcrnn_seq_tc"; returns the number of distinct kernels launched. */
 int stmp_path_counters(const char** names, int64_t* counts, int max_entries);

@@ -100,7 +100,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise StmpError(
                 f"{LIB_PATH} is missing: build it with `python -m pytorch_geometric_temporal_b200.build` "
-                "(nvcc, sm_100a).  There is no CPU/PyTorch fallback for the hot path.")
+                "(nvcc, sm_90a).  There is no CPU/PyTorch fallback for the hot path.")
         h = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(h, name)
@@ -136,7 +136,7 @@ def launch_count() -> int:
 
 
 def path_counters() -> dict:
-    """{kernel name: launches so far} -- lets tests and users assert which path (tcgen05 / FFMA / tiled) served a call."""
+    """{kernel name: launches so far} -- lets tests and users assert which path (wgmma / FFMA / tiled) served a call."""
     n = 96
     names = (c_char_p * n)()
     counts = (c_int64 * n)()

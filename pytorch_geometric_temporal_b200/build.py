@@ -1,4 +1,4 @@
-"""Build libstmp.so (sm_100a) in-tree with nvcc.  `python -m pytorch_geometric_temporal_b200.build`."""
+"""Build libstmp.so (sm_90a, H100) in-tree with nvcc.  `python -m pytorch_geometric_temporal_b200.build`."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libstmp.so")
 SOURCES = ["plan.cu", "spmm.cu", "dcrnn_seq.cu", "dcrnn_seq_tc.cu", "gemm_tc.cu", "cells.cu", "dcrnn_bwd.cu", "tgcn_attn.cu", "gemm_blocks.cu", "astgcn_factors.cu", "train.cu", "wgrad_tc.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
 
@@ -50,7 +50,7 @@ def build(force=False, verbose=False, extra_flags=(), out=None):
         if p.returncode != 0:
             sys.stderr.write("\n".join(log))
             raise RuntimeError(f"nvcc failed on {s}")
-    cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     subprocess.check_call(cmd)
     with open(os.path.join(HERE, "lib", "build.log"), "w") as f:
         f.write("\n".join(log))
@@ -72,7 +72,7 @@ def _build_variant(flags, out):
         o, _ = p.communicate()
         if p.returncode != 0:
             raise RuntimeError(f"nvcc failed on {s}:\n{o}")
-    subprocess.check_call([_nvcc(), "-shared", "-o", out, *objs, "-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call([_nvcc(), "-shared", "-o", out, *objs, "-gencode", "arch=compute_90a,code=sm_90a"])
     return out
 
 

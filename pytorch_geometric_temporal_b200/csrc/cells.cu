@@ -9,7 +9,7 @@ constexpr int kT = 256;
 inline unsigned grid_for(long long n) {
   long long b = (n + kT - 1) / kT;
   if (b < 1) b = 1;
-  if (b > 148ll * 32) b = 148ll * 32;
+  if (b > 132ll * 32) b = 132ll * 32;
   return (unsigned)b;
 }
 

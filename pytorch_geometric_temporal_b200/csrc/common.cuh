@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libstmp (sm_100a only).
+// common.cuh -- shared helpers for libstmp (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -67,7 +67,7 @@ struct stmp_plan {
   stmp::Csr fwd[2];  // by destination
   stmp::Csr bwd[2];  // by source (transposed product)
   int device = 0;
-  // Shared-memory image of the first n_ops operators for the fused tcgen05 kernel (gstart | order | padded edge
+  // Shared-memory image of the first n_ops operators for the fused tensor-core kernel (gstart | order | padded edge
   // entries, exactly as the kernel lays them out), built once at plan creation when the graph fits (N <= 207):
   // the kernel then fetches it with ONE TMA bulk copy instead of re-staging the CSR in every CTA.
   void* gimg[3] = {nullptr, nullptr, nullptr};   // index = n_ops (1, 2)
@@ -78,7 +78,7 @@ namespace stmp {
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
-// ---- small PTX wrappers (sm_100a) ---------------------------------------------------------------------
+// ---- small PTX wrappers (sm_90a) ---------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
@@ -166,6 +166,9 @@ __device__ __forceinline__ uint32_t map_to_peer(const void* p, uint32_t peer) {
 }
 __device__ __forceinline__ void st4_cluster(uint32_t addr, float4 v) {
   asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+__device__ __forceinline__ void st2_cluster(uint32_t addr, float2 v) {
+  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
 }
 
 // 16-byte store into the partner CTA's shared memory that also completes 16 transaction bytes on an mbarrier THERE: the receiver waits on its

@@ -219,7 +219,7 @@ __device__ __forceinline__ void adjoint_at(const Gr<SG> (&g)[2], const float* __
 }
 
 // SPLIT = 2: a thread-block cluster of two CTAs per window (launched when 2 B CTAs still fit the machine, i.e. at the reference's batch of 64
-// on 148 SMs): each CTA owns half of the node rows (a multiple of 8), runs the GEMMs / adjoints / gate derivatives of its rows only, and
+// on 132 SMs): each CTA owns half of the node rows (a multiple of 8), runs the GEMMs / adjoints / gate derivatives of its rows only, and
 // pushes its rows of dS into the partner's buf so that the adjoint gathers stay local.  Behind a GEMM the pair meets at a release / acquire
 // cluster barrier (dS visible); behind a gather phase each CTA only signals "done reading buf" (relaxed arrival) and the matching wait sits
 // in the next GEMM between its FFMA loop and its stores.

@@ -1,4 +1,4 @@
-// dcrnn_common.cuh -- device helpers shared by the fused DCRNN sequence kernels (FFMA and tcgen05 variants).
+// dcrnn_common.cuh -- device helpers shared by the fused DCRNN sequence kernels (FFMA and wgmma variants).
 #pragma once
 #include "common.cuh"
 
@@ -6,23 +6,10 @@ namespace stmp {
 
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
-// Packed fp32 FMA (sm_100 FFMA2): two independent fp32 FMAs per instruction.  A scalar multiplicand is
-// passed as (a,a); ptxas folds it into the .F32 broadcast operand form, so no extra moves are issued.
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\t"
-      "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-      "fma.rn.f32x2 rd, ra, rb, rc;\n\t"
-      "mov.b64 {%0, %1}, rd;\n\t}"
-      : "=f"(d.x), "=f"(d.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-  return d;
-}
+// Two independent fp32 FMAs (round to nearest, as one fma.rn each).
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ void fma4(float4& acc, float w, const float4& x) {
-  const float2 ww = make_float2(w, w);
-  const float2 lo = ffma2(ww, make_float2(x.x, x.y), make_float2(acc.x, acc.y));
-  const float2 hi = ffma2(ww, make_float2(x.z, x.w), make_float2(acc.z, acc.w));
-  acc = make_float4(lo.x, lo.y, hi.x, hi.y);
+  acc = make_float4(fmaf(w, x.x, acc.x), fmaf(w, x.y, acc.y), fmaf(w, x.z, acc.z), fmaf(w, x.w, acc.w));
 }
 
 // Shared-memory form of the two operators, built once per CTA from the plan's CSR:
@@ -99,7 +86,7 @@ __device__ __forceinline__ void stage_graph(const int* __restrict__ grp0, const 
     }
   }
   __syncthreads();
-  // order tasks: rows >= split_row first (the second MMA row tile of the tcgen05 kernel), then by descending
+  // order tasks: rows >= split_row first (the second MMA row tile of the wgmma kernel), then by descending
   // padded length (rank = number of tasks that sort before this one)
   for (int task = tid; task < NTASK; task += NT) {
     const int len = s_gstart[task + 1] - s_gstart[task];

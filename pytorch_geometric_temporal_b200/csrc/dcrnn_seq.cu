@@ -3,7 +3,7 @@
 // Reference path replaced: BatchedDCRNN.forward (nn/recurrent/dcrnn.py:429-475) = Python loop over T of
 // 3 x BatchedDConv (:258-325) + gates (:398-427); with B=T=1 it is DCRNN.forward (:194-219).
 //
-// Design (sm_100a):
+// Design (sm_90a):
 //  * grid = min(B, #SM) persistent CTAs; CTA b owns window b, b+grid, ...  Everything a window needs
 //    lives in shared memory for all T steps: both diffusion operators (CSR, (col,val) packed 8 B/edge),
 //    the three gates' weights, and the basis matrix S[N][NB*CP] = [U | P_o U | P_i U | ...] whose block 0
@@ -25,7 +25,7 @@
 #include "dcrnn_common.cuh"
 
 namespace stmp {
-// tcgen05 variant (dcrnn_seq_tc.cu)
+// wgmma variant (dcrnn_seq_tc.cu)
 extern int g_spmm_variant;
 extern int g_spmm_rows_per_group;
 extern int g_spmm_block;
@@ -52,7 +52,7 @@ int g_use_tc = -1;   // -1: read STMP_DCRNN_TC on first use
 
 namespace {
 
-constexpr int kMaxSmem = 232448;  // 227 KB opt-in limit per CTA on sm_100
+constexpr int kMaxSmem = 232448;  // 227 KB opt-in limit per CTA on sm_90
 
 struct DcrnnParams {
   int N, CIN, K, T;
@@ -424,7 +424,7 @@ using namespace stmp;
 
 extern "C" int stmp_dcrnn_seq_supported(const stmp_plan* plan, int64_t cin, int64_t cout, int64_t K) {
   if (!shape_ok(plan, cin, cout, K)) return 0;
-  if (g_use_tc != 0 && dcrnn_tc_supported(plan, cin, cout, K)) return 1;   // the tcgen05 kernel's envelope is wider in cin than the FFMA kernel's
+  if (g_use_tc != 0 && dcrnn_tc_supported(plan, cin, cout, K)) return 1;   // the wgmma kernel's envelope is wider in cin than the FFMA kernel's
   Layout L;
   return make_layout(plan, (int)cin, (int)cout, (int)K, 12, &L) ? 1 : 0;
 }
@@ -507,7 +507,7 @@ extern "C" int stmp_gru_seq_fwd(const stmp_plan* plan, int n_ops, int64_t B, int
                        h0_bstride, out, stash, wimage, workspace, (cudaStream_t)stream);
 }
 
-/* Test hook: select the kernel family behind stmp_dcrnn_seq_fwd at run time ("dcrnn_tc": 1 tcgen05 / 0 FFMA), so the two
+/* Test hook: select the kernel family behind stmp_dcrnn_seq_fwd at run time ("dcrnn_tc": 1 wgmma / 0 FFMA), so the two
  * independent implementations can be cross-checked against each other at full benchmark size. */
 extern "C" int stmp_set_option(const char* name, int value) {
   STMP_REQUIRE(name != nullptr, STMP_EINVAL, "stmp_set_option: NULL name");
@@ -531,7 +531,7 @@ extern "C" int stmp_dcrnn_pack_weights(int64_t cin, int64_t cout, int64_t K, con
                                        const float* b_z, const float* b_r, const float* b_h, void* image, void* stream) {
   STMP_REQUIRE(w_z && w_r && w_h && image, STMP_EINVAL, "stmp_dcrnn_pack_weights: NULL pointer");
   if (cout != 32 || K != 2 || cin < 1 || cin > 4)
-    return set_error(STMP_EUNSUPPORTED, "weight images exist for the tcgen05 kernel only (cout=32, K=2, cin<=4)");
+    return set_error(STMP_EUNSUPPORTED, "weight images exist for the wgmma kernel only (cout=32, K=2, cin<=4)");
   return tc_pack_weight_image(nullptr, nullptr, w_z, w_r, w_h, b_z, b_r, b_h, (int)cin, image, (cudaStream_t)stream);
 }
 

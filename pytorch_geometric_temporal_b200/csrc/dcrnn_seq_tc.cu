@@ -1,13 +1,12 @@
-// dcrnn_seq_tc.cu -- fused DCRNN recurrence with the dense contraction on the 5th-gen tensor cores.
+// dcrnn_seq_tc.cu -- fused DCRNN recurrence with the dense contraction on the Hopper tensor cores (wgmma).
 //
 // Same contract as k_dcrnn_seq (dcrnn_seq.cu) for K=2, Cout=32, Cin<=4, N<=255; what changes is WHERE the
-// S @ [Wz|Wr] and S @ Wh contractions run: `tcgen05.mma.kind::f16` with accumulators in TMEM instead of
-// FFMA in registers (the FFMA contraction is 58% of a step in the FFMA kernel, profiles/r01_dcrnn_seq_v3).
+// S @ [Wz|Wr] and S @ Wh contractions run: warpgroup MMAs (wgmma, fp32 accumulators in registers) instead of FFMA.
 //
 // fp32 accuracy on fp16 tensor cores: every fp32 operand v is split on the fly into hi = fp16(v) and
 // lo = fp16(v - hi) (22 mantissa bits together; products of fp16 pairs are exact in the fp32 accumulator) and
-// the product is formed as lo*hi + hi*lo + hi*hi -- three MMAs.  Validated stand-alone in tools/tc_probe.cu:
-// max |err| 6e-6 vs fp64 on K=112 dot products, the same order as an fp32 FMA chain (3e-6).
+// the product is formed as lo*hi + hi*lo + hi*hi -- three MMAs.  The tests hold the result to the fp32 oracle at
+// rtol 1e-4 / atol 1e-5 (tests/test_gpu_dcrnn.py).
 //
 // Shared memory (~204 KB of 227), all operands written by hand in the canonical K-major SWIZZLE_128B layout
 // (row pitch 128 B = 64 fp16, 16-byte chunk index XOR (row % 8), 8-row atoms of 1024 B):
@@ -15,12 +14,14 @@
 //   B_hi / B_lo : 2 K-panels x 96 rows    rows = output channels of z | r | h, same k order (7 k-steps of 16)
 //   U  fp32 [208][36] = H (or H*R) + 16 B of row padding: the gather source of the diffusion (tensor cores only see the fp16 split); row 207 = 0
 //   graph image (graph_image.cuh: balanced warp-task lists, 8-bit source rows four per word, values four per 128 bits),
-//   biases, 6 mbarriers, 2 arrival counters.
-// TMEM (256 columns): z|r accumulators of the two 128-row tiles at columns [0,64) [64,128), candidate at
-// [128,160) [160,192).  TMEM lane == row, so thread (warp w, lane l) owns row 128*(w/4) + 32*(w%4) + l for the
-// whole step: it reads its 64+32 accumulator columns with tcgen05.ld, applies the gates, keeps H in
-// registers, and writes H*R / H_t back as fp32 (U), as fp16 hi/lo (A panel) and to HBM.  16 warps: each row is
-// shared by two threads (channel halves), which also doubles the warps available to hide the gather latency.
+//   biases, one mbarrier (prologue TMA).
+// 16 warps = 4 warpgroups; warpgroup = (128-row MMA tile, channel slice).  A warpgroup issues the wgmmas of its tile and slice (two
+// m64 subtiles; z and r of GEMM 1, the candidate of GEMM 2, m64nCW each) and keeps the accumulators in registers, so every thread
+// applies the gates to the (row, channel) pairs its accumulator fragment holds: rows 64 s + 16 w + l/4 (+8) of its tile, channels
+// 8 j + 2 (l % 4) (+1) of its slice.  It keeps H of those pairs in registers and writes H*R / H_t back as fp32 (U), as fp16 hi/lo
+// (A panel) and to HBM.
+// ptxas serializes the wgmmas of this kernel (the issue points sit under warpgroup-uniform branches it cannot prove uniform), so the
+// MMAs of a tile do not overlap the gather of the next; every warpgroup waits for its own MMAs before its epilogue.
 #include <cuda_fp16.h>
 
 #include <cstdlib>
@@ -50,7 +51,6 @@ constexpr int TC_UROWS = 208;              // rows of U; row 207 is the all-zero
 constexpr int TC_AROWS = 208;              // rows stored per A panel (tile 1 over-reads into the next buffer: harmless)
 constexpr int TC_PANEL_A = TC_AROWS * 128;
 constexpr int TC_PANEL_B = 96 * 128;
-constexpr int TC_TMEM_COLS = 256;
 
 struct TcParams {
   int N, CIN, T;
@@ -149,9 +149,11 @@ typedef uint32_t img_idx_t;
 #endif
 static_assert(kImgRowPitchBytes == TC_UP * 4, "graph image offsets are pre-scaled by the gather buffer's row pitch");
 static_assert(kImgZeroRow * kImgRowPitchBytes < 65536, "row offsets must fit 16 bits");
+#if STMP_IMG_OFF16
 __device__ __forceinline__ float4 ld4_off(const float* base, uint32_t byte_off) {
   return *reinterpret_cast<const float4*>(reinterpret_cast<const unsigned char*>(base) + byte_off);
 }
+#endif
 // (u, v) = the task's first group, already loaded (gather_segment fetches it while the previous task is being gathered)
 __device__ __forceinline__ float4 gather_groups(const float* __restrict__ Uj, const img_idx_t* __restrict__ idx4,
                                                 const float4* __restrict__ val4, int g0, int ng, img_idx_t u, float4 v) {
@@ -186,25 +188,30 @@ __device__ __forceinline__ float4 gather_groups(const float* __restrict__ Uj, co
   return gather_groups(Uj, idx4, val4, g0, ng, idx4[g0], val4[g0]);
 }
 
-// Step anatomy (all 16 warps; T_k = MMA row tile k = rows [128k, 128k+128)):
-//   round 1  tid 0 issues the H | X k-steps of GEMM1 for both tiles; all warps gather [P_o H | P_i H] of T_0's rows -> A panels
-//            barrier; tid 0 issues T_0's P_o / P_i k-steps + commit -- the tensor core works on T_0 while the LSU gathers T_1's rows
-//            barrier; tid 0 issues T_1's k-steps + commit
-//   epi 1    wait GEMM1(own tile): R, H*R -> U, A panel                                                          barrier
+// Step anatomy (all 16 warps = 4 warpgroups; T_k = MMA row tile k = rows [128k, 128k+128)):
+//   round 1  every warpgroup issues the H | X k-steps of GEMM1 for its tile; all warps gather [P_o H | P_i H] of T_0's rows -> A panels
+//            barrier; T_0's warpgroups issue their P_o / P_i k-steps, then gather T_1's rows
+//            barrier; T_1's warpgroups issue their k-steps
+//   epi 1    wait GEMM1 (own MMAs): R, H*R; barrier (every MMA has read the A panels); H*R -> U, A panel                      barrier
 //   round 2  same gathers over H*R, GEMM2 (candidate)
-//   epi 2    wait GEMM2(own tile): Z (recomputed from TMEM), H~, H_t -> U, A panel, HBM;  X_{t+1} k-step           barrier
+//   epi 2    wait GEMM2: Z (from the GEMM1 accumulators, still in registers), H~, H_t; barrier; H_t -> U, A panel, HBM;
+//            X_{t+1} k-step                                                                                                  barrier
+// A warpgroup issues the wgmmas of its own (tile, channel slice): the accumulator fragments then sit in the threads that apply the
+// gates, so the epilogue is register-local.  Thread (warp w of the group, lane l) owns rows 64 s + 16 w + l/4 (+8), s = 0, 1, of its tile
+// and channels ch0 + 8 j + 2 (l % 4) (+1) of its slice.
 // The task lists of the gather are balanced over the warps when the plan is built (graph_image.cuh), which is what makes the extra
 // barriers cheap (round 1 profile: 25 % of all warp time was barrier wait behind the warp that always drew the longest rows).
 // X is never gathered per step: P_o X_t, P_i X_t of ALL steps of a window are produced by one gather pass over rows of
 // T*Cin floats in the window prologue and parked in the window's own (not yet written) output rows out[b, t, :, 0:8].
 // SPLIT = 2 (small batches: 2 B CTAs still fit the machine, N > 128): a window is served by a 2-CTA thread-block cluster.  CTA c owns MMA
-// row tile c -- its gather tasks, its MMAs, its epilogue (all 16 warps: thread = (row, channel quarter)) -- and pushes the rows of H*R / H_t it
+// row tile c -- its gather tasks, its MMAs, its epilogue (warpgroup = channel quarter) -- and pushes the rows of H*R / H_t it
 // produces into the partner's gather buffer U through distributed shared memory, so both gathers stay local.  Per round: "done reading U"
 // is a relaxed cluster arrival right after the gather, waited for just before the epilogue overwrites U; the barrier that closes an epilogue is
 // a release / acquire cluster barrier (the pushed rows are visible).
 template <int CIN, int SPLIT>
 __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
-  constexpr int CW = SPLIT == 2 ? 8 : 16;   // channels per thread (two / four threads share a row)
+  constexpr int CW = SPLIT == 2 ? 8 : 16;   // channels per warpgroup (two / four warpgroups share a tile)
+  constexpr int NP = CW / 8;                // channel pairs of a thread per row
   extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int N = p.N, T = p.T;
@@ -220,28 +227,23 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
   const img_idx_t* s_idx = reinterpret_cast<const img_idx_t*>(img + p.gl.off_idx);
   const float4* s_val = reinterpret_cast<const float4*>(img + p.gl.off_val);
   float* Bs = reinterpret_cast<float*>(smem + p.off_bias);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.off_bar);   // [0..3] MMA done (gemm*2+tile), [4] prologue TMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
+  uint64_t* tma_bar = reinterpret_cast<uint64_t*>(smem + p.off_bar);   // prologue TMA (graph and weight images)
 
   const int crank = SPLIT == 2 ? (int)cluster_rank() : 0;
   const long long cta = blockIdx.x / SPLIT, n_cta = gridDim.x / SPLIT;
   if (cta >= p.B) return;
 
   // ---- one-time per CTA ------------------------------------------------------------------------------------
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TC_TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
-    for (int i = 0; i < 5; ++i) mbar_init(&bars[i], 1);
+    mbar_init(tma_bar, 1);
     fence_mbar_init();
     const uint32_t tx = (p.n_ops ? (uint32_t)p.gl.bytes : 0u) + (p.wimage ? (uint32_t)TC_WIMAGE_BYTES : 0u);
     if (tx) {   // graph image and weight image arrive by TMA bulk copies while the CTA zeroes its panels
-      mbar_arrive_expect_tx(&bars[4], tx);
-      if (p.n_ops) tma_bulk_g2s(smem + p.off_img, p.gimg, (uint32_t)p.gl.bytes, &bars[4]);
+      mbar_arrive_expect_tx(tma_bar, tx);
+      if (p.n_ops) tma_bulk_g2s(smem + p.off_img, p.gimg, (uint32_t)p.gl.bytes, tma_bar);
       if (p.wimage) {
-        tma_bulk_g2s(b_hi, p.wimage, 4u * TC_PANEL_B, &bars[4]);
-        tma_bulk_g2s(Bs, reinterpret_cast<const unsigned char*>(p.wimage) + 4 * TC_PANEL_B, 96u * 4u, &bars[4]);
+        tma_bulk_g2s(b_hi, p.wimage, 4u * TC_PANEL_B, tma_bar);
+        tma_bulk_g2s(Bs, reinterpret_cast<const unsigned char*>(p.wimage) + 4 * TC_PANEL_B, 96u * 4u, tma_bar);
       }
     }
   }
@@ -269,63 +271,87 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
       Bs[idx] = p.bcat ? p.bcat[idx] : (bg ? bg[idx & 31] : 0.f);
     }
   }
-  if (p.n_ops || p.wimage) mbar_wait(&bars[4], 0);
+  if (p.n_ops || p.wimage) mbar_wait(tma_bar, 0);
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  // thread = (row, channel half): warp = half*8 + tile*4 + q ; TMEM lane == row, a warp may only touch lanes 32*(warp%4)..
-  // (cluster pair: thread = (row of my tile, channel quarter): warp = quarter*4 + q)
-  const int half = SPLIT == 2 ? (warp >> 2) : (warp >> 3), tile = SPLIT == 2 ? crank : ((warp >> 2) & 1), q = warp & 3;
-  const int row = tile * 128 + q * 32 + lane;
+  // warpgroup wg = (channel slice, tile): SPLIT 1: wg = half * 2 + tile; cluster pair: wg = channel quarter, tile = my rank
+  const int wg = warp >> 2, wt = tid & 127;
+  const int half = SPLIT == 2 ? wg : (wg >> 1), tile = SPLIT == 2 ? crank : (wg & 1);
   const int ch0 = CW * half;
-  const bool live = row < N;
-  const bool owner = live && half == 0;      // the thread that feeds its row's X k-step
-  const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16);
+  const int fr = tile * 128 + 16 * (wt >> 5) + ((wt & 31) >> 2);   // my first row; the others are +8, +64, +72
+  const int fc = 2 * (wt & 3);                                      // my first channel inside the slice; the others are +1, +8, +9
+  auto frow = [&](int e) { return fr + 64 * (e >> 1) + 8 * (e & 1); };   // e = 2 s + (second row of the fragment)
   const uint32_t a_hi_s = smem_u32(a_hi), a_lo_s = smem_u32(a_lo), b_hi_s = smem_u32(b_hi), b_lo_s = smem_u32(b_lo);
-  constexpr uint32_t ID64 = umma_idesc_f16(128, 64), ID32 = umma_idesc_f16(128, 32);
-  uint32_t parity = 0;
   const bool two_tiles = N > 128;
+  const bool has_rows = tile * 128 < N;
+  const bool sub1 = tile * 128 + 64 < N;    // the second 64-row subtile of my tile has rows
   const int j = lane & 7, quarter = lane >> 3;
   const float* Uj = U + 4 * j;
+  // the thread that feeds row `xrow`'s X k-step (one row per thread; the cluster pair feeds the rows of its own tile)
+  const int xrow = SPLIT == 2 ? crank * 128 + tid : tid;
+  const bool x_owner = (SPLIT == 2 ? tid < 128 : true) && xrow < N;
   uint32_t peer_U = 0;
   if constexpr (SPLIT == 2) peer_U = map_to_peer(U, (uint32_t)(crank ^ 1));
-  // store a float4 of my row into U -- and into the partner's U in the cluster-pair variant
-  auto put_u = [&](int off, float4 v) {
-    st4(U + off, v);
-    if constexpr (SPLIT == 2) st4_cluster(peer_U + (uint32_t)off * 4u, v);
+  // store two floats of a row into U -- and into the partner's U in the cluster-pair variant
+  auto put_u = [&](int off, float2 v) {
+    *reinterpret_cast<float2*>(U + off) = v;
+    if constexpr (SPLIT == 2) st2_cluster(peer_U + (uint32_t)off * 4u, v);
+  };
+  // two channels (c, c+1) of a row -> panel 0 as fp16 hi / lo
+  auto store_split2 = [&](int row, int c, float a, float b) {
+    const __half2 h = __floats2half2_rn(a, b);
+    const float2 f = __half22float2(h);
+    const int off = sw128(row, c);
+    *reinterpret_cast<uint32_t*>(a_hi + off) = pack_h2(h);
+    *reinterpret_cast<uint32_t*>(a_lo + off) = pack_h2(__floats2half2_rn(a - f.x, b - f.y));
   };
   // barrier that closes an epilogue / the window prologue: operand + U stores of everybody visible to the MMAs and the next gather
   auto close_phase = [&]() {
     fence_proxy_async();
-    tc_fence_before();
     if constexpr (SPLIT == 2) cluster_sync_all(); else __syncthreads();
-    tc_fence_after();
   };
 
-  // The 3 x 7 MMAs of one (tile, gemm) are issued in three groups, each as soon as its k-steps are in shared memory, each with
-  // its own commit to the (tile, gemm) barrier (count 3):
+  float accz[2][CW / 2], accr[2][CW / 2], acch[2][CW / 2];   // m64 x CW accumulators of my two subtiles: z, r (GEMM 1), candidate (GEMM 2)
+  // The 3 x 7 k-steps of one gemm are issued in three commit groups, each as soon as its k-steps are in shared memory:
   //   group 0: k-steps of H | H*R and X  -- complete when the round starts; its first MMA overwrites the accumulator
   //   group 1: k-steps of P_o H          -- after the last warp finished the tile's P_o tasks
   //   group 2: k-steps of P_i H          -- after the last warp finished the tile's P_i tasks
-  // so the tensor core runs underneath the gather and only the last group's 6 MMAs are exposed at the end of a round.
-  auto issue_group = [&](int tl, int gm, int grp) {
-    const uint32_t dcol = gm == 0 ? 64u * tl : 128u + 32u * tl;
+  // (each group is one wgmma commit group; ptxas serializes them, see the file header).
+  auto issue_group = [&](int gm, int grp) {
     const int ks0 = grp == 0 ? 0 : (grp == 1 ? 2 : 4);
+    wgmma_fence();
 #pragma unroll
     for (int pass = 0; pass < 3; ++pass) {           // lo*hi, hi*lo, hi*hi (small terms first)
-      const uint32_t ab = (pass == 0 ? a_lo_s : a_hi_s) + tl * (128 * 128);
-      const uint32_t bb = (pass == 1 ? b_lo_s : b_hi_s) + (gm ? 64 * 128 : 0);
+      const uint32_t ab = (pass == 0 ? a_lo_s : a_hi_s) + tile * (128 * 128);
+      const uint32_t bb = pass == 1 ? b_lo_s : b_hi_s;
 #pragma unroll
       for (int i = 0; i < 3; ++i) {
         if (i == 2 && grp != 0) continue;
         const int ks = i == 2 ? 6 : ks0 + i;
         const int panel = ks >> 2, kin = (ks & 3) * 16;
-        umma_f16(tmem + dcol, umma_desc(ab + panel * TC_PANEL_A + kin * 2), umma_desc(bb + panel * TC_PANEL_B + kin * 2),
-                 gm == 0 ? ID64 : ID32, (grp == 0 && pass == 0 && i == 0) ? 0u : 1u);
+        const uint32_t sc = (grp == 0 && pass == 0 && i == 0) ? 0u : 1u;
+        const uint32_t bk = bb + panel * TC_PANEL_B + kin * 2;
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          if (s == 1 && !sub1) continue;
+          const uint64_t da = gmma_desc_sw128(ab + s * (64 * 128) + panel * TC_PANEL_A + kin * 2);
+          if (gm == 0) {
+            wgmma_f16<CW>(accz[s], da, gmma_desc_sw128(bk + ch0 * 128), sc);
+            wgmma_f16<CW>(accr[s], da, gmma_desc_sw128(bk + (32 + ch0) * 128), sc);
+          } else {
+            wgmma_f16<CW>(acch[s], da, gmma_desc_sw128(bk + (64 + ch0) * 128), sc);
+          }
+        }
       }
+    }
+    wgmma_commit();
+  };
+  auto wait_gemm = [&](int gm) {
+    if (has_rows) wgmma_wait<0>();
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      if (gm == 0) { acc_fence(accz[s]); acc_fence(accr[s]); } else { acc_fence(acch[s]); }
     }
   };
 
@@ -365,69 +391,59 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
     }
 #endif
   };
-  // One gather round.  tid 0 issues every MMA: the static group (H | X k-steps) of both tiles right away (the block barrier in front of
-  // the round ordered those operand stores), tile 0's P_o / P_i groups behind the barrier that closes tile 0's tasks -- they run on the
-  // tensor core while the LSU gathers tile 1 -- and tile 1's groups behind the closing barrier.  One commit per tile covers all of
-  // that tile's MMAs (same issuing thread => in order).  The task lists are balanced (graph_image.cuh), so the two barriers are cheap;
-  // the closing one also tells the epilogue that nobody reads U any more.
+  // One gather round.  Every warpgroup issues the static group (H | X k-steps) of its tile right away (the block barrier in front of
+  // the round ordered those operand stores), tile 0's warpgroups their P_o / P_i groups behind the barrier that closes tile 0's tasks,
+  // and tile 1's warpgroups theirs behind the closing barrier.  The task
+  // lists are balanced (graph_image.cuh), so the two barriers are cheap; the closing one also tells the epilogue that nobody reads U any more.
   auto gather_round = [&](int gm) {
     if constexpr (SPLIT == 2) {
-      if (tid == 0) issue_group(crank, gm, 0);
+      issue_group(gm, 0);
       if (p.n_ops > 0) gather_segment(2 * crank);
       if (p.n_ops > 1) gather_segment(2 * crank + 1);
       cluster_arrive_relaxed();   // this CTA has finished reading U (waited for by the partner before its epilogue overwrites my U)
       fence_proxy_async();
-      tc_fence_before();
       __syncthreads();
-      tc_fence_after();
-      if (tid == 0) {
-        issue_group(crank, gm, 1);
-        issue_group(crank, gm, 2);
-        umma_commit(&bars[2 * gm + crank]);
-      }
+      issue_group(gm, 1);
+      issue_group(gm, 2);
       return;
     }
-    if (tid == 0) {
-      issue_group(0, gm, 0);
-      if (two_tiles) issue_group(1, gm, 0);
-    }
+    if (has_rows) issue_group(gm, 0);
     if (p.n_ops > 0) gather_segment(0);
     if (p.n_ops > 1) gather_segment(1);
     fence_proxy_async();        // my generic-proxy stores to the A panels -> visible to the tensor core (async proxy)
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    if (tid == 0) {
-      issue_group(0, gm, 1);
-      issue_group(0, gm, 2);
-      umma_commit(&bars[2 * gm]);
+    if (tile == 0) {
+      issue_group(gm, 1);
+      issue_group(gm, 2);
     }
     if (two_tiles) {
       if (p.n_ops > 0) gather_segment(2);
       if (p.n_ops > 1) gather_segment(3);
     }
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    if (tid == 0 && two_tiles) {
-      issue_group(1, gm, 1);
-      issue_group(1, gm, 2);
-      umma_commit(&bars[2 * gm + 1]);
+    if (tile == 1 && two_tiles) {
+      issue_group(gm, 1);
+      issue_group(gm, 2);
     }
+  };
+  // every MMA of the CTA has read the A panels (each is issued by the warpgroup of its channel slice): only then are they overwritten
+  auto operands_free = [&]() {
+    __syncthreads();
+    if constexpr (SPLIT == 2) cluster_wait();       // the partner is done gathering from its U
   };
 
   auto x_base = [&](long long b) -> const float* { return p.x + (p.win_start ? p.win_start[b] * p.x_tstride : b * p.x_bstride); };
-  // [X_t | P_o X_t | P_i X_t] of my row -> k 32..43 of panel 1 (weights of absent channels / operators are zero, but the
+  // [X_t | P_o X_t | P_i X_t] of row xrow -> k 32..43 of panel 1 (weights of absent channels / operators are zero, but the
   // operand itself must be finite: everything not produced is written as 0 -- at store time, so the loads stay in flight)
   auto load_x = [&](const float* xb, long long b, int t, float4& xv, float4& po, float4& pi) {
     float xn[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-    for (int c = 0; c < CIN; ++c) xn[c] = __ldg(xb + t * p.x_tstride + row * CIN + c);
+    for (int c = 0; c < CIN; ++c) xn[c] = __ldg(xb + t * p.x_tstride + xrow * CIN + c);
     xv = make_float4(xn[0], xn[1], xn[2], xn[3]);
     po = pi = make_float4(0.f, 0.f, 0.f, 0.f);
     if (p.ws) {             // per-CTA workspace rows [row][op][t*CIN + c]: rewritten every window, so they stay in L2
-      const float* w0 = p.ws + (((long long)blockIdx.x * N + row) * 2) * p.ws_pitch + t * CIN;
+      const float* w0 = p.ws + (((long long)blockIdx.x * N + xrow) * 2) * p.ws_pitch + t * CIN;
       float a0[4] = {0.f, 0.f, 0.f, 0.f}, a1[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
       for (int c = 0; c < CIN; ++c) {
@@ -438,7 +454,7 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
       pi = make_float4(a1[0], a1[1], a1[2], a1[3]);
       return;
     }
-    const float* sc = p.out + ((b * T + t) * (long long)N + row) * 32;   // parked there by the window prologue (plain loads:
+    const float* sc = p.out + ((b * T + t) * (long long)N + xrow) * 32;  // parked there by the window prologue (plain loads:
     if (p.n_ops >= 1) po = *reinterpret_cast<const float4*>(sc);         //  written by this CTA earlier in this launch)
     if (p.n_ops >= 2) pi = *reinterpret_cast<const float4*>(sc + 4);
   };
@@ -449,9 +465,9 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
     return v;
   };
   auto store_x = [&](const float4& xv, const float4& po, const float4& pi) {
-    store_split4(a_hi + TC_PANEL_A, a_lo + TC_PANEL_A, row, 32, xv);
-    store_split4(a_hi + TC_PANEL_A, a_lo + TC_PANEL_A, row, 36, mask_c(po));
-    store_split4(a_hi + TC_PANEL_A, a_lo + TC_PANEL_A, row, 40, mask_c(pi));
+    store_split4(a_hi + TC_PANEL_A, a_lo + TC_PANEL_A, xrow, 32, xv);
+    store_split4(a_hi + TC_PANEL_A, a_lo + TC_PANEL_A, xrow, 36, mask_c(po));
+    store_split4(a_hi + TC_PANEL_A, a_lo + TC_PANEL_A, xrow, 40, mask_c(pi));
   };
 
   for (long long b = cta; b < p.B; b += n_cta) {
@@ -526,24 +542,30 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
       }
     }
     // ---- window prologue B: H_0 into U (fp32) and the A panels (fp16 hi/lo); the X k-step of step 0 ---------------------------
-    float hreg[CW];
+    float hreg[4][2 * NP];      // [fragment row e][channel 8 jj + fc + x at 2 jj + x]
     if constexpr (SPLIT == 2) {   // the partner has finished the X gather of its prologue: its U may be overwritten
       cluster_arrive_relaxed();
       cluster_wait();
     }
-    if (live) {
 #pragma unroll
-      for (int c = 0; c < CW / 4; ++c) {
-        const float4 h = p.h0 ? __ldg(reinterpret_cast<const float4*>(p.h0 + b * p.h0_bstride + row * 32 + ch0) + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-        hreg[4 * c] = h.x; hreg[4 * c + 1] = h.y; hreg[4 * c + 2] = h.z; hreg[4 * c + 3] = h.w;
-        put_u(row * TC_UP + ch0 + 4 * c, h);
+    for (int e = 0; e < 4; ++e) {
+      const int row = frow(e);
+#pragma unroll
+      for (int jj = 0; jj < NP; ++jj) {
+        const int c = ch0 + 8 * jj + fc;
+        float2 h = make_float2(0.f, 0.f);
+        if (row < N && p.h0) h = __ldg(reinterpret_cast<const float2*>(p.h0 + b * p.h0_bstride + row * 32 + c));
+        hreg[e][2 * jj] = h.x; hreg[e][2 * jj + 1] = h.y;
+        if (row < N) {
+          put_u(row * TC_UP + c, h);
+          store_split2(row, c, h.x, h.y);
+        }
       }
-      store_split_row<CW>(a_hi, a_lo, row, half, hreg);
-      if (owner) {
-        float4 xv, po, pi;
-        load_x(xb, b, 0, xv, po, pi);
-        store_x(xv, po, pi);
-      }
+    }
+    if (x_owner) {
+      float4 xv, po, pi;
+      load_x(xb, b, 0, xv, po, pi);
+      store_x(xv, po, pi);
     }
     close_phase();             // the first MMA group of step 0 is issued right behind this barrier
 
@@ -551,31 +573,32 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
       // ---- round 1: diffuse H ------------------------------------------------------------------------------------------
       gather_round(0);
       // ---- epilogue 1: r gate; H*R ---------------------------------------------------------------------------------------
-      if (tile == 0 || two_tiles) mbar_wait(&bars[tile], parity);   // tile 1 has no rows when N <= 128
-      tc_fence_after();
+      wait_gemm(0);
       const long long obase = (b * T + t) * (long long)N;
       {
-        uint32_t vr[CW];
-        tmem_ld<CW>(trow + 64 * tile + 32 + ch0, vr);
-        tmem_ld_wait();
-        float hr[CW];
+        float hr[4][2 * NP], rv[4][2 * NP];
 #pragma unroll
-        for (int c = 0; c < CW; ++c) {
-          const float r = sigmoid_fast(__uint_as_float(vr[c]) + Bs[32 + ch0 + c]);
-          hr[c] = hreg[c] * r;
-          vr[c] = __float_as_uint(r);
-        }
-        if constexpr (SPLIT == 2) cluster_wait();       // the partner is done gathering from its U
-        if (live) {
+        for (int e = 0; e < 4; ++e)
 #pragma unroll
-          for (int c = 0; c < CW / 4; ++c) put_u(row * TC_UP + ch0 + 4 * c, make_float4(hr[4 * c], hr[4 * c + 1], hr[4 * c + 2], hr[4 * c + 3]));
-          store_split_row<CW>(a_hi, a_lo, row, half, hr);
-          if (p.stash) {
-            float* sp = p.stash + ((obase * 3) + row) * 32 + ch0;
+          for (int jj = 0; jj < NP; ++jj)
 #pragma unroll
-            for (int c = 0; c < CW / 4; ++c) {
-              st4(sp + (long long)N * 32 + 4 * c, make_float4(__uint_as_float(vr[4 * c]), __uint_as_float(vr[4 * c + 1]),
-                                                              __uint_as_float(vr[4 * c + 2]), __uint_as_float(vr[4 * c + 3])));
+            for (int x = 0; x < 2; ++x) {
+              const float r = sigmoid_fast(accr[e >> 1][4 * jj + 2 * (e & 1) + x] + Bs[32 + ch0 + 8 * jj + fc + x]);
+              hr[e][2 * jj + x] = hreg[e][2 * jj + x] * r;
+              rv[e][2 * jj + x] = r;
+            }
+        operands_free();
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int row = frow(e);
+          if (row < N) {
+#pragma unroll
+            for (int jj = 0; jj < NP; ++jj) {
+              const int c = ch0 + 8 * jj + fc;
+              put_u(row * TC_UP + c, make_float2(hr[e][2 * jj], hr[e][2 * jj + 1]));
+              store_split2(row, c, hr[e][2 * jj], hr[e][2 * jj + 1]);
+              if (p.stash)
+                *reinterpret_cast<float2*>(p.stash + ((obase * 3) + row) * 32 + (long long)N * 32 + c) = make_float2(rv[e][2 * jj], rv[e][2 * jj + 1]);
             }
           }
         }
@@ -585,54 +608,52 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
       gather_round(1);
       // ---- epilogue 2: candidate, H_t --------------------------------------------------------------------------------------
       float4 xv, po, pi;
-      const bool feed_x = owner && t + 1 < T;
+      const bool feed_x = x_owner && t + 1 < T;
       if (feed_x) load_x(xb, b, t + 1, xv, po, pi);      // in flight under the MMA wait
-      if (tile == 0 || two_tiles) mbar_wait(&bars[2 + tile], parity);
-      tc_fence_after();
+      wait_gemm(1);
       {
-        // Z is recomputed from its accumulator, which stays in TMEM until the next step's GEMM 1: cheaper than keeping
-        // CW registers alive (and spilling) across the second diffusion round
-        uint32_t vh[CW], vz[CW];
-        tmem_ld<CW>(trow + 128 + 32 * tile + ch0, vh);
-        tmem_ld<CW>(trow + 64 * tile + ch0, vz);
-        tmem_ld_wait();
-        float ht[CW], zreg[CW];
+        // Z comes from its GEMM-1 accumulators, which stay in registers until the next step's GEMM 1
+        float ht[4][2 * NP], zreg[4][2 * NP];
 #pragma unroll
-        for (int c = 0; c < CW; ++c) {
-          zreg[c] = sigmoid_fast(__uint_as_float(vz[c]) + Bs[ch0 + c]);
-          ht[c] = tanh_fast(__uint_as_float(vh[c]) + Bs[64 + ch0 + c]);
-          hreg[c] = zreg[c] * hreg[c] + (1.0f - zreg[c]) * ht[c];   // dcrnn.py:190-192
-        }
-        if constexpr (SPLIT == 2) cluster_wait();
-        if (live) {
-          float* op = p.out + (obase + row) * 32 + ch0;
+        for (int e = 0; e < 4; ++e)
 #pragma unroll
-          for (int c = 0; c < CW / 4; ++c) {
-            const float4 hv = make_float4(hreg[4 * c], hreg[4 * c + 1], hreg[4 * c + 2], hreg[4 * c + 3]);
-            put_u(row * TC_UP + ch0 + 4 * c, hv);
-            st4(op + 4 * c, hv);
-          }
-          store_split_row<CW>(a_hi, a_lo, row, half, hreg);
-          if (p.stash) {
-            float* sp = p.stash + ((obase * 3) + row) * 32 + ch0;
+          for (int jj = 0; jj < NP; ++jj)
 #pragma unroll
-            for (int c = 0; c < CW / 4; ++c) {
-              st4(sp + 4 * c, make_float4(zreg[4 * c], zreg[4 * c + 1], zreg[4 * c + 2], zreg[4 * c + 3]));
-              st4(sp + 2 * (long long)N * 32 + 4 * c, make_float4(ht[4 * c], ht[4 * c + 1], ht[4 * c + 2], ht[4 * c + 3]));
+            for (int x = 0; x < 2; ++x) {
+              const int c = ch0 + 8 * jj + fc + x, a = 4 * jj + 2 * (e & 1) + x;
+              const float z = sigmoid_fast(accz[e >> 1][a] + Bs[c]);
+              const float h = tanh_fast(acch[e >> 1][a] + Bs[64 + c]);
+              zreg[e][2 * jj + x] = z;
+              ht[e][2 * jj + x] = h;
+              hreg[e][2 * jj + x] = z * hreg[e][2 * jj + x] + (1.0f - z) * h;   // dcrnn.py:190-192
+            }
+        operands_free();
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int row = frow(e);
+          if (row < N) {
+            float* op = p.out + (obase + row) * 32;
+#pragma unroll
+            for (int jj = 0; jj < NP; ++jj) {
+              const int c = ch0 + 8 * jj + fc;
+              const float2 hv = make_float2(hreg[e][2 * jj], hreg[e][2 * jj + 1]);
+              put_u(row * TC_UP + c, hv);
+              *reinterpret_cast<float2*>(op + c) = hv;
+              store_split2(row, c, hv.x, hv.y);
+              if (p.stash) {
+                float* sp = p.stash + ((obase * 3) + row) * 32;
+                *reinterpret_cast<float2*>(sp + c) = make_float2(zreg[e][2 * jj], zreg[e][2 * jj + 1]);
+                *reinterpret_cast<float2*>(sp + 2 * (long long)N * 32 + c) = make_float2(ht[e][2 * jj], ht[e][2 * jj + 1]);
+              }
             }
           }
-          if (feed_x) store_x(xv, po, pi);
         }
+        if (feed_x) store_x(xv, po, pi);
       }
-      parity ^= 1u;
       close_phase();
     }
   }
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TC_TMEM_COLS));
 }
-
-
-inline int align_up(int v, int a) { return (v + a - 1) / a * a; }
 
 // shared-memory layout for `n_ops` operators of `plan`
 bool tc_layout(const stmp_plan* plan, int n_ops, TcParams* p, int* smem_bytes) {
@@ -645,7 +666,7 @@ bool tc_layout(const stmp_plan* plan, int n_ops, TcParams* p, int* smem_bytes) {
   p->gl = graph_image_layout(n_ops * plan->n, nnz);
   p->off_img = off; off += n_ops ? p->gl.bytes : 0;
   p->off_bias = off; off += 96 * 4;
-  p->off_bar = off; off += 64;
+  p->off_bar = off; off += 8;
   *smem_bytes = off;
   return off <= kMaxSmemTc;
 }
@@ -655,7 +676,7 @@ bool tc_layout(const stmp_plan* plan, int n_ops, TcParams* p, int* smem_bytes) {
 int tc_ws_pitch(long long T, long long cin) { return (int)((T * cin + 7) / 8 * 8); }   // floats per (row, operator): whole 32-byte sectors
 
 long long tc_workspace_bytes(const stmp_plan* plan, long long T, long long cin) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return (long long)sms * plan->n * 2 * tc_ws_pitch(T, cin) * 4;
 }
@@ -710,9 +731,9 @@ int gru_tc_launch(const stmp_plan* plan, int n_ops, long long B, long long T, lo
 static int tc_launch_params(const stmp_plan* plan, TcParams& p, cudaStream_t st) {
   int smem = 0;
   const long long B = p.B;
-  if (!tc_layout(plan, p.n_ops, &p, &smem)) return set_error(STMP_EUNSUPPORTED, "tcgen05 graph-GRU kernel needs %d B of shared memory", smem);
+  if (!tc_layout(plan, p.n_ops, &p, &smem)) return set_error(STMP_EUNSUPPORTED, "tensor-core graph-GRU kernel needs %d B of shared memory", smem);
   p.gimg = p.n_ops ? plan->gimg[p.n_ops] : nullptr;
-  if (p.n_ops && !p.gimg) return set_error(STMP_EUNSUPPORTED, "tcgen05 graph-GRU kernel: the plan has no shared-memory graph image");
+  if (p.n_ops && !p.gimg) return set_error(STMP_EUNSUPPORTED, "tensor-core graph-GRU kernel: the plan has no shared-memory graph image");
   int dev = 0, sms = 0;
   STMP_CUDA_OK(cudaGetDevice(&dev));
   STMP_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -739,7 +760,7 @@ static int tc_launch_params(const stmp_plan* plan, TcParams& p, cudaStream_t st)
     break;
     STMP_TC_CASE(1) STMP_TC_CASE(2) STMP_TC_CASE(3) STMP_TC_CASE(4)
 #undef STMP_TC_CASE
-    default: return set_error(STMP_EUNSUPPORTED, "tcgen05 graph-GRU kernel: cin %d not in 1..4", p.CIN);
+    default: return set_error(STMP_EUNSUPPORTED, "tensor-core graph-GRU kernel: cin %d not in 1..4", p.CIN);
   }
   STMP_LAUNCH_OK("k_dcrnn_seq_tc");
   if (split) { static const int slot2 = path_slot("k_dcrnn_seq_tc[cluster2]"); count_path(slot2); }

@@ -1,4 +1,4 @@
-// gemm_blocks.cu -- the dense products of an ASTGCN block (nn/attention/astgcn.py) on the 5th-gen tensor cores, fp32 in / fp32 out,
+// gemm_blocks.cu -- the dense products of an ASTGCN block (nn/attention/astgcn.py) on the Hopper tensor cores (wgmma), fp32 in / fp32 out,
 // with the operand GATHER and the pointwise tail of each product fused into one kernel:
 //
 //   C[m, :] = epilogue( sum_blocks  A_blk[row(m) + shift_blk, 0:width_blk] @ W_blk  + bias )
@@ -13,10 +13,10 @@
 // * MODE_SPATT generates the A operand instead of loading it: spatial attention (astgcn.py:245-262)
 //     S = softmax_dim1( Vs @ sigmoid(LHS @ RHS + bs) )   is computed TRANSPOSED,  S^T[b] = sigmoid(...)^T @ Vs^T, rows (b, j):
 //     A[(b,j)][k] = sigmoid( sum_t LHS[b,k,t] RHS[b,t,j] + bs[k][j] )  is formed on the fly from the two (B,N,T) factors, and the
-//     softmax over dim 1 of S becomes a softmax over the COLUMNS of each output row -- thread-local in the epilogue (TMEM lane ==
-//     row).  2 B N^3 FLOPs, the one GEMM of the model SURVEY calls a tensor-core target, never materialises the N x N sigmoid.
-// * fp32-class accuracy from fp16 tensor cores: operands split into hi = fp16(v), lo = fp16(v - hi), three tcgen05.mma.kind::f16
-//   passes lo*hi + hi*lo + hi*hi into the fp32 TMEM accumulator (as gemm_tc.cu / dcrnn_seq_tc.cu; tools/tc_probe.cu).
+//     softmax over dim 1 of S becomes a softmax over the COLUMNS of each output row -- thread-local in the epilogue (the accumulators are
+//     staged in shared memory, one thread per row).  2 B N^3 FLOPs, the one GEMM of the model SURVEY calls a tensor-core target, never materialises the N x N sigmoid.
+// * fp32-class accuracy from fp16 tensor cores: operands split into hi = fp16(v), lo = fp16(v - hi), three wgmma f16 passes
+//   lo*hi + hi*lo + hi*hi into fp32 register accumulators (as gemm_tc.cu / dcrnn_seq_tc.cu).
 // One CTA = 128 rows x all N (<= 320) columns; N > 256 runs as two MMA column halves.  2-stage pipeline: the tile of k-block i+1 is
 // loaded / generated / converted while the MMAs of k-block i run.
 #include "common.cuh"
@@ -29,6 +29,7 @@ constexpr int GB_NT = 256;
 constexpr int GB_BM = 128;
 constexpr int GB_A_BYTES = GB_BM * 128;   // one K-block of A (hi or lo): 128 rows x 64 fp16
 constexpr int GB_MAXBLK = 12;
+constexpr int GB_MAXN = 320;
 
 enum { EPI_BIAS = 0, EPI_RELU = 1, EPI_RELU_LN = 2, EPI_SOFTMAX = 3 };
 
@@ -62,31 +63,26 @@ struct GbParams {
 
 __device__ __forceinline__ float sigmoid_g(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
 
-template <int EPI>
-__global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_blocks(const GbParams p) {
+// NCH: accumulator column chunks of 16 compiled in (N <= 16 NCH); the small-N instance keeps two CTAs per SM
+template <int EPI, int NCH>
+__global__ void __launch_bounds__(GB_NT, (EPI == EPI_SOFTMAX || NCH > 4) ? 1 : 2) k_gemm_blocks(const GbParams p) {
   constexpr bool SPATT = EPI == EPI_SOFTMAX;         // spatial attention: generated A operand + row-softmax epilogue
   extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int N = p.N;
   const int b_bytes = N * 128;                       // one K-block of B (hi or lo)
   const int stage_bytes = 2 * GB_A_BYTES + 2 * b_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);   // [0,1] MMAs of a stage drained; [2,3] B tile of a stage landed (TMA)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);   // [2,3] B tile of a stage landed (TMA)
   float* red = reinterpret_cast<float*>(bars + 6);     // [2][128] epilogue exchange (EPI_SOFTMAX)
 
-  const int tm_cols = N > 256 ? 512 : 256;
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tm_cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     for (int i = 0; i < 4; ++i) mbar_init(&bars[i], 1);
     fence_mbar_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
+  // warpgroup g owns rows [64 g, 64 g + 64) of the tile and all N columns, as N / 16 accumulators of m64n16
+  const int wg = warp >> 2, wt = tid & 127;
+  float acc[NCH][8];
   // row tiles: plain GEMMs tile M; spatial attention tiles every batch element separately (ceil(Nn/128) tiles each), so all rows of
   // a tile share their batch index (warp-uniform LHS addresses, no divergence at batch boundaries)
   const int sp_tiles = SPATT ? (p.Nn + GB_BM - 1) / GB_BM : 1;
@@ -95,8 +91,6 @@ __global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_bloc
   const long long m0 = SPATT ? (long long)sp_bt * p.Nn + sp_j0 : (long long)blockIdx.x * GB_BM;
   const int rows_here = SPATT ? min(GB_BM, p.Nn - sp_j0) : (int)min((long long)GB_BM, (long long)p.M - m0);
   const int nkb = p.nblk, Kpad = p.nblk * 64;
-  const int nh = N > 256 ? 2 : 1, Nh = N / nh;        // MMA column halves
-  const uint32_t idesc = umma_idesc_f16(128, Nh);
 
   // MODE_SPATT register tile: thread = 4 consecutive rows (b, j..j+3) x 8 k of every k-block.  RHS columns of my rows live in
   // registers for the whole tile; LHS rows are warp-uniform addresses (a warp shares k and the tile shares b): broadcast 16-byte loads.
@@ -155,9 +149,9 @@ __global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_bloc
     unsigned char* a_lo = a_hi + GB_A_BYTES;
     unsigned char* b_hi = a_lo + GB_A_BYTES;
     unsigned char* b_lo = b_hi + b_bytes;
-    if (kb >= 2) {  // the MMAs of k-block kb-2 must have drained this stage
-      mbar_wait(&bars[s], (uint32_t)((kb >> 1) - 1) & 1u);
-      tc_fence_after();
+    if (kb >= 2) {  // the MMAs of k-block kb-2 (both warpgroups) must have drained this stage; those of kb-1 keep running
+      wgmma_wait<1>();
+      __syncthreads();
     }
     const int k0 = kb * 64;
     if (p.w_img && tid == 0) {
@@ -245,44 +239,48 @@ __global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_bloc
         }
       }
     }
-    fence_proxy_async();
-    tc_fence_before();
+    fence_proxy_async();        // generic-proxy operand stores -> visible to the tensor core (async proxy)
     __syncthreads();
-    tc_fence_after();
-    if (tid == 0) {
-      if (p.w_img) mbar_wait(&bars[2 + s], (uint32_t)(kb >> 1) & 1u);
-      const uint32_t ah = smem_u32(a_hi), al = smem_u32(a_lo), bh = smem_u32(b_hi), bl = smem_u32(b_lo);
-      for (int hh = 0; hh < nh; ++hh) {
+    if (p.w_img) mbar_wait(&bars[2 + s], (uint32_t)(kb >> 1) & 1u);
+    const uint32_t ah = smem_u32(a_hi) + wg * 64 * 128, al = smem_u32(a_lo) + wg * 64 * 128, bh = smem_u32(b_hi), bl = smem_u32(b_lo);
+    wgmma_fence();
 #pragma unroll
-        for (int pass = 0; pass < 3; ++pass) {          // lo*hi, hi*lo, hi*hi
-          const uint32_t ab = pass == 0 ? al : ah, bb = (pass == 1 ? bl : bh) + hh * Nh * 128;
+    for (int pass = 0; pass < 3; ++pass) {          // lo*hi, hi*lo, hi*hi
+      const uint32_t ab = pass == 0 ? al : ah, bb = pass == 1 ? bl : bh;
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks)
-            umma_f16(tmem + hh * Nh, umma_desc(ab + ks * 32), umma_desc(bb + ks * 32), idesc, (kb | pass | ks) ? 1u : 0u);
-        }
+      for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+        for (int c = 0; c < NCH; ++c)
+          if (16 * c < N)
+            wgmma_f16_n16(acc[c], gmma_desc_sw128(ab + ks * 32), gmma_desc_sw128(bb + c * 16 * 128 + ks * 32), (kb | pass | ks) ? 1u : 0u);
       }
-      umma_commit(&bars[s]);
     }
+    wgmma_commit();
   }
-  {  // all MMAs complete in order: waiting for the last commit is enough
-    const int last = nkb - 1;
-    mbar_wait(&bars[last & 1], (uint32_t)(last >> 1) & 1u);
-    tc_fence_after();
-  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int c = 0; c < NCH; ++c) acc_fence(acc[c]);
+  // the accumulators go to a row-major fp32 tile over the (now idle) operand stages, so that the epilogue walks rows
+  __syncthreads();              // the other warpgroup's MMAs have read the stages too
+  float* ct = reinterpret_cast<float*>(smem);
+  const int cp = N + 8;         // row pitch (floats): the fragment's 8-row float2 stores hit 2 bank wavefronts per warp
+#pragma unroll
+  for (int c = 0; c < NCH; ++c)
+    if (16 * c < N) acc_store(ct, cp, 64 * wg, 16 * c, wt, acc[c]);
+  __syncthreads();
 
-  // ---- epilogue: TMEM lane == row ----------------------------------------------------------------------------------------
+  // ---- epilogue: thread == row ---------------------------------------------------------------------------------------------
   const int q = warp & 3, half = warp >> 2;
-  const long long row = m0 + q * 32 + lane;
-  const bool live = (q * 32 + lane) < rows_here;
-  const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16);
+  const int trow = q * 32 + lane;
+  const long long row = m0 + trow;
+  const bool live = trow < rows_here;
   if (EPI == EPI_BIAS || EPI == EPI_RELU) {
     // warps 0-3 / 4-7 split the 16-column chunks
     const int nchunk = N / 16;
     for (int ch = half; ch < nchunk; ch += 2) {
       const int c0 = ch * 16;
       uint32_t v[16];
-      tmem_ld16(trow + c0, v);
-      tmem_ld_wait();
+      acc_ld<16>(ct, cp, trow, c0, v);
       if (live) {
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj) {
@@ -309,14 +307,13 @@ __global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_bloc
   } else if (EPI == EPI_RELU_LN) {
     // y = LayerNorm(relu(acc + bias)) over the row's 64 columns (torch: biased variance, eps inside the sqrt); warps 0-3 own the rows
     if (half == 0) {
-      // pass 1: mean and (two-pass) variance straight from TMEM; pass 2: normalise and store -- 16 values live at a time, so the
+      // pass 1: mean and (two-pass) variance from the staged accumulator tile; pass 2: normalise and store -- 16 values live at a time, so the
       // kernel fits two CTAs per SM
       float mean = 0.f;
 #pragma unroll
       for (int ch = 0; ch < 4; ++ch) {
         uint32_t v[16];
-        tmem_ld16(trow + 16 * ch, v);
-        tmem_ld_wait();
+        acc_ld<16>(ct, cp, trow, 16 * ch, v);
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj) mean += fmaxf(__uint_as_float(v[jj]) + (p.bias ? __ldg(p.bias + 16 * ch + jj) : 0.f), 0.f);
       }
@@ -325,8 +322,7 @@ __global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_bloc
 #pragma unroll
       for (int ch = 0; ch < 4; ++ch) {
         uint32_t v[16];
-        tmem_ld16(trow + 16 * ch, v);
-        tmem_ld_wait();
+        acc_ld<16>(ct, cp, trow, 16 * ch, v);
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj) {
           const float d = fmaxf(__uint_as_float(v[jj]) + (p.bias ? __ldg(p.bias + 16 * ch + jj) : 0.f), 0.f) - mean;
@@ -337,8 +333,7 @@ __global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_bloc
 #pragma unroll
       for (int ch = 0; ch < 4; ++ch) {
         uint32_t v[16];
-        tmem_ld16(trow + 16 * ch, v);
-        tmem_ld_wait();
+        acc_ld<16>(ct, cp, trow, 16 * ch, v);
         if (live) {
           float* dst = p.C + row * p.ldc + 16 * ch;
 #pragma unroll
@@ -362,8 +357,7 @@ __global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_bloc
     float mx = -INFINITY;
     for (int ch = half; ch < nchunk; ch += 2) {
       uint32_t v[16];
-      tmem_ld16(trow + 16 * ch, v);
-      tmem_ld_wait();
+      acc_ld<16>(ct, cp, trow, 16 * ch, v);
 #pragma unroll
       for (int jj = 0; jj < 16; ++jj)
         if (16 * ch + jj < p.ncols) mx = fmaxf(mx, __uint_as_float(v[jj]));
@@ -375,8 +369,7 @@ __global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_bloc
     float sum = 0.f;
     for (int ch = half; ch < nchunk; ch += 2) {
       uint32_t v[16];
-      tmem_ld16(trow + 16 * ch, v);
-      tmem_ld_wait();
+      acc_ld<16>(ct, cp, trow, 16 * ch, v);
 #pragma unroll
       for (int jj = 0; jj < 16; ++jj)
         if (16 * ch + jj < p.ncols) sum += __expf(__uint_as_float(v[jj]) - mx);
@@ -386,8 +379,7 @@ __global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_bloc
     const float inv = 1.0f / (red[r128] + red[128 + r128]);
     for (int ch = half; ch < nchunk; ch += 2) {
       uint32_t v[16];
-      tmem_ld16(trow + 16 * ch, v);
-      tmem_ld_wait();
+      acc_ld<16>(ct, cp, trow, 16 * ch, v);
       if (live) {
         float* dst = p.C + row * p.ldc + 16 * ch;      // ldc % 4 == 0, C 16-byte aligned (checked on the host)
 #pragma unroll
@@ -400,9 +392,6 @@ __global__ void __launch_bounds__(GB_NT, EPI == EPI_SOFTMAX ? 1 : 2) k_gemm_bloc
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tm_cols));
 }
 
 // packed [N][Kpad] hi | lo  ->  per k-block [hi tile | lo tile], each N x 128 B in the SWIZZLE_128B layout of the kernel's B stage
@@ -420,15 +409,22 @@ __global__ void k_gb_weight_image(const __half* __restrict__ hi, const __half* _
   *reinterpret_cast<uint4*>(img + ((size_t)kb * 2 + half) * N * 128 + n * 128 + ((c ^ (n & 7)) << 4)) = v;
 }
 
-template <int EPI>
-int gb_launch(GbParams& p, cudaStream_t st) {
+template <int EPI, int NCH>
+int gb_launch_n(GbParams& p, cudaStream_t st) {
   const int smem = 2 * (2 * GB_A_BYTES + 2 * p.N * 128) + 48 + 256 * 4;
   if (smem > 232448) return set_error(STMP_EUNSUPPORTED, "blocked GEMM: N=%d needs %d B of shared memory", p.N, smem);
-  STMP_CUDA_OK(cudaFuncSetAttribute(k_gemm_blocks<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  STMP_CUDA_OK(cudaFuncSetAttribute(k_gemm_blocks<EPI, NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const unsigned grid = EPI == EPI_SOFTMAX ? (unsigned)((p.M / p.Nn) * ((p.Nn + GB_BM - 1) / GB_BM)) : (unsigned)((p.M + GB_BM - 1) / GB_BM);
-  k_gemm_blocks<EPI><<<grid, GB_NT, smem, st>>>(p);
+  k_gemm_blocks<EPI, NCH><<<grid, GB_NT, smem, st>>>(p);
   STMP_LAUNCH_OK("k_gemm_blocks");
   return STMP_OK;
+}
+template <int EPI>
+int gb_launch(GbParams& p, cudaStream_t st) {
+  // the accumulator registers are compiled in per instance: the smallest one that holds N
+  if (EPI != EPI_SOFTMAX && p.N <= 64) return gb_launch_n<EPI, 4>(p, st);   // the block GEMMs of ASTGCN (N = 64), two CTAs per SM
+  if (p.N <= 128) return gb_launch_n<EPI, 8>(p, st);
+  return gb_launch_n<EPI, GB_MAXN / 16>(p, st);
 }
 
 int gb_dispatch(GbParams& p, int epi, cudaStream_t st) {

@@ -1,14 +1,14 @@
 // gemm_tc.cu -- K4 (+K5): the dense node-feature x weight contraction of the tiled (large-graph) path on the
-// 5th-gen tensor cores, fp32 in / fp32 out:   C[M,N] = A[M,K] @ W[K,N] + bias
+// Hopper tensor cores (wgmma), fp32 in / fp32 out:   C[M,N] = A[M,K] @ W[K,N] + bias
 // optionally fused with the peephole-LSTM gate epilogue of GConvLSTM (gconv_lstm.py:168-202), so the gate
 // pre-activations never reach HBM.
 //
 // fp32-class accuracy from fp16 tensor cores: every operand is split into hi = fp16(v), lo = fp16(v - hi) and the
-// product is accumulated as lo*hi + hi*lo + hi*hi in the fp32 TMEM accumulator (three tcgen05.mma.kind::f16 passes;
-// validated in tools/tc_probe.cu).  The weights are split ONCE (stmp_gemm_prepack); activations are split on the
-// fly while they are staged: 256 threads stream a 128 x 64 fp32 tile from HBM (coalesced float4), convert, and
-// write both halves into the hand-swizzled K-major SWIZZLE_128B layout the UMMA descriptors expect.  Two stages:
-// the tile of k-block i+1 is loaded/converted while the MMAs of k-block i run (tcgen05.commit -> mbarrier).
+// product is accumulated as lo*hi + hi*lo + hi*hi in fp32 register accumulators (three wgmma f16 passes).  The weights
+// are split ONCE (stmp_gemm_prepack); activations are split on the fly while they are staged: 256 threads stream a
+// 128 x 64 fp32 tile from HBM (coalesced float4), convert, and write both halves into the hand-swizzled K-major
+// SWIZZLE_128B layout the GMMA descriptors expect.  Two stages: the tile of k-block i+1 is loaded/converted while the
+// asynchronous MMAs of k-block i run (wgmma.wait_group 1 keeps one k-block in flight).
 //
 // One CTA = 128 rows x all N (<= 256) columns, so A is read from HBM exactly once: algorithmic bytes
 // 4*M*K + 4*M*N (+ the L2-resident weights).  This is a true dense GEMM (cfg5: 80 000 x 384 x 256), the one place on
@@ -23,6 +23,7 @@ constexpr int GM_NT = 256;
 constexpr int GM_BM = 128;
 constexpr int GM_BK = 64;
 constexpr int GM_A_BYTES = GM_BM * 128;   // one K-block of A (hi or lo): 128 rows x 128 B
+constexpr int GM_NCH = 8;                 // accumulator column chunks of 32 (N <= 256)
 
 struct GemmParams {
   const float* A; long long lda;
@@ -58,25 +59,11 @@ __global__ void __launch_bounds__(GM_NT, 1) k_gemm_split(const GemmParams p) {
   const int N = p.N;
   const int b_bytes = N * 128;                       // one K-block of B (hi or lo)
   const int stage_bytes = 2 * GM_A_BYTES + 2 * b_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
-
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (tid == 0) {
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    fence_mbar_init();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const long long m0 = (long long)blockIdx.x * GM_BM;
   const int nkb = p.Kpad / GM_BK;
-  const uint32_t idesc = umma_idesc_f16(128, N);
+  // warpgroup g owns rows [64 g, 64 g + 64) of the tile and all N columns, as N / 32 accumulators of m64n32
+  const int wg = warp >> 2, wt = tid & 127;
+  float acc[GM_NCH][16];
 
   float4 av[8];
   auto load_a = [&](int kb) {
@@ -98,9 +85,9 @@ __global__ void __launch_bounds__(GM_NT, 1) k_gemm_split(const GemmParams p) {
     unsigned char* a_lo = a_hi + GM_A_BYTES;
     unsigned char* b_hi = a_lo + GM_A_BYTES;
     unsigned char* b_lo = b_hi + b_bytes;
-    if (kb >= 2) {  // the MMAs of k-block kb-2 must have drained this stage
-      mbar_wait(&bars[s], (uint32_t)((kb >> 1) - 1) & 1u);
-      tc_fence_after();
+    if (kb >= 2) {  // the MMAs of k-block kb-2 (both warpgroups) must have drained this stage; those of kb-1 keep running
+      wgmma_wait<1>();
+      __syncthreads();
     }
     const int k0 = kb * GM_BK;
     // A: 128 x 64 fp32 -> hi/lo fp16, swizzled.  16 lanes cover one row's 256 B contiguously.  The 8 loads of k-block kb+1 are
@@ -136,39 +123,45 @@ __global__ void __launch_bounds__(GM_NT, 1) k_gemm_split(const GemmParams p) {
         }
       }
     }
-    fence_proxy_async();
-    tc_fence_before();
+    fence_proxy_async();        // generic-proxy operand stores -> visible to the tensor core (async proxy)
     __syncthreads();
-    tc_fence_after();
-    if (tid == 0) {
-      const uint32_t ah = smem_u32(a_hi), al = smem_u32(a_lo), bh = smem_u32(b_hi), bl = smem_u32(b_lo);
+    const uint32_t ah = smem_u32(a_hi) + wg * 64 * 128, al = smem_u32(a_lo) + wg * 64 * 128, bh = smem_u32(b_hi), bl = smem_u32(b_lo);
+    wgmma_fence();
 #pragma unroll
-      for (int pass = 0; pass < 3; ++pass) {          // lo*hi, hi*lo, hi*hi
-        const uint32_t ab = pass == 0 ? al : ah, bb = pass == 1 ? bl : bh;
+    for (int pass = 0; pass < 3; ++pass) {          // lo*hi, hi*lo, hi*hi
+      const uint32_t ab = pass == 0 ? al : ah, bb = pass == 1 ? bl : bh;
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks)
-          umma_f16(tmem, umma_desc(ab + ks * 32), umma_desc(bb + ks * 32), idesc, (kb | pass | ks) ? 1u : 0u);
+      for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+        for (int c = 0; c < GM_NCH; ++c)
+          if (32 * c < N)
+            wgmma_f16_n32(acc[c], gmma_desc_sw128(ab + ks * 32), gmma_desc_sw128(bb + c * 32 * 128 + ks * 32), (kb | pass | ks) ? 1u : 0u);
       }
-      umma_commit(&bars[s]);
     }
+    wgmma_commit();
   }
-  {  // all MMAs complete in order: waiting for the last commit is enough
-    const int last = nkb - 1;
-    mbar_wait(&bars[last & 1], (uint32_t)(last >> 1) & 1u);
-    tc_fence_after();
-  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int c = 0; c < GM_NCH; ++c) acc_fence(acc[c]);
+  // the accumulators go to a row-major fp32 tile over the (now idle) operand stages, so that the epilogue walks rows
+  __syncthreads();              // the other warpgroup's MMAs have read the stages too
+  float* ct = reinterpret_cast<float*>(smem);
+  const int cp = N + 8;         // row pitch (floats): the fragment's 8-row float2 stores hit 2 bank wavefronts per warp
+#pragma unroll
+  for (int c = 0; c < GM_NCH; ++c)
+    if (32 * c < N) acc_store(ct, cp, 64 * wg, 32 * c, wt, acc[c]);
+  __syncthreads();
 
-  // ---- epilogue: TMEM lane == row; warps 0-3 / 4-7 split the columns ------------------------------------------
+  // ---- epilogue: thread == row; warps 0-3 / 4-7 split the columns ---------------------------------------------
   const int q = warp & 3, half = warp >> 2;
-  const long long row = m0 + q * 32 + lane;
+  const int trow = q * 32 + lane;
+  const long long row = m0 + trow;
   const bool live = row < p.M;
-  const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16);
   if (EPI == 0) {
     const int ncol = N / 2;   // N % 32 == 0 on this path
     for (int c0 = half * ncol; c0 < (half + 1) * ncol; c0 += 16) {
       uint32_t v[16];
-      tmem_ld16(trow + c0, v);
-      tmem_ld_wait();
+      acc_ld<16>(ct, cp, trow, c0, v);
       if (live) {
         float* dst = p.C + row * p.ldc + c0;
 #pragma unroll
@@ -189,11 +182,10 @@ __global__ void __launch_bounds__(GM_NT, 1) k_gemm_split(const GemmParams p) {
     const int Co = p.Co, nch = Co / 2;
     for (int ch = half * nch; ch < (half + 1) * nch; ch += 16) {
       uint32_t vi[16], vf[16], vc[16], vo[16];
-      tmem_ld16(trow + ch, vi);
-      tmem_ld16(trow + Co + ch, vf);
-      tmem_ld16(trow + 2 * Co + ch, vc);
-      tmem_ld16(trow + 3 * Co + ch, vo);
-      tmem_ld_wait();
+      acc_ld<16>(ct, cp, trow, ch, vi);
+      acc_ld<16>(ct, cp, trow, Co + ch, vf);
+      acc_ld<16>(ct, cp, trow, 2 * Co + ch, vc);
+      acc_ld<16>(ct, cp, trow, 3 * Co + ch, vo);
       if (live) {
         float cold[16], hn[16], cn[16];
 #pragma unroll
@@ -221,9 +213,6 @@ __global__ void __launch_bounds__(GM_NT, 1) k_gemm_split(const GemmParams p) {
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(256));
 }
 
 inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
@@ -231,7 +220,7 @@ inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) =
 int gemm_check(int64_t M, int64_t K, int64_t N, const float* A, int64_t lda) {
   STMP_REQUIRE(M >= 0 && K > 0 && N > 0, STMP_EINVAL, "stmp_gemm: bad sizes");
   if (N > 256 || N % 32 != 0 || K % 4 != 0 || lda % 4 != 0 || !al16(A) || M >= (1ll << 31) - 128)
-    return set_error(STMP_EUNSUPPORTED, "tcgen05 GEMM needs N<=256, N%%32==0, K%%4==0 and 16-byte aligned rows (M=%lld K=%lld N=%lld)",
+    return set_error(STMP_EUNSUPPORTED, "tensor-core GEMM needs N<=256, N%%32==0, K%%4==0 and 16-byte aligned rows (M=%lld K=%lld N=%lld)",
                      (long long)M, (long long)K, (long long)N);
   return STMP_OK;
 }

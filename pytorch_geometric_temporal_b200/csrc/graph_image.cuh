@@ -1,4 +1,4 @@
-// graph_image.cuh -- the shared-memory image of a plan's operators that the fused tcgen05 graph-GRU kernel gathers from
+// graph_image.cuh -- the shared-memory image of a plan's operators that the fused wgmma graph-GRU kernel gathers from
 // (built once per plan by plan.cu::k_build_graph_image, fetched by every CTA with ONE TMA bulk copy).
 //
 // A *task* = one (destination row, operator) pair: the weighted sum of the source rows of its CSR row.  The 16 warps of

@@ -594,7 +594,7 @@ int build_gcn(Builder& b, stmp_plan* p, int n, int e, const int* row, const int*
 #define STMP_LPT_B 3
 #endif
 
-// ---- shared-memory graph image for the fused tcgen05 kernel (graph_image.cuh) ---------------------------------------
+// ---- shared-memory graph image for the fused wgmma kernel (graph_image.cuh) ---------------------------------------
 // One CTA.  Tasks (row, op) are rank-sorted per segment (destination row tile, operator) by descending group count, cut into
 // warp-tasks of four, and dealt longest-first to the least loaded of the 16 warps (loads carry over between the segments,
 // so the whole round is balanced, not each segment); then the padded edge groups are written.
@@ -877,7 +877,7 @@ extern "C" int stmp_plan_export(const stmp_plan* p, int op, int transposed, int3
 }
 
 extern "C" const char* stmp_last_error(void) { return err_buf(); }
-extern "C" const char* stmp_version(void) { return "stmp 0.1.0 sm_100a"; }
+extern "C" const char* stmp_version(void) { return "stmp 0.1.0 sm_90a"; }
 extern "C" int64_t stmp_launch_count(void) { return g_launches.load(); }
 extern "C" int stmp_path_counters(const char** names, int64_t* counts, int max_entries) {
   const int n = stmp::g_n_paths.load();

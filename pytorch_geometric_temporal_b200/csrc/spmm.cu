@@ -1,12 +1,10 @@
 // spmm.cu -- K1/K3: gather of source-node rows -> edge-weighted accumulate per destination, with the
 // Chebyshev/diffusion axpby fused into the epilogue.  One group of G lanes owns one (batch, destination) row, lanes are
 // vectorised along the feature axis (float4/float2/float), edge metadata is one 64-bit load per edge, 4 gathers in flight.
-// A CTA owns 8 x (256 / G) consecutive destination rows of one batch element (1855 GB/s at the cfg5 probe; one row per group: 1451).
+// A CTA owns 8 x (256 / G) consecutive destination rows of one batch element.
 // Bound (cfg5 probe, random 10^4-node graph): L2 throughput -- 4*nnz*F*B = 1.8 GB of gathered rows per launch on top of the 0.33 GB of
-// compulsory HBM traffic leave L2 at 12.0 TB/s, the LTS cap (~6300 B/clk).  Measured dead ends, all bit-identical and all at or below this
-// kernel (tests/perf/spmm_variants.py, spmm_blocked.py, profiles/r02_spmm_*.json): entries preloaded once + shuffles with 4 / 8 gathers in
-// flight (0.92x / 0.72x), predicated batches without a scalar tail (0.98x / 0.58x), TMA-staged source rows (k_spmm_tma below, kept
-// selectable: 0.90x / 0.95x), 1024-thread CTAs (0.94x).
+// compulsory HBM traffic.  Variants kept selectable for A/B runs (tests/perf/spmm_variants.py, spmm_blocked.py): entries preloaded once
+// + shuffles, predicated batches without a scalar tail, TMA-staged source rows (k_spmm_tma below), 1024-thread CTAs.
 // Deterministic: per destination the sum runs in the reference's scatter order with separate
 // multiply and add, which makes the result bit-identical to CPU index_select -> mul -> scatter_add_.
 #include <cstdlib>

@@ -1,6 +1,11 @@
-// tc_common.cuh -- tcgen05 / TMEM building blocks shared by the fused graph-GRU kernel and the split-fp16 GEMM:
-// UMMA shared-memory / instruction descriptors, MMA issue + commit, TMEM loads, the hand-written SWIZZLE_128B
-// K-major operand layout and the fp32 -> fp16 (hi, lo) operand split.
+// tc_common.cuh -- Hopper warpgroup MMA (wgmma) building blocks shared by the fused graph-GRU kernel, the split-fp16 GEMMs and the
+// weight-gradient contraction: GMMA shared-memory descriptors, wgmma issue / commit / wait, the accumulator fragment layout, the
+// hand-written SWIZZLE_128B K-major operand layout and the fp32 -> fp16 (hi, lo) operand split.
+//
+// A wgmma is issued by a whole warpgroup (4 consecutive warps, 128 threads) and accumulates an M = 64 row tile in the registers of that
+// warpgroup.  Fragment of an m64nN fp32 accumulator d[N/2]: thread (warp w of the group, lane l) holds, for every 8-column group j,
+//   d[4j + 0, 1] = D[16w + l/4    ][8j + 2(l%4) + 0, 1]
+//   d[4j + 2, 3] = D[16w + l/4 + 8][8j + 2(l%4) + 0, 1]
 #pragma once
 #include <cuda_fp16.h>
 
@@ -8,54 +13,88 @@
 
 namespace stmp {
 
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  // cute::UMMA::SmemDescriptor: start>>4 [0,14) | LBO>>4 [16,30) (unused: swizzled K-major) | SBO>>4 [32,46) = 1024 B |
-  // version [46,48) = 1 (sm_100) | layout_type [61,64) = 2 (SWIZZLE_128B)
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+// GmmaDescriptor (sm_90): start>>4 [0,14) | LBO>>4 [16,30) (unused by swizzled K-major layouts: 1) | SBO>>4 [32,46) = bytes between
+// 8-row groups | layout_type [62,64) (1 = SWIZZLE_128B, 2 = SWIZZLE_64B).  Operand tiles start on a swizzle-atom boundary; a k-step
+// inside the atom advances the start address (the hardware applies the XOR pattern to the absolute address bits).
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t sbo, uint32_t layout) {
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(sbo >> 4) << 32) | ((uint64_t)layout << 62);
 }
-__device__ __forceinline__ constexpr uint32_t umma_idesc_f16(int m, int n) {
-  // cute::UMMA::InstrDescriptor: c_format [4,6) = 1 (F32); a/b_format = 0 (F16); a/b_major = 0 (K); n>>3 at [17,23); m>>4 at [24,29)
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+// K-major, SWIZZLE_128B, 128-byte rows (64 fp16): 8-row atoms of 1024 B
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) { return gmma_desc(saddr, 1024, 1); }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// keeps the compiler from moving accumulator reads / writes across a wgmma fence or wait
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 operands (K-major in shared memory), fp32 accumulator; scale_d == 0 overwrites D
+__device__ __forceinline__ void wgmma_f16_n8(float (&d)[4], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+__device__ __forceinline__ void wgmma_f16_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,"
-      "%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-        "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]),
-        "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+__device__ __forceinline__ void wgmma_f16_n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr));
+template <int N> __device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_f16<8>(float (&d)[4], uint64_t da, uint64_t db, uint32_t s) { wgmma_f16_n8(d, da, db, s); }
+template <> __device__ __forceinline__ void wgmma_f16<16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t s) { wgmma_f16_n16(d, da, db, s); }
+template <> __device__ __forceinline__ void wgmma_f16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t s) { wgmma_f16_n32(d, da, db, s); }
+
+// D[64 x 32] += A[64 x 8] * B[32 x 8]^T, TF32 operands (K-major), fp32 accumulator
+__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db));
 }
-template <int CW> __device__ __forceinline__ void tmem_ld(uint32_t taddr, uint32_t (&v)[CW]);
-template <> __device__ __forceinline__ void tmem_ld<8>(uint32_t taddr, uint32_t (&v)[8]) { tmem_ld8(taddr, v); }
-template <> __device__ __forceinline__ void tmem_ld<32>(uint32_t taddr, uint32_t (&v)[32]) { tmem_ld32(taddr, v); }
-template <> __device__ __forceinline__ void tmem_ld<16>(uint32_t taddr, uint32_t (&v)[16]) { tmem_ld16(taddr, v); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
+// Writes an m64nN accumulator fragment (N = 2 R) of warpgroup-thread `wt` (0..127) into a row-major fp32 tile:
+// rows row0 .. row0 + 63, columns col0 .. col0 + N - 1, `pitch` floats per row.
+template <int R>
+__device__ __forceinline__ void acc_store(float* tile, int pitch, int row0, int col0, int wt, const float (&d)[R]) {
+  const int r = row0 + 16 * (wt >> 5) + ((wt & 31) >> 2), c = col0 + 2 * (wt & 3);
+#pragma unroll
+  for (int j = 0; j < R / 4; ++j) {
+    *reinterpret_cast<float2*>(tile + (size_t)r * pitch + c + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(tile + (size_t)(r + 8) * pitch + c + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+// CW consecutive accumulator values of one row of such a tile (col % 4 == 0, pitch % 4 == 0)
+template <int CW>
+__device__ __forceinline__ void acc_ld(const float* tile, int pitch, int row, int col, uint32_t (&v)[CW]) {
+  const float4* src = reinterpret_cast<const float4*>(tile + (size_t)row * pitch + col);
+#pragma unroll
+  for (int j = 0; j < CW / 4; ++j) {
+    const float4 q = src[j];
+    v[4 * j] = __float_as_uint(q.x); v[4 * j + 1] = __float_as_uint(q.y); v[4 * j + 2] = __float_as_uint(q.z); v[4 * j + 3] = __float_as_uint(q.w);
+  }
+}
 
 // byte offset of element (row, kin) inside a K-panel (kin in [0,64))
 __device__ __forceinline__ int sw128(int row, int kin) { return row * 128 + ((((kin >> 3) ^ (row & 7))) << 4) + ((kin & 7) << 1); }

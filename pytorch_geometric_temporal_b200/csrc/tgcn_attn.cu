@@ -1,5 +1,5 @@
 // tgcn_attn.cu -- fused temporal-attention + GCN-GRU kernel: A3TGCN / A3TGCN2 (and a TGCN / TGCN2 cell as the one-period case)
-// for graphs of ANY size (the tcgen05 graph-GRU kernel stops at 207 nodes; PEMS-BAY has 325).
+// for graphs of ANY size (the wgmma graph-GRU kernel stops at 207 nodes; PEMS-BAY has 325).
 //
 // Reference (nn/recurrent/attentiontemporalgcn.py:130-157, temporalgcn.py:187-233): for every period t
 //     G_g = GCNConv_g(X[..., t])            three GCNConvs = gcn_norm + Linear(in,out) + propagate over `out` channels

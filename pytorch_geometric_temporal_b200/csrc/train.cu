@@ -18,12 +18,12 @@
 #include "common.cuh"
 
 namespace stmp {
-int g_wgrad_tc = -1;      // 1: tcgen05 contraction (wgrad_tc.cu); 0: the fp32 FFMA kernel below (stmp_set_option("dcrnn_wgrad_tc") / STMP_WGRAD_TC)
+int g_wgrad_tc = -1;      // 1: wgmma contraction (wgrad_tc.cu); 0: the fp32 FFMA kernel below (stmp_set_option("dcrnn_wgrad_tc") / STMP_WGRAD_TC)
 int wgrad_tc_launch(int cin, long long rows, int ld, const float* S1, const float* S2, const float* dpzr, const float* dph, float* partial,
                     int max_parts, cudaStream_t st, int* parts);
 namespace {
 
-constexpr int kWgradTcDefault = 1;    // in the training step: 0.837 ms (tcgen05) vs 0.866 ms (FFMA), A/B on one box
+constexpr int kWgradTcDefault = 1;    // the tensor-core contraction (wgrad_tc.cu)
 constexpr int kWgTK = 16;            // rows per staged tile
 constexpr int kWgStages = 4;         // tiles in flight per CTA: 3 x 19 KB x 2 CTAs per SM keeps ~115 KB per SM on the wire (2 stages of 32 rows were load-latency bound)
 constexpr int kWgThreads = 192;      // >= 12 * ceil(3C/8) for cin <= 4
@@ -210,7 +210,7 @@ __global__ void __launch_bounds__(256) k_adam_flat(long long n, float* __restric
 using namespace stmp;
 
 static int wgrad_grid() {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return 2 * sms;
 }

@@ -1,30 +1,31 @@
-// wgrad_tc.cu -- the DCRNN weight / bias gradient contraction on the tensor cores (tcgen05, kind::tf32, MN-major operands).
+// wgrad_tc.cu -- the DCRNN weight / bias gradient contraction on the tensor cores (wgmma, TF32, K-major operands).
 //
 //   dW_zr [3C x 64] = S1^T dpre_zr,   dW_h [3C x 32] = S2^T dpre_h,   db = 1^T dpre        over all rows = T*B*N (159 k at B = 64)
 //
 // (what autograd accumulates for the matmul(basis, W) + bias of torch_geometric_temporal/nn/recurrent/dcrnn.py:86-111 across steps, gates
-// and hops).  The contraction axis is the ROW axis of the row-major operands, i.e. both UMMA operands are MN-major: a 16-row tile of
-// S (16 x 104 fp32) IS A^T[k][m] with m contiguous.  fp16 hi/lo splits (the forward kernel's trick) would need a gradient scale -- d
-// pre-activations of a mean loss are ~1e-5 and fall into fp16 subnormals -- so the split is TF32 hi + TF32 lo (fp32 exponent range, 21+
-// mantissa bits together): three kind::tf32 passes hi*hi + lo*hi + hi*lo per product, accumulators in TMEM (D_zr 128 x 64, D_h 128 x 32; four sets used round-robin).
+// and hops).  The contraction axis is the ROW axis of the row-major operands; TF32 wgmma takes K-major operands only, so a 16-row tile
+// is transposed while it is converted: operand row m (a column of S, or of dpre) holds the tile's 16 k values, 64 bytes, in the
+// canonical K-major SWIZZLE_64B layout (8-row atoms of 512 B, the four 16-byte chunks of a row XOR-ed with (row / 2) % 4).  fp16 hi/lo
+// splits (the forward kernel's trick) would need a gradient scale -- d pre-activations of a mean loss are ~1e-5 and fall into fp16
+// subnormals -- so the split is TF32 hi + TF32 lo (fp32 exponent range, 21+ mantissa bits together): three passes hi*hi + lo*hi + hi*lo
+// per product, accumulators in registers (two sets used alternately).
 //
-// Per CTA (one per SM; 8 converting warps + 1 producer / issuer warp): a 6-stage ring of 16-row fp32 tiles S1 | S2 | dpre_zr | dpre_h filled by TMA bulk copies; all warps
-// convert a tile into the canonical MN-major layout of 32-bit operands -- SWIZZLE_128B_BASE32B, the only one the tensor core accepts for
-// MN-major TF32: atoms of 4 k-rows x 128 B (32 elements along MN), the four 32-byte chunks of a row XOR-ed with the row index -- as hi and
-// lo copies, two operand buffers; the issuer lane fires the 12 MMAs of a tile when the eight warps have arrived on the buffer's "full" mbarrier and commits them to its "free" mbarrier (no block-wide barrier in the loop); the bias row-sums ride along as
-// a column of ones at m = 127 of the A operands.  The kernel is then bound by reading the 193 MB of operands once.  Epilogue: TMEM ->
-// one partial per CTA, summed in a fixed order by k_dcrnn_wgrad_reduce (train.cu) straight into the module's weight layout.
+// Per CTA (one per SM; 8 converting warps = 2 warpgroups + 1 TMA producer warp): a 6-stage ring of 16-row fp32 tiles S1 | S2 | dpre_zr |
+// dpre_h filled by TMA bulk copies; the two warpgroups convert a tile into one of two operand buffers (hi and lo copies) and then each
+// issues the MMAs of its 64 rows of the weight gradient.  (ptxas serializes these wgmmas -- the accumulator set is chosen per tile -- so
+// a tile's MMAs complete before the next tile is converted; the two operand buffers still let the TMA ring run ahead.)
+// The bias row-sums ride along as a row of ones at m = 127 of the A operands.  Epilogue: one partial per CTA, summed in a fixed order by
+// k_dcrnn_wgrad_reduce (train.cu) straight into the module's weight layout.
 #include "tc_common.cuh"
 
 namespace stmp {
 namespace {
 
 constexpr int kCo = 32;
-constexpr int kTK = 16;                  // rows per tile = two k-groups of 8 (one kind::tf32 MMA consumes K = 8)
+constexpr int kTK = 16;                  // rows per tile = two k-steps of 8 (one TF32 wgmma consumes K = 8)
 constexpr int kStages = 6;
-constexpr int kConvThreads = 256;        // warps 0..7 convert (and run the epilogue); warp 8 = TMA producer + MMA issuer
+constexpr int kConvThreads = 256;        // warps 0..7 convert and issue the MMAs (two warpgroups); warp 8 = TMA producer
 constexpr int kThreads = kConvThreads + 32;
-constexpr int kAccSets = 4;              // TMEM accumulator sets of 96 columns (D_zr 64 | D_h 32)
 constexpr int kObBytes = 45056;          // one operand buffer: A1 hi|lo 2 x 8 KB, A2 hi|lo 2 x 8 KB, B1 hi|lo 2 x 4 KB, B2 hi|lo 2 x 2 KB
 constexpr int kOffA1 = 0, kOffA2 = 16384, kOffB1 = 32768, kOffB2 = 40960;
 constexpr int kLoA = 8192, kLoB1 = 4096, kLoB2 = 2048;   // offset of the lo copy behind the hi copy
@@ -36,36 +37,19 @@ struct WgTcParams {
   float* partial;                        // [grid][MG*8*96 + 96]
 };
 
-// SmemDescriptor of an MN-major SWIZZLE_128B_BASE32B operand: start>>4 [0,14) | LBO>>4 [16,30) (between 32-element MN blocks) |
-// SBO>>4 [32,46) (between 4-row k atoms) | version [46,48) = 1 | layout_type [61,64) = 1
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)1 << 61);
-}
-// InstrDescriptor: c_format [4,6) = 1 (F32) | a_format [7,10) = b_format [10,13) = 2 (TF32) | a_major [15] = b_major [16] = 1 (MN) |
-// n>>3 [17,23) | m>>4 [24,29)
-__device__ __forceinline__ constexpr uint32_t umma_idesc_tf32_mn(int m, int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// barrier of the converting warps only (the producer warp has left)
+__device__ __forceinline__ void conv_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConvThreads) : "memory"); }
 __device__ __forceinline__ float tf32_rna(float v) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
   return __uint_as_float(r);
 }
-// byte offset, inside one 512-byte atom (4 k-rows x 128 B), of the 16 bytes holding elements 4q..4q+3 (q = 0..7) of k-row k4
-__device__ __forceinline__ int atom_chunk(int k4, int q) { return k4 * 128 + ((((q >> 1) ^ k4)) << 5) + ((q & 1) << 4); }
-// operand tile layouts (16 k-rows = 4 k atoms): offset(k, mn) = (k >> 2) * SBO + (mn >> 5) * 512 + atom_chunk(k & 3, (mn & 31) >> 2) + (mn & 3) * 4
-constexpr int kLbo = 512, kSboA = 2048, kSboB1 = 1024, kSboB2 = 512;
+// byte offset of k values 4q..4q+3 (q = 0..3) of operand row m: K-major SWIZZLE_64B
+__device__ __forceinline__ int kmaj64(int m, int q) { return (m >> 3) * 512 + (m & 7) * 64 + ((q ^ ((m >> 1) & 3)) << 4); }
+__device__ __forceinline__ uint64_t desc64(uint32_t saddr) { return gmma_desc(saddr, 512, 2); }
 
 __device__ __forceinline__ void store_split_tf32(unsigned char* hi, int lo_off, int off, float4 v) {
   const float4 h = make_float4(tf32_rna(v.x), tf32_rna(v.y), tf32_rna(v.z), tf32_rna(v.w));
@@ -73,45 +57,32 @@ __device__ __forceinline__ void store_split_tf32(unsigned char* hi, int lo_off, 
   *reinterpret_cast<float4*>(hi + lo_off + off) = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
 }
 
+struct WgAcc { float z0[16], z1[16], h[16]; };   // m64 rows of D_zr columns [0,32) [32,64) and of D_h
+
 __global__ void __launch_bounds__(kThreads, 1) k_dcrnn_wgrad_tc(WgTcParams p) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int ld = p.ld, ld4 = ld >> 2;
+  const int ld = p.ld;
   const int stage_bytes = kTK * (2 * ld + 3 * kCo) * 4;
-  unsigned char* ob0 = smem;                                   // two operand buffers (1024-byte aligned atoms)
+  unsigned char* ob0 = smem;                                   // two operand buffers (1024-byte aligned)
   unsigned char* raw = smem + 2 * kObBytes;                    // kStages raw fp32 tiles
-  // mbarriers: raw_full[s] (TMA bytes landed) | raw_free[s] (the 4 warps converting that tile are done with the stage) | ob_full[b] (4 warps have written the
-  // operand buffer) | ob_free[b] (tcgen05.commit: the MMAs that read it are done)
+  // mbarriers: raw_full[s] (TMA bytes landed) | raw_free[s] (both warpgroups have read the stage)
   uint64_t* raw_full = reinterpret_cast<uint64_t*>(raw + (size_t)kStages * stage_bytes);
   uint64_t* raw_free = raw_full + kStages;
-  uint64_t* ob_full = raw_free + kStages;
-  uint64_t* ob_free = ob_full + 2;
-  uint64_t* done = ob_free + 2;                                  // one phase: every MMA of the CTA has completed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
 
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
-    for (int i = 0; i < kStages; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_free[i], kConvThreads / 64); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&ob_full[i], kConvThreads / 64); mbar_init(&ob_free[i], 1); }
-    mbar_init(done, 1);
+    for (int i = 0; i < kStages; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_free[i], kConvThreads / 32); }
     fence_mbar_init();
   }
-  // operand buffers: zero (columns >= ld of A are never written again), then the column of ones at m = 127 of A1 hi / A2 hi
+  // operand buffers: zero (rows >= ld of A are never written again), then the row of ones at m = 127 of A1 hi / A2 hi
   for (int i = tid; i < 2 * kObBytes / 16; i += kThreads) reinterpret_cast<uint4*>(ob0)[i] = make_uint4(0, 0, 0, 0);
+  __syncthreads();
+  if (tid < 2 * 2 * 4) {                                       // (buffer, operand, k chunk)
+    const int q = tid & 3, which = (tid >> 2) & 1, b = tid >> 3;
+    *reinterpret_cast<float4*>(ob0 + b * kObBytes + (which ? kOffA2 : kOffA1) + kmaj64(127, q)) = make_float4(1.f, 1.f, 1.f, 1.f);
+  }
   fence_proxy_async();
   __syncthreads();
-  if (tid < 2 * 2 * kTK) {                                     // (buffer, operand, k)
-    const int k = tid & (kTK - 1), which = (tid >> 4) & 1, b = tid >> 5;
-    unsigned char* a = ob0 + b * kObBytes + (which ? kOffA2 : kOffA1);
-    *reinterpret_cast<float*>(a + (k >> 2) * kSboA + 3 * kLbo + atom_chunk(k & 3, 7) + 12) = 1.0f;
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
   auto issue_tma = [&](int tile, int s) {
     const long long r0 = (long long)tile * kTK;
@@ -124,147 +95,125 @@ __global__ void __launch_bounds__(kThreads, 1) k_dcrnn_wgrad_tc(WgTcParams p) {
     tma_bulk_g2s(st + 2 * kTK * ld, p.dpzr + r0 * 2 * kCo, bzr, &raw_full[s]);
     tma_bulk_g2s(st + 2 * kTK * ld + kTK * 2 * kCo, p.dph + r0 * kCo, bh, &raw_full[s]);
   };
-  constexpr uint32_t ID64 = umma_idesc_tf32_mn(128, 64), ID32 = umma_idesc_tf32_mn(128, 32);
-  // The eight converting warps work as two groups of four: group g converts the tiles with (it & 1) == g into operand buffer g, so the
-  // serial chain of a tile (wait -> LDS -> cvt -> STS -> proxy fence -> arrive, ~1 k cycles of latency) of one group runs under the other's.
-  // Conversion work of a thread is the same for every tile, so its source / destination offsets are computed once (gt = thread in group):
-  //   S1, S2     rows (gt >> 5) + 4 j, j = 0..3, float4 chunk m4 = gt & 31 (idle when m4 >= ld / 4)
-  //   dpre_zr    rows (gt >> 4) and (gt >> 4) + 8, chunk gt & 15            dpre_h    row gt >> 3, chunk gt & 7
-  const int grp = (tid >> 7) & 1, gt = tid & 127;
-  const int m4 = gt & 31, mrow = gt >> 5, m = 4 * m4;
-  const bool a_on = m4 < ld4;
-  const int a_src = mrow * ld + m;                                                   // + 4 j ld
-  const int a_dst = (m >> 5) * kLbo + atom_chunk(mrow, m4 & 7);                      // + j kSboA   ((mrow + 4 j) >> 2 == j, & 3 == mrow)
-  const bool z0 = m >= p.C3, z1 = m + 1 >= p.C3, z2 = m + 2 >= p.C3, z3 = m + 3 >= p.C3;
-  const int b1k = gt >> 4, b1n4 = gt & 15;
-  const int b1_src = 2 * kTK * ld + b1k * 2 * kCo + 4 * b1n4;                        // + 8 rows
-  const int b1_dst = (b1k >> 2) * kSboB1 + (b1n4 >> 3) * kLbo + atom_chunk(b1k & 3, b1n4 & 7);   // + 2 kSboB1
-  const int b2k = gt >> 3, b2n4 = gt & 7;
-  const int b2_src = 2 * kTK * ld + kTK * 2 * kCo + b2k * kCo + 4 * b2n4;
-  const int b2_dst = (b2k >> 2) * kSboB2 + atom_chunk(b2k & 3, b2n4);
-  const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-  auto mask_cols = [&](float4 v) {
-    if (z0) v.x = 0.f;
-    if (z1) v.y = 0.f;
-    if (z2) v.z = 0.f;
-    if (z3) v.w = 0.f;
-    return v;
-  };
 
   int n_local = 0;                                               // tiles of this CTA
   for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) ++n_local;
 
   if (warp == kConvThreads / 32) {
-    // ---- producer / issuer warp: one lane keeps the TMA ring full and issues the 12 MMAs of every tile as soon as its operand buffer is
-    // complete -- the converting warps never wait for the ~150 serial instructions of descriptor set-up and MMA issue.  (Letting all 32
-    // lanes of this warp run the loop and its waits, with one lane issuing, measured slower: 85 vs 77 us.)  Profile of this version
-    // (profiles/r02_dcrnn_wgrad_tc.txt): 69 us, the converting warps spend 56 % of their time waiting for the MMAs of tile it - 2 to retire
-    // (tensor pipe active 17 %): the six dependent K = 8 MMAs per accumulator and tile are latency-, not throughput-bound.
+    // ---- producer warp: one lane keeps the TMA ring full -------------------------------------------------------------------------
     if (lane == 0) {
-      for (int q = 0; q < kStages - 1 && q < n_local; ++q) issue_tma(blockIdx.x + q * gridDim.x, q);
-      for (int it = 0; it < n_local; ++it) {
-        const int ob = it & 1, nxt = it + kStages - 1;
-        if (nxt < n_local) {
-          const int sp = nxt % kStages;                          // last used by tile it - 1
-          if (it >= 1) mbar_wait(&raw_free[sp], ((it - 1) / kStages) & 1);
-          issue_tma(blockIdx.x + nxt * gridDim.x, sp);
-        }
-        mbar_wait(&ob_full[ob], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t ob_s = smem_u32(ob0 + ob * kObBytes);
-#pragma unroll
-        for (int kg = 0; kg < 2; ++kg) {
-          // one kind::tf32 MMA consumes K = 8 = two k atoms (SBO apart), starting at atom 2 kg
-          const uint64_t a1h = umma_desc_mn(ob_s + kOffA1 + kg * 2 * kSboA, kLbo, kSboA), a1l = umma_desc_mn(ob_s + kOffA1 + kLoA + kg * 2 * kSboA, kLbo, kSboA);
-          const uint64_t a2h = umma_desc_mn(ob_s + kOffA2 + kg * 2 * kSboA, kLbo, kSboA), a2l = umma_desc_mn(ob_s + kOffA2 + kLoA + kg * 2 * kSboA, kLbo, kSboA);
-          const uint64_t b1h = umma_desc_mn(ob_s + kOffB1 + kg * 2 * kSboB1, kLbo, kSboB1), b1l = umma_desc_mn(ob_s + kOffB1 + kLoB1 + kg * 2 * kSboB1, kLbo, kSboB1);
-          const uint64_t b2h = umma_desc_mn(ob_s + kOffB2 + kg * 2 * kSboB2, kLbo, kSboB2), b2l = umma_desc_mn(ob_s + kOffB2 + kLoB2 + kg * 2 * kSboB2, kLbo, kSboB2);
-          // four accumulator sets used round-robin: the tensor core's fp32 accumulation is not round-to-nearest, a 4x shorter chain per
-          // set (and an fp32 sum of the sets in the epilogue) keeps the result close to the fp32 FFMA kernel
-          const uint32_t first = (it < kAccSets && kg == 0) ? 0u : 1u, dz = tmem + (uint32_t)(it & (kAccSets - 1)) * 96u, dh = dz + 64u;
-          umma_tf32(dz, a1l, b1h, ID64, first);        // small terms first
-          umma_tf32(dz, a1h, b1l, ID64, 1u);
-          umma_tf32(dz, a1h, b1h, ID64, 1u);
-          umma_tf32(dh, a2l, b2h, ID32, first);
-          umma_tf32(dh, a2h, b2l, ID32, 1u);
-          umma_tf32(dh, a2h, b2h, ID32, 1u);
-        }
-        umma_commit(&ob_free[ob]);
+      for (int q = 0; q < kStages && q < n_local; ++q) issue_tma(blockIdx.x + q * gridDim.x, q);
+      for (int it = kStages; it < n_local; ++it) {
+        const int sp = it % kStages;                             // last used by tile it - kStages
+        mbar_wait(&raw_free[sp], ((it - kStages) / kStages) & 1);
+        issue_tma(blockIdx.x + it * gridDim.x, sp);
       }
-      umma_commit(done);          // (a wait on ob_free's parity would alias for threads that have not followed that barrier phase by phase)
     }
-  } else {
-    // ---- converting warps --------------------------------------------------------------------------------------------------------
-    for (int it = grp; it < n_local; it += 2) {
-      const int s = it % kStages;
-      const long long r0 = ((long long)blockIdx.x + (long long)it * gridDim.x) * kTK;
-      const int nr = (int)((p.rows - r0) < kTK ? (p.rows - r0) : kTK);                  // < 16 only for the last tile: missing rows become zeros
-      mbar_wait(&raw_full[s], (it / kStages) & 1);
-      const float* st = reinterpret_cast<const float*>(raw + (size_t)s * stage_bytes);
-      float4 s1[4], s2[4], v1[2], v2 = zero4;
+    return;
+  }
+
+  // ---- converting / MMA warps ------------------------------------------------------------------------------------------------------
+  // Conversion work of a thread is the same for every tile (k = row of the raw tile):
+  //   A1, A2     operand row m = tid & 127, k chunk pair (tid >> 7) * 2 + {0, 1}   (idle when m >= ld)
+  //   B1         row n = tid & 63, k chunk tid >> 6                                 B2   row n = tid & 31, k chunk tid >> 5 (tid < 128)
+  const int wg = warp >> 2, wt = tid & 127;
+  const int am = tid & 127, aq0 = (tid >> 7) * 2;
+  const bool a_on = am < ld;
+  const bool a_zero = am >= p.C3;                                // padding columns of S hold garbage: they must never reach a result
+  const int b1n = tid & 63, b1q = tid >> 6, b2n = tid & 31, b2q = tid >> 5;
+  WgAcc acc[2];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        s1[j] = s2[j] = zero4;
-        if (a_on && mrow + 4 * j < nr) {
-          s1[j] = *reinterpret_cast<const float4*>(st + a_src + 4 * j * ld);
-          s2[j] = *reinterpret_cast<const float4*>(st + kTK * ld + a_src + 4 * j * ld);
-        }
+  for (int s = 0; s < 2; ++s)
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[s].z0[i] = acc[s].z1[i] = acc[s].h[i] = 0.f;
+
+  auto issue = [&](WgAcc& a, uint32_t ob_s) {
+    wgmma_fence();
+#pragma unroll
+    for (int kg = 0; kg < 2; ++kg) {
+      // one TF32 wgmma consumes K = 8 = 32 bytes of each operand row
+      const uint32_t a1 = ob_s + kOffA1 + wg * 64 * 64 + kg * 32, a2 = ob_s + kOffA2 + wg * 64 * 64 + kg * 32;
+      const uint32_t b1 = ob_s + kOffB1 + kg * 32, b2 = ob_s + kOffB2 + kg * 32;
+#pragma unroll
+      for (int pass = 0; pass < 3; ++pass) {           // lo*hi, hi*lo, hi*hi (small terms first)
+        const uint32_t ao = pass == 0 ? kLoA : 0, b1o = pass == 1 ? kLoB1 : 0, b2o = pass == 1 ? kLoB2 : 0;
+        wgmma_tf32_n32(a.z0, desc64(a1 + ao), desc64(b1 + b1o));
+        wgmma_tf32_n32(a.z1, desc64(a1 + ao), desc64(b1 + b1o + 32 * 64));
+        wgmma_tf32_n32(a.h, desc64(a2 + ao), desc64(b2 + b2o));
       }
+    }
+    wgmma_commit();
+  };
+
+  for (int it = 0; it < n_local; ++it) {
+    const int s = it % kStages, ob = it & 1;
+    const long long r0 = ((long long)blockIdx.x + (long long)it * gridDim.x) * kTK;
+    const int nr = (int)((p.rows - r0) < kTK ? (p.rows - r0) : kTK);                  // < 16 only for the last tile: missing rows become zeros
+    mbar_wait(&raw_full[s], (it / kStages) & 1);
+    const float* st = reinterpret_cast<const float*>(raw + (size_t)s * stage_bytes);
+    auto col4 = [&](const float* base, int pitch, int q, int n) {                      // rows 4q..4q+3 of column n
+      float v[4];
 #pragma unroll
-      for (int j = 0; j < 2; ++j) v1[j] = b1k + 8 * j < nr ? *reinterpret_cast<const float4*>(st + b1_src + 8 * j * 2 * kCo) : zero4;
-      if (b2k < nr) v2 = *reinterpret_cast<const float4*>(st + b2_src);
-      if (it >= 2) mbar_wait(&ob_free[grp], ((it >> 1) - 1) & 1);                      // the MMAs of tile it - 2 have read this operand buffer
-      tc_fence_after();
-      unsigned char* o = ob0 + grp * kObBytes;
-      if (a_on) {
+      for (int e = 0; e < 4; ++e) v[e] = 4 * q + e < nr ? base[(4 * q + e) * pitch + n] : 0.f;
+      return make_float4(v[0], v[1], v[2], v[3]);
+    };
+    const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 s1[2], s2[2];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          store_split_tf32(o + kOffA1, kLoA, a_dst + j * kSboA, mask_cols(s1[j]));
-          store_split_tf32(o + kOffA2, kLoA, a_dst + j * kSboA, mask_cols(s2[j]));
-        }
+    for (int i = 0; i < 2; ++i) {
+      s1[i] = (a_on && !a_zero) ? col4(st, ld, aq0 + i, am) : zero4;
+      s2[i] = (a_on && !a_zero) ? col4(st + kTK * ld, ld, aq0 + i, am) : zero4;
+    }
+    const float4 v1 = col4(st + 2 * kTK * ld, 2 * kCo, b1q, b1n);
+    const float4 v2 = tid < 128 ? col4(st + 2 * kTK * ld + kTK * 2 * kCo, kCo, b2q, b2n) : zero4;
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&raw_free[s]);
+    wgmma_wait<1>();            // my MMAs of tile it - 2 (operand buffer ob) are done; those of tile it - 1 keep running
+    conv_sync();                // ... and the other warpgroup's
+    unsigned char* o = ob0 + ob * kObBytes;
+    if (a_on) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        store_split_tf32(o + kOffA1, kLoA, kmaj64(am, aq0 + i), s1[i]);
+        store_split_tf32(o + kOffA2, kLoA, kmaj64(am, aq0 + i), s2[i]);
       }
+    }
+    store_split_tf32(o + kOffB1, kLoB1, kmaj64(b1n, b1q), v1);
+    if (tid < 128) store_split_tf32(o + kOffB2, kLoB2, kmaj64(b2n, b2q), v2);
+    fence_proxy_async();          // generic-proxy operand stores -> visible to the tensor core
+    conv_sync();
+    // two accumulator sets used alternately: the tensor core's fp32 accumulation is not round-to-nearest, a shorter chain per set (and an
+    // fp32 sum of the sets in the epilogue) keeps the result close to the fp32 FFMA kernel
+    if (it & 1) issue(acc[1], smem_u32(o)); else issue(acc[0], smem_u32(o));
+  }
+  wgmma_wait<0>();
 #pragma unroll
-      for (int j = 0; j < 2; ++j) store_split_tf32(o + kOffB1, kLoB1, b1_dst + j * 2 * kSboB1, v1[j]);
-      store_split_tf32(o + kOffB2, kLoB2, b2_dst, v2);
-      fence_proxy_async();          // generic-proxy operand stores -> visible to the tensor core
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(&ob_full[grp]); mbar_arrive(&raw_free[s]); }
+  for (int s = 0; s < 2; ++s) { acc_fence(acc[s].z0); acc_fence(acc[s].z1); acc_fence(acc[s].h); }
+
+  // ---- epilogue: fragment rows m = 64 wg + 16 (wt / 32) + (lane / 4) (+8), columns 8 j + 2 (lane % 4) (+1) ------------------------
+  const int MG8 = p.MG * 8;
+  float* out = p.partial + (size_t)blockIdx.x * ((size_t)MG8 * 3 * kCo + 3 * kCo);
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int m = 64 * wg + 16 * (wt >> 5) + ((wt & 31) >> 2) + 8 * hr;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int n = 8 * j + 2 * (wt & 3), a = 4 * j + 2 * hr;
+      const float2 z0 = make_float2(acc[0].z0[a] + acc[1].z0[a], acc[0].z0[a + 1] + acc[1].z0[a + 1]);
+      const float2 z1 = make_float2(acc[0].z1[a] + acc[1].z1[a], acc[0].z1[a + 1] + acc[1].z1[a + 1]);
+      const float2 h = make_float2(acc[0].h[a] + acc[1].h[a], acc[0].h[a + 1] + acc[1].h[a + 1]);
+      if (m < MG8) {
+        *reinterpret_cast<float2*>(out + (size_t)m * 2 * kCo + n) = z0;
+        *reinterpret_cast<float2*>(out + (size_t)m * 2 * kCo + 32 + n) = z1;
+        *reinterpret_cast<float2*>(out + (size_t)MG8 * 2 * kCo + (size_t)m * kCo + n) = h;
+      } else if (m == 127) {                                    // the ones row: bias sums z | r | h
+        float* bsum = out + (size_t)MG8 * 3 * kCo;
+        *reinterpret_cast<float2*>(bsum + n) = z0;
+        *reinterpret_cast<float2*>(bsum + 32 + n) = z1;
+        *reinterpret_cast<float2*>(bsum + 64 + n) = h;
+      }
     }
   }
-  const int it = n_local;
-  // ---- epilogue: the last commit covers every MMA issued by thread 0 ------------------------------------------------------------
-  mbar_wait(done, 0);
-  tc_fence_after();
-  if (warp < 4) {
-    const int m = 32 * warp + lane, MG8 = p.MG * 8;
-    float* out = p.partial + (size_t)blockIdx.x * ((size_t)MG8 * 3 * kCo + 3 * kCo);
-    const uint32_t trow = tmem + ((uint32_t)(32 * warp) << 16);
-    const int nsets = it < kAccSets ? it : kAccSets;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {                                // columns [0,32) [32,64) of D_zr, [64,96) = D_h, summed over the sets
-      uint32_t v[32], w[32];
-      tmem_ld32(trow + 32 * c, v);
-      tmem_ld_wait();
-      for (int js = 1; js < nsets; ++js) {
-        tmem_ld32(trow + 96 * js + 32 * c, w);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(w[j]));
-      }
-      float* dst = nullptr;
-      if (m < MG8) dst = c < 2 ? out + (size_t)m * 2 * kCo + 32 * c : out + (size_t)MG8 * 2 * kCo + (size_t)m * kCo;
-      else if (m == 127) dst = out + (size_t)MG8 * 3 * kCo + 32 * c;        // the ones column: bias sums z | r | h
-      if (dst) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          reinterpret_cast<float4*>(dst)[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                                          __uint_as_float(v[4 * j + 3]));
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
 }
 
 }  // namespace
@@ -277,12 +226,12 @@ int wgrad_tc_launch(int cin, long long rows, int ld, const float* S1, const floa
   p.C3 = 3 * (cin + kCo); p.MG = (p.C3 + 7) / 8;
   p.n_tiles = (int)((rows + kTK - 1) / kTK);
   p.partial = partial;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   STMP_CUDA_OK(cudaGetDevice(&dev));
   STMP_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   int grid = sms < max_parts ? sms : max_parts;
   if (p.n_tiles < grid) grid = p.n_tiles > 0 ? p.n_tiles : 1;
-  const int smem = 2 * kObBytes + kStages * kTK * (2 * ld + 3 * kCo) * 4 + (2 * kStages + 5) * 8 + 16;
+  const int smem = 2 * kObBytes + kStages * kTK * (2 * ld + 3 * kCo) * 4 + 2 * kStages * 8;
   STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_wgrad_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   k_dcrnn_wgrad_tc<<<grid, kThreads, smem, st>>>(p);
   STMP_LAUNCH_OK("k_dcrnn_wgrad_tc");

@@ -6,7 +6,7 @@ There is no network here, so nothing is downloaded: `raw_data_dir` must already 
 archives -- `adj_mat.npy (N,N)` + `node_values.npy (T,N,F)` for METR-LA, `pems_adj_mat.npy` + `pems_node_values.npy`
 for PEMS-BAY (metr_la.py:66-77, pems_bay.py:72-84); a missing file raises FileNotFoundError naming it.
 
-B200-side addition: `get_index_loaders(...)` returns `signal.IndexBatchLoader`s over a series that lives in HBM
+Addition of this package: `get_index_loaders(...)` returns `signal.IndexBatchLoader`s over a series that lives in HBM
 (z-scored on the device, metr_la.py:180-190), sharded per rank with DistributedSampler semantics -- the feed the
 fused DCRNN sequence kernel consumes without materialising windows."""
 import os

@@ -12,7 +12,7 @@ What runs where
   launch per hop covers every timestep; the dense `(I*S)^T @ x` used for a diagonal scale (:160-165) is
   a broadcast multiply;
 * inference on a static graph (N <= 320, T <= 12, 64 time filters, stride 1) keeps the activations channels-last
-  (B, N, T, F) between blocks and runs every large product on tcgen05 with its neighbours fused (csrc/gemm_blocks.cu):
+  (B, N, T, F) between blocks and runs every large product on wgmma with its neighbours fused (csrc/gemm_blocks.cu):
   spatial attention `softmax(Vs @ sigmoid(LHS @ RHS + bs))` in ONE kernel (the N x N sigmoid is generated in the operand
   stage, the softmax is the epilogue; the result is kept transposed and consumed so by `stmp_spmm_att_t`); the Chebyshev
   contraction + ReLU; time convolution + residual convolution + ReLU + LayerNorm; the final convolution; and the small-matrix
@@ -214,7 +214,7 @@ class ASTGCNBlock(nn.Module):
             self._lam_cache[key] = hit
         return hit[0]
 
-    # ---- native inference path: channels-last activations, fused tcgen05 products ------------------------------------
+    # ---- native inference path: channels-last activations, fused wgmma products ------------------------------------
     def _native_ok(self, N, Fi, T):
         tc, rc = self._time_convolution, self._residual_convolution
         K = self._chebconv_attention._weight.size(0)

@@ -133,7 +133,7 @@ class _DcrnnSeqFn(torch.autograd.Function):
             dX = torch.empty(X.shape, **f32) if ctx.needs_input_grad[0] else None   # dense: the kernels write (B,T,N,Cin) row-major
             dH0 = torch.empty(B, N, Co, **f32)
             # the bases depend only on forward results, the recurrence only on gout: run them side by side -- the
-            # recurrence occupies one SM per window (64 of 148 at the reference's batch size), the basis kernel fills the
+            # recurrence occupies one SM per window (64 of 132 at the reference's batch size), the basis kernel fills the
             # rest.  Fork/join with events, so a CUDA-graph capture records two parallel branches.
             main = torch.cuda.current_stream(X.device)
             side = _side_stream(X.device)
@@ -314,7 +314,7 @@ class DCRNN(torch.nn.Module):
                 self.conv_x_z.bias, self.conv_x_r.bias, self.conv_x_h.bias)
 
     def _weight_image(self):
-        """B-operand image for the tcgen05 kernel, rebuilt only when a parameter changes."""
+        """B-operand image for the wgmma kernel, rebuilt only when a parameter changes."""
         return self._wimg.get(list(self.parameters()),
                               lambda: ops.dcrnn_weight_image(*self._params(), self.in_channels, self.K))
 

@@ -6,7 +6,7 @@ lambda_max) -> (H, C)`, state_dict keys `conv_{i,f,c,o}.lins.{k}.weight/.bias`, 
 The reference runs four ChebConvs on the same H (4(K-1) propagations) and four `X @ W_g` products.  Here
 T_k(H) is computed once ((K-1) SpMMs on `out` channels, written in place into the basis buffer
 S = [X | T_0(H) | .. | T_{K-1}(H)]) and ONE GEMM produces all four gate pre-activations; without autograd that GEMM
-is the tcgen05 kernel with the LSTM gate chain in its epilogue (`stmp_gemm_lstm_f32`, zero peepholes -- GCLSTM has
+is the wgmma kernel with the LSTM gate chain in its epilogue (`stmp_gemm_lstm_f32`, zero peepholes -- GCLSTM has
 none, and its output gate therefore does not depend on the new cell state, gc_lstm.py:139-145)."""
 import torch
 

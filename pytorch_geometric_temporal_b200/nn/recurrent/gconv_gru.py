@@ -70,7 +70,7 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
         if H is None:
             H = torch.zeros(*X.shape[:-1], Co, device=X.device, dtype=X.dtype)
         plan = self._cheb_plan(edge_index, edge_weight, N, self.normalization, lambda_max)
-        if self._fused_ok(plan, X, H):   # one tcgen05 launch for the whole cell (stmp_gru_seq_fwd)
+        if self._fused_ok(plan, X, H):   # one wgmma launch for the whole cell (stmp_gru_seq_fwd)
             W, b, img = self._packed()
             return ops.gru_seq_fwd(plan, 1 if K > 1 else 0, X.reshape(1, 1, N, Ci), W, b, h0=H.reshape(1, N, Co), wimage=img)[0, 0]
         TU = cheb_basis(plan, torch.cat([X, H], dim=-1), K)              # K x (N, Ci+Co)

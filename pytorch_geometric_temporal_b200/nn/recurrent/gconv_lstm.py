@@ -27,9 +27,9 @@ def _chunked_tn(A: torch.Tensor, B: torch.Tensor) -> torch.Tensor:
 class _LstmCellFn(torch.autograd.Function):
     """Training path of one GConvLSTM step on a large graph (gconv_lstm.py:204-238) with a hand-written backward.
 
-    forward : Chebyshev basis S = [T_0|..|T_{K-1}]([X|H]) built in place by `stmp_spmm`, then ONE tcgen05 launch computes S @ W and
+    forward : Chebyshev basis S = [T_0|..|T_{K-1}]([X|H]) built in place by `stmp_spmm`, then ONE wgmma launch computes S @ W and
               the whole peephole gate chain in its epilogue (`stmp_gemm_lstm_f32`).  Only S, C_{t-1}, C_t are kept.
-    backward: pre = S @ W recomputed on tcgen05 -> `stmp_lstm_gate_bwd` (gate derivatives) -> dS = dpre @ W^T (tcgen05, two column
+    backward: pre = S @ W recomputed on wgmma -> `stmp_lstm_gate_bwd` (gate derivatives) -> dS = dpre @ W^T (wgmma, two column
               halves) -> adjoint of the Chebyshev recurrence by TRANSPOSED SpMMs in place -> dX, dH;  dW = S^T dpre as a chunked
               GEMM; peephole / bias gradients as column reductions.  ~14 launches instead of the ~90 autograd records."""
 
@@ -153,7 +153,7 @@ class GConvLSTM(torch.nn.Module, ChebPlanMixin):
                                                   or H.requires_grad or C.requires_grad)
         Cw = self.in_channels + Co
         if not needs_grad and Co in (32, 64) and (self.K * Cw) % 4 == 0 and Cw % 4 == 0:
-            # large-graph inference: T_k written in place into S = [T_0|T_1|..] by the SpMM kernel, then ONE tcgen05
+            # large-graph inference: T_k written in place into S = [T_0|T_1|..] by the SpMM kernel, then ONE wgmma
             # launch does S @ W and the whole peephole-LSTM gate chain in its epilogue (stmp_gemm_lstm_f32)
             S = torch.empty(*X.shape[:-1], self.K * Cw, device=X.device, dtype=torch.float32)
             S[..., :self.in_channels] = X

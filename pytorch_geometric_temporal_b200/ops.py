@@ -260,7 +260,7 @@ def gemm_prepack(W: torch.Tensor) -> torch.Tensor:
 
 def gemm(A: torch.Tensor, packed: torch.Tensor, K: int, N: int, bias: Optional[torch.Tensor] = None,
          out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """C = A @ W + bias on tcgen05 with the fp16 hi/lo operand split (fp32-class accuracy).  A (..., K) contiguous.
+    """C = A @ W + bias on wgmma with the fp16 hi/lo operand split (fp32-class accuracy).  A (..., K) contiguous.
     `out`: a 2-D (M, N) view with unit column stride (e.g. a column block of a wider buffer) to write into."""
     A = _f32c(A, "A")
     M = A.numel() // K
@@ -393,7 +393,7 @@ def gemm_lstm(A: torch.Tensor, packed: torch.Tensor, K: int, cout: int, conv_bia
 
 
 def dcrnn_weight_image(wz, wr, wh, bz, br, bh, cin: int, K: int) -> Optional[torch.Tensor]:
-    """B-operand image of the tcgen05 kernel for DConv weights (None when the configuration has no tensor kernel)."""
+    """B-operand image of the wgmma kernel for DConv weights (None when the configuration has no tensor kernel)."""
     cout = wz.size(-1)
     if cout != 32 or K != 2 or not (1 <= cin <= 4):
         return None

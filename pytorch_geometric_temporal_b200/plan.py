@@ -17,7 +17,7 @@ def _require_cuda(t: torch.Tensor, name: str):
     if not t.is_cuda:
         raise RuntimeError(
             f"{name} is on {t.device}: pytorch_geometric_temporal_b200 runs the hot path on CUDA only "
-            "(hand-written sm_100a kernels, no CPU fallback).")
+            "(hand-written sm_90a kernels, no CPU fallback).")
 
 
 class GraphPlan:

@@ -6,7 +6,7 @@ batch 32 per GPU, data-parallel.
   python -m torch.distributed.run --nnodes=1 --nproc-per-node 4 --master-addr 127.0.0.1 --master-port 29512 tests/perf/bench_cfg4_ddp.py
 
 Two numbers (rank 0 prints one JSON line; device-timed, max over ranks):
-  * inference: windows/s through the native channels-last path (fused spatial attention + blocked tcgen05 GEMMs), replicas, no collective;
+  * inference: windows/s through the native channels-last path (fused spatial attention + blocked wgmma GEMMs), replicas, no collective;
   * training:  windows/s of forward + backward (autograd around stmp_spmm / stmp_spmm_att_grad) + ONE flat NCCL all-reduce + Adam."""
 import argparse
 import json

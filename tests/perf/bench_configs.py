@@ -125,7 +125,7 @@ def main():
         cms = cpu_time(cpu5, budget=8) * 6 * 8  # 2 of 12 steps, 1 of 8 windows, scaled
         out.append({"config": "cfg5 GConvLSTM(64,64,K=3), 10k nodes / 100k edges, 8 windows x 12 steps per GPU, forward", "launch": how,
                     "ours_ms": ms, "ours_snapshots_per_s": 8 / ms * 1e3, "cpu_oracle_ms_scaled": cms, "cpu_snapshots_per_s": 8 / cms * 1e3})
-        # K4 probe: the tcgen05 split-fp16 GEMM alone at the cfg5 size, vs cuBLAS fp32 (torch.matmul)
+        # K4 probe: the wgmma split-fp16 GEMM alone at the cfg5 size, vs cuBLAS fp32 (torch.matmul)
         from pytorch_geometric_temporal_b200 import ops
         A = torch.randn(80000, 384, device=DEV); W = torch.randn(384, 256, device=DEV) * 0.1
         packed = ops.gemm_prepack(W)
@@ -135,8 +135,8 @@ def main():
         pk_b = ops.gemm_blocks_prepack([W[64 * i:64 * i + 64].contiguous() for i in range(6)])
         Cb = torch.empty(80000, 256, device=DEV)
         ms_gb = gpu_time(lambda: ops.gemm_blocks([(A[:, 64 * i:64 * i + 64], 64, 0) for i in range(6)], pk_b, 256, 256, None, ops.EPI_BIAS, out=Cb), iters=20)
-        out.append({"config": "K4 probe: C[80000,256] = A[80000,384] @ W, fp32 in/out", "tcgen05_split_fp16_ms": ms_tc, "cublas_fp32_ms": ms_cb,
-                    "tcgen05_blocked_ms (TMA weight image, prefetched A)": ms_gb,
+        out.append({"config": "K4 probe: C[80000,256] = A[80000,384] @ W, fp32 in/out", "wgmma_split_fp16_ms": ms_tc, "cublas_fp32_ms": ms_cb,
+                    "wgmma_blocked_ms (TMA weight image, prefetched A)": ms_gb,
                     "algorithmic_bytes": byt, "achieved_gbs": byt / ms_tc / 1e6, "blocked_achieved_gbs": byt / ms_gb / 1e6,
                     "tflops_fp32_equiv": 2 * 80000 * 384 * 256 / ms_tc / 1e9})
     for o in out:

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Weight-gradient contraction of the DCRNN training step at the reference's batch size (rows = 12 * 64 * 207): fp32 FFMA kernel vs the
-tcgen05 TF32-split kernel, both against a float64 contraction.  One JSON line."""
+wgmma TF32-split kernel, both against a float64 contraction.  One JSON line."""
 import json
 import os
 import sys
@@ -38,6 +38,6 @@ for tc in (0, 1):
         e1.record()
         torch.cuda.synchronize()
         ts.append(e0.elapsed_time(e1) * 1e3)
-    res["tcgen05" if tc else "ffma"] = {"us_cold": round(min(ts), 1), "rel_err_vs_fp64": err}
+    res["wgmma" if tc else "ffma"] = {"us_cold": round(min(ts), 1), "rel_err_vs_fp64": err}
 _lib.set_option("dcrnn_wgrad_tc", 1)
 print(json.dumps(res))

@@ -80,22 +80,17 @@ def test_masked_mae():
     assert abs(float(D.masked_mae_loss(y, t)) - 0.75) < 1e-6
 
 
-def test_masked_mae_matches_reference_example_util():
+def test_masked_mae_matches_reference_example_util(golden_dir):
     """The op-for-op form (the checker of the fused CUDA loss) against the unmodified reference function
-    examples/indexBatching/DCRNN/utils.py:10-18, loaded by path where /root/reference exists."""
-    import importlib.util
+    examples/indexBatching/DCRNN/utils.py:10-18: its losses on these three seeded (prediction, target) pairs with 0 %, 30 % and
+    100 % missing targets are stored in tests/golden/masked_mae_reference.pt."""
     import os
-    path = "/root/reference/examples/indexBatching/DCRNN/utils.py"
-    if not os.path.isfile(path):
-        pytest.skip("/root/reference not present")
-    spec = importlib.util.spec_from_file_location("ref_dcrnn_utils", path)
-    ref = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(ref)
+    want = torch.load(os.path.join(golden_dir, "masked_mae_reference.pt"))
     torch.manual_seed(0)
-    for zero_frac in (0.0, 0.3, 1.0):
+    for zero_frac, b in zip((0.0, 0.3, 1.0), want):
         y = torch.randn(64, 207)
         y[torch.rand(64, 207) < zero_frac] = 0.0
         p = torch.randn(64, 207)
-        a, b = D.masked_mae_loss_reference(p, y), ref.masked_mae_loss(p, y)
+        a = D.masked_mae_loss_reference(p, y)
         assert torch.equal(a, b)
         assert torch.equal(D.masked_mae_loss(p, y), b)          # CPU tensors take the op-for-op form

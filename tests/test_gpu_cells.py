@@ -100,7 +100,7 @@ def test_tgcn_goldens(golden_dir):
 @pytest.mark.parametrize("fused", [True, False])
 def test_gconv_lstm_cfg5_cell_sequence_gradients_vs_reference_golden(golden_dir, fused):
     """GConvLSTM(64,64,K=3) unrolled over 6 steps: final state AND every gradient against the UNMODIFIED reference's autograd
-    (tests/golden/make_goldens_r2.py) -- through the hand-written cell backward (_LstmCellFn: tcgen05 GEMM + LSTM epilogue forward,
+    (tests/golden/make_goldens_r2.py) -- through the hand-written cell backward (_LstmCellFn: wgmma GEMM + LSTM epilogue forward,
     recompute + stmp_lstm_gate_bwd + transposed SpMM backward) and through the op-for-op autograd path."""
     g = _load(golden_dir, "gconv_lstm_cfg5seq")
     ei, ew = g["edge_index"].to(DEV), g["edge_weight"].to(DEV)
@@ -207,7 +207,7 @@ def test_astgcn_goldens(golden_dir):
 def test_astgcn_config4_shape_vs_reference_golden(golden_dir):
     """BASELINE configs[3] AT SHAPE: ASTGCN(3 blocks, K=3, 64/64 filters) on 307 nodes, batch 32 (and normalization None on 8
     rows), against the UNMODIFIED reference (tests/golden/make_goldens_r2.py) at the STRICT tolerance rtol 1e-4 / atol 1e-5,
-    through the native channels-last path: fused spatial attention, blocked tcgen05 GEMMs (k_gemm_blocks), attention SpMM."""
+    through the native channels-last path: fused spatial attention, blocked wgmma GEMMs (k_gemm_blocks), attention SpMM."""
     g = _load(golden_dir, "astgcn_cfg4")
     ei = g["edge_index"].to(DEV)
     for c in g["cases"].values():
@@ -369,7 +369,7 @@ def test_astgcn_backward_runs_and_matches_oracle_grad(golden_dir):
         _close(prm.grad, p[k].grad, rtol=2e-3, atol=2e-4)
 
 
-# ---- the generic fused graph-GRU kernel (stmp_gru_seq_fwd, tcgen05) behind GConvGRU / TGCN / A3TGCN -----------------
+# ---- the generic fused graph-GRU kernel (stmp_gru_seq_fwd, wgmma) behind GConvGRU / TGCN / A3TGCN -----------------
 def _metr():
     ei, ew, _ = synthetic.metr_la_like(0, 16)
     return torch.from_numpy(ei), torch.from_numpy(ew)

@@ -160,7 +160,7 @@ def test_unsupported_shapes_fall_back_to_tiled_not_cpu():
 
 
 def test_full_bench_size_two_independent_kernels_agree():
-    """Full BASELINE size (1184 windows x 12 steps, METR-LA shape): the tcgen05 kernel (fp16 hi/lo split operands, TMEM)
+    """Full BASELINE size (1184 windows x 12 steps, METR-LA shape): the wgmma kernel (fp16 hi/lo split operands, register accumulators)
     and the FFMA kernel (exact fp32, different thread mapping, TMA-staged inputs) are independent implementations of the
     same recurrence; they must agree to fp32 rounding on every one of the 94 M outputs, and a few windows are spot-checked
     against the oracle."""
@@ -304,7 +304,7 @@ def test_cfg2_training_gradients_vs_reference_golden(golden_dir, fused_bwd):
         _DcrnnSeqFn.fused_backward = True
     after = _lib.path_counters()
     ran = {k for k, v in after.items() if v > before.get(k, 0)}
-    assert "k_dcrnn_seq_tc" in ran                                     # the tcgen05 forward served the training call
+    assert "k_dcrnn_seq_tc" in ran                                     # the wgmma forward served the training call
     assert ("k_dcrnn_bwd_seq" in ran) == fused_bwd                     # and the persistent backward exactly when asked
     _close(out, g["out"])
     _close(X.grad, g["gX"], 1e-3, 1e-3 * g["gX"].abs().max().item())

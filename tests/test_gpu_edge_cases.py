@@ -40,7 +40,7 @@ def test_single_node_and_tiny_graphs():
     torch.manual_seed(0)
     m = TGCN(3, 4)
     _close(m.to(DEV)(x.to(DEV), ei.to(DEV)), R.tgcn_cell(m.cpu().state_dict(), x, ei))
-    m = DCRNN(3, 32, 2)   # N=1 through the fused tcgen05 kernel
+    m = DCRNN(3, 32, 2)   # N=1 through the fused wgmma kernel
     want = R.dcrnn_cell(m.state_dict(), x, ei)
     with torch.no_grad():
         _close(m.to(DEV)(x.to(DEV), ei.to(DEV)), want)

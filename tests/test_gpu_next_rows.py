@@ -46,7 +46,7 @@ def test_gc_lstm_goldens(golden_dir):
         x, h, cc = c["X"].to(DEV), c["H"].to(DEV), c["C"].to(DEV)
         n0 = _lib.launch_count()
         with torch.no_grad():
-            ho, co = m(x, ei, ew, h, cc, lm)                      # in-place basis + fused gate kernels / tcgen05 epilogue
+            ho, co = m(x, ei, ew, h, cc, lm)                      # in-place basis + fused gate kernels / wgmma epilogue
             _close(ho, c["outH"]); _close(co, c["outC"])
             if "outH0" in c:
                 ho, co = m(x, ei, lambda_max=lm)

@@ -235,7 +235,7 @@ def test_index_batch_loader_host_batches_and_forward_indexed_match_materialised_
             assert torch.equal(m.forward_indexed(sd, st, 12, ei_t, ew_t), m(x, ei_t, ew_t))
 
 
-# ---- K4: tcgen05 split-fp16 GEMM (stmp_gemm_f32) and its fused LSTM epilogue ------------------------------------------
+# ---- K4: wgmma split-fp16 GEMM (stmp_gemm_f32) and its fused LSTM epilogue ------------------------------------------
 @pytest.mark.parametrize("M,K,N", [(1, 4, 32), (127, 36, 64), (128, 64, 96), (1000, 384, 256), (20000, 132, 128)])
 def test_gemm_tc_matches_fp64(M, K, N):
     g = torch.Generator().manual_seed(M + K + N)

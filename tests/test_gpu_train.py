@@ -75,7 +75,7 @@ def test_flat_adam_cuda_graph_replay_counts_steps_on_device():
 @pytest.mark.parametrize("tc", [0, 1])
 @pytest.mark.parametrize("cin,rows", [(2, 12 * 5 * 207), (1, 1000), (4, 207 * 3 + 5), (2, 7)])
 def test_dcrnn_wgrad_vs_float64(cin, rows, tc):
-    """tc = 1: the tcgen05 contraction (TF32 hi/lo split, MN-major operands); tc = 0: the fp32 FFMA kernel."""
+    """tc = 1: the wgmma contraction (TF32 hi/lo split, K-major operands); tc = 0: the fp32 FFMA kernel."""
     _lib.set_option("dcrnn_wgrad_tc", tc)
     try:
         _wgrad_case(cin, rows, "k_dcrnn_wgrad_tc" if tc else "k_dcrnn_wgrad")

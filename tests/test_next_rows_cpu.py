@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import refload
+from oracle import golden
 from pytorch_geometric_temporal_b200.dataset import METRLADatasetLoader, PemsBayDatasetLoader, dense_to_sparse
 from pytorch_geometric_temporal_b200.signal import StaticGraphTemporalSignalBatch, temporal_signal_split
 
@@ -98,35 +98,26 @@ def test_offline_loader_errors(tmp_path):
         METRLADatasetLoader(raw_data_dir=str(tmp_path)).get_index_dataset()
 
 
-@pytest.mark.skipif(not refload.available(), reason="/root/reference not present")
 @pytest.mark.parametrize("mod,name,prefix", [("dataset.metr_la", "METRLADatasetLoader", ""), ("dataset.pems_bay", "PemsBayDatasetLoader", "pems_")])
 def test_offline_loaders_match_reference(tmp_path, mod, name, prefix):
+    """Against the unmodified reference loader `mod`.`name` run on the same archive (digests in tests/golden/ref_compare.pt.gz)."""
     tmp = str(tmp_path)
     _archive(tmp, 9, 2, 60, prefix)
-    open(os.path.join(tmp, "METR-LA.zip" if prefix == "" else "PEMS-BAY.zip"), "wb").close()      # the reference checks the zip exists
-    # the reference loader does `from ..signal import StaticGraphTemporalSignal`; its signal/__init__ pulls every iterator
-    # (PyG Batch/HeteroData), so expose just that one unmodified class on the path-only parent package refload registers
-    import sys
-    sig = refload.load("signal.static_graph_temporal_signal")
-    sys.modules["torch_geometric_temporal.signal"].StaticGraphTemporalSignal = sig.StaticGraphTemporalSignal
-    ref_cls = getattr(refload.load(mod), name)
+    want = golden.load()["loaders"][name]
     ours_cls = METRLADatasetLoader if prefix == "" else PemsBayDatasetLoader
-    want, got = ref_cls(raw_data_dir=tmp).get_dataset(6, 6), ours_cls(raw_data_dir=tmp).get_dataset(6, 6)
-    assert want.snapshot_count == got.snapshot_count
-    for a, b in zip(want, got):
-        assert torch.equal(a.x, b.x) and torch.equal(a.y, b.y) and torch.equal(a.edge_index, b.edge_index) and torch.equal(a.edge_attr, b.edge_attr)
-    w = ref_cls(raw_data_dir=tmp, index=True).get_index_dataset(lags=6, batch_size=4)
+    got = ours_cls(raw_data_dir=tmp).get_dataset(6, 6)
+    assert len(want["snapshots"]) == got.snapshot_count
+    for a, b in zip(want["snapshots"], got):
+        assert a == tuple(golden.digest(t) for t in (b.x, b.y, b.edge_index, b.edge_attr))
     g = ours_cls(raw_data_dir=tmp, index=True).get_index_dataset(lags=6, batch_size=4)
     for i in range(3):
-        for (xa, ya), (xb, yb) in zip(w[i], g[i]):
-            assert torch.equal(xa, xb) and torch.equal(ya, yb)
+        batches = [(golden.digest(xb), golden.digest(yb)) for xb, yb in g[i]]
+        assert batches == want["loaders"][i]
     for i in range(3, 7):
-        assert torch.equal(w[i], g[i])
+        assert golden.digest(g[i]) == want["rest"][i - 3]
     # DistributedSampler shards
-    w = ref_cls(raw_data_dir=tmp, index=True).get_index_dataset(lags=6, batch_size=4, shuffle=True, world_size=2, ddp_rank=1)
     g = ours_cls(raw_data_dir=tmp, index=True).get_index_dataset(lags=6, batch_size=4, shuffle=True, world_size=2, ddp_rank=1)
-    for (xa, ya), (xb, yb) in zip(w[0], g[0]):
-        assert torch.equal(xa, xb) and torch.equal(ya, yb)
+    assert [(golden.digest(xb), golden.digest(yb)) for xb, yb in g[0]] == want["ddp_rank1"]
 
 
 # ---- SURVEY 8f rank 4: dynamic-graph iterators ------------------------------------------------------------------------
@@ -184,27 +175,28 @@ def test_dynamic_signals_iteration_typing_slicing():
     assert pc[0].edge_index is pc[1].edge_index and pc[1].edge_index is not pc[2].edge_index
 
 
-@pytest.mark.skipif(not refload.available(), reason="/root/reference not present")
 def test_dynamic_signals_match_reference():
+    """Against the unmodified reference iterators on the same data (digests in tests/golden/ref_compare.pt.gz)."""
     eis, ews, xs, ys, bs, marks = _dynamic_case(seed=3)
-    pairs = [
-        (refload.load("signal.dynamic_graph_temporal_signal").DynamicGraphTemporalSignal, DynamicGraphTemporalSignal, (eis, ews, xs, ys)),
-        (refload.load("signal.dynamic_graph_static_signal").DynamicGraphStaticSignal, DynamicGraphStaticSignal, (eis, ews, xs[0], ys)),
-        (refload.load("signal.dynamic_graph_temporal_signal_batch").DynamicGraphTemporalSignalBatch, DynamicGraphTemporalSignalBatch, (eis, ews, xs, ys, bs)),
-        (refload.load("signal.dynamic_graph_static_signal_batch").DynamicGraphStaticSignalBatch, DynamicGraphStaticSignalBatch, (eis, ews, xs[0], ys, bs)),
-        (refload.load("signal.static_graph_temporal_signal_batch").StaticGraphTemporalSignalBatch, StaticGraphTemporalSignalBatch, (eis[0], ews[0], xs, ys, bs[0])),
-    ]
-    for ref_cls, our_cls, args in pairs:
-        want, got = ref_cls(*args, marks=marks), our_cls(*args, marks=marks)
-        assert want.snapshot_count == got.snapshot_count
-        for a, b in zip(want, got):
+    ours = {
+        "DynamicGraphTemporalSignal": (DynamicGraphTemporalSignal, (eis, ews, xs, ys)),
+        "DynamicGraphStaticSignal": (DynamicGraphStaticSignal, (eis, ews, xs[0], ys)),
+        "DynamicGraphTemporalSignalBatch": (DynamicGraphTemporalSignalBatch, (eis, ews, xs, ys, bs)),
+        "DynamicGraphStaticSignalBatch": (DynamicGraphStaticSignalBatch, (eis, ews, xs[0], ys, bs)),
+        "StaticGraphTemporalSignalBatch": (StaticGraphTemporalSignalBatch, (eis[0], ews[0], xs, ys, bs[0])),
+    }
+    ref = golden.load()["dynamic"]
+    for name, (our_cls, args) in ours.items():
+        want, got = ref[name], our_cls(*args, marks=marks)
+        assert want["count"] == got.snapshot_count
+        for a, b in zip(want["snapshots"], got):
             for key in ("x", "edge_index", "edge_attr", "y", "marks"):
-                ta, tb = getattr(a, key), getattr(b, key)
-                assert ta.dtype == tb.dtype and torch.equal(ta, tb)
-            if hasattr(a, "batch") and a.batch is not None:
-                assert torch.equal(a.batch, b.batch)
-        wa, ga = want[1:4], got[1:4]
-        assert wa.snapshot_count == ga.snapshot_count and torch.equal(wa[0].x, ga[0].x) and torch.equal(wa[2].edge_index, ga[2].edge_index)
+                assert a[key] == golden.digest(getattr(b, key))          # dtype, shape and bytes
+            if a["batch"] is not None:
+                assert a["batch"] == golden.digest(b.batch)
+        ga = got[1:4]
+        assert want["slice_count"] == ga.snapshot_count and want["slice_x0"] == golden.digest(ga[0].x)
+        assert want["slice_ei2"] == golden.digest(ga[2].edge_index)
 
 
 # ---- host-side algebra of the hand-written DCRNN backward ---------------------------------------------------------------

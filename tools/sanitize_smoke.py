@@ -1,5 +1,5 @@
-"""One small invocation of every hand-synchronised kernel (mbarriers, TMEM alloc, proxy fences, last-arriver MMA issue, TMA bulk copies)
-for compute-sanitizer:   tools/sanitize.sh   runs this under --tool memcheck and --tool racecheck and keeps the logs in profiles/."""
+"""One small invocation of every hand-synchronised kernel (mbarriers, wgmma, proxy fences, TMA bulk copies, cluster pairs)
+for compute-sanitizer:   tools/sanitize.sh   runs this under --tool memcheck and --tool racecheck."""
 import os
 import sys
 
@@ -18,7 +18,7 @@ ei_t, ew_t = torch.from_numpy(ei).to(dev), torch.from_numpy(ew).to(dev)
 X = torch.from_numpy(series[:36]).reshape(3, 12, 207, 2).to(dev)
 m = BatchedDCRNN(2, 32, 2).to(dev)
 with torch.no_grad():
-    m(X, ei_t, ew_t)                                             # k_dcrnn_seq_tc (tcgen05, TMA images, MMA groups)
+    m(X, ei_t, ew_t)                                             # k_dcrnn_seq_tc (wgmma, TMA images, MMA groups)
 m(X[:2], ei_t, ew_t).square().mean().backward()                  # + stash; CTA-pair (cluster) forward and backward, k_dcrnn_bwd_basis, k_dcrnn_wgrad_tc
 for opt in ("dcrnn_fwd_split", "dcrnn_bwd_split", "dcrnn_wgrad_tc"):
     _lib.set_option(opt, 0)
