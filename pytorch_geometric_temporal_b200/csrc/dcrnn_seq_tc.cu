@@ -15,13 +15,14 @@
 //   U  fp32 [208][36] = H (or H*R) + 16 B of row padding: the gather source of the diffusion (tensor cores only see the fp16 split); row 207 = 0
 //   graph image (graph_image.cuh: balanced warp-task lists, 8-bit source rows four per word, values four per 128 bits),
 //   biases, one mbarrier (prologue TMA).
-// 16 warps = 4 warpgroups; warpgroup = (128-row MMA tile, channel slice).  A warpgroup issues the wgmmas of its tile and slice (two
-// m64 subtiles; z and r of GEMM 1, the candidate of GEMM 2, m64nCW each) and keeps the accumulators in registers, so every thread
-// applies the gates to the (row, channel) pairs its accumulator fragment holds: rows 64 s + 16 w + l/4 (+8) of its tile, channels
-// 8 j + 2 (l % 4) (+1) of its slice.  It keeps H of those pairs in registers and writes H*R / H_t back as fp32 (U), as fp16 hi/lo
-// (A panel) and to HBM.
-// ptxas serializes the wgmmas of this kernel (the issue points sit under warpgroup-uniform branches it cannot prove uniform), so the
-// MMAs of a tile do not overlap the gather of the next; every warpgroup waits for its own MMAs before its epilogue.
+// 16 warps = 4 warpgroups; warpgroup wg = one 64-row MMA subtile, rows [64 wg, 64 wg + 64) (warpgroups 0-1 form row tile 0, 2-3 tile 1).
+// Per k-step and pass it issues one m64n64k16 for GEMM 1 (B rows 0..63 = z | r) and one m64n32k16 for GEMM 2 (the candidate), so the
+// A rows of a subtile are read once per MMA k-step, and keeps the accumulators in registers: every thread applies the gates to the
+// (row, channel) pairs its fragment holds -- rows 64 wg + 16 w + l/4 (+8), channels 8 jj + 2 (l % 4) (+1), jj = 0..3 -- with z, r
+// and the candidate of a pair in the same thread.  It keeps H of those pairs in registers and writes H*R / H_t back as fp32 (U), as
+// fp16 hi/lo (A panel) and to HBM.
+// The wgmmas are issued on paths ptxas can prove warpgroup-uniform (no run-time row guards; the role comes from a warp broadcast), so
+// they run asynchronously: the H | X group under the gather of tile 0, tile 0's P groups under the gather of tile 1.
 #include <cuda_fp16.h>
 
 #include <cstdlib>
@@ -41,14 +42,14 @@
 #define STMP_TC_UNROLL(n) STMP_TC_PRAGMA(unroll n)
 
 namespace stmp {
-int g_fwd_split = 1;      // 1: a CTA pair per window for small batches (stmp_set_option("dcrnn_fwd_split")): 64 windows 160.8 -> 132.2 us
+int g_fwd_split = 1;      // 1: a CTA pair per window for small batches (stmp_set_option("dcrnn_fwd_split")): 64 windows 200 -> 171 us (H100 SXM, 700 W)
 namespace {
 
 constexpr int kMaxSmemTc = 232448;
 constexpr int TC_UP = 36;                  // U row pitch (floats): a 128-byte row of H (or of T*Cin X values in the window prologue) + 16 B, so that the
                                            // epilogue's row-strided 16-byte stores rotate through the banks (pitch 32: 8-way conflicts, measured -14 %)
 constexpr int TC_UROWS = 208;              // rows of U; row 207 is the all-zero row that pad entries of the graph image point at
-constexpr int TC_AROWS = 208;              // rows stored per A panel (tile 1 over-reads into the next buffer: harmless)
+constexpr int TC_AROWS = 208;              // rows stored per A panel (subtile 3 over-reads into the next buffer: harmless)
 constexpr int TC_PANEL_A = TC_AROWS * 128;
 constexpr int TC_PANEL_B = 96 * 128;
 
@@ -189,29 +190,29 @@ __device__ __forceinline__ float4 gather_groups(const float* __restrict__ Uj, co
 }
 
 // Step anatomy (all 16 warps = 4 warpgroups; T_k = MMA row tile k = rows [128k, 128k+128)):
-//   round 1  every warpgroup issues the H | X k-steps of GEMM1 for its tile; all warps gather [P_o H | P_i H] of T_0's rows -> A panels
-//            barrier; T_0's warpgroups issue their P_o / P_i k-steps, then gather T_1's rows
+//   round 1  every warpgroup issues the H | X k-steps of GEMM1 for its subtile; all warps gather [P_o H | P_i H] of T_0's rows -> A panels
+//            barrier; T_0's warpgroups issue their P_o / P_i k-steps, then (with their MMAs in flight) gather T_1's rows
 //            barrier; T_1's warpgroups issue their k-steps
 //   epi 1    wait GEMM1 (own MMAs): R, H*R; barrier (every MMA has read the A panels); H*R -> U, A panel                      barrier
 //   round 2  same gathers over H*R, GEMM2 (candidate)
 //   epi 2    wait GEMM2: Z (from the GEMM1 accumulators, still in registers), H~, H_t; barrier; H_t -> U, A panel, HBM;
 //            X_{t+1} k-step                                                                                                  barrier
-// A warpgroup issues the wgmmas of its own (tile, channel slice): the accumulator fragments then sit in the threads that apply the
-// gates, so the epilogue is register-local.  Thread (warp w of the group, lane l) owns rows 64 s + 16 w + l/4 (+8), s = 0, 1, of its tile
-// and channels ch0 + 8 j + 2 (l % 4) (+1) of its slice.
+// A warpgroup issues the wgmmas of its own subtile: the accumulator fragments then sit in the threads that apply the gates, so the
+// epilogue is register-local.  Thread (warp w of the group, lane l) owns rows row0 + 16 w + l/4 (+8) and channels ch0 + 8 jj + 2 (l % 4)
+// (+1), jj < NJ.
 // The task lists of the gather are balanced over the warps when the plan is built (graph_image.cuh), which is what makes the extra
 // barriers cheap (round 1 profile: 25 % of all warp time was barrier wait behind the warp that always drew the longest rows).
 // X is never gathered per step: P_o X_t, P_i X_t of ALL steps of a window are produced by one gather pass over rows of
 // T*Cin floats in the window prologue and parked in the window's own (not yet written) output rows out[b, t, :, 0:8].
 // SPLIT = 2 (small batches: 2 B CTAs still fit the machine, N > 128): a window is served by a 2-CTA thread-block cluster.  CTA c owns MMA
-// row tile c -- its gather tasks, its MMAs, its epilogue (warpgroup = channel quarter) -- and pushes the rows of H*R / H_t it
+// row tile c -- its gather tasks, its MMAs, its epilogue (warpgroup = subtile x channel half: m64n16 per gate) -- and pushes the rows of H*R / H_t it
 // produces into the partner's gather buffer U through distributed shared memory, so both gathers stay local.  Per round: "done reading U"
 // is a relaxed cluster arrival right after the gather, waited for just before the epilogue overwrites U; the barrier that closes an epilogue is
 // a release / acquire cluster barrier (the pushed rows are visible).
 template <int CIN, int SPLIT>
 __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
-  constexpr int CW = SPLIT == 2 ? 8 : 16;   // channels per warpgroup (two / four warpgroups share a tile)
-  constexpr int NP = CW / 8;                // channel pairs of a thread per row
+  constexpr int NJ = SPLIT == 2 ? 2 : 4;    // 8-channel groups of a warpgroup (all 32 channels / a half)
+  constexpr int NE = 2;                     // rows of a thread's accumulator fragment
   extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int N = p.N, T = p.T;
@@ -275,17 +276,18 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
   fence_proxy_async();
   __syncthreads();
 
-  // warpgroup wg = (channel slice, tile): SPLIT 1: wg = half * 2 + tile; cluster pair: wg = channel quarter, tile = my rank
-  const int wg = warp >> 2, wt = tid & 127;
-  const int half = SPLIT == 2 ? wg : (wg >> 1), tile = SPLIT == 2 ? crank : (wg & 1);
-  const int ch0 = CW * half;
-  const int fr = tile * 128 + 16 * (wt >> 5) + ((wt & 31) >> 2);   // my first row; the others are +8, +64, +72
-  const int fc = 2 * (wt & 3);                                      // my first channel inside the slice; the others are +1, +8, +9
-  auto frow = [&](int e) { return fr + 64 * (e >> 1) + 8 * (e & 1); };   // e = 2 s + (second row of the fragment)
+  // Warpgroup wg owns one 64-row subtile (rows [64 sub, 64 sub + 64)) and 8 NJ channels of it.  SPLIT 1: sub = wg, all channels (tile
+  // wg / 2); cluster pair: sub = 2 rank + wg % 2, channel half wg / 2.  wg is broadcast from lane 0 so that the compiler knows it is
+  // warp-uniform: the wgmma issue branches on it, and a branch it cannot prove uniform makes ptxas serialize every wgmma of the kernel.
+  const int wg = __shfl_sync(~0u, tid >> 7, 0), wt = tid & 127;
+  const int tile = SPLIT == 2 ? crank : (wg >> 1);
+  const int ch0 = SPLIT == 2 ? 16 * (wg >> 1) : 0;                  // my first channel
+  const int row0 = 64 * (SPLIT == 2 ? 2 * crank + (wg & 1) : wg);   // first row of my subtile
+  const int fr = row0 + 16 * (wt >> 5) + ((wt & 31) >> 2);          // my first row; the other is +8
+  const int fc = 2 * (wt & 3);                                      // my first channel offset; the others are +1 and +8 jj, +8 jj + 1
+  auto frow = [&](int e) { return fr + 8 * e; };                    // e = row of the fragment
   const uint32_t a_hi_s = smem_u32(a_hi), a_lo_s = smem_u32(a_lo), b_hi_s = smem_u32(b_hi), b_lo_s = smem_u32(b_lo);
   const bool two_tiles = N > 128;
-  const bool has_rows = tile * 128 < N;
-  const bool sub1 = tile * 128 + 64 < N;    // the second 64-row subtile of my tile has rows
   const int j = lane & 7, quarter = lane >> 3;
   const float* Uj = U + 4 * j;
   // the thread that feeds row `xrow`'s X k-step (one row per thread; the cluster pair feeds the rows of its own tile)
@@ -312,18 +314,23 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
     if constexpr (SPLIT == 2) cluster_sync_all(); else __syncthreads();
   };
 
-  float accz[2][CW / 2], accr[2][CW / 2], acch[2][CW / 2];   // m64 x CW accumulators of my two subtiles: z, r (GEMM 1), candidate (GEMM 2)
+  // Accumulators of my subtile.  GEMM 1: z in fragment columns [0, 8 NJ), r in [8 NJ, 16 NJ); GEMM 2: the candidate.  SPLIT 1 issues a
+  // k-step as one m64n64 (B rows 0..63 = z | r) and one m64n32 (rows 64..95), the cluster pair as one m64n16 per gate.
+  // Thread (warp w of the group, lane l) holds for fragment row e (row frow(e)) and channel ch0 + 8 jj + fc + x:
+  //   z = acc1[4 jj + 2 e + x],  r = acc1[4 NJ + 4 jj + 2 e + x],  candidate = acc2[4 jj + 2 e + x]
+  float acc1[8 * NJ], acc2[4 * NJ];
   // The 3 x 7 k-steps of one gemm are issued in three commit groups, each as soon as its k-steps are in shared memory:
   //   group 0: k-steps of H | H*R and X  -- complete when the round starts; its first MMA overwrites the accumulator
   //   group 1: k-steps of P_o H          -- after the last warp finished the tile's P_o tasks
   //   group 2: k-steps of P_i H          -- after the last warp finished the tile's P_i tasks
-  // (each group is one wgmma commit group; ptxas serializes them, see the file header).
+  // No MMA is skipped at run time (a wgmma under a branch ptxas cannot prove uniform is serialized): rows past N are issued too.  Their
+  // operands are finite -- zeroed, or over-read from the buffer behind the panel -- and their results are never stored.
   auto issue_group = [&](int gm, int grp) {
     const int ks0 = grp == 0 ? 0 : (grp == 1 ? 2 : 4);
     wgmma_fence();
 #pragma unroll
     for (int pass = 0; pass < 3; ++pass) {           // lo*hi, hi*lo, hi*hi (small terms first)
-      const uint32_t ab = (pass == 0 ? a_lo_s : a_hi_s) + tile * (128 * 128);
+      const uint32_t ab = (pass == 0 ? a_lo_s : a_hi_s) + row0 * 128;
       const uint32_t bb = pass == 1 ? b_lo_s : b_hi_s;
 #pragma unroll
       for (int i = 0; i < 3; ++i) {
@@ -332,27 +339,22 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
         const int panel = ks >> 2, kin = (ks & 3) * 16;
         const uint32_t sc = (grp == 0 && pass == 0 && i == 0) ? 0u : 1u;
         const uint32_t bk = bb + panel * TC_PANEL_B + kin * 2;
-#pragma unroll
-        for (int s = 0; s < 2; ++s) {
-          if (s == 1 && !sub1) continue;
-          const uint64_t da = gmma_desc_sw128(ab + s * (64 * 128) + panel * TC_PANEL_A + kin * 2);
-          if (gm == 0) {
-            wgmma_f16<CW>(accz[s], da, gmma_desc_sw128(bk + ch0 * 128), sc);
-            wgmma_f16<CW>(accr[s], da, gmma_desc_sw128(bk + (32 + ch0) * 128), sc);
-          } else {
-            wgmma_f16<CW>(acch[s], da, gmma_desc_sw128(bk + (64 + ch0) * 128), sc);
-          }
+        const uint64_t da = gmma_desc_sw128(ab + panel * TC_PANEL_A + kin * 2);
+        if (gm == 1) {
+          wgmma_f16<8 * NJ>(acc2, da, gmma_desc_sw128(bk + (64 + ch0) * 128), sc);
+        } else if constexpr (NJ == 4) {
+          wgmma_f16<64>(acc1, da, gmma_desc_sw128(bk), sc);
+        } else {
+          wgmma_f16<16>(*reinterpret_cast<float(*)[8]>(&acc1[0]), da, gmma_desc_sw128(bk + ch0 * 128), sc);
+          wgmma_f16<16>(*reinterpret_cast<float(*)[8]>(&acc1[8]), da, gmma_desc_sw128(bk + (32 + ch0) * 128), sc);
         }
       }
     }
     wgmma_commit();
   };
   auto wait_gemm = [&](int gm) {
-    if (has_rows) wgmma_wait<0>();
-#pragma unroll
-    for (int s = 0; s < 2; ++s) {
-      if (gm == 0) { acc_fence(accz[s]); acc_fence(accr[s]); } else { acc_fence(acch[s]); }
-    }
+    wgmma_wait<0>();
+    if (gm == 0) acc_fence(acc1); else acc_fence(acc2);
   };
 
   // this warp's warp-tasks of segment `seg` = (MMA tile of the destination rows) * 2 + operator: results -> A panels as fp16 hi/lo
@@ -407,7 +409,7 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
       issue_group(gm, 2);
       return;
     }
-    if (has_rows) issue_group(gm, 0);
+    issue_group(gm, 0);
     if (p.n_ops > 0) gather_segment(0);
     if (p.n_ops > 1) gather_segment(1);
     fence_proxy_async();        // my generic-proxy stores to the A panels -> visible to the tensor core (async proxy)
@@ -422,12 +424,13 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
     }
     fence_proxy_async();
     __syncthreads();
-    if (tile == 1 && two_tiles) {
+    if (tile == 1) {
       issue_group(gm, 1);
       issue_group(gm, 2);
     }
   };
-  // every MMA of the CTA has read the A panels (each is issued by the warpgroup of its channel slice): only then are they overwritten
+  // every MMA of the CTA has read the A panels (each is issued by the warpgroup of its subtile / channel quarter): only then are they
+  // overwritten
   auto operands_free = [&]() {
     __syncthreads();
     if constexpr (SPLIT == 2) cluster_wait();       // the partner is done gathering from its U
@@ -542,16 +545,16 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
       }
     }
     // ---- window prologue B: H_0 into U (fp32) and the A panels (fp16 hi/lo); the X k-step of step 0 ---------------------------
-    float hreg[4][2 * NP];      // [fragment row e][channel 8 jj + fc + x at 2 jj + x]
+    float hreg[NE][2 * NJ];     // [fragment row e][channel ch0 + 8 jj + fc + x at 2 jj + x]
     if constexpr (SPLIT == 2) {   // the partner has finished the X gather of its prologue: its U may be overwritten
       cluster_arrive_relaxed();
       cluster_wait();
     }
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
+    for (int e = 0; e < NE; ++e) {
       const int row = frow(e);
 #pragma unroll
-      for (int jj = 0; jj < NP; ++jj) {
+      for (int jj = 0; jj < NJ; ++jj) {
         const int c = ch0 + 8 * jj + fc;
         float2 h = make_float2(0.f, 0.f);
         if (row < N && p.h0) h = __ldg(reinterpret_cast<const float2*>(p.h0 + b * p.h0_bstride + row * 32 + c));
@@ -576,24 +579,24 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
       wait_gemm(0);
       const long long obase = (b * T + t) * (long long)N;
       {
-        float hr[4][2 * NP], rv[4][2 * NP];
+        float hr[NE][2 * NJ], rv[NE][2 * NJ];
 #pragma unroll
-        for (int e = 0; e < 4; ++e)
+        for (int e = 0; e < NE; ++e)
 #pragma unroll
-          for (int jj = 0; jj < NP; ++jj)
+          for (int jj = 0; jj < NJ; ++jj)
 #pragma unroll
             for (int x = 0; x < 2; ++x) {
-              const float r = sigmoid_fast(accr[e >> 1][4 * jj + 2 * (e & 1) + x] + Bs[32 + ch0 + 8 * jj + fc + x]);
+              const float r = sigmoid_fast(acc1[4 * NJ + 4 * jj + 2 * e + x] + Bs[32 + ch0 + 8 * jj + fc + x]);
               hr[e][2 * jj + x] = hreg[e][2 * jj + x] * r;
               rv[e][2 * jj + x] = r;
             }
         operands_free();
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
+        for (int e = 0; e < NE; ++e) {
           const int row = frow(e);
           if (row < N) {
 #pragma unroll
-            for (int jj = 0; jj < NP; ++jj) {
+            for (int jj = 0; jj < NJ; ++jj) {
               const int c = ch0 + 8 * jj + fc;
               put_u(row * TC_UP + c, make_float2(hr[e][2 * jj], hr[e][2 * jj + 1]));
               store_split2(row, c, hr[e][2 * jj], hr[e][2 * jj + 1]);
@@ -613,28 +616,28 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
       wait_gemm(1);
       {
         // Z comes from its GEMM-1 accumulators, which stay in registers until the next step's GEMM 1
-        float ht[4][2 * NP], zreg[4][2 * NP];
+        float ht[NE][2 * NJ], zreg[NE][2 * NJ];
 #pragma unroll
-        for (int e = 0; e < 4; ++e)
+        for (int e = 0; e < NE; ++e)
 #pragma unroll
-          for (int jj = 0; jj < NP; ++jj)
+          for (int jj = 0; jj < NJ; ++jj)
 #pragma unroll
             for (int x = 0; x < 2; ++x) {
-              const int c = ch0 + 8 * jj + fc + x, a = 4 * jj + 2 * (e & 1) + x;
-              const float z = sigmoid_fast(accz[e >> 1][a] + Bs[c]);
-              const float h = tanh_fast(acch[e >> 1][a] + Bs[64 + c]);
+              const int c = ch0 + 8 * jj + fc + x, a = 4 * jj + 2 * e + x;
+              const float z = sigmoid_fast(acc1[a] + Bs[c]);
+              const float h = tanh_fast(acc2[a] + Bs[64 + c]);
               zreg[e][2 * jj + x] = z;
               ht[e][2 * jj + x] = h;
               hreg[e][2 * jj + x] = z * hreg[e][2 * jj + x] + (1.0f - z) * h;   // dcrnn.py:190-192
             }
         operands_free();
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
+        for (int e = 0; e < NE; ++e) {
           const int row = frow(e);
           if (row < N) {
             float* op = p.out + (obase + row) * 32;
 #pragma unroll
-            for (int jj = 0; jj < NP; ++jj) {
+            for (int jj = 0; jj < NJ; ++jj) {
               const int c = ch0 + 8 * jj + fc;
               const float2 hv = make_float2(hreg[e][2 * jj], hreg[e][2 * jj + 1]);
               put_u(row * TC_UP + c, hv);

@@ -36,13 +36,6 @@ __device__ __forceinline__ void acc_fence(float (&d)[R]) {
 }
 
 // D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 operands (K-major in shared memory), fp32 accumulator; scale_d == 0 overwrites D
-__device__ __forceinline__ void wgmma_f16_n8(float (&d)[4], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
 __device__ __forceinline__ void wgmma_f16_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
@@ -59,10 +52,21 @@ __device__ __forceinline__ void wgmma_f16_n32(float (&d)[16], uint64_t da, uint6
         "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
       : "l"(da), "l"(db), "r"(scale_d));
 }
+__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
 template <int N> __device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
-template <> __device__ __forceinline__ void wgmma_f16<8>(float (&d)[4], uint64_t da, uint64_t db, uint32_t s) { wgmma_f16_n8(d, da, db, s); }
 template <> __device__ __forceinline__ void wgmma_f16<16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t s) { wgmma_f16_n16(d, da, db, s); }
 template <> __device__ __forceinline__ void wgmma_f16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t s) { wgmma_f16_n32(d, da, db, s); }
+template <> __device__ __forceinline__ void wgmma_f16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t s) { wgmma_f16_n64(d, da, db, s); }
 
 // D[64 x 32] += A[64 x 8] * B[32 x 8]^T, TF32 operands (K-major), fp32 accumulator
 __device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], uint64_t da, uint64_t db) {
