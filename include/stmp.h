@@ -345,11 +345,11 @@ int stmp_gemm_blocks_image(const void* packed, int64_t N, int64_t nblk, void* im
 int stmp_window_gather(const float* series, int64_t t_total, int64_t row_elems, const int64_t* start,
                        int64_t B, int64_t horizon, float* x, float* y, void* stream);
 
-/* Run-time switches for tests: "dcrnn_tc" = 1 (wgmma kernel, default) / 0 (FFMA kernel) behind stmp_dcrnn_seq_fwd; "spmm_variant" = 0
- * (register gather, default) / 1, 2 (TMA-staged rows, 8 / 16 per warp); "dcrnn_bwd_all_cin" = 1 (default) / 0 (persistent backward only for cin == 2); "dcrnn_bwd_split" = 1 (default: a 2-CTA cluster per window
- * when 2 B <= SM count) / 0 (one CTA per window); "dcrnn_fwd_split" = 1 (default: the fused forward also runs on a 2-CTA cluster per window when 2 B <= SM count and N > 128) / 0;
- * "dcrnn_wgrad_tc" = 1 (default, wgmma) / 0 (FFMA); "spmm_rows_per_group" (default 8) and
- * "spmm_block" (256 / 1024): the SpMM's row blocking. */
+/* Run-time switches for tests, each selecting an implementation or launch shape that a test compares the default against:
+ * "dcrnn_tc" = 1 (wgmma kernel, default) / 0 (FFMA kernel) behind stmp_dcrnn_seq_fwd; "dcrnn_fwd_split" = 1 (default: the fused
+ * forward runs on a 2-CTA cluster per window when 2 B <= SM count and N > 128) / 0 (one CTA per window); "dcrnn_bwd_split" = 1
+ * (default: a 2-CTA cluster per window when 2 B <= SM count) / 0 (one CTA per window); "dcrnn_wgrad_tc" = 1 (default, wgmma) /
+ * 0 (FFMA).  Any other name returns STMP_EINVAL. */
 int stmp_set_option(const char* name, int value);
 
 /* ---- misc ---------------------------------------------------------------------------------------- */

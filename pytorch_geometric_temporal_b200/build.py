@@ -28,11 +28,8 @@ def needs_build():
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build(force=False, verbose=False, extra_flags=(), out=None):
-    """`extra_flags` / `out`: build a VARIANT of the library (e.g. -DSTMP_X=1 into lib/libstmp_x.so) next to the product one, to A/B it on
-    one GPU box through the STMP_LIB environment variable (tests/perf only; the product build takes neither)."""
-    if out is not None:
-        return _build_variant(list(extra_flags), out)
+def build(force=False, verbose=False):
+    """To A/B two versions of the library, build each in its own checkout and point STMP_LIB (_lib.py) at one of them."""
     if not force and not needs_build():
         return LIB
     os.makedirs(os.path.dirname(LIB), exist_ok=True)
@@ -57,23 +54,6 @@ def build(force=False, verbose=False, extra_flags=(), out=None):
     if verbose:
         print("\n".join(log))
     return LIB
-
-
-def _build_variant(flags, out):
-    objdir = os.path.join(HERE, "lib", "variant_" + os.path.basename(out).replace(".so", ""))
-    os.makedirs(objdir, exist_ok=True)
-    procs, objs = [], []
-    for s in SOURCES:
-        o = os.path.join(objdir, s.replace(".cu", ".o"))
-        cmd = [_nvcc(), *[f for f in NVCC_FLAGS if f not in ("-Xptxas", "-v")], *flags, "-c", os.path.join(CSRC, s), "-o", o]
-        procs.append((s, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
-        objs.append(o)
-    for s, p in procs:
-        o, _ = p.communicate()
-        if p.returncode != 0:
-            raise RuntimeError(f"nvcc failed on {s}:\n{o}")
-    subprocess.check_call([_nvcc(), "-shared", "-o", out, *objs, "-gencode", "arch=compute_90a,code=sm_90a"])
-    return out
 
 
 if __name__ == "__main__":

@@ -19,6 +19,13 @@ inline void count_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_
 int path_slot(const char* name);
 void count_path(int slot);
 
+// ---- run-time switches (stmp_set_option, plan.cu) ----------------------------------------------------
+// Each selects an independent implementation or a launch shape that a test compares the default against.
+extern int g_dcrnn_tc;     // "dcrnn_tc": 1 wgmma forward (dcrnn_seq_tc.cu) / 0 exact-fp32 FFMA forward (dcrnn_seq.cu)
+extern int g_fwd_split;    // "dcrnn_fwd_split": 1 a CTA pair per window for small batches / 0 one CTA per window (wgmma forward)
+extern int g_bwd_split;    // "dcrnn_bwd_split": the same choice for the persistent backward (dcrnn_bwd.cu)
+extern int g_wgrad_tc;     // "dcrnn_wgrad_tc": 1 wgmma weight-gradient contraction (wgrad_tc.cu) / 0 FFMA (train.cu)
+
 #define STMP_CUDA_OK(expr)                                                                    \
   do {                                                                                        \
     cudaError_t _e = (expr);                                                                  \

@@ -19,8 +19,6 @@
 #include "dcrnn_common.cuh"
 
 namespace stmp {
-int g_bwd_all_cin = 1;
-int g_bwd_split = 1;      // 1: a CTA pair per window when 2 B CTAs fit the machine; 0: always one CTA per window
 namespace {
 
 constexpr int kCo = 32;          // hidden size served by these kernels
@@ -434,9 +432,7 @@ inline bool bwd_supported(const stmp_plan* plan, long long cin, long long cout, 
   if (!plan || plan->flavor != STMP_FLAVOR_DCONV || plan->n_ops != 2) return false;
   if (K != 2 || cout != kCo || cin < 1 || cin > 4) return false;
   // cin == 2 (float2 slots, 104 columns) is the benchmark configuration; cin 1, 3, 4 (scalar slots / 112 columns) are served too
-  // (tests/test_gpu_dcrnn.py::test_training_persistent_backward_other_channel_counts); stmp_set_option("dcrnn_bwd_all_cin", 0)
-  // restricts the persistent kernel to cin == 2 again.
-  if (cin != 2 && !g_bwd_all_cin) return false;
+  // (tests/test_gpu_dcrnn.py::test_training_persistent_backward_other_channel_counts).
   return ((plan->n + 7) / 8) * (ncol_of((int)cin) / 8) <= kBwdThreads && seq_smem_base(plan->n, (int)cin) <= 227 * 1024 &&
          2 * sizeof(float) * (size_t)plan->n * (cin + kCo) <= 100 * 1024;
 }

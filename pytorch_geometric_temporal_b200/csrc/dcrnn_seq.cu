@@ -18,21 +18,11 @@
 //    channels 4w..4w+3 of every gate, lane l owns rows l, l+32, ...; A rows are read as float4 along K
 //    with LD/4 odd => conflict-free LDS.128; B is a warp-uniform broadcast.  The gate epilogue
 //    (sigmoid/tanh/Hadamard/convex combine) runs on the accumulators in registers.
-#include <cstdlib>
-#include <cstring>
-
 #include "common.cuh"
 #include "dcrnn_common.cuh"
 
 namespace stmp {
 // wgmma variant (dcrnn_seq_tc.cu)
-extern int g_spmm_variant;
-extern int g_spmm_rows_per_group;
-extern int g_spmm_block;
-extern int g_wgrad_tc;
-extern int g_fwd_split;
-extern int g_bwd_all_cin;
-extern int g_bwd_split;
 bool dcrnn_tc_supported(const stmp_plan* plan, long long cin, long long cout, long long K);
 int dcrnn_tc_launch(const stmp_plan* plan, long long B, long long T, long long cin, const float* x, const long long* win_start,
                     long long x_bstride, long long x_tstride, const float* w_z, const float* w_r, const float* w_h, const float* b_z,
@@ -47,8 +37,6 @@ int gru_tc_launch(const stmp_plan* plan, int n_ops, long long B, long long T, lo
                   long long x_bstride, long long x_tstride, const float* wcat, const float* bcat, const float* h0, long long h0_bstride,
                   float* out, float* stash, const void* wimage, void* workspace, cudaStream_t st);
 long long tc_workspace_bytes(const stmp_plan* plan, long long T, long long cin);
-
-int g_use_tc = -1;   // -1: read STMP_DCRNN_TC on first use
 
 namespace {
 
@@ -397,10 +385,9 @@ int launch(const Layout& L, int grid, cudaStream_t st) {
 
 // rows covered = NW * (128/OUT) * RT
 template <int OUT>
-int launch_rt(const Layout& L, int grid, cudaStream_t st, int variant) {
+int launch_rt(const Layout& L, int grid, cudaStream_t st) {
   constexpr int RQ = 128 / OUT;
   const int n = L.p.N;
-  if (variant == 1 && n <= 16 * RQ * 4) return launch<OUT, 4, 16>(L, grid, st);  // 16 warps x 4 row tiles
   if (n <= 8 * RQ * 1) return launch<OUT, 1, 8>(L, grid, st);
   if (n <= 8 * RQ * 2) return launch<OUT, 2, 8>(L, grid, st);
   if (n <= 8 * RQ * 4) return launch<OUT, 4, 8>(L, grid, st);
@@ -424,7 +411,7 @@ using namespace stmp;
 
 extern "C" int stmp_dcrnn_seq_supported(const stmp_plan* plan, int64_t cin, int64_t cout, int64_t K) {
   if (!shape_ok(plan, cin, cout, K)) return 0;
-  if (g_use_tc != 0 && dcrnn_tc_supported(plan, cin, cout, K)) return 1;   // the wgmma kernel's envelope is wider in cin than the FFMA kernel's
+  if (g_dcrnn_tc && dcrnn_tc_supported(plan, cin, cout, K)) return 1;   // the wgmma kernel's envelope is wider in cin than the FFMA kernel's
   Layout L;
   return make_layout(plan, (int)cin, (int)cout, (int)K, 12, &L) ? 1 : 0;
 }
@@ -443,15 +430,10 @@ extern "C" int stmp_dcrnn_seq_fwd(const stmp_plan* plan, int64_t B, int64_t T, i
     return set_error(STMP_EUNSUPPORTED, "fused DCRNN kernel supports N<=256 (cout 32), cin<=4, cout in {16,32}, K<=4 (got N=%d cin=%lld cout=%lld K=%lld)",
                      plan->n, (long long)cin, (long long)cout, (long long)K);
   if (B == 0 || T == 0) return STMP_OK;
-  {  // tensor-core variant unless disabled (STMP_DCRNN_TC=0 / stmp_set_option) or outside its envelope
-    if (g_use_tc < 0) {
-      const char* v = getenv("STMP_DCRNN_TC");
-      g_use_tc = v ? atoi(v) : 1;
-    }
-    if (g_use_tc && dcrnn_tc_supported(plan, cin, cout, K))
-      return dcrnn_tc_launch(plan, B, T, cin, x, reinterpret_cast<const long long*>(win_start), x_bstride, x_tstride, w_z, w_r, w_h,
-                             b_z, b_r, b_h, h0, out, stash, wimage, workspace, (cudaStream_t)stream);
-  }
+  // tensor-core variant unless disabled (stmp_set_option("dcrnn_tc", 0)) or outside its envelope
+  if (g_dcrnn_tc && dcrnn_tc_supported(plan, cin, cout, K))
+    return dcrnn_tc_launch(plan, B, T, cin, x, reinterpret_cast<const long long*>(win_start), x_bstride, x_tstride, w_z, w_r, w_h,
+                           b_z, b_r, b_h, h0, out, stash, wimage, workspace, (cudaStream_t)stream);
   STMP_REQUIRE(T * (long long)plan->n * cin < (1ll << 24), STMP_ESHAPE, "window too long for the shared-memory X buffer");
   Layout L;
   if (!make_layout(plan, (int)cin, (int)cout, (int)K, (int)T, &L))
@@ -478,13 +460,8 @@ extern "C" int stmp_dcrnn_seq_fwd(const stmp_plan* plan, int64_t B, int64_t T, i
   STMP_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   int grid = (int)(B < sms ? B : sms);
   cudaStream_t st = (cudaStream_t)stream;
-  static int variant = -1;
-  if (variant < 0) {
-    const char* v = getenv("STMP_DCRNN_VARIANT");
-    variant = v ? atoi(v) : 0;
-  }
-  if (cout == 16) return launch_rt<16>(L, grid, st, variant);
-  return launch_rt<32>(L, grid, st, variant);
+  if (cout == 16) return launch_rt<16>(L, grid, st);
+  return launch_rt<32>(L, grid, st);
 }
 
 extern "C" int stmp_gru_seq_supported(const stmp_plan* plan, int n_ops, int64_t cin, int64_t cout) {
@@ -505,21 +482,6 @@ extern "C" int stmp_gru_seq_fwd(const stmp_plan* plan, int n_ops, int64_t B, int
   if (B == 0 || T == 0) return STMP_OK;
   return gru_tc_launch(plan, n_ops, B, T, cin, x, reinterpret_cast<const long long*>(win_start), x_bstride, x_tstride, wcat, bcat, h0,
                        h0_bstride, out, stash, wimage, workspace, (cudaStream_t)stream);
-}
-
-/* Test hook: select the kernel family behind stmp_dcrnn_seq_fwd at run time ("dcrnn_tc": 1 wgmma / 0 FFMA), so the two
- * independent implementations can be cross-checked against each other at full benchmark size. */
-extern "C" int stmp_set_option(const char* name, int value) {
-  STMP_REQUIRE(name != nullptr, STMP_EINVAL, "stmp_set_option: NULL name");
-  if (strcmp(name, "dcrnn_tc") == 0) { g_use_tc = value ? 1 : 0; return STMP_OK; }
-  if (strcmp(name, "spmm_variant") == 0) { g_spmm_variant = value; return STMP_OK; }
-  if (strcmp(name, "spmm_rows_per_group") == 0) { g_spmm_rows_per_group = value < 1 ? 1 : value; return STMP_OK; }
-  if (strcmp(name, "dcrnn_fwd_split") == 0) { g_fwd_split = value ? 1 : 0; return STMP_OK; }
-  if (strcmp(name, "dcrnn_wgrad_tc") == 0) { g_wgrad_tc = value ? 1 : 0; return STMP_OK; }
-  if (strcmp(name, "spmm_block") == 0) { g_spmm_block = value == 1024 ? 1024 : 256; return STMP_OK; }
-  if (strcmp(name, "dcrnn_bwd_all_cin") == 0) { g_bwd_all_cin = value ? 1 : 0; return STMP_OK; }
-  if (strcmp(name, "dcrnn_bwd_split") == 0) { g_bwd_split = value ? 1 : 0; return STMP_OK; }
-  return set_error(STMP_EINVAL, "stmp_set_option: unknown option '%s'", name);
 }
 
 extern "C" int64_t stmp_gru_weight_image_bytes(void) { return tc_weight_image_bytes(); }

@@ -32,17 +32,7 @@
 #include "graph_image.cuh"
 #include "tc_common.cuh"
 
-#ifndef STMP_TC_GUNROLL
-#define STMP_TC_GUNROLL 2
-#endif
-#ifndef STMP_TC_PREFETCH
-#define STMP_TC_PREFETCH 0
-#endif
-#define STMP_TC_PRAGMA(x) _Pragma(#x)
-#define STMP_TC_UNROLL(n) STMP_TC_PRAGMA(unroll n)
-
 namespace stmp {
-int g_fwd_split = 1;      // 1: a CTA pair per window for small batches (stmp_set_option("dcrnn_fwd_split")): 64 windows 200 -> 171 us (H100 SXM, 700 W)
 namespace {
 
 constexpr int kMaxSmemTc = 232448;
@@ -143,38 +133,20 @@ __device__ __forceinline__ float tanh_fast(float x) { return 2.0f * __fdividef(1
 // Four edges per group: one broadcast 32-bit load carries their four 8-bit source rows, one 128-bit load their values; the
 // next group's entries are fetched while the current group's four feature rows are in flight.  Summation order = CSR order
 // (the reference's scatter order), products by FMA as in the round-1 kernel.
-#if STMP_IMG_OFF16
-typedef uint2 img_idx_t;
-#else
-typedef uint32_t img_idx_t;
-#endif
-static_assert(kImgRowPitchBytes == TC_UP * 4, "graph image offsets are pre-scaled by the gather buffer's row pitch");
-static_assert(kImgZeroRow * kImgRowPitchBytes < 65536, "row offsets must fit 16 bits");
-#if STMP_IMG_OFF16
-__device__ __forceinline__ float4 ld4_off(const float* base, uint32_t byte_off) {
-  return *reinterpret_cast<const float4*>(reinterpret_cast<const unsigned char*>(base) + byte_off);
-}
-#endif
-// (u, v) = the task's first group, already loaded (gather_segment fetches it while the previous task is being gathered)
-__device__ __forceinline__ float4 gather_groups(const float* __restrict__ Uj, const img_idx_t* __restrict__ idx4,
-                                                const float4* __restrict__ val4, int g0, int ng, img_idx_t u, float4 v) {
+__device__ __forceinline__ float4 gather_groups(const float* __restrict__ Uj, const uint32_t* __restrict__ idx4,
+                                                const float4* __restrict__ val4, int g0, int ng) {
   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-  STMP_TC_UNROLL(STMP_TC_GUNROLL)    // 2: +6 % over the rolled loop (A/B on one box: 886 k -> 942 k snapshots/s) -- a task has 2-3 groups on average,
-  for (int g = 1; g <= ng; ++g) {    // the loop branch and its convergence barrier were 10 % of the issued instructions
-    const img_idx_t un = idx4[g0 + g];     // (one spare group at the end of the arrays)
+  uint32_t u = idx4[g0];
+  float4 v = val4[g0];
+#pragma unroll 2    // a task has 2-3 groups on average: the rolled loop's branch and convergence barrier were 10 % of the issued instructions
+  for (int g = 1; g <= ng; ++g) {
+    const uint32_t un = idx4[g0 + g];      // (one spare group at the end of the arrays)
     const float4 vn = val4[g0 + g];
     // (predicating the loads of pad entries off saves their wavefronts but costs more in compares / selects: measured -2 %, A/B on one box)
-#if STMP_IMG_OFF16
-    const float4 x0 = ld4_off(Uj, u.x & 0xffffu);
-    const float4 x1 = ld4_off(Uj, u.x >> 16);
-    const float4 x2 = ld4_off(Uj, u.y & 0xffffu);
-    const float4 x3 = ld4_off(Uj, u.y >> 16);
-#else
     const float4 x0 = ld4(Uj + (u & 0xffu) * TC_UP);
     const float4 x1 = ld4(Uj + ((u >> 8) & 0xffu) * TC_UP);
     const float4 x2 = ld4(Uj + ((u >> 16) & 0xffu) * TC_UP);
     const float4 x3 = ld4(Uj + (u >> 24) * TC_UP);
-#endif
     fma4(acc, v.x, x0);
     fma4(acc, v.y, x1);
     fma4(acc, v.z, x2);
@@ -183,10 +155,6 @@ __device__ __forceinline__ float4 gather_groups(const float* __restrict__ Uj, co
     v = vn;
   }
   return acc;
-}
-__device__ __forceinline__ float4 gather_groups(const float* __restrict__ Uj, const img_idx_t* __restrict__ idx4,
-                                                const float4* __restrict__ val4, int g0, int ng) {
-  return gather_groups(Uj, idx4, val4, g0, ng, idx4[g0], val4[g0]);
 }
 
 // Step anatomy (all 16 warps = 4 warpgroups; T_k = MMA row tile k = rows [128k, 128k+128)):
@@ -225,7 +193,7 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
   const uint16_t* s_wstart = reinterpret_cast<const uint16_t*>(img + p.gl.off_wstart);
   const uint16_t* s_wcount = reinterpret_cast<const uint16_t*>(img + p.gl.off_wcount);
   const uint32_t* s_wt = reinterpret_cast<const uint32_t*>(img + p.gl.off_wt);
-  const img_idx_t* s_idx = reinterpret_cast<const img_idx_t*>(img + p.gl.off_idx);
+  const uint32_t* s_idx = reinterpret_cast<const uint32_t*>(img + p.gl.off_idx);
   const float4* s_val = reinterpret_cast<const float4*>(img + p.gl.off_val);
   float* Bs = reinterpret_cast<float*>(smem + p.off_bias);
   uint64_t* tma_bar = reinterpret_cast<uint64_t*>(smem + p.off_bar);   // prologue TMA (graph and weight images)
@@ -365,25 +333,6 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
     unsigned char* dh = a_hi + (op ? TC_PANEL_A : 0);
     unsigned char* dl = a_lo + (op ? TC_PANEL_A : 0);
     const int kcol = (op ? 0 : 32) + 4 * j;
-#if STMP_TC_PREFETCH
-    // the next task's descriptor and first edge group are fetched while the current task is gathered: the chain descriptor -> group ->
-    // feature rows (three dependent shared-memory latencies per task) is taken off the critical path
-    uint32_t d = wc > 0 ? s_wt[ws * 4 + quarter] : kImgNoTask;
-    int g0 = d == kImgNoTask ? 0 : (int)(d >> 16);
-    img_idx_t u0 = s_idx[g0];
-    float4 v0 = s_val[g0];
-    for (int i = 0; i < wc; ++i) {
-      const uint32_t dn = i + 1 < wc ? s_wt[(ws + i + 1) * 4 + quarter] : kImgNoTask;
-      const int g0n = dn == kImgNoTask ? 0 : (int)(dn >> 16);
-      const img_idx_t un0 = s_idx[g0n];
-      const float4 vn0 = s_val[g0n];
-      if (d != kImgNoTask) {
-        const float4 acc = gather_groups(Uj, s_idx, s_val, g0, (int)((d >> 9) & 0x7f), u0, v0);
-        store_split4(dh, dl, (int)(d & 0xff), kcol, acc);
-      }
-      d = dn; g0 = g0n; u0 = un0; v0 = vn0;
-    }
-#else
     for (int i = 0; i < wc; ++i) {
       const uint32_t d = s_wt[(ws + i) * 4 + quarter];
       if (d != kImgNoTask) {
@@ -391,7 +340,6 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
         store_split4(dh, dl, (int)(d & 0xff), kcol, acc);
       }
     }
-#endif
   };
   // One gather round.  Every warpgroup issues the static group (H | X k-steps) of its tile right away (the block barrier in front of
   // the round ordered those operand stores), tile 0's warpgroups their P_o / P_i groups behind the barrier that closes tile 0's tasks,

@@ -9,9 +9,7 @@
 //   wstart   [16][4]  u16  first warp-task of warp w in segment s = 2 * (MMA row tile of the destination: rows <128 | >=128) + operator
 //   wcount   [16][4]  u16  number of warp-tasks of warp w in segment s
 //   wt       [n_warp_tasks][4] u32 task descriptors: row | op << 8 | n_groups << 9 | first_group << 16  (0xFFFFFFFF = none)
-//   idx4     [n_groups + 1]  four source rows of an edge group (pad entries point at the all-zero row 207): 8-bit row numbers in one u32
-//                            (shift + mask + two multiply-adds per address) -- or, built with -DSTMP_IMG_OFF16=1, 16-bit BYTE OFFSETS of the
-//                            rows in the gather buffer (one 64-bit load, one extract + one add per address; measured 0.6 % slower)
+//   idx4     [n_groups + 1]  u32: four source rows of an edge group (pad entries point at the all-zero row 207), 8-bit row numbers
 //   val4     [n_groups + 1]  float4: their four values (pad = 0)
 //
 // Edge order inside a task is the plan's CSR order (= the reference's scatter order).  Warp-tasks are dealt to warps by
@@ -28,11 +26,6 @@ constexpr int kImgWarps = 16;
 constexpr int kImgSegs = 4;
 constexpr int kImgZeroRow = 207;
 constexpr uint32_t kImgNoTask = 0xFFFFFFFFu;
-#ifndef STMP_IMG_OFF16
-#define STMP_IMG_OFF16 0     // A/B on one box (tests/perf/flagship_variants.py): 8-bit rows 942.8 k snapshots/s, 16-bit pre-scaled offsets 937.5 k
-#endif
-constexpr int kImgIdxBytes = STMP_IMG_OFF16 ? 8 : 4;     // bytes per edge group in idx4
-constexpr int kImgRowPitchBytes = 144;                  // pitch of the kernel's gather buffer (dcrnn_seq_tc.cu: TC_UP floats)
 
 struct GraphImageLayout {
   int off_wstart, off_wcount, off_wt, off_idx, off_val, bytes;
@@ -52,7 +45,7 @@ __host__ __device__ inline GraphImageLayout graph_image_layout(int n_tasks, int 
   L.off_wcount = off; off += kImgWarps * kImgSegs * 2;
   off = gi_align16(off);
   L.off_wt = off; off += gi_align16(L.cap_wt * 16);
-  L.off_idx = off; off += gi_align16(L.cap_groups * kImgIdxBytes);
+  L.off_idx = off; off += gi_align16(L.cap_groups * 4);
   L.off_val = off; off += L.cap_groups * 16;
   L.bytes = gi_align16(off);
   return L;

@@ -26,6 +26,12 @@ namespace stmp {
 // ---------------------------------------------------------------------------------------------------------
 std::atomic<long long> g_launches{0};
 
+// run-time switches (common.cuh, stmp_set_option below)
+int g_dcrnn_tc = 1;
+int g_fwd_split = 1;       // 64 windows: 200 -> 171 us (H100 SXM, 700 W)
+int g_bwd_split = 1;
+int g_wgrad_tc = 1;
+
 // ---- per-kernel launch counters (stmp_path_counters) ----------------------------------------------------
 constexpr int kMaxPaths = 96;
 static const char* g_path_names[kMaxPaths];
@@ -583,16 +589,10 @@ int build_gcn(Builder& b, stmp_plan* p, int n, int e, const int* row, const int*
   return 0;
 }
 
-// cost model of the static longest-first deal (tunable at build time for A/B runs: tests/perf/flagship_variants.py)
-#ifndef STMP_LPT_HANDICAP
-#define STMP_LPT_HANDICAP 24
-#endif
-#ifndef STMP_LPT_A
-#define STMP_LPT_A 2
-#endif
-#ifndef STMP_LPT_B
-#define STMP_LPT_B 3
-#endif
+// cost model of the static longest-first deal
+constexpr int kLptHandicap = 24;
+constexpr int kLptA = 2;
+constexpr int kLptB = 3;
 
 // ---- shared-memory graph image for the fused wgmma kernel (graph_image.cuh) ---------------------------------------
 // One CTA.  Tasks (row, op) are rank-sorted per segment (destination row tile, operator) by descending group count, cut into
@@ -647,7 +647,7 @@ __global__ void __launch_bounds__(512) k_build_graph_image(const int* rp0, const
   if (tid == 0) {
     int load[kImgWarps], cntw[kImgWarps], pos[kImgWarps];
     for (int w = 0; w < kImgWarps; ++w) load[w] = 0;
-    load[0] = STMP_LPT_HANDICAP;                         // warp 0 also issues the round's MMAs (~42 x 8 issue slots)
+    load[0] = kLptHandicap;                              // warp 0 also issues the round's MMAs (~42 x 8 issue slots)
     int nwt = 0;
     int base = 0;
     for (int seg = 0; seg < kImgSegs; base += s_segcount[seg], ++seg) {
@@ -658,7 +658,7 @@ __global__ void __launch_bounds__(512) k_build_graph_image(const int* rp0, const
         for (int w = 1; w < kImgWarps; ++w)
           if (load[w] < load[best]) best = w;
         s_owner[k] = (unsigned char)best;
-        load[best] += STMP_LPT_A * s_ng[s_sorted[base + 4 * k]] + STMP_LPT_B;   // ~ issue slots: per group 6 loads + 8 FMA2, per task a split store
+        load[best] += kLptA * s_ng[s_sorted[base + 4 * k]] + kLptB;   // ~ issue slots: per group 6 loads + 8 FMA2, per task a split store
         ++cntw[best];
       }
       int run = nwt;
@@ -695,24 +695,20 @@ __global__ void __launch_bounds__(512) k_build_graph_image(const int* rp0, const
     const int2* cv = op ? cv1 : cv0;
     const int beg = rp[i], len = rp[i + 1] - beg;
     for (int g = 0; g < s_ng[task]; ++g) {
-      uint32_t u = 0, w[2] = {0u, 0u};
+      uint32_t u = 0;
       float v[4];
       for (int e = 0; e < 4; ++e) {
         const int k = 4 * g + e;
         const int2 c = k < len ? cv[beg + k] : make_int2(kImgZeroRow, 0);
         u |= ((uint32_t)c.x & 0xffu) << (8 * e);
-        w[e >> 1] |= ((uint32_t)c.x * kImgRowPitchBytes) << (16 * (e & 1));
         v[e] = __int_as_float(c.y);
       }
-      if (STMP_IMG_OFF16) reinterpret_cast<uint2*>(idx4)[s_g0[task] + g] = make_uint2(w[0], w[1]);
-      else idx4[s_g0[task] + g] = u;
+      idx4[s_g0[task] + g] = u;
       val4[s_g0[task] + g] = make_float4(v[0], v[1], v[2], v[3]);
     }
   }
   if (tid == 0) {   // the spare group the gather loop prefetches past the last task
-    const uint32_t z = (uint32_t)kImgZeroRow * kImgRowPitchBytes;
-    if (STMP_IMG_OFF16) reinterpret_cast<uint2*>(idx4)[s_g0[NT]] = make_uint2(z | (z << 16), z | (z << 16));
-    else idx4[s_g0[NT]] = kImgZeroRow * 0x01010101u;
+    idx4[s_g0[NT]] = kImgZeroRow * 0x01010101u;
     val4[s_g0[NT]] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
@@ -874,6 +870,16 @@ extern "C" int stmp_plan_export(const stmp_plan* p, int op, int transposed, int3
     STMP_LAUNCH_OK("k_export");
   }
   return STMP_OK;
+}
+
+/* Test hook: select, at run time, the implementation or launch shape a test cross-checks against the default (common.cuh). */
+extern "C" int stmp_set_option(const char* name, int value) {
+  STMP_REQUIRE(name != nullptr, STMP_EINVAL, "stmp_set_option: NULL name");
+  if (strcmp(name, "dcrnn_tc") == 0) { g_dcrnn_tc = value ? 1 : 0; return STMP_OK; }
+  if (strcmp(name, "dcrnn_fwd_split") == 0) { g_fwd_split = value ? 1 : 0; return STMP_OK; }
+  if (strcmp(name, "dcrnn_bwd_split") == 0) { g_bwd_split = value ? 1 : 0; return STMP_OK; }
+  if (strcmp(name, "dcrnn_wgrad_tc") == 0) { g_wgrad_tc = value ? 1 : 0; return STMP_OK; }
+  return set_error(STMP_EINVAL, "stmp_set_option: unknown option '%s'", name);
 }
 
 extern "C" const char* stmp_last_error(void) { return err_buf(); }

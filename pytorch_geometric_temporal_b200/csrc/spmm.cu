@@ -1,22 +1,19 @@
 // spmm.cu -- K1/K3: gather of source-node rows -> edge-weighted accumulate per destination, with the
 // Chebyshev/diffusion axpby fused into the epilogue.  One group of G lanes owns one (batch, destination) row, lanes are
 // vectorised along the feature axis (float4/float2/float), edge metadata is one 64-bit load per edge, 4 gathers in flight.
-// A CTA owns 8 x (256 / G) consecutive destination rows of one batch element.
+// A CTA of 256 threads owns 8 x (256 / G) consecutive destination rows of one batch element.
 // Bound (cfg5 probe, random 10^4-node graph): L2 throughput -- 4*nnz*F*B = 1.8 GB of gathered rows per launch on top of the 0.33 GB of
-// compulsory HBM traffic.  Variants kept selectable for A/B runs (tests/perf/spmm_variants.py, spmm_blocked.py): entries preloaded once
-// + shuffles, predicated batches without a scalar tail, TMA-staged source rows (k_spmm_tma below), 1024-thread CTAs.
+// compulsory HBM traffic.  Measured dead ends (B200): TMA-staged source rows 0.90x / 0.95x, 1024-thread CTAs 0.94x.
 // Deterministic: per destination the sum runs in the reference's scatter order with separate
 // multiply and add, which makes the result bit-identical to CPU index_select -> mul -> scatter_add_.
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace stmp {
-int g_spmm_rows_per_group = 8;   // consecutive destination rows walked by one lane group (stmp_set_option("spmm_rows_per_group")): cfg5 probe
-                                 // 1: 1451 GB/s, 4: 1810, 8: 1855, 16: 1700 on the random graph; 1533 / 1920 / 1986 / 1879 on a banded one
-int g_spmm_block = 256;          // threads per CTA (stmp_set_option("spmm_block"): 256 or 1024)
-int g_spmm_variant = -1;   // 0 (default): k_spmm register gather; 1 / 2: k_spmm_tma with 8 / 16 staged rows per warp
 namespace {
+
+constexpr int kSpmmThreads = 256;
+constexpr int kSpmmRowsPerGroup = 8;   // consecutive destination rows walked by one lane group: cfg5 probe (B200) 1: 1451 GB/s, 4: 1810,
+                                       // 8: 1855, 16: 1700 on the random graph; 1533 / 1920 / 1986 / 1879 on a banded one
 
 template <int VEC> struct VecT;
 template <> struct VecT<1> { using T = float; };
@@ -60,10 +57,10 @@ struct SpmmArgs {
 // A CTA owns `rpg` * (256 / G) CONSECUTIVE destination rows of one batch element and walks them 256 / G rows at a time: with a node
 // numbering that has locality (sensor networks numbered along the roads) the source rows of neighbouring destinations overlap and are
 // re-used out of L1 instead of crossing the L2 -> SM crossbar once per edge.
-template <int VEC, int BLOCK>
-__global__ void __launch_bounds__(BLOCK) k_spmm(SpmmArgs a, int G, int log2G, int rpg, int blocks_per_b) {
+template <int VEC>
+__global__ void __launch_bounds__(kSpmmThreads) k_spmm(SpmmArgs a, int G, int log2G, int rpg, int blocks_per_b) {
   const int lane_in_group = threadIdx.x & (G - 1);
-  const int gpc = BLOCK >> log2G;
+  const int gpc = kSpmmThreads >> log2G;
   const long long b = blockIdx.x / blocks_per_b;
   const int blk = blockIdx.x - (int)(b * blocks_per_b);
   const float* xb = a.x + b * a.bsx;
@@ -123,80 +120,6 @@ __global__ void __launch_bounds__(BLOCK) k_spmm(SpmmArgs a, int G, int log2G, in
     }
     st_vec<VEC>(a.y + b * a.bsy + (long long)i * a.ldy + f0, o);
   }
-  }
-}
-
-// ---- TMA-staged gather ---------------------------------------------------------------------------------------------------------
-// One warp per (batch, destination) row, persistent over rows.  The source rows of the destination's CSR row are fetched by TMA bulk
-// copies (cp.async.bulk global -> shared, one per edge, 4*f bytes each, completion on the warp's mbarrier) into the warp's slots in
-// shared memory, up to SLOTS rows per batch -- the loads in flight are bounded by shared memory (SLOTS x 4f bytes per warp), not by
-// the L1's outstanding-load tracking that caps the register gather (k_spmm: ~64 KB per SM in flight whatever the unroll depth:
-// tests/perf/spmm_variants.py).  Lanes then read their float4 of every staged row (conflict-free) and accumulate in CSR order with
-// separate multiply and add -- bit-identical to k_spmm.  Needs f % 4 == 0, 16-byte aligned rows, f <= 32 * 4 * JMAX, no attention.
-template <int SLOTS, int JMAX>
-__global__ void __launch_bounds__(256) k_spmm_tma(SpmmArgs a) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int rowbytes = a.f * 4;
-  float* slots = reinterpret_cast<float*>(smem_raw) + (size_t)warp * SLOTS * a.f;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw + (size_t)8 * SLOTS * rowbytes) + warp;
-  if (lane == 0) {
-    mbar_init(bar, 1);
-    fence_mbar_init();
-  }
-  __syncwarp();
-  const long long total = a.batch * (long long)a.n;
-  uint32_t parity = 0;
-  for (long long group = (long long)blockIdx.x * 8 + warp; group < total; group += (long long)gridDim.x * 8) {
-    const int i = (int)(group % a.n);
-    const long long b = group / a.n;
-    const float* xb = a.x + b * a.bsx;
-    const int beg = __ldg(a.rowptr + i), end = __ldg(a.rowptr + i + 1);
-    float acc[JMAX][4];
-#pragma unroll
-    for (int j = 0; j < JMAX; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
-    for (int c0 = beg; c0 < end; c0 += SLOTS) {
-      const int nh = min(SLOTS, end - c0);
-      const int2 mine = lane < nh ? __ldg(a.cv + c0 + lane) : make_int2(0, 0);
-      if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)(nh * rowbytes));
-      __syncwarp();
-      if (lane < nh) tma_bulk_g2s(slots + (size_t)lane * a.f, xb + (long long)mine.x * a.ldx, (uint32_t)rowbytes, bar);
-      mbar_wait(bar, parity);
-      parity ^= 1u;
-      for (int u = 0; u < nh; ++u) {
-        const float w = __int_as_float(__shfl_sync(0xffffffffu, mine.y, u));
-#pragma unroll
-        for (int j = 0; j < JMAX; ++j) {
-          const int f0 = (j * 32 + lane) * 4;
-          if (f0 < a.f) {
-            const float4 xv = *reinterpret_cast<const float4*>(slots + (size_t)u * a.f + f0);
-            acc[j][0] = __fadd_rn(acc[j][0], __fmul_rn(w, xv.x));
-            acc[j][1] = __fadd_rn(acc[j][1], __fmul_rn(w, xv.y));
-            acc[j][2] = __fadd_rn(acc[j][2], __fmul_rn(w, xv.z));
-            acc[j][3] = __fadd_rn(acc[j][3], __fmul_rn(w, xv.w));
-          }
-        }
-      }
-      __syncwarp();          // every lane is done with the slots before the next batch of copies overwrites them
-    }
-#pragma unroll
-    for (int j = 0; j < JMAX; ++j) {
-      const int f0 = (j * 32 + lane) * 4;
-      if (f0 < a.f) {
-        float o[4];
-        if (a.z) {
-          const float4 zv = __ldg(reinterpret_cast<const float4*>(a.z + b * a.bsz + (long long)i * a.ldz + f0));
-          o[0] = __fadd_rn(__fmul_rn(a.alpha, acc[j][0]), __fmul_rn(a.beta, zv.x));
-          o[1] = __fadd_rn(__fmul_rn(a.alpha, acc[j][1]), __fmul_rn(a.beta, zv.y));
-          o[2] = __fadd_rn(__fmul_rn(a.alpha, acc[j][2]), __fmul_rn(a.beta, zv.z));
-          o[3] = __fadd_rn(__fmul_rn(a.alpha, acc[j][3]), __fmul_rn(a.beta, zv.w));
-        } else {
-#pragma unroll
-          for (int v = 0; v < 4; ++v) o[v] = (a.alpha == 1.0f) ? acc[j][v] : __fmul_rn(a.alpha, acc[j][v]);
-        }
-        *reinterpret_cast<float4*>(a.y + b * a.bsy + (long long)i * a.ldy + f0) = make_float4(o[0], o[1], o[2], o[3]);
-      }
-    }
   }
 }
 
@@ -277,59 +200,17 @@ static int spmm_impl(const stmp_plan* plan, int op, int transposed, int64_t batc
   int lanes = (int)((f + vec - 1) / vec);
   int G = 1, lg = 0;
   while (G < lanes && G < 32) { G <<= 1; ++lg; }
-  long long groups = batch * (long long)c.n;
-  const int blk = g_spmm_block == 1024 ? 1024 : 256;
-  const int gpc = blk / G;
-  int rpg = g_spmm_rows_per_group;
-  if (rpg < 1) rpg = 1;
+  const int gpc = kSpmmThreads / G;
+  int rpg = kSpmmRowsPerGroup;
   // small problems keep one row per group: the row blocks must still fill the machine (>= 8 CTAs of 256 threads per SM's worth of blocks)
   while (rpg > 1 && batch * ((c.n + (long long)gpc * rpg - 1) / ((long long)gpc * rpg)) < 1184) rpg >>= 1;
   const int blocks_per_b = (int)((c.n + (long long)gpc * rpg - 1) / ((long long)gpc * rpg));
   long long blocks = batch * (long long)blocks_per_b;
   STMP_REQUIRE(blocks < (1ll << 31), STMP_ESHAPE, "stmp_spmm: problem too large for one launch");
   cudaStream_t st = (cudaStream_t)stream;
-  if (g_spmm_variant < 0) {
-    const char* v = getenv("STMP_SPMM_VARIANT");
-    g_spmm_variant = v ? atoi(v) : 0;
-  }
-  if ((g_spmm_variant == 1 || g_spmm_variant == 2) && !att && vec == 4 && f <= 512 && (long long)groups >= 8) {
-    // TMA-staged gather: SLOTS x 4f bytes of shared memory per warp
-    const int slots = g_spmm_variant == 1 ? 8 : 16;
-    const size_t smem = (size_t)8 * slots * f * 4 + 8 * 8;
-    if (smem <= 200 * 1024) {
-      int dev = 0, sms = 0;
-      STMP_CUDA_OK(cudaGetDevice(&dev));
-      STMP_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-      int per_sm = (int)((220 * 1024) / (smem + 1024));
-      if (per_sm > 8) per_sm = 8;
-      if (per_sm < 1) per_sm = 1;
-      long long want = (groups + 7) / 8;
-      unsigned grid = (unsigned)(want < (long long)sms * per_sm ? want : (long long)sms * per_sm);
-      const int jm = (int)((f + 127) / 128);
-#define STMP_TMA_LAUNCH(S, J)                                                                                          \
-  do {                                                                                                                 \
-    STMP_CUDA_OK(cudaFuncSetAttribute(k_spmm_tma<S, J>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));      \
-    k_spmm_tma<S, J><<<grid, 256, smem, st>>>(a);                                                                      \
-  } while (0)
-      if (slots == 8) {
-        if (jm == 1) STMP_TMA_LAUNCH(8, 1); else if (jm == 2) STMP_TMA_LAUNCH(8, 2); else STMP_TMA_LAUNCH(8, 4);
-      } else {
-        if (jm == 1) STMP_TMA_LAUNCH(16, 1); else if (jm == 2) STMP_TMA_LAUNCH(16, 2); else STMP_TMA_LAUNCH(16, 4);
-      }
-#undef STMP_TMA_LAUNCH
-      STMP_LAUNCH_OK("k_spmm_tma");
-      return STMP_OK;
-    }
-  }
-  if (blk == 1024) {
-    if (vec == 4) k_spmm<4, 1024><<<(unsigned)blocks, 1024, 0, st>>>(a, G, lg, rpg, blocks_per_b);
-    else if (vec == 2) k_spmm<2, 1024><<<(unsigned)blocks, 1024, 0, st>>>(a, G, lg, rpg, blocks_per_b);
-    else k_spmm<1, 1024><<<(unsigned)blocks, 1024, 0, st>>>(a, G, lg, rpg, blocks_per_b);
-  } else {
-    if (vec == 4) k_spmm<4, 256><<<(unsigned)blocks, 256, 0, st>>>(a, G, lg, rpg, blocks_per_b);
-    else if (vec == 2) k_spmm<2, 256><<<(unsigned)blocks, 256, 0, st>>>(a, G, lg, rpg, blocks_per_b);
-    else k_spmm<1, 256><<<(unsigned)blocks, 256, 0, st>>>(a, G, lg, rpg, blocks_per_b);
-  }
+  if (vec == 4) k_spmm<4><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(a, G, lg, rpg, blocks_per_b);
+  else if (vec == 2) k_spmm<2><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(a, G, lg, rpg, blocks_per_b);
+  else k_spmm<1><<<(unsigned)blocks, kSpmmThreads, 0, st>>>(a, G, lg, rpg, blocks_per_b);
   STMP_LAUNCH_OK("k_spmm");
   return STMP_OK;
 }

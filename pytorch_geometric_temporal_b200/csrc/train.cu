@@ -13,17 +13,13 @@
 //                               parameter / gradient buffer of distributed.FlatGradSync: one launch instead of the ~35 of the
 //                               capturable foreach implementation; the step counter lives on the device (CUDA-graph replay), the
 //                               gradient average over ranks and the zeroing of the gradient buffer are folded in.
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace stmp {
-int g_wgrad_tc = -1;      // 1: wgmma contraction (wgrad_tc.cu); 0: the fp32 FFMA kernel below (stmp_set_option("dcrnn_wgrad_tc") / STMP_WGRAD_TC)
 int wgrad_tc_launch(int cin, long long rows, int ld, const float* S1, const float* S2, const float* dpzr, const float* dph, float* partial,
                     int max_parts, cudaStream_t st, int* parts);
 namespace {
 
-constexpr int kWgradTcDefault = 1;    // the tensor-core contraction (wgrad_tc.cu)
 constexpr int kWgTK = 16;            // rows per staged tile
 constexpr int kWgStages = 4;         // tiles in flight per CTA: 3 x 19 KB x 2 CTAs per SM keeps ~115 KB per SM on the wire (2 stages of 32 rows were load-latency bound)
 constexpr int kWgThreads = 192;      // >= 12 * ceil(3C/8) for cin <= 4
@@ -243,10 +239,6 @@ extern "C" int stmp_dcrnn_bwd_wgrad(int64_t cin, int64_t cout, int64_t K, int64_
   p.n_tiles = (int)((rows + kWgTK - 1) / kWgTK);
   p.partial = reinterpret_cast<float*>(workspace);
   int grid = wgrad_grid();
-  if (g_wgrad_tc < 0) {
-    const char* v = getenv("STMP_WGRAD_TC");
-    g_wgrad_tc = v ? (atoi(v) ? 1 : 0) : kWgradTcDefault;
-  }
   if (g_wgrad_tc) {
     const int rc = wgrad_tc_launch((int)cin, rows, (int)ld, S1, S2, dpzr, dph, p.partial, grid, st, &grid);
     if (rc != STMP_OK) return rc;
