@@ -132,6 +132,10 @@ int stmp_spmm_att_grad(const stmp_plan* plan, int op, int64_t batch, int64_t f, 
  *   w_z,w_r,w_h: DConv.weight [2,K,cin+cout,cout]; b_*: [cout] or NULL (dcrnn.py:26-37)
  *   h0: [B,N,cout] or NULL; out: [B,T,N,cout]
  *   stash (nullable): [B,T,3,N,cout] receives (Z,R,Htilde) per step for the backward pass.
+ * Kernels: cout = 32, K = 2 the wgmma kernel; cout in {16, 32} the FFMA kernel; cout in 1..4 (cin in 1..4, K in 1..4: the
+ * reference's BatchedDCRNN(F, F, K=3) training model) the narrow-state kernel, whose CTAs serve up to 8 windows side by side
+ * ("dcrnn_narrow_pack", stmp_set_option; fewer where N * P would exceed 1024 in the forward or 512 in the backward) and which ignores
+ * wimage / workspace.
  * Returns STMP_EUNSUPPORTED when (N, nnz, cin, cout, K) do not fit the fused kernel. */
 int stmp_dcrnn_seq_fwd(const stmp_plan* plan, int64_t B, int64_t T, int64_t cin, int64_t cout, int64_t K,
                        const float* x, const int64_t* win_start, int64_t x_bstride, int64_t x_tstride,
@@ -223,6 +227,18 @@ int stmp_dcrnn_bwd_basis(const stmp_plan* plan, int64_t B, int64_t T, int64_t ci
 int stmp_dcrnn_bwd_seq(const stmp_plan* plan, int64_t B, int64_t T, int64_t cin, int64_t cout, const float* gout,
                        const float* out, const float* h0, const float* stash, const float* whsT, const float* wzrT,
                        float* dph_all, float* dpzr_all, float* dx, float* dh0, void* stream);
+
+/* ---- backward of the fused DCRNN sequence for narrow states (cout <= 4): the reference's training model BatchedDCRNN(F, F, K=3) ----
+ * Served when stmp_dcrnn_narrow_bwd_supported(plan, cin, cout, K) != 0 (DCONV plan, cin and cout in 1..4, K in 1..4, graph and state
+ * buffers fit one SM's shared memory: PEMS-BAY's 325 nodes at K = 3 do).  stmp_dcrnn_narrow_bwd_seq is the reverse-time recurrence in
+ * one persistent launch, with the contract of stmp_dcrnn_bwd_seq plus K: gout (B,T,N,cout), out and stash (B,T,3,N,cout) of the
+ * forward, h0 (B,N,cout; nullable), whsT (cout, (2K-1)C) / wzrT (2cout, (2K-1)C) from stmp_dcrnn_pack_bwd_weights -> dph_all
+ * (T,B,N,cout), dpzr_all (T,B,N,2cout), dx (B,T,N,cin; nullable), dh0 (B,N,cout).  Deterministic, no atomics; the results do not
+ * depend on how many windows a CTA serves ("dcrnn_narrow_pack"). */
+int stmp_dcrnn_narrow_bwd_supported(const stmp_plan* plan, int64_t cin, int64_t cout, int64_t K);
+int stmp_dcrnn_narrow_bwd_seq(const stmp_plan* plan, int64_t B, int64_t T, int64_t cin, int64_t cout, int64_t K, const float* gout,
+                              const float* out, const float* h0, const float* stash, const float* whsT, const float* wzrT,
+                              float* dph_all, float* dpzr_all, float* dx, float* dh0, void* stream);
 
 /* Backward of stmp_tgcn_attn_fwd for H = NULL (the training configuration of the reference's A3TGCN2 example; what autograd records for
  * attentiontemporalgcn.py:130-157 / temporalgcn.py:187-233 over all periods): given gout (B, N, 32) it recomputes A^X and the gates and
@@ -349,7 +365,8 @@ int stmp_window_gather(const float* series, int64_t t_total, int64_t row_elems, 
  * "dcrnn_tc" = 1 (wgmma kernel, default) / 0 (FFMA kernel) behind stmp_dcrnn_seq_fwd; "dcrnn_fwd_split" = 1 (default: the fused
  * forward runs on a 2-CTA cluster per window when 2 B <= SM count and N > 128) / 0 (one CTA per window); "dcrnn_bwd_split" = 1
  * (default: a 2-CTA cluster per window when 2 B <= SM count) / 0 (one CTA per window); "dcrnn_wgrad_tc" = 1 (default, wgmma) /
- * 0 (FFMA).  Any other name returns STMP_EINVAL. */
+ * 0 (FFMA); "dcrnn_narrow_pack" = 0 (default: automatic) / P in 1..8, the number of windows one CTA of the narrow-state DCRNN kernels
+ * serves side by side (lowered if the layout does not fit; outputs do not depend on it).  Any other name returns STMP_EINVAL. */
 int stmp_set_option(const char* name, int value);
 
 /* ---- misc ---------------------------------------------------------------------------------------- */

@@ -25,6 +25,7 @@ extern int g_dcrnn_tc;     // "dcrnn_tc": 1 wgmma forward (dcrnn_seq_tc.cu) / 0 
 extern int g_fwd_split;    // "dcrnn_fwd_split": 1 a CTA pair per window for small batches / 0 one CTA per window (wgmma forward)
 extern int g_bwd_split;    // "dcrnn_bwd_split": the same choice for the persistent backward (dcrnn_bwd.cu)
 extern int g_wgrad_tc;     // "dcrnn_wgrad_tc": 1 wgmma weight-gradient contraction (wgrad_tc.cu) / 0 FFMA (train.cu)
+extern int g_narrow_pack;  // "dcrnn_narrow_pack": windows per CTA of the narrow DCRNN kernels (dcrnn_narrow.cu), 0 = automatic
 
 #define STMP_CUDA_OK(expr)                                                                    \
   do {                                                                                        \

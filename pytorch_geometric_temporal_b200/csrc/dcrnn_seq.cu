@@ -38,6 +38,13 @@ int gru_tc_launch(const stmp_plan* plan, int n_ops, long long B, long long T, lo
                   float* out, float* stash, const void* wimage, void* workspace, cudaStream_t st);
 long long tc_workspace_bytes(const stmp_plan* plan, long long T, long long cin);
 
+// narrow-state variant, cout <= 4 (dcrnn_narrow.cu)
+bool dcrnn_narrow_supported(const stmp_plan* plan, long long cin, long long cout, long long K);
+int dcrnn_narrow_launch(const stmp_plan* plan, long long B, long long T, long long cin, long long cout, long long K, const float* x,
+                        const long long* win_start, long long x_bstride, long long x_tstride, const float* w_z, const float* w_r,
+                        const float* w_h, const float* b_z, const float* b_r, const float* b_h, const float* h0, float* out, float* stash,
+                        cudaStream_t st);
+
 namespace {
 
 constexpr int kMaxSmem = 232448;  // 227 KB opt-in limit per CTA on sm_90
@@ -410,6 +417,7 @@ bool shape_ok(const stmp_plan* plan, int64_t cin, int64_t cout, int64_t K) {
 using namespace stmp;
 
 extern "C" int stmp_dcrnn_seq_supported(const stmp_plan* plan, int64_t cin, int64_t cout, int64_t K) {
+  if (cout >= 1 && cout <= 4) return dcrnn_narrow_supported(plan, cin, cout, K) ? 1 : 0;   // narrow states: dcrnn_narrow.cu
   if (!shape_ok(plan, cin, cout, K)) return 0;
   if (g_dcrnn_tc && dcrnn_tc_supported(plan, cin, cout, K)) return 1;   // the wgmma kernel's envelope is wider in cin than the FFMA kernel's
   Layout L;
@@ -426,6 +434,14 @@ extern "C" int stmp_dcrnn_seq_fwd(const stmp_plan* plan, int64_t B, int64_t T, i
   STMP_REQUIRE(B >= 0 && T >= 0, STMP_EINVAL, "stmp_dcrnn_seq_fwd: negative B/T");
   STMP_REQUIRE(K > 0, STMP_EINVAL, "K must be > 0");  // assert K > 0, dcrnn.py:23
   STMP_REQUIRE(x && w_z && w_r && w_h && out, STMP_EINVAL, "stmp_dcrnn_seq_fwd: NULL tensor");
+  if (cout >= 1 && cout <= 4) {   // narrow states (the reference's BatchedDCRNN(F, F, K) training model): dcrnn_narrow.cu
+    if (!dcrnn_narrow_supported(plan, cin, cout, K))
+      return set_error(STMP_EUNSUPPORTED, "narrow DCRNN kernel supports cin in 1..4, K in 1..4 and graphs whose layout fits shared memory "
+                       "(got N=%d cin=%lld cout=%lld K=%lld)", plan->n, (long long)cin, (long long)cout, (long long)K);
+    if (B == 0 || T == 0) return STMP_OK;
+    return dcrnn_narrow_launch(plan, B, T, cin, cout, K, x, reinterpret_cast<const long long*>(win_start), x_bstride, x_tstride, w_z, w_r,
+                               w_h, b_z, b_r, b_h, h0, out, stash, (cudaStream_t)stream);
+  }
   if (!shape_ok(plan, cin, cout, K))
     return set_error(STMP_EUNSUPPORTED, "fused DCRNN kernel supports N<=256 (cout 32), cin<=4, cout in {16,32}, K<=4 (got N=%d cin=%lld cout=%lld K=%lld)",
                      plan->n, (long long)cin, (long long)cout, (long long)K);

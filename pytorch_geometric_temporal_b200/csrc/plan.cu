@@ -31,6 +31,7 @@ int g_dcrnn_tc = 1;
 int g_fwd_split = 1;       // 64 windows: 200 -> 171 us (H100 SXM, 700 W)
 int g_bwd_split = 1;
 int g_wgrad_tc = 1;
+int g_narrow_pack = 0;
 
 // ---- per-kernel launch counters (stmp_path_counters) ----------------------------------------------------
 constexpr int kMaxPaths = 96;
@@ -879,6 +880,11 @@ extern "C" int stmp_set_option(const char* name, int value) {
   if (strcmp(name, "dcrnn_fwd_split") == 0) { g_fwd_split = value ? 1 : 0; return STMP_OK; }
   if (strcmp(name, "dcrnn_bwd_split") == 0) { g_bwd_split = value ? 1 : 0; return STMP_OK; }
   if (strcmp(name, "dcrnn_wgrad_tc") == 0) { g_wgrad_tc = value ? 1 : 0; return STMP_OK; }
+  if (strcmp(name, "dcrnn_narrow_pack") == 0) {
+    STMP_REQUIRE(value >= 0 && value <= 8, STMP_EINVAL, "stmp_set_option: dcrnn_narrow_pack must be 0 (automatic) .. 8");
+    g_narrow_pack = value;
+    return STMP_OK;
+  }
   return set_error(STMP_EINVAL, "stmp_set_option: unknown option '%s'", name);
 }
 

@@ -97,7 +97,7 @@ class _DcrnnSeqFn(torch.autograd.Function):
     hand-written reverse-time loop over the stash (transposed SpMM for the diffusion adjoints, cuBLAS for the
     contractions).  Replaces autograd's replay of the ~1500-launch tiled graph."""
 
-    fused_backward = True    # False forces the per-step backward even where the persistent kernel is available (tests)
+    fused_backward = True    # False forces the per-step backward even where a persistent kernel is available (tests)
 
     @staticmethod
     def forward(ctx, X, H0, wz, wr, wh, bz, br, bh, plan, K, wimage):
@@ -112,7 +112,9 @@ class _DcrnnSeqFn(torch.autograd.Function):
         """Reverse-time loop with 8 launches per step: [carry] -> GEMM -> 2 transposed SpMMs (in-place adjoint) -> [zr] ->
         GEMM -> 2 transposed SpMMs.  Everything that does not depend on the dH recurrence is hoisted out: both bases of
         every step are built with 4 batched SpMMs straight into their column blocks, and the weight gradients are two
-        large GEMMs over all (t, b, n) rows after the loop."""
+        large GEMMs over all (t, b, n) rows after the loop.  Two persistent kernels replace the loop where they apply: hidden 32 / K = 2
+        (`dcrnn_bwd_seq`, with its own bases and weight-gradient kernels) and narrow states, cout <= 4 (`dcrnn_narrow_bwd_seq`, after the
+        same hoisted bases and before the same `_finish`)."""
         X, H0, wz, wr, wh, out, stash = ctx.saved_tensors
         plan, K = ctx.plan, ctx.K
         B, T, N, Ci = X.shape
@@ -170,9 +172,15 @@ class _DcrnnSeqFn(torch.autograd.Function):
                         ops.spmm_cols(plan, o, S, 0, dst, C)
                     else:
                         ops.spmm_cols(plan, o, S, dst - 2 * C, dst, C, alpha=2.0, z_col=0, beta=-1.0)
-        # ---- the recurrence ---------------------------------------------------------------------------------------------
         dph_all = torch.empty(T, B, N, Co, **f32)
         dpzr_all = torch.empty(T, B, N, 2 * Co, **f32)
+        if _DcrnnSeqFn.fused_backward and Co <= 4 and ops.dcrnn_narrow_bwd_supported(plan, Ci, Co, K):
+            # narrow states (cout <= 4): the whole reverse recurrence is ONE persistent launch, dL/dH stays on chip
+            dX = torch.empty(X.shape, **f32) if ctx.needs_input_grad[0] else None
+            dH0 = torch.empty(B, N, Co, **f32)
+            ops.dcrnn_narrow_bwd_seq(plan, Ci, K, gout, out, H0, stash, WhsT, WzrT, dph_all, dpzr_all, dX, dH0)
+            return _DcrnnSeqFn._finish(ctx, S1, S2, dph_all, dpzr_all, dX, dH0, K, C, Co)
+        # ---- the recurrence ---------------------------------------------------------------------------------------------
         buf2 = torch.empty(B, N, nb * C, **f32)                                            # dL/dS2 -> (in place) dL/d[X | H*R]
         buf1 = torch.empty(B, N, nb * C, **f32)                                            # dL/dS1 -> (in place) dL/d[X | H_{t-1}]
         g = torch.empty(B, N, Co, **f32)

@@ -473,6 +473,22 @@ def dcrnn_bwd_seq(plan: GraphPlan, cin: int, gout, out, h0, stash, whsT, wzrT, d
                                                  _lib.ptr(dpzr_all), _lib.ptr(dx), _lib.ptr(dh0), _lib.stream_ptr()))
 
 
+def dcrnn_narrow_bwd_supported(plan: GraphPlan, cin: int, cout: int, K: int) -> bool:
+    return bool(_lib.lib().stmp_dcrnn_narrow_bwd_supported(plan.handle, cin, cout, K))
+
+
+def dcrnn_narrow_bwd_seq(plan: GraphPlan, cin: int, K: int, gout, out, h0, stash, whsT, wzrT, dph_all, dpzr_all, dx, dh0):
+    """The reverse-time recurrence of the narrow-state DCRNN backward (cout <= 4, any K <= 4) in one persistent launch."""
+    gout, out, stash = _f32c(gout, "gout"), _f32c(out, "out"), _f32c(stash, "stash")
+    B, T, N, Co = gout.shape
+    h0 = None if h0 is None else _f32c(h0, "h0")
+    with torch.cuda.device(gout.device):
+        _lib.check(_lib.lib().stmp_dcrnn_narrow_bwd_seq(plan.handle, B, T, cin, Co, K, _lib.ptr(gout), _lib.ptr(out), _lib.ptr(h0),
+                                                        _lib.ptr(stash), _lib.ptr(_f32c(whsT, "whsT")), _lib.ptr(_f32c(wzrT, "wzrT")),
+                                                        _lib.ptr(dph_all), _lib.ptr(dpzr_all), _lib.ptr(dx), _lib.ptr(dh0),
+                                                        _lib.stream_ptr()))
+
+
 def dcrnn_bwd_basis_ld(cin: int, cout: int, K: int) -> int:
     """Row pitch of the stacked bases: (2K-1)(cin+cout) rounded up to 8 floats (16-byte rows for the weight-gradient kernel's tiles)."""
     return ((2 * K - 1) * (cin + cout) + 7) // 8 * 8

@@ -49,6 +49,18 @@ with torch.no_grad():
     eg, wg = torch.from_numpy(eg).to(dev), torch.from_numpy(wg).to(dev)
     lstm = GConvLSTM(64, 64, 3).to(dev)
     lstm(torch.randn(2000, 64, device=dev), eg, wg)              # k_spmm + k_gemm_split<LSTM epilogue>
+    nm = BatchedDCRNN(2, 2, 3).to(dev)
+    _lib.set_option("dcrnn_narrow_pack", 3)
+    nm(X[:5, :4], ei_t, ew_t)                                    # k_dcrnn_narrow_seq, 3 windows per CTA (one group half empty)
+    _lib.set_option("dcrnn_narrow_pack", 0)
+(nm(X[:3, :4], ei_t, ew_t) * torch.randn(3, 4, X.size(2), 2, device=dev)).sum().backward()   # k_dcrnn_narrow_bwd, one window per CTA
+_lib.set_option("dcrnn_narrow_pack", 2)
+(nm(X[:3, :4], ei_t, ew_t) * torch.randn(3, 4, X.size(2), 2, device=dev)).sum().backward()   # packed: 2 windows per CTA, 2 tasks per thread
+e8 = torch.stack([torch.arange(40), (torch.arange(40) * 7 + 1) % 40]).to(dev)
+nm8 = BatchedDCRNN(4, 4, 3).to(dev)
+_lib.set_option("dcrnn_narrow_pack", 8)
+(nm8(torch.randn(10, 3, 40, 4, device=dev), e8, torch.ones(40, device=dev)) ** 2).sum().backward()   # CP = 8, 8 windows per CTA, tail group
+_lib.set_option("dcrnn_narrow_pack", 0)
 x = torch.randn(2, 2000, 64, device=dev, requires_grad=True)
 h, c = lstm(x, eg, wg)
 (h.sum() + c.sum()).backward()                                   # _LstmCellFn backward: k_gemm_split, k_lstm_gate_bwd, transposed SpMM
