@@ -251,6 +251,18 @@ int stmp_tgcn_attn_bwd(const stmp_plan* plan, int64_t B, int64_t fin, int64_t pe
                        const float* c, const float* probs, const float* gout, void* workspace, float* dA, float* dc,
                        float* dprobs, void* stream);
 
+/* Backward of ONE TGCN cell step with an incoming state: stmp_tgcn_attn_fwd with periods = 1, probs = NULL and h != NULL (what autograd
+ * records for temporalgcn.py:104-130 / :212-233 on the steps t >= 1 of the reference's BatchedTGCN loop, H carried).  x (B, N, fin), h
+ * (B, N, 32) at batch stride h_bstride, A (fin, 96), Bm (32, 96), c (96) are the forward's operands, gout = dL/dH_new (B, N, 32).  It
+ * recomputes A^X and the gates and writes dh = dL/dH (B, N, 32, contiguous; skipped when dh is NULL) and the folded-weight gradients
+ * dA (fin, 96), dBm (32, 96) and dc (96), reduced over all (batch row, node).  No gradient w.r.t. X.  Two launches (k_tgcn_cell_bwd:
+ * per-CTA partials; k_tgcn_cell_bwd_reduce: fixed-order sum), deterministic; workspace of stmp_tgcn_cell_bwd_workspace_bytes(plan, B)
+ * bytes.  STMP_EUNSUPPORTED for fin outside 1..4, STMP_EINVAL for a NULL tensor or B < 1, STMP_ESHAPE for B >= 65536. */
+int64_t stmp_tgcn_cell_bwd_workspace_bytes(const stmp_plan* plan, int64_t B);
+int stmp_tgcn_cell_bwd(const stmp_plan* plan, int64_t B, int64_t fin, const float* x, const float* h, int64_t h_bstride, const float* A,
+                       const float* Bm, const float* c, const float* gout, void* workspace, float* dh, float* dA, float* dBm, float* dc,
+                       void* stream);
+
 /* Weight / bias gradients of the three DCRNN gates over all (t, b, n) rows (what autograd accumulates for the `matmul(basis, W)` and
  * `+ bias` of dcrnn.py:86-111 across steps, gates and hops): S1 / S2 (rows, ld) are stmp_dcrnn_bwd_basis' bases (ld = 3(cin+cout) rounded
  * up to 8), dpzr (rows, 2cout) / dph (rows, cout) stmp_dcrnn_bwd_seq's d pre-activations.  Writes gz / gr / gh in the module's

@@ -41,6 +41,50 @@ __device__ __forceinline__ float tanh_f(float x) { return 2.0f * __fdividef(1.0f
 
 constexpr int kNodesPerBlock = 64;
 
+// Thread 0 starts ONE TMA bulk copy of X[b] into shared memory; the CTA waits for it with __syncthreads() + mbar_wait(bar, 0).
+__device__ __forceinline__ void stage_x_begin(uint64_t* bar, float* Xs, const float* xb, uint32_t bytes) {
+  if (threadIdx.x == 0) {
+    mbar_init(bar, 1);
+    fence_mbar_init();
+    mbar_arrive_expect_tx(bar, bytes);
+    tma_bulk_g2s(Xs, xb, bytes, bar);
+  }
+}
+
+// A^X of node n for all periods, in the reference's edge order: lane holds entries (q*32 + lane) of the node's FP-float row of X[b]
+// (Xg: shared memory when staged, global memory otherwise).
+template <int NQ>
+__device__ __forceinline__ void gather_ax(const int* rowptr, const int2* cv, const float* Xg, int FP, int stage, int n, int lane,
+                                          float (&ax)[NQ]) {
+#pragma unroll
+  for (int q = 0; q < NQ; ++q) ax[q] = 0.f;
+  const int beg = __ldg(rowptr + n), end = __ldg(rowptr + n + 1);
+  for (int k = beg; k < end; ++k) {
+    const int2 e = __ldg(cv + k);
+    const float w = __int_as_float(e.y);
+    const float* xr = Xg + (long long)e.x * FP;
+#pragma unroll
+    for (int q = 0; q < NQ; ++q)
+      if (q * 32 + lane < FP) ax[q] = __fadd_rn(ax[q], __fmul_rn(w, stage ? xr[q * 32 + lane] : __ldg(xr + q * 32 + lane)));
+  }
+}
+
+// Sum of column i of `parts` per-CTA partials (row length `width`) in a fixed association: warp w sums its contiguous share of the
+// partials, then the 8 sub-sums are added in warp order.  Valid in warp 0 only; i may depend on the lane only.
+__device__ __forceinline__ float sum_partials(int parts, int width, const float* __restrict__ partial, int i, float (&sub)[8][32]) {
+  const int x = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int per = (parts + 7) / 8, q0 = w * per, q1 = (q0 + per < parts) ? q0 + per : parts;
+  float s = 0.f;
+  if (i < width)
+    for (int q = q0; q < q1; ++q) s += partial[(size_t)q * width + i];
+  sub[w][x] = s;
+  __syncthreads();
+  float t = sub[0][x];
+#pragma unroll
+  for (int k = 1; k < 8; ++k) t += sub[k][x];
+  return t;
+}
+
 template <int NQ, bool HAS_H>
 __global__ void __launch_bounds__(256) k_tgcn_attn(const TgcnArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -50,15 +94,7 @@ __global__ void __launch_bounds__(256) k_tgcn_attn(const TgcnArgs a) {
   const long long b = blockIdx.y;
   const int n0 = blockIdx.x * kNodesPerBlock;
   const float* xb = a.x + b * (long long)a.N * a.FP;
-  if (a.stage) {
-    if (threadIdx.x == 0) {
-      mbar_init(&bar, 1);
-      fence_mbar_init();
-      const uint32_t bytes = (uint32_t)a.N * a.FP * 4u;
-      mbar_arrive_expect_tx(&bar, bytes);
-      tma_bulk_g2s(Xs, xb, bytes, &bar);
-    }
-  }
+  if (a.stage) stage_x_begin(&bar, Xs, xb, (uint32_t)a.N * a.FP * 4u);
   // weights of my output channel (lane) while the copy is in flight
   float Az[4], Ar[4], Ah[4];
 #pragma unroll
@@ -87,17 +123,7 @@ __global__ void __launch_bounds__(256) k_tgcn_attn(const TgcnArgs a) {
   for (int n = n0 + warp; n < nend; n += 8) {
     // ---- A^X for all periods: lane holds entries (q*32 + lane) of the node's in*periods row, reference's edge order --------
     float ax[NQ];
-#pragma unroll
-    for (int q = 0; q < NQ; ++q) ax[q] = 0.f;
-    const int beg = __ldg(a.rowptr + n), end = __ldg(a.rowptr + n + 1);
-    for (int k = beg; k < end; ++k) {
-      const int2 e = __ldg(a.cv + k);
-      const float w = __int_as_float(e.y);
-      const float* xr = Xg + (long long)e.x * FP;
-#pragma unroll
-      for (int q = 0; q < NQ; ++q)
-        if (q * 32 + lane < FP) ax[q] = __fadd_rn(ax[q], __fmul_rn(w, a.stage ? xr[q * 32 + lane] : __ldg(xr + q * 32 + lane)));
-    }
+    gather_ax<NQ>(a.rowptr, a.cv, Xg, FP, a.stage, n, lane, ax);
     float h = 0.f, hz = cz, hr = cr;
     if (HAS_H) {
       h = __ldg(a.h + b * a.h_bstride + (long long)n * 32 + lane);
@@ -168,13 +194,7 @@ __global__ void __launch_bounds__(256) k_tgcn_attn_bwd(const TgcnBwdArgs a) {
   const long long b = blockIdx.y;
   const int n0 = blockIdx.x * kNodesPerBlock;
   const float* xb = a.x + b * (long long)a.N * a.FP;
-  if (a.stage && threadIdx.x == 0) {
-    mbar_init(&bar, 1);
-    fence_mbar_init();
-    const uint32_t bytes = (uint32_t)a.N * a.FP * 4u;
-    mbar_arrive_expect_tx(&bar, bytes);
-    tma_bulk_g2s(Xs, xb, bytes, &bar);
-  }
+  if (a.stage) stage_x_begin(&bar, Xs, xb, (uint32_t)a.N * a.FP * 4u);
   float Az[4], Ah[4];
 #pragma unroll
   for (int f = 0; f < 4; ++f) {
@@ -192,17 +212,7 @@ __global__ void __launch_bounds__(256) k_tgcn_attn_bwd(const TgcnBwdArgs a) {
   float dAz[4] = {0.f, 0.f, 0.f, 0.f}, dAh[4] = {0.f, 0.f, 0.f, 0.f}, dcz = 0.f, dch = 0.f, dpr[4] = {0.f, 0.f, 0.f, 0.f};
   for (int n = n0 + warp; n < nend; n += 8) {
     float ax[NQ];
-#pragma unroll
-    for (int q = 0; q < NQ; ++q) ax[q] = 0.f;
-    const int beg = __ldg(a.rowptr + n), end = __ldg(a.rowptr + n + 1);
-    for (int k = beg; k < end; ++k) {
-      const int2 e = __ldg(a.cv + k);
-      const float w = __int_as_float(e.y);
-      const float* xr = Xg + (long long)e.x * FP;
-#pragma unroll
-      for (int q = 0; q < NQ; ++q)
-        if (q * 32 + lane < FP) ax[q] = __fadd_rn(ax[q], __fmul_rn(w, a.stage ? xr[q * 32 + lane] : __ldg(xr + q * 32 + lane)));
-    }
+    gather_ax<NQ>(a.rowptr, a.cv, Xg, FP, a.stage, n, lane, ax);
     const float g = __ldg(a.gout + (b * a.N + n) * 32 + lane);
     for (int t = 0; t < P; ++t) {
       float pz = cz, ph = ch, v[4] = {0.f, 0.f, 0.f, 0.f};
@@ -260,23 +270,177 @@ __global__ void __launch_bounds__(256) k_tgcn_attn_bwd(const TgcnBwdArgs a) {
 __global__ void __launch_bounds__(256) k_tgcn_attn_bwd_reduce(int parts, int FIN, int P, const float* __restrict__ partial, float* __restrict__ dA,
                                                               float* __restrict__ dc, float* __restrict__ dprobs) {
   __shared__ float sub[8][32];
-  const int x = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int i = blockIdx.x * 32 + x;                     // index into the partial layout
-  const int per = (parts + 7) / 8, q0 = w * per, q1 = (q0 + per < parts) ? q0 + per : parts;
-  float s = 0.f;
-  if (i < kBwdPartial)
-    for (int q = q0; q < q1; ++q) s += partial[(size_t)q * kBwdPartial + i];
-  sub[w][x] = s;
-  __syncthreads();
-  if (w != 0 || i >= kBwdPartial) return;
-  float t = sub[0][x];
-#pragma unroll
-  for (int k = 1; k < 8; ++k) t += sub[k][x];
+  const int i = blockIdx.x * 32 + (threadIdx.x & 31);   // index into the partial layout
+  const float t = sum_partials(parts, kBwdPartial, partial, i, sub);
+  if (threadIdx.x >= 32 || i >= kBwdPartial) return;
   if (i < 128) { const int f = i >> 5; if (f < FIN) dA[f * 96 + (i & 31)] = t; }
   else if (i < 256) { const int f = (i - 128) >> 5; if (f < FIN) dA[f * 96 + 64 + (i & 31)] = t; }
   else if (i < 288) dc[i - 256] = t;
   else if (i < 320) dc[64 + i - 288] = t;
   else if (i - 320 < P && dprobs) dprobs[i - 320] = t;
+}
+
+// ---- backward of one TGCN cell step WITH an incoming state (periods = 1): the steps t >= 1 of the reference's BatchedTGCN loop ----
+// Forward (k_tgcn_attn<1, true>):  pre_g = (A^X) A_g + H' Bm_g + c_g,  Z = sigma(pre_z), R = sigma(pre_r) with H' = H,
+// H~ = tanh(pre_h) with H' = H*R,  H_new = Z*H + (1-Z)*H~.  Given g = dL/dH_new the kernel recomputes A^X (the forward's gather) and
+// the gates, then per (row, node), lane j = output channel:
+//     dpz = g (H - H~) Z (1-Z),  dph = g (1-Z)(1 - H~^2),  d(H*R)_j = sum_k dph_k Bm_h[j][k],  dpr = d(H*R) H R (1-R)
+//     dH_j = g_j Z_j + d(H*R)_j R_j + sum_k dpz_k Bm_z[j][k] + sum_k dpr_k Bm_r[j][k]            (only when dh != NULL)
+// and accumulates  dA_g[f][j] += A^X_f dp_g,  dBm_{z,r}[k][j] += H_k dp_{z,r},  dBm_h[k][j] += (H*R)_k dph,  dc_g[j] += dp_g.
+// The graph only touches X, so no transposed SpMM is needed.  Bm is staged in shared memory with a padded row (kBmLd = 97) so that
+// both the column reads of the recompute (lane = column) and the row reads of the transposed products (lane = row) are free of bank
+// conflicts; the 96 dBm accumulators of a lane stay in registers.  Per-CTA partials are summed over the 8 warps in warp order, and
+// k_tgcn_cell_bwd_reduce adds the partials in a fixed association: the same inputs give the same bits.
+struct TgcnCellBwdArgs {
+  const int* rowptr;
+  const int2* cv;
+  int N, FIN;
+  const float* x;         // [B][N][FIN] contiguous
+  const float* h;         // [B][N][32] at h_bstride
+  long long h_bstride;
+  const float* A; const float* Bm; const float* c;
+  const float* gout;      // [B][N][32]
+  float* dh;              // [B][N][32] or null
+  float* partial;         // [gridDim.y * gridDim.x][kCellPartial]: dA[4][96] | dBm[32][96] | dc[96] (the output layouts)
+  int stage;
+};
+constexpr int kCellPartial = 4 * 96 + 32 * 96 + 96;
+constexpr int kBmLd = 97;
+
+__global__ void __launch_bounds__(256, 1) k_tgcn_cell_bwd(const TgcnCellBwdArgs a) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  float* Xs = reinterpret_cast<float*>(smem_raw);
+  __shared__ __align__(8) uint64_t bar;
+  __shared__ float Bs[32 * kBmLd];
+  __shared__ float red[8][1024];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long b = blockIdx.y;
+  const int n0 = blockIdx.x * kNodesPerBlock;
+  const float* xb = a.x + b * (long long)a.N * a.FIN;
+  if (a.stage) stage_x_begin(&bar, Xs, xb, (uint32_t)a.N * a.FIN * 4u);
+  for (int i = threadIdx.x; i < 32 * 96; i += 256) Bs[(i / 96) * kBmLd + i % 96] = __ldg(a.Bm + i);
+  float Az[4], Ar[4], Ah[4];
+#pragma unroll
+  for (int f = 0; f < 4; ++f) {
+    Az[f] = f < a.FIN ? __ldg(a.A + f * 96 + lane) : 0.f;
+    Ar[f] = f < a.FIN ? __ldg(a.A + f * 96 + 32 + lane) : 0.f;
+    Ah[f] = f < a.FIN ? __ldg(a.A + f * 96 + 64 + lane) : 0.f;
+  }
+  const float cz = __ldg(a.c + lane), cr = __ldg(a.c + 32 + lane), ch = __ldg(a.c + 64 + lane);
+  __syncthreads();            // Bs written; barrier initialised before anyone waits on it
+  if (a.stage) mbar_wait(&bar, 0);
+  const float* Xg = a.stage ? Xs : xb;
+  const float* Bl = Bs + lane * kBmLd;          // row `lane` of Bm (transposed products)
+  const int nend = min(n0 + kNodesPerBlock, a.N);
+  float dAz[4] = {0.f, 0.f, 0.f, 0.f}, dAr[4] = {0.f, 0.f, 0.f, 0.f}, dAh[4] = {0.f, 0.f, 0.f, 0.f};
+  float dcz = 0.f, dcr = 0.f, dch = 0.f;
+  float dBz[32], dBr[32], dBh[32];
+#pragma unroll
+  for (int k = 0; k < 32; ++k) dBz[k] = dBr[k] = dBh[k] = 0.f;
+  for (int n = n0 + warp; n < nend; n += 8) {
+    float ax[1];
+    gather_ax<1>(a.rowptr, a.cv, Xg, a.FIN, a.stage, n, lane, ax);
+    // ---- recompute the gates in the forward's order of operations -----------------------------------------------------------
+    const float h = __ldg(a.h + b * a.h_bstride + (long long)n * 32 + lane);
+    float pz = cz, pr = cr, ph = ch;
+#pragma unroll
+    for (int k = 0; k < 32; ++k) {
+      const float hk = __shfl_sync(0xffffffffu, h, k);
+      pz = fmaf(hk, Bs[k * kBmLd + lane], pz);
+      pr = fmaf(hk, Bs[k * kBmLd + 32 + lane], pr);
+    }
+    float v[4];
+#pragma unroll
+    for (int f = 0; f < 4; ++f) {
+      v[f] = __shfl_sync(0xffffffffu, ax[0], f);
+      if (f < a.FIN) {
+        pz = fmaf(v[f], Az[f], pz);
+        pr = fmaf(v[f], Ar[f], pr);
+        ph = fmaf(v[f], Ah[f], ph);
+      } else {
+        v[f] = 0.f;
+      }
+    }
+    const float Z = sigmoid_f(pz), R = sigmoid_f(pr), hr = h * R;
+#pragma unroll
+    for (int k = 0; k < 32; ++k) ph = fmaf(__shfl_sync(0xffffffffu, hr, k), Bs[k * kBmLd + 64 + lane], ph);
+    const float Ht = tanh_f(ph);
+    // ---- gate backward ------------------------------------------------------------------------------------------------------
+    const long long row = b * a.N + n;
+    const float g = __ldg(a.gout + row * 32 + lane);
+    const float dpz = g * (h - Ht) * Z * (1.0f - Z);
+    const float dph = g * (1.0f - Z) * (1.0f - Ht * Ht);
+    float dhr = 0.f;
+#pragma unroll
+    for (int k = 0; k < 32; ++k) dhr = fmaf(__shfl_sync(0xffffffffu, dph, k), Bl[64 + k], dhr);
+    const float dpr = dhr * h * R * (1.0f - R);
+    if (a.dh) {
+      float d = fmaf(g, Z, dhr * R);
+#pragma unroll
+      for (int k = 0; k < 32; ++k) {
+        d = fmaf(__shfl_sync(0xffffffffu, dpz, k), Bl[k], d);
+        d = fmaf(__shfl_sync(0xffffffffu, dpr, k), Bl[32 + k], d);
+      }
+      a.dh[row * 32 + lane] = d;
+    }
+    // ---- weight-gradient accumulation ---------------------------------------------------------------------------------------
+#pragma unroll
+    for (int f = 0; f < 4; ++f) {
+      dAz[f] = fmaf(v[f], dpz, dAz[f]);
+      dAr[f] = fmaf(v[f], dpr, dAr[f]);
+      dAh[f] = fmaf(v[f], dph, dAh[f]);
+    }
+    dcz += dpz;
+    dcr += dpr;
+    dch += dph;
+#pragma unroll
+    for (int k = 0; k < 32; ++k) {
+      const float hk = __shfl_sync(0xffffffffu, h, k), hrk = __shfl_sync(0xffffffffu, hr, k);
+      dBz[k] = fmaf(hk, dpz, dBz[k]);
+      dBr[k] = fmaf(hk, dpr, dBr[k]);
+      dBh[k] = fmaf(hrk, dph, dBh[k]);
+    }
+  }
+  // ---- CTA reduction in warp order, one partial per CTA: dBm one gate (32 x 32) at a time, then dA | dc ----------------------
+  float* out = a.partial + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * kCellPartial;
+  float* r = red[warp];
+#pragma unroll
+  for (int gt = 0; gt < 3; ++gt) {
+#pragma unroll
+    for (int k = 0; k < 32; ++k) r[k * 32 + lane] = gt == 0 ? dBz[k] : (gt == 1 ? dBr[k] : dBh[k]);
+    __syncthreads();
+    for (int i = threadIdx.x; i < 1024; i += 256) {
+      float s = red[0][i];
+#pragma unroll
+      for (int w = 1; w < 8; ++w) s += red[w][i];
+      out[4 * 96 + (i >> 5) * 96 + gt * 32 + (i & 31)] = s;
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int f = 0; f < 4; ++f) { r[f * 96 + lane] = dAz[f]; r[f * 96 + 32 + lane] = dAr[f]; r[f * 96 + 64 + lane] = dAh[f]; }
+  r[384 + lane] = dcz;
+  r[416 + lane] = dcr;
+  r[448 + lane] = dch;
+  __syncthreads();
+  for (int i = threadIdx.x; i < 480; i += 256) {
+    float s = red[0][i];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) s += red[w][i];
+    out[i < 384 ? i : 4 * 96 + 32 * 96 + (i - 384)] = s;
+  }
+}
+
+// dA (FIN x 96), dBm (32 x 96), dc (96): sums of the per-CTA partials, 8 sub-sums per output in a fixed association
+__global__ void __launch_bounds__(256) k_tgcn_cell_bwd_reduce(int parts, int FIN, const float* __restrict__ partial, float* __restrict__ dA,
+                                                              float* __restrict__ dBm, float* __restrict__ dc) {
+  __shared__ float sub[8][32];
+  const int i = blockIdx.x * 32 + (threadIdx.x & 31);
+  const float t = sum_partials(parts, kCellPartial, partial, i, sub);
+  if (threadIdx.x >= 32 || i >= kCellPartial) return;
+  if (i < 4 * 96) { if (i / 96 < FIN) dA[i] = t; }
+  else if (i < 4 * 96 + 32 * 96) dBm[i - 4 * 96] = t;
+  else dc[i - 4 * 96 - 32 * 96] = t;
 }
 
 template <int NQ>
@@ -370,5 +534,38 @@ extern "C" int stmp_tgcn_attn_bwd(const stmp_plan* plan, int64_t B, int64_t fin,
   STMP_LAUNCH_OK("k_tgcn_attn_bwd");
   k_tgcn_attn_bwd_reduce<<<(kBwdPartial + 31) / 32, 256, 0, st>>>((int)(grid.x * grid.y), (int)fin, (int)periods, a.partial, dA, dc, dprobs);
   STMP_LAUNCH_OK("k_tgcn_attn_bwd_reduce");
+  return STMP_OK;
+}
+
+extern "C" int64_t stmp_tgcn_cell_bwd_workspace_bytes(const stmp_plan* plan, int64_t B) {
+  if (!plan || B < 0) return 0;
+  return (int64_t)B * ((plan->n + kNodesPerBlock - 1) / kNodesPerBlock) * kCellPartial * 4;
+}
+
+extern "C" int stmp_tgcn_cell_bwd(const stmp_plan* plan, int64_t B, int64_t fin, const float* x, const float* h, int64_t h_bstride,
+                                  const float* A, const float* Bm, const float* c, const float* gout, void* workspace, float* dh,
+                                  float* dA, float* dBm, float* dc, void* stream) {
+  STMP_REQUIRE(plan != nullptr, STMP_EINVAL, "stmp_tgcn_cell_bwd: plan is NULL");
+  STMP_REQUIRE(plan->n_ops >= 1, STMP_EINVAL, "stmp_tgcn_cell_bwd: plan has no operator");
+  if (fin < 1 || fin > 4)
+    return set_error(STMP_EUNSUPPORTED, "fused TGCN cell backward takes in_channels <= 4 (got %lld)", (long long)fin);
+  STMP_REQUIRE(x && h && A && Bm && c && gout && workspace && dA && dBm && dc, STMP_EINVAL, "stmp_tgcn_cell_bwd: NULL tensor");
+  STMP_REQUIRE(B >= 1, STMP_EINVAL, "stmp_tgcn_cell_bwd: bad B");
+  STMP_REQUIRE(B < 65536, STMP_ESHAPE, "stmp_tgcn_cell_bwd: batch too large for one launch");
+  cudaStream_t st = (cudaStream_t)stream;
+  TgcnCellBwdArgs a;
+  a.rowptr = plan->fwd[0].rowptr; a.cv = plan->fwd[0].cv;
+  a.N = plan->n; a.FIN = (int)fin;
+  a.x = x; a.h = h; a.h_bstride = h_bstride; a.A = A; a.Bm = Bm; a.c = c; a.gout = gout; a.dh = dh;
+  a.partial = reinterpret_cast<float*>(workspace);
+  const size_t bytes = (size_t)a.N * a.FIN * 4;
+  a.stage = (bytes <= 128 * 1024 && bytes % 16 == 0 && (reinterpret_cast<uintptr_t>(x) % 16) == 0) ? 1 : 0;
+  const size_t smem = a.stage ? bytes : 0;
+  dim3 grid((unsigned)((a.N + kNodesPerBlock - 1) / kNodesPerBlock), (unsigned)B);
+  STMP_CUDA_OK(cudaFuncSetAttribute(k_tgcn_cell_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_tgcn_cell_bwd<<<grid, 256, smem, st>>>(a);
+  STMP_LAUNCH_OK("k_tgcn_cell_bwd");
+  k_tgcn_cell_bwd_reduce<<<(kCellPartial + 31) / 32, 256, 0, st>>>((int)(grid.x * grid.y), (int)fin, a.partial, dA, dBm, dc);
+  STMP_LAUNCH_OK("k_tgcn_cell_bwd_reduce");
   return STMP_OK;
 }

@@ -106,6 +106,13 @@ class TGCN(torch.nn.Module):
         return (H is None and torch.is_grad_enabled() and not X.requires_grad and self.out_channels == 32 and self.in_channels <= 4
                 and self.in_channels * periods <= 128 and self.fused_training)
 
+    def _cell_train_ok(self, X, H):
+        """The steps after the first of a training loop that carries the state (the reference's BatchedTGCN, tgcn_example.py): the
+        same forward launch with H + the hand-written cell backward (dH and the folded-weight gradients).  No gradient w.r.t. X,
+        out_channels == 32, in_channels <= 4, H of shape X.shape[:-1] + (32,)."""
+        return (H is not None and torch.is_grad_enabled() and not X.requires_grad and self.out_channels == 32 and self.in_channels <= 4
+                and tuple(H.shape) == tuple(X.shape[:-1]) + (32,) and self.fused_training)
+
     fused_training = True     # False: train through autograd over SpMM + cuBLAS (tests compare the two)
 
     def _no_grad_needed(self, X, H, *extra):
@@ -142,6 +149,11 @@ class TGCN(torch.nn.Module):
             A, Bm, c = self._fold3()
             N, Ci = X.shape[-2], X.shape[-1]
             out = ops.tgcn_attn_train(plan, X.reshape(-1, N, Ci, 1), A, Bm, c, None)
+            return out.reshape(*X.shape[:-1], self.out_channels)
+        if self._cell_train_ok(X, H):
+            A, Bm, c = self._fold3()
+            N, Ci = X.shape[-2], X.shape[-1]
+            out = ops.tgcn_cell_train(plan, X.reshape(-1, N, Ci, 1), H.reshape(-1, N, 32), A, Bm, c)
             return out.reshape(*X.shape[:-1], self.out_channels)
         if H is None:
             H = torch.zeros(*X.shape[:-1], self.out_channels, device=X.device, dtype=X.dtype)

@@ -227,6 +227,46 @@ def tgcn_attn_train(plan: GraphPlan, x, A, Bm, c, probs=None) -> torch.Tensor:
     return _TgcnAttnFn.apply(plan, x, A, Bm, c, probs)
 
 
+class _TgcnCellFn(torch.autograd.Function):
+    """Training form of one TGCN / TGCN2 cell step with an incoming state: forward = `stmp_tgcn_attn_fwd` (periods = 1, H given; the
+    same launch as inference, so the output is bit-identical to it), backward = `stmp_tgcn_cell_bwd` (gates recomputed; dH and the
+    gradients of the folded weights A, Bm, c).  No gradient w.r.t. X."""
+
+    @staticmethod
+    def forward(ctx, plan, x, h, A, Bm, c):
+        A, Bm, c, h = A.detach(), Bm.detach(), c.detach(), _f32c(h.detach(), "H")
+        out = tgcn_attn_fwd(plan, x, A, Bm, c, None, h)
+        ctx.plan = plan
+        ctx.save_for_backward(x, h, A, Bm, c)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, h, A, Bm, c = ctx.saved_tensors
+        B, N, fin = x.shape[:3]
+        dev = x.device
+        want_dh = ctx.needs_input_grad[2]
+        dh = torch.empty(B, N, 32, dtype=torch.float32, device=dev) if want_dh else None
+        if B == 0:                                  # nothing to launch (empty tensors have NULL data pointers)
+            return None, None, dh, torch.zeros_like(A), torch.zeros_like(Bm), torch.zeros_like(c)
+        dA = torch.empty(fin, 96, dtype=torch.float32, device=dev)
+        dBm = torch.empty(32, 96, dtype=torch.float32, device=dev)
+        dc = torch.empty(96, dtype=torch.float32, device=dev)
+        gout = _f32c(gout, "gout")
+        handle = ctx.plan.handle
+        ws = torch.empty(int(_lib.lib().stmp_tgcn_cell_bwd_workspace_bytes(handle, B)), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().stmp_tgcn_cell_bwd(handle, B, fin, _lib.ptr(_f32c(x, "X")), _lib.ptr(h), N * 32, _lib.ptr(A),
+                                                     _lib.ptr(Bm), _lib.ptr(c), _lib.ptr(gout), _lib.ptr(ws), _lib.ptr(dh), _lib.ptr(dA),
+                                                     _lib.ptr(dBm), _lib.ptr(dc), _lib.stream_ptr()))
+        return None, None, dh, dA, dBm, dc
+
+
+def tgcn_cell_train(plan: GraphPlan, x, h, A, Bm, c) -> torch.Tensor:
+    """Differentiable (w.r.t. h, A, Bm, c) fused TGCN(2) cell step with an incoming state.  x (B,N,Fin,1), h (B,N,32) -> (B,N,32)."""
+    return _TgcnCellFn.apply(plan, x, h, A, Bm, c)
+
+
 def spmm_cols(plan: GraphPlan, op: int, buf: torch.Tensor, src_col: int, dst_col: int, width: int, alpha: float = 1.0,
               z_col: Optional[int] = None, beta: float = 0.0, transposed: bool = False):
     """In-place column-block product inside one basis buffer `buf` (..., N, LD):

@@ -9,7 +9,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from pytorch_geometric_temporal_b200 import _lib, ops                                        # noqa: E402
 from pytorch_geometric_temporal_b200.dataset import synthetic                               # noqa: E402
 from pytorch_geometric_temporal_b200.nn.attention import ASTGCN                              # noqa: E402
-from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, GConvGRU, GConvLSTM   # noqa: E402
+from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, GConvGRU, GConvLSTM, TGCN2   # noqa: E402
 
 dev = torch.device("cuda")
 torch.manual_seed(0)
@@ -42,6 +42,10 @@ with torch.no_grad():
        torch.randn(4, 325, 32, device=dev))                      # k_tgcn_attn (TMA-staged X)
 with torch.enable_grad():
     a3(torch.randn(4, 325, 2, 12, device=dev), torch.from_numpy(e3).to(dev), torch.from_numpy(w3).to(dev)).square().mean().backward()   # k_tgcn_attn_bwd
+    t2, h = TGCN2(4, 32, 3).to(dev), None
+    for t in range(3):                                           # TGCN2 training with the state carried: step 0 k_tgcn_attn_bwd,
+        h = t2(torch.randn(3, 207, 4, device=dev), ei_t, ew_t, h)   # then k_tgcn_cell_bwd (TMA-staged X, staged Bm) + its reduce
+    h.square().mean().backward()
 with torch.no_grad():
     e4 = torch.from_numpy(synthetic.pems04_like(0)).to(dev)
     ASTGCN(2, 1, 3, 64, 64, 1, 12, 12, 307, normalization="sym").to(dev)(torch.randn(2, 307, 1, 12, device=dev), e4)   # k_gemm_blocks x7
