@@ -316,8 +316,12 @@ int stmp_gru_bwd_zr(int64_t B, int64_t N, int64_t cin, int64_t cout, int64_t du_
 
 /* ---- K4: dense node-feature x weight contraction on the tensor cores (wgmma), fp32 in / fp32 out ------------------
  * C[M,N] = A[M,K] @ W[K,N] + bias.  Replaces `torch.matmul(Tx_k, weight[..][k])` / ChebConv `lins[k](Tx_k)` / GCNConv
- * `lin(x)` (dcrnn.py:81-105; PyG) for the large-graph (tiled) path.  fp32-class accuracy: operands are split into fp16
- * hi/lo halves and multiplied in three wgmma passes with fp32 register accumulators.
+ * `lin(x)` (dcrnn.py:81-105; PyG) for the large-graph (tiled) path.  Operands are split into fp16 hi = fp16(v), lo = fp16(v - hi)
+ * and multiplied in three wgmma passes (lo*hi + hi*lo + hi*hi) with fp32 register accumulators.  Accuracy envelope (also of
+ * stmp_gemm_blocks_f32): |C - A W| <= ~8 (2^-22 (|A||W|)_mn + 2^-25 (sum_k |A_mk| + sum_k |W_kn|)),
+ * i.e. fp32-class relative accuracy only while |operands| lie between about 2^-3 and 2^15; below that an absolute floor of about
+ * 2^-25 per operand element (elements under 3e-8 become zero).  Callers must keep |operands| < 65504 (larger overflow the hi half
+ * to inf) and prescale small operands such as gradients by an exact power of two (see nn/recurrent/gconv_lstm.py::_split_prescale).
  *   stmp_gemm_packed_elems(K,N): number of fp16 elements of the packed weight buffer
  *   stmp_gemm_prepack: W [K,N] row-major (row stride ldw) -> packed (hi/lo, K-major, K padded to 64); once per weight update
  *   stmp_gemm_f32: A row-major (row stride lda), C row-major (ldc); needs N <= 256, N % 32 == 0, K % 4 == 0, 16-byte aligned

@@ -24,13 +24,26 @@ def _chunked_tn(A: torch.Tensor, B: torch.Tensor) -> torch.Tensor:
     return torch.bmm(A.view(chunks, per, -1).transpose(1, 2), B.view(chunks, per, -1)).sum(0)
 
 
+def _split_prescale(g: torch.Tensor):
+    """(s, 1/s): exact powers of two, as 0-dim device tensors, that put max|g| in [2^13, 2^14).
+
+    The wgmma GEMM splits its A operand into fp16 hi = fp16(v), lo = fp16(v - hi); both halves are normal only for |v| between
+    about 2^-3 and 2^15, and below 3e-8 both round to zero.  Gradients of a mean loss are 1e-6 .. 1e-10, so they are scaled into
+    the top of fp16's range first.  Computed on the device (no host sync, capturable in a CUDA graph) from the exponent of the
+    maximum, so s * g and the result times 1/s are exact, and a loss scaled by 2^e gives gradients scaled by exactly 2^e.
+    An all-zero g gives s = 2^14; inf / NaN propagate through the products."""
+    ex = torch.frexp(torch.linalg.vector_norm(g, float("inf"))).exponent      # max|g| = m * 2^ex, m in [0.5, 1)
+    e = (14 - ex).clamp_(-126, 126)                                           # s and 1/s stay normal fp32
+    return ((e + 127) << 23).view(torch.float32), ((127 - e) << 23).view(torch.float32)
+
+
 class _LstmCellFn(torch.autograd.Function):
     """Training path of one GConvLSTM step on a large graph (gconv_lstm.py:204-238) with a hand-written backward.
 
     forward : Chebyshev basis S = [T_0|..|T_{K-1}]([X|H]) built in place by `stmp_spmm`, then ONE wgmma launch computes S @ W and
               the whole peephole gate chain in its epilogue (`stmp_gemm_lstm_f32`).  Only S, C_{t-1}, C_t are kept.
     backward: pre = S @ W recomputed on wgmma -> `stmp_lstm_gate_bwd` (gate derivatives) -> dS = dpre @ W^T (wgmma, two column
-              halves) -> adjoint of the Chebyshev recurrence by TRANSPOSED SpMMs in place -> dX, dH;  dW = S^T dpre as a chunked
+              halves, dpre prescaled by a power of two into the fp16 split's range, see `_split_prescale`) -> adjoint of the Chebyshev recurrence by TRANSPOSED SpMMs in place -> dX, dH;  dW = S^T dpre as a chunked
               GEMM; peephole / bias gradients as column reductions.  ~14 launches instead of the ~90 autograd records."""
 
     @staticmethod
@@ -64,8 +77,10 @@ class _LstmCellFn(torch.autograd.Function):
         dS = torch.empty_like(S)
         dS2 = dS.view(rows, KCw)
         half = KCw // 2
+        s, inv_s = _split_prescale(dpre)
+        dpre_s = dpre * s
         for j in range(2):                                                                 # dS = dpre @ W^T, N split in two (N <= 256)
-            ops.gemm(dpre, ctx.packedT[j], 4 * Co, half, None, out=dS2[:, j * half:(j + 1) * half])
+            ops.gemm(dpre_s, ctx.packedT[j], 4 * Co, half, None, out=dS2[:, j * half:(j + 1) * half])
         dW = _chunked_tn(S2, dpre) if ctx.needs_input_grad[3] else None
         colsum = dpre.sum(0)
         dcb = colsum if ctx.has_cb else None
@@ -80,6 +95,7 @@ class _LstmCellFn(torch.autograd.Function):
             dS[..., (k - 2) * Cw:(k - 1) * Cw].sub_(dS[..., k * Cw:(k + 1) * Cw])
         if K > 1:
             ops.spmm_cols(plan, 0, dS, Cw, 0, Cw, z_col=0, beta=1.0, transposed=True)
+        dS[..., :Cw].mul_(inv_s)                                                           # the adjoint is linear: undo the prescale on dX | dH only
         dX = dS[..., :Ci] if ctx.needs_input_grad[0] else None
         dH = dS[..., Ci:Cw] if ctx.needs_input_grad[1] else None
         return (dX, dH, dC.view_as(C), dW, dcb, dwci, dwcf, dwco, dbi, dbf, dbc, dbo, None, None, None, None)

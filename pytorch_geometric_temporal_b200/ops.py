@@ -300,7 +300,8 @@ def gemm_prepack(W: torch.Tensor) -> torch.Tensor:
 
 def gemm(A: torch.Tensor, packed: torch.Tensor, K: int, N: int, bias: Optional[torch.Tensor] = None,
          out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """C = A @ W + bias on wgmma with the fp16 hi/lo operand split (fp32-class accuracy).  A (..., K) contiguous.
+    """C = A @ W + bias on wgmma with the fp16 hi/lo operand split: fp32-class accuracy for |operands| between about 2^-3 and 2^15,
+    an absolute floor of about 2^-25 per operand element below that (include/stmp.h, K4).  A (..., K) contiguous.
     `out`: a 2-D (M, N) view with unit column stride (e.g. a column block of a wider buffer) to write into."""
     A = _f32c(A, "A")
     M = A.numel() // K
