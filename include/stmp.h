@@ -228,6 +228,35 @@ int stmp_dcrnn_bwd_seq(const stmp_plan* plan, int64_t B, int64_t T, int64_t cin,
                        const float* out, const float* h0, const float* stash, const float* whsT, const float* wzrT,
                        float* dph_all, float* dpzr_all, float* dx, float* dh0, void* stream);
 
+/* ---- backward of the generic graph-GRU recurrence (the twin of stmp_gru_seq_fwd: what autograd records for gconv_gru.py:119-139, and
+ * for the DCRNN cell on any n_ops <= 2 operators of `plan`), graphs that fit one SM -- the kernels of stmp_dcrnn_bwd_* for n_ops operators:
+ * the basis of U = [X | H] is [U | Op0 U | .. | Op_{n_ops-1} U] (width (n_ops+1)(cin+32)), its adjoint dU = dS_0 + sum_op Op^T dS_{1+op}
+ * (the plan's transposed CSRs).  Envelope: cout = 32, cin 1..4, n_ops <= plan's operators, graph and per-window buffers fit one SM's shared
+ * memory (stmp_gru_bwd_supported).  B windows x T steps; x, out (B,T,N,32) and stash (B,T,3,N,32) are those of the forward
+ * (stmp_gru_seq_fwd with a stash); h0 (B,N,32) dense (h0_bstride = N*32) or NULL (zeros).  A shared h0 (h0_bstride = 0) returns
+ * STMP_EUNSUPPORTED.  Deterministic: no atomics, fixed reduction order.
+ *   stmp_gru_pack_bwd_weights: the transposed stacked weights of the backward GEMMs from the forward's wcat [96][112], basis order
+ *                              [X | H] per block: whsT (32, (n_ops+1)(cin+32)) from the h rows, wzrT (64, ..) from the z | r rows.  One launch.
+ *   stmp_gru_bwd_basis:        S1[t*B+b] = basis of [X_t | H_{t-1}], S2 = basis of [X_t | H_{t-1} * R_t], row pitch
+ *                              ld = (n_ops+1)(cin+32) rounded up to 8.  One launch.
+ *   stmp_gru_bwd_seq:          the reverse-time recurrence, one CTA (or a 2-CTA cluster) per window: gout = dL/dout (B,T,N,32) ->
+ *                              dph_all (T,B,N,32), dpzr_all (T,B,N,64), dx (B,T,N,cin; nullable), dh0 (B,N,32).  One launch.
+ *   stmp_gru_bwd_wgrad:        dwcat [96][112] in wcat's layout (columns of absent operators / channels and the padding zero) and dbcat [96]
+ *                              (nullable) over all T*B*N = rows rows: TF32 wgmma per-CTA partials + a fixed-order sum (two launches);
+ *                              workspace of stmp_gru_bwd_wgrad_workspace_bytes(n_ops, cin) bytes.
+ * STMP_EINVAL for NULL tensors, STMP_ESHAPE for bad sizes, pitches or alignment, STMP_EUNSUPPORTED outside the envelope. */
+int stmp_gru_bwd_supported(const stmp_plan* plan, int n_ops, int64_t cin, int64_t cout);
+int stmp_gru_pack_bwd_weights(int n_ops, int64_t cin, const float* wcat, float* whsT, float* wzrT, void* stream);
+int stmp_gru_bwd_basis(const stmp_plan* plan, int n_ops, int64_t B, int64_t T, int64_t cin, const float* x, int64_t x_bstride,
+                       int64_t x_tstride, const float* out, const float* h0, int64_t h0_bstride, const float* stash, float* S1,
+                       float* S2, int64_t ld, void* stream);
+int stmp_gru_bwd_seq(const stmp_plan* plan, int n_ops, int64_t B, int64_t T, int64_t cin, const float* gout, const float* out,
+                     const float* h0, int64_t h0_bstride, const float* stash, const float* whsT, const float* wzrT, float* dph_all,
+                     float* dpzr_all, float* dx, float* dh0, void* stream);
+int64_t stmp_gru_bwd_wgrad_workspace_bytes(int n_ops, int64_t cin);
+int stmp_gru_bwd_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
+                       const float* dph, void* workspace, float* dwcat, float* dbcat, void* stream);
+
 /* ---- backward of the fused DCRNN sequence for narrow states (cout <= 4): the reference's training model BatchedDCRNN(F, F, K=3) ----
  * Served when stmp_dcrnn_narrow_bwd_supported(plan, cin, cout, K) != 0 (DCONV plan, cin and cout in 1..4, K in 1..4, graph and state
  * buffers fit one SM's shared memory: PEMS-BAY's 325 nodes at K = 3 do).  stmp_dcrnn_narrow_bwd_seq is the reverse-time recurrence in

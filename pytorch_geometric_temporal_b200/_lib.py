@@ -63,7 +63,13 @@ _SIGNATURES = {
     "stmp_dcrnn_narrow_bwd_supported": (c_int, [_P, c_int64, c_int64, c_int64]),
     "stmp_dcrnn_narrow_bwd_seq": (c_int, [_P] + [c_int64] * 5 + [_P] * 11),
     "stmp_dcrnn_pack_bwd_weights": (c_int, [c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, _P]),
-    "stmp_tgcn_attn_bwd_workspace_bytes": (c_int64, [_P, c_int64]),
+    "stmp_gru_bwd_supported": (c_int, [_P, c_int, c_int64, c_int64]),
+    "stmp_gru_pack_bwd_weights": (c_int, [c_int, c_int64, _P, _P, _P, _P]),
+    "stmp_gru_bwd_basis": (c_int, [_P, c_int, c_int64, c_int64, c_int64, _P, c_int64, c_int64, _P, _P, c_int64, _P, _P, _P, c_int64, _P]),
+    "stmp_gru_bwd_seq": (c_int, [_P, c_int, c_int64, c_int64, c_int64, _P, _P, _P, c_int64] + [_P] * 8),
+    "stmp_gru_bwd_wgrad_workspace_bytes": (c_int64, [c_int, c_int64]),
+    "stmp_gru_bwd_wgrad": (c_int, [c_int, c_int64, c_int64, c_int64] + [_P] * 8),
+    "stmp_tgcn_attn_bwd_workspace_bytes":(c_int64, [_P, c_int64]),
     "stmp_tgcn_attn_bwd": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "stmp_tgcn_cell_bwd_workspace_bytes": (c_int64, [_P, c_int64]),
     "stmp_tgcn_cell_bwd": (c_int, [_P, c_int64, c_int64, _P, _P, c_int64] + [_P] * 10),

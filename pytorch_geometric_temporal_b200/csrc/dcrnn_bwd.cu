@@ -25,7 +25,8 @@ constexpr int kCo = 32;          // hidden size served by these kernels
 constexpr int kBwdThreads = 512;
 constexpr int kBatch = 4;        // vector slots per thread whose global operands are fetched together (latency paid once)
 
-__host__ __device__ constexpr int ncol_of(int cin) { return (3 * (cin + kCo) + 7) / 8 * 8; }
+// basis width [U | Op_0 U | .. | Op_{nops-1} U], U = [X | H], rounded up to whole 8-column groups
+__host__ __device__ constexpr int ncol_of(int cin, int nops = 2) { return ((nops + 1) * (cin + kCo) + 7) / 8 * 8; }
 
 // ---- 1- or 2-float vector access (rows have C = cin + 32 channels; C even -> float2 slots halve the instruction count)
 template <int V> __device__ __forceinline__ void ldv(const float* p, float (&v)[V]);
@@ -62,7 +63,7 @@ struct BasisParams {
   float* S1; float* S2;                     // (T*B, N, ld), ld >= 3*(cin+Co)
 };
 
-template <int CIN>
+template <int CIN, int NOPS>
 __global__ void __launch_bounds__(256) k_dcrnn_bwd_basis(BasisParams p) {
   constexpr int C = CIN + kCo, V = (C % 2 == 0) ? 2 : 1, CP = C / V;
   extern __shared__ __align__(16) float sm[];
@@ -107,7 +108,7 @@ __global__ void __launch_bounds__(256) k_dcrnn_bwd_basis(BasisParams p) {
   }
   __syncthreads();
 #pragma unroll
-  for (int op = 0; op < 2; ++op) {
+  for (int op = 0; op < NOPS; ++op) {
     const Gr<false> g{p.rp[op], p.cv[op]};
     for (int s = threadIdx.x; s < NP; s += 256) {
       const int n = s / CP, c0 = (s - n * CP) * V;
@@ -196,12 +197,12 @@ __device__ __forceinline__ void gemm_tiles(const float* __restrict__ dpT, int dp
   }
 }
 
-// dU[n][c..c+V) = dS[n][c..] + sum_op sum_{edges of row n of A_op^T} val * dS[col][(1+op)*C + c..]   (adjoint of U -> [U|P_oU|P_iU])
-template <int NCOL, int C, int V, bool SG>
-__device__ __forceinline__ void adjoint_at(const Gr<SG> (&g)[2], const float* __restrict__ buf, int n, int c, float (&v)[V]) {
+// dU[n][c..c+V) = dS[n][c..] + sum_op sum_{edges of row n of A_op^T} val * dS[col][(1+op)*C + c..]   (adjoint of U -> [U|Op_0 U|..])
+template <int NOPS, int NCOL, int C, int V, bool SG, int NG>
+__device__ __forceinline__ void adjoint_at(const Gr<SG> (&g)[NG], const float* __restrict__ buf, int n, int c, float (&v)[V]) {
   ldv<V>(buf + n * NCOL + c, v);
 #pragma unroll
-  for (int op = 0; op < 2; ++op) {
+  for (int op = 0; op < NOPS; ++op) {
     const int k1 = g[op].end(n);
     const float* src = buf + (1 + op) * C + c;
 #pragma unroll 4
@@ -221,9 +222,10 @@ __device__ __forceinline__ void adjoint_at(const Gr<SG> (&g)[2], const float* __
 // pushes its rows of dS into the partner's buf so that the adjoint gathers stay local.  Behind a GEMM the pair meets at a release / acquire
 // cluster barrier (dS visible); behind a gather phase each CTA only signals "done reading buf" (relaxed arrival) and the matching wait sits
 // in the next GEMM between its FFMA loop and its stores.
-template <int CIN, bool SG, int SPLIT>
+// NOPS: operators of the basis (2: DCRNN's P_o, P_i; 1: a Chebyshev K = 2 / GCN operator; 0: none).
+template <int CIN, bool SG, int SPLIT, int NOPS>
 __global__ void __launch_bounds__(kBwdThreads, 1) k_dcrnn_bwd_seq(BwdParams p) {
-  constexpr int C = CIN + kCo, NCOL = ncol_of(CIN), V = (C % 2 == 0) ? 2 : 1, CP = C / V, RT = SPLIT == 2 ? 4 : 8;
+  constexpr int C = CIN + kCo, NB = NOPS + 1, NCOL = ncol_of(CIN, NOPS), V = (C % 2 == 0) ? 2 : 1, CP = C / V, RT = SPLIT == 2 ? 4 : 8;
   extern __shared__ __align__(16) float sm[];
   const int N = p.N, T = p.T, b = blockIdx.x / SPLIT, tid = threadIdx.x;
   const int RG = (N + 7) / 8, dpp = RG * 8 + 4, NH = N * kCo;
@@ -240,13 +242,13 @@ __global__ void __launch_bounds__(kBwdThreads, 1) k_dcrnn_bwd_seq(BwdParams p) {
   float* dpT = buf + RG * 8 * NCOL;          // [2Co][dpp]  d pre-activations, k-major (transposed)
   float* G = dpT + 2 * kCo * dpp;            // [N][Co]     dL/dH_t (open) -> partial dL/dH_{t-1}
   float* dXp = G + N * kCo;                  // [N][4]      dU2[:, :cin] waiting for dU1
-  Gr<SG> g[2];
-  if constexpr (SG) {                        // compressed copy of both transposed operators: val f32 | col u8 | rowptr u16
+  Gr<SG> g[NOPS > 0 ? NOPS : 1];
+  if constexpr (SG) {                        // compressed copy of the transposed operators: val f32 | col u8 | rowptr u16 (nnz of absent ones = 0)
     float* gval = dXp + N * 4;
     unsigned char* gcol = reinterpret_cast<unsigned char*>(gval + p.nnz[0] + p.nnz[1]);
     unsigned short* grp = reinterpret_cast<unsigned short*>(gcol + ((p.nnz[0] + p.nnz[1] + 3) & ~3));
 #pragma unroll
-    for (int op = 0; op < 2; ++op) {
+    for (int op = 0; op < NOPS; ++op) {
       float* val = gval + (op ? p.nnz[0] : 0);
       unsigned char* col = gcol + (op ? p.nnz[0] : 0);
       unsigned short* rp = grp + op * (N + 1);
@@ -256,13 +258,13 @@ __global__ void __launch_bounds__(kBwdThreads, 1) k_dcrnn_bwd_seq(BwdParams p) {
     }
   } else {
 #pragma unroll
-    for (int op = 0; op < 2; ++op) { g[op].rp = p.rp[op]; g[op].cv = p.cv[op]; }
+    for (int op = 0; op < NOPS; ++op) { g[op].rp = p.rp[op]; g[op].cv = p.cv[op]; }
   }
   // ---- weights, zero padded to NCOL columns; padded rows of dpT stay zero for the whole kernel
   for (int i = tid; i < 3 * kCo * NCOL; i += kBwdThreads) {
     const int r = i / NCOL, c = i - r * NCOL;
     float v = 0.f;
-    if (c < 3 * C) v = r < kCo ? __ldg(p.whsT + r * 3 * C + c) : __ldg(p.wzrT + (r - kCo) * 3 * C + c);
+    if (c < NB * C) v = r < kCo ? __ldg(p.whsT + r * NB * C + c) : __ldg(p.wzrT + (r - kCo) * NB * C + c);
     sm[i] = v;
   }
   for (int i = tid; i < 2 * kCo * dpp; i += kBwdThreads) dpT[i] = 0.f;
@@ -335,7 +337,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) k_dcrnn_bwd_seq(BwdParams p) {
         if (s < NP) {
           const int n = s / CP, c0 = (s - n * CP) * V;
           float v[V];
-          adjoint_at<NCOL, C, V, SG>(g, buf, n, c0, v);
+          adjoint_at<NOPS, NCOL, C, V, SG>(g, buf, n, c0, v);
           if (c0 < CIN) {
 #pragma unroll
             for (int e = 0; e < V; ++e) dXp[n * 4 + c0 + e] = v[e];
@@ -383,7 +385,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) k_dcrnn_bwd_seq(BwdParams p) {
         if (s < NP) {
           const int n = s / CP, c0 = (s - n * CP) * V;
           float v[V];
-          adjoint_at<NCOL, C, V, SG>(g, buf, n, c0, v);
+          adjoint_at<NOPS, NCOL, C, V, SG>(g, buf, n, c0, v);
           if (c0 < CIN) {
             if (p.dx) {
 #pragma unroll
@@ -416,49 +418,137 @@ __global__ void __launch_bounds__(kBwdThreads, 1) k_dcrnn_bwd_seq(BwdParams p) {
   if constexpr (SPLIT == 2) cluster_wait();      // pairs with the last arrival; nobody leaves while the partner may still be in its phase
 }
 
-inline size_t seq_smem_base(int N, int cin) {
-  const int ncol = ncol_of(cin), rg = (N + 7) / 8;
+inline size_t seq_smem_base(int N, int cin, int nops = 2) {
+  const int ncol = ncol_of(cin, nops), rg = (N + 7) / 8;
   return sizeof(float) * ((size_t)3 * kCo * ncol + (size_t)rg * 8 * ncol + (size_t)2 * kCo * (rg * 8 + 4) + (size_t)N * (kCo + 4));
 }
-inline size_t seq_smem_graph(const stmp_plan* plan) {
-  const size_t nnz = (size_t)plan->bwd[0].nnz + plan->bwd[1].nnz;
-  return 4 * nnz + ((nnz + 3) & ~(size_t)3) + 2 * 2 * ((size_t)plan->n + 1) + 8;
+inline size_t seq_smem_graph(const stmp_plan* plan, int nops = 2) {
+  size_t nnz = 0;
+  for (int op = 0; op < nops; ++op) nnz += (size_t)plan->bwd[op].nnz;
+  return 4 * nnz + ((nnz + 3) & ~(size_t)3) + 2 * (size_t)nops * ((size_t)plan->n + 1) + 8;
 }
-inline bool graph_in_smem(const stmp_plan* plan, int cin) {
-  return plan->n <= 256 && plan->bwd[0].nnz < 65536 && plan->bwd[1].nnz < 65536 &&
-         seq_smem_base(plan->n, cin) + seq_smem_graph(plan) <= 227 * 1024;
+inline bool graph_in_smem(const stmp_plan* plan, int cin, int nops = 2) {
+  if (nops == 0) return false;                   // nothing to stage
+  for (int op = 0; op < nops; ++op)
+    if (plan->bwd[op].nnz >= 65536) return false;
+  return plan->n <= 256 && seq_smem_base(plan->n, cin, nops) + seq_smem_graph(plan, nops) <= 227 * 1024;
+}
+// the graph fits one SM: the GEMM tiles fit the block, the per-window buffers its shared memory, the basis kernel's [X|H] copies 100 KB
+inline bool fits_one_sm(const stmp_plan* plan, long long cin, int nops) {
+  return ((plan->n + 7) / 8) * (ncol_of((int)cin, nops) / 8) <= kBwdThreads && seq_smem_base(plan->n, (int)cin, nops) <= 227 * 1024 &&
+         2 * sizeof(float) * (size_t)plan->n * (cin + kCo) <= 100 * 1024;
 }
 inline bool bwd_supported(const stmp_plan* plan, long long cin, long long cout, long long K) {
   if (!plan || plan->flavor != STMP_FLAVOR_DCONV || plan->n_ops != 2) return false;
   if (K != 2 || cout != kCo || cin < 1 || cin > 4) return false;
   // cin == 2 (float2 slots, 104 columns) is the benchmark configuration; cin 1, 3, 4 (scalar slots / 112 columns) are served too
   // (tests/test_gpu_dcrnn.py::test_training_persistent_backward_other_channel_counts).
-  return ((plan->n + 7) / 8) * (ncol_of((int)cin) / 8) <= kBwdThreads && seq_smem_base(plan->n, (int)cin) <= 227 * 1024 &&
-         2 * sizeof(float) * (size_t)plan->n * (cin + kCo) <= 100 * 1024;
+  return fits_one_sm(plan, cin, 2);
+}
+inline bool gru_bwd_supported(const stmp_plan* plan, long long n_ops, long long cin, long long cout) {
+  if (!plan || n_ops < 0 || n_ops > 2 || n_ops > plan->n_ops) return false;
+  if (cout != kCo || cin < 1 || cin > 4) return false;
+  return fits_one_sm(plan, cin, (int)n_ops);
 }
 
-template <int CIN>
+template <int CIN, int NOPS>
 int launch_basis(const BasisParams& p, size_t smem, cudaStream_t st) {
-  STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_bwd_basis<CIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_dcrnn_bwd_basis<CIN><<<(unsigned)(p.B * p.T), 256, smem, st>>>(p);
+  STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_bwd_basis<CIN, NOPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_dcrnn_bwd_basis<CIN, NOPS><<<(unsigned)(p.B * p.T), 256, smem, st>>>(p);
   return STMP_OK;
 }
-template <int CIN, bool SG>
+template <int NOPS>
+int dispatch_basis(const BasisParams& p, int cin, size_t smem, cudaStream_t st) {
+  switch (cin) {
+    case 1: return launch_basis<1, NOPS>(p, smem, st);
+    case 2: return launch_basis<2, NOPS>(p, smem, st);
+    case 3: return launch_basis<3, NOPS>(p, smem, st);
+    default: return launch_basis<4, NOPS>(p, smem, st);
+  }
+}
+template <int CIN, bool SG, int NOPS>
 int launch_seq(const BwdParams& p, size_t smem, int split, cudaStream_t st) {
   if (split == 2) {
-    STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_bwd_seq<CIN, SG, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_bwd_seq<CIN, SG, 2, NOPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)p.B * 2); cfg.blockDim = dim3(kBwdThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeClusterDimension;
     at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-    STMP_CUDA_OK(cudaLaunchKernelEx(&cfg, k_dcrnn_bwd_seq<CIN, SG, 2>, p));
+    STMP_CUDA_OK(cudaLaunchKernelEx(&cfg, k_dcrnn_bwd_seq<CIN, SG, 2, NOPS>, p));
     return STMP_OK;
   }
-  STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_bwd_seq<CIN, SG, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_dcrnn_bwd_seq<CIN, SG, 1><<<(unsigned)p.B, kBwdThreads, smem, st>>>(p);
+  STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_bwd_seq<CIN, SG, 1, NOPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_dcrnn_bwd_seq<CIN, SG, 1, NOPS><<<(unsigned)p.B, kBwdThreads, smem, st>>>(p);
   return STMP_OK;
+}
+template <int CIN, int NOPS>
+int launch_seq_sg(const BwdParams& p, bool sg, size_t smem, int split, cudaStream_t st) {
+  if constexpr (NOPS > 0) {
+    if (sg) return launch_seq<CIN, true, NOPS>(p, smem, split, st);
+  }
+  return launch_seq<CIN, false, NOPS>(p, smem, split, st);
+}
+template <int NOPS>
+int dispatch_seq(const BwdParams& p, int cin, bool sg, size_t smem, int split, cudaStream_t st) {
+  switch (cin) {
+    case 1: return launch_seq_sg<1, NOPS>(p, sg, smem, split, st);
+    case 2: return launch_seq_sg<2, NOPS>(p, sg, smem, split, st);
+    case 3: return launch_seq_sg<3, NOPS>(p, sg, smem, split, st);
+    default: return launch_seq_sg<4, NOPS>(p, sg, smem, split, st);
+  }
+}
+
+// Splits the prepacked forward weights wcat [96][112] (columns H | Op0 H | Op1 H | X | Op0 X | Op1 X | pad) into the transposed stacked weights
+// of the backward GEMMs in basis order [X | H] per block: whsT (32, NB C) from the candidate rows, wzrT (64, NB C) from the z | r rows.
+__global__ void k_gru_pack_bwd_weights(int cin, int nb, const float* __restrict__ wcat, float* __restrict__ whsT, float* __restrict__ wzrT) {
+  const int C = cin + kCo, W = nb * C;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 3 * kCo * W) return;
+  const int r = i / W, m = i - r * W, blk = m / C, c = m - blk * C;
+  const int col = c < cin ? 96 + 4 * blk + c : 32 * blk + (c - cin);
+  if (r < kCo) whsT[r * W + m] = wcat[(2 * kCo + r) * 112 + col];
+  else wzrT[(r - kCo) * W + m] = wcat[(r - kCo) * 112 + col];
+}
+
+int basis_impl(const stmp_plan* plan, int nops, int64_t B, int64_t T, int64_t cin, const float* x, int64_t x_bstride, int64_t x_tstride,
+               const float* out, const float* h0, const float* stash, float* S1, float* S2, int64_t ld, cudaStream_t st) {
+  BasisParams p;
+  for (int o = 0; o < 2; ++o) { p.rp[o] = o < nops ? plan->fwd[o].rowptr : nullptr; p.cv[o] = o < nops ? plan->fwd[o].cv : nullptr; }
+  p.N = plan->n; p.B = (int)B; p.T = (int)T; p.ld = (int)ld;
+  p.x = x; p.x_bs = x_bstride; p.x_ts = x_tstride; p.out = out; p.h0 = h0; p.stash = stash; p.S1 = S1; p.S2 = S2;
+  const size_t smem = sizeof(float) * 2 * (size_t)plan->n * (cin + kCo);
+  switch (nops) {
+    case 0: return dispatch_basis<0>(p, (int)cin, smem, st);
+    case 1: return dispatch_basis<1>(p, (int)cin, smem, st);
+    default: return dispatch_basis<2>(p, (int)cin, smem, st);
+  }
+}
+
+int seq_impl(const stmp_plan* plan, int nops, int64_t B, int64_t T, int64_t cin, const float* gout, const float* out, const float* h0,
+             const float* stash, const float* whsT, const float* wzrT, float* dph_all, float* dpzr_all, float* dx, float* dh0, cudaStream_t st,
+             int* split_out) {
+  BwdParams p;
+  for (int o = 0; o < 2; ++o) {
+    const bool on = o < nops;
+    p.rp[o] = on ? plan->bwd[o].rowptr : nullptr; p.cv[o] = on ? plan->bwd[o].cv : nullptr; p.nnz[o] = on ? plan->bwd[o].nnz : 0;
+  }
+  p.N = plan->n; p.B = (int)B; p.T = (int)T;
+  p.gout = gout; p.out = out; p.h0 = h0; p.stash = stash; p.whsT = whsT; p.wzrT = wzrT;
+  p.dph_all = dph_all; p.dpzr_all = dpzr_all; p.dx = dx; p.dh0 = dh0;
+  const bool sg = graph_in_smem(plan, (int)cin, nops);
+  const size_t smem = seq_smem_base(plan->n, (int)cin, nops) + (sg ? seq_smem_graph(plan, nops) : 0);
+  int dev = 0, sms = 0;
+  STMP_CUDA_OK(cudaGetDevice(&dev));
+  STMP_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int split = (g_bwd_split && 2 * B <= sms && plan->n >= 16) ? 2 : 1;      // small batches: two CTAs per window (cluster), rows halved
+  *split_out = split;
+  switch (nops) {
+    case 0: return dispatch_seq<0>(p, (int)cin, sg, smem, split, st);
+    case 1: return dispatch_seq<1>(p, (int)cin, sg, smem, split, st);
+    default: return dispatch_seq<2>(p, (int)cin, sg, smem, split, st);
+  }
 }
 
 }  // namespace
@@ -481,19 +571,7 @@ extern "C" int stmp_dcrnn_bwd_basis(const stmp_plan* plan, int64_t B, int64_t T,
   STMP_REQUIRE(!vec2 || (ld % 2 == 0 && x_bstride % 2 == 0 && x_tstride % 2 == 0 && ((uintptr_t)x % 8) == 0 && ((uintptr_t)S1 % 8) == 0 &&
                          ((uintptr_t)S2 % 8) == 0), STMP_ESHAPE, "stmp_dcrnn_bwd_basis: operands must be 8-byte aligned with even strides");
   if (B == 0) return STMP_OK;
-  BasisParams p;
-  for (int o = 0; o < 2; ++o) { p.rp[o] = plan->fwd[o].rowptr; p.cv[o] = plan->fwd[o].cv; }
-  p.N = plan->n; p.B = (int)B; p.T = (int)T; p.ld = (int)ld;
-  p.x = x; p.x_bs = x_bstride; p.x_ts = x_tstride; p.out = out; p.h0 = h0; p.stash = stash; p.S1 = S1; p.S2 = S2;
-  const size_t smem = sizeof(float) * 2 * (size_t)plan->n * (cin + cout);
-  cudaStream_t st = (cudaStream_t)stream;
-  int rc = STMP_OK;
-  switch (cin) {
-    case 1: rc = launch_basis<1>(p, smem, st); break;
-    case 2: rc = launch_basis<2>(p, smem, st); break;
-    case 3: rc = launch_basis<3>(p, smem, st); break;
-    default: rc = launch_basis<4>(p, smem, st); break;
-  }
+  const int rc = basis_impl(plan, 2, B, T, cin, x, x_bstride, x_tstride, out, h0, stash, S1, S2, ld, (cudaStream_t)stream);
   if (rc != STMP_OK) return rc;
   STMP_LAUNCH_OK("k_dcrnn_bwd_basis");
   return STMP_OK;
@@ -510,31 +588,66 @@ extern "C" int stmp_dcrnn_bwd_seq(const stmp_plan* plan, int64_t B, int64_t T, i
   STMP_REQUIRE(al8(gout) && al8(out) && al8(stash) && al8(dph_all) && al8(dpzr_all) && al8(dh0) && (!h0 || al8(h0)), STMP_ESHAPE,
                "stmp_dcrnn_bwd_seq: operands must be 8-byte aligned");
   if (B == 0) return STMP_OK;
-  BwdParams p;
-  for (int o = 0; o < 2; ++o) { p.rp[o] = plan->bwd[o].rowptr; p.cv[o] = plan->bwd[o].cv; p.nnz[o] = plan->bwd[o].nnz; }
-  p.N = plan->n; p.B = (int)B; p.T = (int)T;
-  p.gout = gout; p.out = out; p.h0 = h0; p.stash = stash; p.whsT = whsT; p.wzrT = wzrT;
-  p.dph_all = dph_all; p.dpzr_all = dpzr_all; p.dx = dx; p.dh0 = dh0;
-  const bool sg = graph_in_smem(plan, (int)cin);
-  const size_t smem = seq_smem_base(plan->n, (int)cin) + (sg ? seq_smem_graph(plan) : 0);
-  cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, sms = 0;
-  STMP_CUDA_OK(cudaGetDevice(&dev));
-  STMP_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int split = (g_bwd_split && 2 * B <= sms && plan->n >= 16) ? 2 : 1;      // small batches: two CTAs per window (cluster), rows halved
-  int rc = STMP_OK;
-  switch ((int)cin * 2 + (sg ? 1 : 0)) {
-    case 2: rc = launch_seq<1, false>(p, smem, split, st); break;
-    case 3: rc = launch_seq<1, true>(p, smem, split, st); break;
-    case 4: rc = launch_seq<2, false>(p, smem, split, st); break;
-    case 5: rc = launch_seq<2, true>(p, smem, split, st); break;
-    case 6: rc = launch_seq<3, false>(p, smem, split, st); break;
-    case 7: rc = launch_seq<3, true>(p, smem, split, st); break;
-    case 8: rc = launch_seq<4, false>(p, smem, split, st); break;
-    default: rc = launch_seq<4, true>(p, smem, split, st); break;
-  }
+  int split = 1;
+  const int rc = seq_impl(plan, 2, B, T, cin, gout, out, h0, stash, whsT, wzrT, dph_all, dpzr_all, dx, dh0, (cudaStream_t)stream, &split);
   if (rc != STMP_OK) return rc;
   STMP_LAUNCH_OK("k_dcrnn_bwd_seq");
   if (split == 2) { static const int slot2 = path_slot("k_dcrnn_bwd_seq[cluster2]"); count_path(slot2); }
+  return STMP_OK;
+}
+
+// ---- generic graph-GRU backward (the twin of stmp_gru_seq_fwd): the same kernels with n_ops operators of any plan flavor --------------
+extern "C" int stmp_gru_bwd_supported(const stmp_plan* plan, int n_ops, int64_t cin, int64_t cout) {
+  return gru_bwd_supported(plan, n_ops, cin, cout) ? 1 : 0;
+}
+
+extern "C" int stmp_gru_bwd_basis(const stmp_plan* plan, int n_ops, int64_t B, int64_t T, int64_t cin, const float* x, int64_t x_bstride,
+                                  int64_t x_tstride, const float* out, const float* h0, int64_t h0_bstride, const float* stash, float* S1,
+                                  float* S2, int64_t ld, void* stream) {
+  STMP_REQUIRE(plan != nullptr, STMP_EINVAL, "stmp_gru_bwd_basis: plan is NULL");
+  STMP_REQUIRE(gru_bwd_supported(plan, n_ops, cin, kCo), STMP_EUNSUPPORTED,
+               "stmp_gru_bwd_basis: configuration not served (n_ops <= plan's, cout = 32, cin <= 4, graph fits one SM)");
+  STMP_REQUIRE(!h0 || h0_bstride != 0, STMP_EUNSUPPORTED, "stmp_gru_bwd_basis: a shared h0 (batch stride 0) is not served");
+  STMP_REQUIRE(x && out && stash && S1 && S2, STMP_EINVAL, "stmp_gru_bwd_basis: NULL tensor");
+  const int64_t C = cin + kCo;
+  STMP_REQUIRE(B >= 0 && T > 0 && ld == ncol_of((int)cin, n_ops) && (!h0 || h0_bstride == (int64_t)plan->n * kCo), STMP_ESHAPE,
+               "stmp_gru_bwd_basis: bad sizes (ld must be (n_ops+1)(cin+32) rounded up to 8, h0 (B, N, 32) dense)");
+  STMP_REQUIRE(C % 2 != 0 || (x_bstride % 2 == 0 && x_tstride % 2 == 0 && ((uintptr_t)x % 8) == 0 && ((uintptr_t)S1 % 8) == 0 &&
+                              ((uintptr_t)S2 % 8) == 0), STMP_ESHAPE, "stmp_gru_bwd_basis: operands must be 8-byte aligned with even strides");
+  if (B == 0) return STMP_OK;
+  const int rc = basis_impl(plan, n_ops, B, T, cin, x, x_bstride, x_tstride, out, h0, stash, S1, S2, ld, (cudaStream_t)stream);
+  if (rc != STMP_OK) return rc;
+  STMP_LAUNCH_OK("k_gru_bwd_basis");
+  return STMP_OK;
+}
+
+extern "C" int stmp_gru_bwd_seq(const stmp_plan* plan, int n_ops, int64_t B, int64_t T, int64_t cin, const float* gout, const float* out,
+                                const float* h0, int64_t h0_bstride, const float* stash, const float* whsT, const float* wzrT, float* dph_all,
+                                float* dpzr_all, float* dx, float* dh0, void* stream) {
+  STMP_REQUIRE(plan != nullptr, STMP_EINVAL, "stmp_gru_bwd_seq: plan is NULL");
+  STMP_REQUIRE(gru_bwd_supported(plan, n_ops, cin, kCo), STMP_EUNSUPPORTED,
+               "stmp_gru_bwd_seq: configuration not served (n_ops <= plan's, cout = 32, cin <= 4, graph fits one SM)");
+  STMP_REQUIRE(!h0 || h0_bstride != 0, STMP_EUNSUPPORTED, "stmp_gru_bwd_seq: a shared h0 (batch stride 0) is not served");
+  STMP_REQUIRE(gout && out && stash && whsT && wzrT && dph_all && dpzr_all && dh0, STMP_EINVAL, "stmp_gru_bwd_seq: NULL tensor");
+  STMP_REQUIRE(B >= 0 && T > 0 && (!h0 || h0_bstride == (int64_t)plan->n * kCo), STMP_ESHAPE,
+               "stmp_gru_bwd_seq: bad sizes (h0 must be (B, N, 32) dense)");
+  auto al8 = [](const void* q) { return ((uintptr_t)q % 8) == 0; };
+  STMP_REQUIRE(al8(gout) && al8(out) && al8(stash) && al8(dph_all) && al8(dpzr_all) && al8(dh0) && (!h0 || al8(h0)), STMP_ESHAPE,
+               "stmp_gru_bwd_seq: operands must be 8-byte aligned");
+  if (B == 0) return STMP_OK;
+  int split = 1;
+  const int rc = seq_impl(plan, n_ops, B, T, cin, gout, out, h0, stash, whsT, wzrT, dph_all, dpzr_all, dx, dh0, (cudaStream_t)stream, &split);
+  if (rc != STMP_OK) return rc;
+  STMP_LAUNCH_OK("k_gru_bwd_seq");
+  if (split == 2) { static const int slot2 = path_slot("k_gru_bwd_seq[cluster2]"); count_path(slot2); }
+  return STMP_OK;
+}
+
+extern "C" int stmp_gru_pack_bwd_weights(int n_ops, int64_t cin, const float* wcat, float* whsT, float* wzrT, void* stream) {
+  STMP_REQUIRE(wcat && whsT && wzrT, STMP_EINVAL, "stmp_gru_pack_bwd_weights: NULL tensor");
+  STMP_REQUIRE(n_ops >= 0 && n_ops <= 2 && cin >= 1 && cin <= 4, STMP_EUNSUPPORTED, "stmp_gru_pack_bwd_weights: n_ops <= 2, cin <= 4 only");
+  const int total = 3 * kCo * (n_ops + 1) * (int)(cin + kCo);
+  k_gru_pack_bwd_weights<<<(total + 255) / 256, 256, 0, (cudaStream_t)stream>>>((int)cin, n_ops + 1, wcat, whsT, wzrT);
+  STMP_LAUNCH_OK("k_gru_pack_bwd_weights");
   return STMP_OK;
 }

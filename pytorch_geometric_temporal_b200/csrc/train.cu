@@ -16,7 +16,7 @@
 #include "common.cuh"
 
 namespace stmp {
-int wgrad_tc_launch(int cin, long long rows, int ld, const float* S1, const float* S2, const float* dpzr, const float* dph, float* partial,
+int wgrad_tc_launch(int c3, long long rows, int ld, const float* S1, const float* S2, const float* dpzr, const float* dph, float* partial,
                     int max_parts, cudaStream_t st, int* parts);
 namespace {
 
@@ -170,6 +170,51 @@ __global__ void __launch_bounds__(256) k_dcrnn_wgrad_reduce(int parts, int MG, i
   }
 }
 
+// The same fixed-order sum for the generic graph-GRU (bases [U | Op_0 U | ..] of nb = n_ops + 1 blocks), scattered straight into the layout
+// of the forward's prepacked weights: dwcat [96][112] (row gate*32 + o; columns H | Op0 H | Op1 H | X | Op0 X | Op1 X | pad -- zero for absent
+// operators, absent X channels and the padding) and dbcat [96] (nullable).
+__global__ void __launch_bounds__(256) k_gru_wgrad_reduce(int parts, int MG, int cin, int nb, const float* __restrict__ partial,
+                                                          float* __restrict__ dwcat, float* __restrict__ dbcat) {
+  __shared__ float sub[8][32];
+  const int C = cin + kCo;
+  const int x = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int i = blockIdx.x * 32 + x;
+  const size_t stride = (size_t)MG * 8 * 3 * kCo + 3 * kCo;
+  size_t src = 0;
+  float* dst = nullptr;
+  bool zero = false;
+  if (i < 96 * 112) {
+    const int row = i / 112, col = i - row * 112, gate = row >> 5, o = row & 31;
+    const int blk = col < 96 ? col >> 5 : (col - 96) >> 2, c = col < 96 ? cin + (col & 31) : (col - 96) & 3;
+    dst = dwcat + i;
+    zero = blk >= nb || (col >= 96 && c >= cin);
+    const int m = blk * C + c;                                   // column of the basis
+    src = gate == 2 ? (size_t)MG * 8 * 2 * kCo + (size_t)m * kCo + o : (size_t)m * 2 * kCo + gate * kCo + o;
+  } else if (i < 96 * 112 + 3 * kCo) {
+    const int b = i - 96 * 112;                                  // bias sums are stored z | r | h
+    src = (size_t)MG * 8 * 3 * kCo + b;
+    dst = dbcat ? dbcat + b : nullptr;
+  }
+  const int per = (parts + 7) / 8, q0 = w * per, q1 = (q0 + per < parts) ? q0 + per : parts;
+  float s0 = 0.f, s1 = 0.f;
+  if (dst && !zero) {
+    int q = q0;
+    for (; q + 2 <= q1; q += 2) {
+      s0 += partial[(size_t)q * stride + src];
+      s1 += partial[(size_t)(q + 1) * stride + src];
+    }
+    if (q < q1) s0 += partial[(size_t)q * stride + src];
+  }
+  sub[w][x] = s0 + s1;
+  __syncthreads();
+  if (w == 0 && dst) {
+    float t = sub[0][x];
+#pragma unroll
+    for (int k = 1; k < 8; ++k) t += sub[k][x];
+    *dst = zero ? 0.f : t;
+  }
+}
+
 // ---- Adam over one flat buffer -------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_adam_flat(long long n, float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
                                                    float* __restrict__ v, float* step, unsigned* ticket, float lr, float b1, float b2,
@@ -240,7 +285,7 @@ extern "C" int stmp_dcrnn_bwd_wgrad(int64_t cin, int64_t cout, int64_t K, int64_
   p.partial = reinterpret_cast<float*>(workspace);
   int grid = wgrad_grid();
   if (g_wgrad_tc) {
-    const int rc = wgrad_tc_launch((int)cin, rows, (int)ld, S1, S2, dpzr, dph, p.partial, grid, st, &grid);
+    const int rc = wgrad_tc_launch(3 * (int)(cin + kCo), rows, (int)ld, S1, S2, dpzr, dph, p.partial, grid, st, &grid);
     if (rc != STMP_OK) return rc;
   } else {
     if (p.n_tiles < grid) grid = p.n_tiles > 0 ? p.n_tiles : 1;
@@ -252,6 +297,33 @@ extern "C" int stmp_dcrnn_bwd_wgrad(int64_t cin, int64_t cout, int64_t K, int64_
   const int total = 3 * 4 * C * kCo + 3 * kCo;
   k_dcrnn_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(grid, MG, C, p.partial, gz, gr, gh, gbz, gbr, gbh);
   STMP_LAUNCH_OK("k_dcrnn_wgrad_reduce");
+  return STMP_OK;
+}
+
+extern "C" int64_t stmp_gru_bwd_wgrad_workspace_bytes(int n_ops, int64_t cin) {
+  const int64_t MG = ((n_ops + 1) * (cin + kCo) + 7) / 8;
+  return (int64_t)wgrad_grid() * (MG * 8 * 3 * kCo + 3 * kCo) * 4;
+}
+
+extern "C" int stmp_gru_bwd_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
+                                  const float* dph, void* workspace, float* dwcat, float* dbcat, void* stream) {
+  STMP_REQUIRE(S1 && S2 && dpzr && dph && workspace && dwcat && rows >= 0, STMP_EINVAL, "stmp_gru_bwd_wgrad: bad argument");
+  STMP_REQUIRE(n_ops >= 0 && n_ops <= 2 && cin >= 1 && cin <= 4, STMP_EUNSUPPORTED, "stmp_gru_bwd_wgrad: n_ops <= 2, cin <= 4 only");
+  const int C = (int)cin + kCo, C3 = (n_ops + 1) * C, MG = (C3 + 7) / 8;
+  STMP_REQUIRE(ld == 8 * MG, STMP_ESHAPE, "stmp_gru_bwd_wgrad: the basis row pitch must be (n_ops+1)(cin+32) rounded up to 8");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rows == 0) {                                   // nothing to contract: the gradients are zero
+    STMP_CUDA_OK(cudaMemsetAsync(dwcat, 0, (size_t)96 * 112 * 4, st));
+    if (dbcat) STMP_CUDA_OK(cudaMemsetAsync(dbcat, 0, (size_t)96 * 4, st));
+    return STMP_OK;
+  }
+  float* partial = reinterpret_cast<float*>(workspace);
+  int grid = wgrad_grid();
+  const int rc = wgrad_tc_launch(C3, rows, (int)ld, S1, S2, dpzr, dph, partial, grid, st, &grid);
+  if (rc != STMP_OK) return rc;
+  const int total = 96 * 112 + 3 * kCo;
+  k_gru_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(grid, MG, (int)cin, n_ops + 1, partial, dwcat, dbcat);
+  STMP_LAUNCH_OK("k_gru_wgrad_reduce");
   return STMP_OK;
 }
 

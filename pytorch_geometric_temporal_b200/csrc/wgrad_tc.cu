@@ -33,7 +33,7 @@ constexpr int kLoA = 8192, kLoB1 = 4096, kLoB2 = 2048;   // offset of the lo cop
 struct WgTcParams {
   const float* S1; const float* S2; const float* dpzr; const float* dph;
   long long rows;
-  int ld, n_tiles, MG, C3;               // C3 = 3 (cin + cout): columns >= C3 of S are padding
+  int ld, n_tiles, MG, C3;               // C3 = (n_ops + 1)(cin + cout) (DCRNN: 3 blocks): columns >= C3 of S are padding
   float* partial;                        // [grid][MG*8*96 + 96]
 };
 
@@ -218,12 +218,12 @@ __global__ void __launch_bounds__(kThreads, 1) k_dcrnn_wgrad_tc(WgTcParams p) {
 
 }  // namespace
 
-// launched by stmp_dcrnn_bwd_wgrad (train.cu); returns the number of partials written (= grid)
-int wgrad_tc_launch(int cin, long long rows, int ld, const float* S1, const float* S2, const float* dpzr, const float* dph, float* partial,
+// launched by stmp_dcrnn_bwd_wgrad / stmp_gru_bwd_wgrad (train.cu), c3 = used basis columns; returns the number of partials written (= grid)
+int wgrad_tc_launch(int c3, long long rows, int ld, const float* S1, const float* S2, const float* dpzr, const float* dph, float* partial,
                     int max_parts, cudaStream_t st, int* parts) {
   WgTcParams p;
   p.S1 = S1; p.S2 = S2; p.dpzr = dpzr; p.dph = dph; p.rows = rows; p.ld = ld;
-  p.C3 = 3 * (cin + kCo); p.MG = (p.C3 + 7) / 8;
+  p.C3 = c3; p.MG = (p.C3 + 7) / 8;
   p.n_tiles = (int)((rows + kTK - 1) / kTK);
   p.partial = partial;
   int dev = 0, sms = 132;

@@ -2,7 +2,11 @@
 constructor `(in_channels, out_channels, K, normalization="sym", bias=True)`, `forward(X, edge_index,
 edge_weight=None, H=None, lambda_max=None)`, state_dict keys `conv_{x,h}_{z,r,h}.lins.{k}.weight`,
 `.bias`.  The six ChebConvs of the reference renormalise the graph and re-propagate per gate; here the
-scaled Laplacian is a cached plan and T_k([X|H]) is computed once and shared by all gates."""
+scaled Laplacian is a cached plan and T_k([X|H]) is computed once and shared by all gates.
+
+Inside the fused envelope (K <= 2, out_channels = 32, in_channels <= 4, a graph that fits one SM) inference is one launch of the
+generic graph-GRU kernel, and training is that same launch plus a hand-written backward (ops.gru_seq_train): the gradients of the
+prepacked weights are handed to the parameters as blocks, so the cached fold needs no autograd graph."""
 import torch
 
 from ... import ops
@@ -20,6 +24,7 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
             setattr(self, f"conv_h_{g}", ChebParams(out_channels, out_channels, K, bias))
         self._init_plans()
         self._pack = ops.PackCache()
+        self.fused_training = True      # False: op-for-op autograd path (tests compare the two)
 
     def _gate_weight(self, g, x_only=False, h_only=False):
         """Rows follow the basis [T_0 | T_1 | ...] of U=[X|H]: block k = [Wx_k^T ; Wh_k^T]."""
@@ -55,6 +60,35 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
             return W, b, ops.gru_weight_image(W, b)
         return self._pack.get(list(self.parameters()), build)
 
+    def _param_spec(self):
+        """(spec, params) of ops.gru_seq_train: where each parameter's gradient sits in (dwcat, dbcat) -- the inverse of `_packed`.
+        Both ChebConvs of a gate add their biases, so both receive that gate's block of dbcat."""
+        spec, params = [], []
+        for gi, g in enumerate("zrh"):
+            cx, ch = getattr(self, f"conv_x_{g}"), getattr(self, f"conv_h_{g}")
+            for k in range(self.K):
+                spec.append(("w", 32 * gi, 32, 32 * k, 32))
+                params.append(ch.lins[k].weight)
+                spec.append(("w", 32 * gi, 32, 96 + 4 * k, self.in_channels))
+                params.append(cx.lins[k].weight)
+            if cx.bias is not None:
+                spec += [("b", 32 * gi, 32), ("b", 32 * gi, 32)]
+                params += [cx.bias, ch.bias]
+        return spec, params
+
+    def _train_ok(self, plan, X, H):
+        """The fused training route: grad enabled and something requires it, inside the envelope of both the forward and the
+        backward kernels for n_ops = K - 1."""
+        if not self.fused_training or self.K > 2 or self.out_channels != 32 or self.in_channels > 4 or X.dim() != 2:
+            return False
+        if not (torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters()) or X.requires_grad or H.requires_grad)):
+            return False
+        if H.shape != (X.size(0), 32) or X.dtype != torch.float32 or H.dtype != torch.float32:
+            return False
+        n_ops = self.K - 1
+        return (ops.gru_seq_supported(plan, n_ops, self.in_channels, self.out_channels)
+                and ops.gru_bwd_supported(plan, n_ops, self.in_channels, self.out_channels))
+
     def _fused_ok(self, plan, X, H):
         if self.K > 2 or self.out_channels != 32 or X.dim() != 2:
             return False
@@ -67,12 +101,18 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
                 H: torch.FloatTensor = None, lambda_max: torch.Tensor = None) -> torch.FloatTensor:
         _require_cuda(X, "X")
         N, Ci, Co, K = X.size(-2), self.in_channels, self.out_channels, self.K
+        H_given = H
         if H is None:
             H = torch.zeros(*X.shape[:-1], Co, device=X.device, dtype=X.dtype)
         plan = self._cheb_plan(edge_index, edge_weight, N, self.normalization, lambda_max)
         if self._fused_ok(plan, X, H):   # one wgmma launch for the whole cell (stmp_gru_seq_fwd)
             W, b, img = self._packed()
             return ops.gru_seq_fwd(plan, 1 if K > 1 else 0, X.reshape(1, 1, N, Ci), W, b, h0=H.reshape(1, N, Co), wimage=img)[0, 0]
+        if self._train_ok(plan, X, H):   # the same launch with a stash, and a hand-written backward
+            W, b, img = self._packed()
+            spec, params = self._param_spec()
+            h0 = None if H_given is None else H_given.reshape(1, N, Co)      # None: zeros, and no dH
+            return ops.gru_seq_train(plan, K - 1, X.reshape(1, 1, N, Ci), h0, W, b, img, spec, params)[0, 0]
         TU = cheb_basis(plan, torch.cat([X, H], dim=-1), K)              # K x (N, Ci+Co)
         S = torch.cat(TU, dim=-1)
         pre = torch.matmul(S, torch.cat([self._gate_weight("z"), self._gate_weight("r")], dim=1))

@@ -141,9 +141,10 @@ def gru_seq_supported(plan: GraphPlan, n_ops: int, cin: int, cout: int) -> bool:
 
 
 def gru_seq_fwd(plan: GraphPlan, n_ops: int, x: torch.Tensor, wcat: torch.Tensor, bcat: torch.Tensor, h0=None,
-                h0_shared: bool = False, wimage: Optional[torch.Tensor] = None):
-    """Generic fused graph-GRU recurrence (stmp_gru_seq_fwd).  x (B,T,N,Cin) -> (B,T,N,32).
-    h0: (B,N,32), or (N,32)/(1,N,32) with h0_shared=True (every window starts from the same state), or None."""
+                h0_shared: bool = False, wimage: Optional[torch.Tensor] = None, stash: bool = False):
+    """Generic fused graph-GRU recurrence (stmp_gru_seq_fwd).  x (B,T,N,Cin) -> out (B,T,N,32) [, stash (B,T,3,N,32) = (Z, R, H~)
+    per step, the operand of the backward].  h0: (B,N,32), or (N,32)/(1,N,32) with h0_shared=True (every window starts from the same
+    state), or None."""
     x = _f32c(x, "X")
     N = plan.num_nodes
     if x.dim() != 4 or x.size(2) != N:
@@ -153,18 +154,127 @@ def gru_seq_fwd(plan: GraphPlan, n_ops: int, x: torch.Tensor, wcat: torch.Tensor
     if wcat.shape != (96, 112) or bcat.numel() != 96:
         raise RuntimeError("wcat must be (96,112) and bcat (96,)")
     out = torch.empty((B, T, N, 32), dtype=torch.float32, device=x.device)
+    st = torch.empty((B, T, 3, N, 32), dtype=torch.float32, device=x.device) if stash else None
     if B == 0 or T == 0:
-        return out
+        return (out, st) if stash else out
     h0c, hs = None, 0
     if h0 is not None:
         h0c = _f32c(h0, "H")
         hs = 0 if h0_shared else N * 32
     with torch.cuda.device(x.device):
         rc = _lib.lib().stmp_gru_seq_fwd(plan.handle, n_ops, B, T, cin, _lib.ptr(x), None, T * N * cin, N * cin, _lib.ptr(wcat),
-                                         _lib.ptr(bcat), _lib.ptr(h0c), hs, _lib.ptr(out), None, _lib.ptr(wimage),
+                                         _lib.ptr(bcat), _lib.ptr(h0c), hs, _lib.ptr(out), _lib.ptr(st), _lib.ptr(wimage),
                                          _lib.ptr(_seq_workspace(plan, T, cin, x.device)), _lib.stream_ptr())
     _lib.check(rc)
-    return out
+    return (out, st) if stash else out
+
+
+def gru_bwd_supported(plan: GraphPlan, n_ops: int, cin: int, cout: int) -> bool:
+    return bool(_lib.lib().stmp_gru_bwd_supported(plan.handle, n_ops, cin, cout))
+
+
+def gru_bwd_basis_ld(n_ops: int, cin: int) -> int:
+    """Row pitch of the graph-GRU bases [U | Op0 U | ..]: (n_ops+1)(cin+32) rounded up to 8 floats."""
+    return ((n_ops + 1) * (cin + 32) + 7) // 8 * 8
+
+
+def gru_pack_bwd_weights(n_ops: int, cin: int, wcat: torch.Tensor):
+    """(whsT (32, (n_ops+1)(cin+32)), wzrT (64, ..)): the backward GEMMs' weights in basis order from the forward's wcat, one launch."""
+    nb = (n_ops + 1) * (cin + 32)
+    whsT = torch.empty(32, nb, device=wcat.device, dtype=torch.float32)
+    wzrT = torch.empty(64, nb, device=wcat.device, dtype=torch.float32)
+    with torch.cuda.device(wcat.device):
+        _lib.check(_lib.lib().stmp_gru_pack_bwd_weights(n_ops, cin, _lib.ptr(_f32c(wcat, "wcat")), _lib.ptr(whsT), _lib.ptr(wzrT),
+                                                        _lib.stream_ptr()))
+    return whsT, wzrT
+
+
+def gru_bwd_basis(plan: GraphPlan, n_ops: int, x, out, h0, stash, S1, S2):
+    """S1 / S2 (T*B, N, ld) <- bases of [X_t | H_{t-1}] and [X_t | H_{t-1}*R_t] for every (t, b): one launch."""
+    B, T, N, Ci = x.shape
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.lib().stmp_gru_bwd_basis(plan.handle, n_ops, B, T, Ci, _lib.ptr(x), T * N * Ci, N * Ci, _lib.ptr(out), _lib.ptr(h0),
+                                                 N * 32, _lib.ptr(stash), _lib.ptr(S1), _lib.ptr(S2), S1.size(-1), _lib.stream_ptr()))
+
+
+def gru_bwd_seq(plan: GraphPlan, n_ops: int, cin: int, gout, out, h0, stash, whsT, wzrT, dph_all, dpzr_all, dx, dh0):
+    """The reverse-time recurrence of the graph-GRU backward in one persistent launch (one CTA or CTA pair per window)."""
+    B, T, N, _ = gout.shape
+    with torch.cuda.device(gout.device):
+        _lib.check(_lib.lib().stmp_gru_bwd_seq(plan.handle, n_ops, B, T, cin, _lib.ptr(gout), _lib.ptr(out), _lib.ptr(h0), N * 32,
+                                               _lib.ptr(stash), _lib.ptr(whsT), _lib.ptr(wzrT), _lib.ptr(dph_all), _lib.ptr(dpzr_all),
+                                               _lib.ptr(dx), _lib.ptr(dh0), _lib.stream_ptr()))
+
+
+def gru_bwd_wgrad(n_ops: int, cin: int, S1, S2, dpzr_all, dph_all, has_bias: bool):
+    """(dwcat (96, 112), dbcat (96,) or None): gradients of the forward's prepacked weights over all (t, b, n) rows, two launches."""
+    dev = S1.device
+    key = (dev, torch.cuda.current_stream(dev).cuda_stream, "gru", n_ops, cin)
+    ws = _WGRAD_WS.get(key)
+    if ws is None:
+        ws = torch.empty(int(_lib.lib().stmp_gru_bwd_wgrad_workspace_bytes(n_ops, cin)), device=dev, dtype=torch.uint8)
+        _WGRAD_WS[key] = ws
+    dwcat = torch.empty(96, 112, device=dev, dtype=torch.float32)
+    dbcat = torch.empty(96, device=dev, dtype=torch.float32) if has_bias else None
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().stmp_gru_bwd_wgrad(n_ops, cin, S1.size(0) * S1.size(1), S1.size(-1), _lib.ptr(S1), _lib.ptr(S2),
+                                                 _lib.ptr(dpzr_all), _lib.ptr(dph_all), _lib.ptr(ws), _lib.ptr(dwcat), _lib.ptr(dbcat),
+                                                 _lib.stream_ptr()))
+    return dwcat, dbcat
+
+
+class _GruSeqFn(torch.autograd.Function):
+    """Training form of the generic fused graph-GRU recurrence.  forward = `stmp_gru_seq_fwd` with a stash: the same launch as inference,
+    so the output is bit-identical to the `no_grad` one.  backward = pack -> basis -> reverse-time recurrence -> weight gradients
+    (`stmp_gru_pack_bwd_weights`, `stmp_gru_bwd_basis`, `stmp_gru_bwd_seq`, `stmp_gru_bwd_wgrad`): dX (when x requires grad), dH0 (when
+    h0 requires grad), dwcat and dbcat.  `params` receive their gradients as blocks of dwcat / dbcat, described by `spec`:
+    ("w", row, n_rows, col, n_cols) -> dwcat[row:row+n_rows, col:col+n_cols], ("b", row, n_rows) -> dbcat[row:row+n_rows] -- so a module
+    whose prepacked weights are a cached fold of its parameters needs no differentiable fold."""
+
+    @staticmethod
+    def forward(ctx, plan, n_ops, x, h0, wcat, bcat, wimage, spec, *params):
+        x = _f32c(x.detach(), "X")
+        h0c = None if h0 is None else _f32c(h0.detach(), "H")
+        out, stash = gru_seq_fwd(plan, n_ops, x, wcat, bcat, h0=h0c, wimage=wimage, stash=True)
+        ctx.plan, ctx.n_ops, ctx.spec, ctx.has_h0 = plan, n_ops, spec, h0 is not None
+        ctx.save_for_backward(x, h0c, out, stash, wcat)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, h0, out, stash, wcat = ctx.saved_tensors
+        plan, n_ops = ctx.plan, ctx.n_ops
+        B, T, N, Ci = x.shape
+        f32 = dict(device=x.device, dtype=torch.float32)
+        gout = _f32c(gout, "gout")
+        whsT, wzrT = gru_pack_bwd_weights(n_ops, Ci, wcat)
+        ld = gru_bwd_basis_ld(n_ops, Ci)
+        S1 = torch.empty(T * B, N, ld, **f32)
+        S2 = torch.empty(T * B, N, ld, **f32)
+        dph_all = torch.empty(T, B, N, 32, **f32)
+        dpzr_all = torch.empty(T, B, N, 64, **f32)
+        dX = torch.empty(x.shape, **f32) if ctx.needs_input_grad[2] else None
+        dH0 = torch.empty(B, N, 32, **f32)
+        gru_bwd_basis(plan, n_ops, x, out, h0, stash, S1, S2)
+        gru_bwd_seq(plan, n_ops, Ci, gout, out, h0, stash, whsT, wzrT, dph_all, dpzr_all, dX, dH0)
+        grads = [None] * len(ctx.spec)
+        if any(ctx.needs_input_grad[8:]):
+            dwcat, dbcat = gru_bwd_wgrad(n_ops, Ci, S1, S2, dpzr_all, dph_all, any(s[0] == "b" for s in ctx.spec))
+            db = None
+            for i, s in enumerate(ctx.spec):
+                if s[0] == "w":
+                    grads[i] = dwcat[s[1]:s[1] + s[2], s[3]:s[3] + s[4]]
+                else:
+                    if db is None:     # one copy per parameter that shares a dbcat block, so no two .grad tensors alias
+                        db = dbcat.expand(sum(1 for q in ctx.spec if q[0] == "b"), 96).clone()
+                    grads[i] = db[sum(1 for q in ctx.spec[:i] if q[0] == "b"), s[1]:s[1] + s[2]]
+        gH0 = dH0 if (ctx.has_h0 and ctx.needs_input_grad[3]) else None
+        return (None, None, dX, gH0, None, None, None, None, *grads)
+
+
+def gru_seq_train(plan: GraphPlan, n_ops: int, x, h0, wcat, bcat, wimage, spec, params) -> torch.Tensor:
+    """Differentiable (w.r.t. x, h0 and `params`, see _GruSeqFn) fused graph-GRU recurrence.  x (B,T,N,Cin), h0 (B,N,32) or None."""
+    return _GruSeqFn.apply(plan, n_ops, x, h0, wcat, bcat, wimage, tuple(spec), *params)
 
 
 def tgcn_attn_fwd(plan: GraphPlan, x: torch.Tensor, A: torch.Tensor, Bm: torch.Tensor, c: torch.Tensor,

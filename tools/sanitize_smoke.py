@@ -46,8 +46,11 @@ with torch.enable_grad():
     for t in range(3):                                           # TGCN2 training with the state carried: step 0 k_tgcn_attn_bwd,
         h = t2(torch.randn(3, 207, 4, device=dev), ei_t, ew_t, h)   # then k_tgcn_cell_bwd (TMA-staged X, staged Bm) + its reduce
     h.square().mean().backward()
+    for K in (1, 2):                                             # GConvGRU training: stashing forward, k_gru_pack_bwd_weights,
+        gg = GConvGRU(2, 32, K).to(dev)                          # k_gru_bwd_basis, k_gru_bwd_seq (CTA pair), k_dcrnn_wgrad_tc, k_gru_wgrad_reduce
+        gg(X[0, 0], ei_t, ew_t, torch.randn(207, 32, device=dev, requires_grad=True)).square().mean().backward()
 with torch.no_grad():
-    e4 = torch.from_numpy(synthetic.pems04_like(0)).to(dev)
+    e4 =torch.from_numpy(synthetic.pems04_like(0)).to(dev)
     ASTGCN(2, 1, 3, 64, 64, 1, 12, 12, 307, normalization="sym").to(dev)(torch.randn(2, 307, 1, 12, device=dev), e4)   # k_gemm_blocks x7
     eg, wg = synthetic.large_graph(2000, 20000, 0)
     eg, wg = torch.from_numpy(eg).to(dev), torch.from_numpy(wg).to(dev)
