@@ -257,6 +257,41 @@ int64_t stmp_gru_bwd_wgrad_workspace_bytes(int n_ops, int64_t cin);
 int stmp_gru_bwd_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
                        const float* dph, void* workspace, float* dwcat, float* dbcat, void* stream);
 
+/* ---- the generic graph-GRU cell on graphs of ANY size, split over CTAs by destination rows (gru_rows.cu): GConvGRU K <= 2 on a
+ * Chebyshev plan (gconv_gru.py:119-139), one graph and one step per call.  Envelope: cout = 32, cin 1..16, n_ops 0..1 and at most the
+ * plan's operators (stmp_gru_rows_supported), any number of nodes and any degree.  Exact fp32 FFMA; deterministic (no atomics, every
+ * reduction in a fixed order); no host sync and no allocation: scratch and workspace come from the caller, so a call can be captured.
+ *   packed weights w [96][nb], nb = (n_ops+1)(cin+32): row gate*32 + o (gates z | r | h), column m of the basis [X | H | Op X | Op H]
+ *   (X channels first in each block); b [96] = the sum of a gate's two biases (zeros without biases).
+ *   stmp_gru_rows_pack_weights: w, b from the parameters' layout: wx [3][n_ops+1][32][cin], wh [3][n_ops+1][32][32] (gate, Chebyshev
+ *                               order, out, in), bx / bh [3][32] (both or neither).  One launch.
+ *   stmp_gru_rows_fwd:          x (N,cin), h (N,32) or NULL (H = None) -> out (N,32).  H given: two launches (Op[X | H] -> Z, R, H*R;
+ *                               Op(H*R) -> H'), scratch of N*96 floats; H = None: one launch, no scratch.  Training adds (all nullable)
+ *                               stash (3,N,32) = Z | R | Ht (R unwritten for H = None) and the weight-gradient bases S1 = [U | Op U],
+ *                               S2 = [X | H*R | Op X | Op(H*R)] (N, ld), ld = nb rounded up to 8, 16-byte aligned; for H = None S1 = S2
+ *                               (pass S2 = NULL).  The output does not depend on which of them are given.
+ *   stmp_gru_rows_bwd:          gout = dL/dH' (N,32), h, stash and w of the forward -> dph (N,32), dpzr (N,64) (the weight-gradient
+ *                               operands; dpr = 0 for H = None), dx (N,cin; nullable), dh (N,32; nullable, NULL for H = None).  H given:
+ *                               rowwise dS2 = dph W_h^T; Op^T of dS2's H*R block -> dpr, dS1 = [dpz | dpr] W_zr^T; Op^T of the operator
+ *                               blocks -> dH, dX (skipped when neither is asked for or n_ops = 0).  H = None: one rowwise launch, plus
+ *                               one Op^T gather for dx.  scratch of stmp_gru_rows_scratch_bytes(plan) bytes (N*192 floats).
+ *   stmp_gru_rows_wgrad:        dw [96][nb] (the packed layout) and db [96] (nullable) = S1^T [dpz | dpr], S2^T dph and the column sums
+ *                               over `rows` rows: fp32 FFMA per-CTA partials + a fixed-order sum (two launches); workspace of
+ *                               stmp_gru_rows_wgrad_workspace_bytes(n_ops, cin) bytes, 16-byte aligned operands.
+ * STMP_EINVAL for NULL tensors, STMP_ESHAPE for bad sizes, pitches or alignment, STMP_EUNSUPPORTED for cin > 16, n_ops > 1, cout != 32
+ * or n_ops above the plan's operators. */
+int stmp_gru_rows_supported(const stmp_plan* plan, int n_ops, int64_t cin, int64_t cout);
+int stmp_gru_rows_pack_weights(int n_ops, int64_t cin, const float* wx, const float* wh, const float* bx, const float* bh, float* w,
+                               float* b, void* stream);
+int stmp_gru_rows_fwd(const stmp_plan* plan, int n_ops, int64_t cin, const float* x, const float* h, const float* w, const float* b,
+                      float* scratch, float* out, float* stash, float* S1, float* S2, int64_t ld, void* stream);
+int64_t stmp_gru_rows_scratch_bytes(const stmp_plan* plan);
+int stmp_gru_rows_bwd(const stmp_plan* plan, int n_ops, int64_t cin, const float* gout, const float* h, const float* stash,
+                      const float* w, float* scratch, float* dph, float* dpzr, float* dx, float* dh, void* stream);
+int64_t stmp_gru_rows_wgrad_workspace_bytes(int n_ops, int64_t cin);
+int stmp_gru_rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
+                        const float* dph, void* workspace, float* dw, float* db, void* stream);
+
 /* ---- backward of the fused DCRNN sequence for narrow states (cout <= 4): the reference's training model BatchedDCRNN(F, F, K=3) ----
  * Served when stmp_dcrnn_narrow_bwd_supported(plan, cin, cout, K) != 0 (DCONV plan, cin and cout in 1..4, K in 1..4, graph and state
  * buffers fit one SM's shared memory: PEMS-BAY's 325 nodes at K = 3 do).  stmp_dcrnn_narrow_bwd_seq is the reverse-time recurrence in

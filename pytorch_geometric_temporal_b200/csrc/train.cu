@@ -215,6 +215,45 @@ __global__ void __launch_bounds__(256) k_gru_wgrad_reduce(int parts, int MG, int
   }
 }
 
+// The same fixed-order sum for the row-split graph-GRU cell (gru_rows.cu), scattered into its packed layout dw [96][nb] (row gate*32 + o,
+// column m of the basis [X | H | Op X | Op H]) and db [96] (nullable).
+__global__ void __launch_bounds__(256) k_gru_rows_wgrad_reduce(int parts, int MG, int nb, const float* __restrict__ partial,
+                                                               float* __restrict__ dw, float* __restrict__ db) {
+  __shared__ float sub[8][32];
+  const int x = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int i = blockIdx.x * 32 + x;
+  const size_t stride = (size_t)MG * 8 * 3 * kCo + 3 * kCo;
+  size_t src = 0;
+  float* dst = nullptr;
+  if (i < 96 * nb) {
+    const int row = i / nb, m = i - row * nb, gate = row >> 5, o = row & 31;
+    src = gate == 2 ? (size_t)MG * 8 * 2 * kCo + (size_t)m * kCo + o : (size_t)m * 2 * kCo + gate * kCo + o;
+    dst = dw + i;
+  } else if (i < 96 * nb + 3 * kCo) {
+    const int b = i - 96 * nb;                                   // bias sums are stored z | r | h
+    src = (size_t)MG * 8 * 3 * kCo + b;
+    dst = db ? db + b : nullptr;
+  }
+  const int per = (parts + 7) / 8, q0 = w * per, q1 = (q0 + per < parts) ? q0 + per : parts;
+  float s0 = 0.f, s1 = 0.f;
+  if (dst) {
+    int q = q0;
+    for (; q + 2 <= q1; q += 2) {
+      s0 += partial[(size_t)q * stride + src];
+      s1 += partial[(size_t)(q + 1) * stride + src];
+    }
+    if (q < q1) s0 += partial[(size_t)q * stride + src];
+  }
+  sub[w][x] = s0 + s1;
+  __syncthreads();
+  if (w == 0 && dst) {
+    float t = sub[0][x];
+#pragma unroll
+    for (int k = 1; k < 8; ++k) t += sub[k][x];
+    *dst = t;
+  }
+}
+
 // ---- Adam over one flat buffer -------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_adam_flat(long long n, float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
                                                    float* __restrict__ v, float* step, unsigned* ticket, float lr, float b1, float b2,
@@ -324,6 +363,42 @@ extern "C" int stmp_gru_bwd_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t 
   const int total = 96 * 112 + 3 * kCo;
   k_gru_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(grid, MG, (int)cin, n_ops + 1, partial, dwcat, dbcat);
   STMP_LAUNCH_OK("k_gru_wgrad_reduce");
+  return STMP_OK;
+}
+
+extern "C" int64_t stmp_gru_rows_wgrad_workspace_bytes(int n_ops, int64_t cin) {
+  const int64_t MG = ((n_ops + 1) * (cin + kCo) + 7) / 8;
+  return (int64_t)wgrad_grid() * (MG * 8 * 3 * kCo + 3 * kCo) * 4;
+}
+
+// Exact fp32: the FFMA contraction k_dcrnn_wgrad (per-CTA partials over strided 16-row tiles) and k_gru_rows_wgrad_reduce.
+extern "C" int stmp_gru_rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
+                                   const float* dph, void* workspace, float* dw, float* db, void* stream) {
+  STMP_REQUIRE(S1 && S2 && dpzr && dph && workspace && dw && rows >= 0, STMP_EINVAL, "stmp_gru_rows_wgrad: bad argument");
+  STMP_REQUIRE(n_ops >= 0 && n_ops <= 1 && cin >= 1 && cin <= 16, STMP_EUNSUPPORTED, "stmp_gru_rows_wgrad: n_ops <= 1, cin 1..16 only");
+  const int nb = (n_ops + 1) * ((int)cin + kCo), MG = (nb + 7) / 8;
+  STMP_REQUIRE(ld == 8 * MG, STMP_ESHAPE, "stmp_gru_rows_wgrad: the basis row pitch must be (n_ops+1)(cin+32) rounded up to 8");
+  STMP_REQUIRE((((uintptr_t)S1 | (uintptr_t)S2 | (uintptr_t)dpzr | (uintptr_t)dph | (uintptr_t)workspace) & 15u) == 0, STMP_ESHAPE,
+               "stmp_gru_rows_wgrad: S1, S2, dpzr, dph and the workspace must be 16-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rows == 0) {
+    STMP_CUDA_OK(cudaMemsetAsync(dw, 0, (size_t)96 * nb * 4, st));
+    if (db) STMP_CUDA_OK(cudaMemsetAsync(db, 0, (size_t)96 * 4, st));
+    return STMP_OK;
+  }
+  WgradParams p;
+  p.S1 = S1; p.S2 = S2; p.dpzr = dpzr; p.dph = dph; p.rows = rows; p.ld = (int)ld; p.MG = MG;
+  p.n_tiles = (int)((rows + kWgTK - 1) / kWgTK);
+  p.partial = reinterpret_cast<float*>(workspace);
+  int grid = wgrad_grid();
+  if (p.n_tiles < grid) grid = p.n_tiles;
+  const int smem = kWgStages * kWgTK * (2 * (int)ld + 3 * kCo) * 4 + 64;
+  STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  k_dcrnn_wgrad<<<grid, kWgThreads, smem, st>>>(p);
+  STMP_LAUNCH_OK("k_dcrnn_wgrad");
+  const int total = 96 * nb + 3 * kCo;
+  k_gru_rows_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(grid, MG, nb, p.partial, dw, db);
+  STMP_LAUNCH_OK("k_gru_rows_wgrad_reduce");
   return STMP_OK;
 }
 

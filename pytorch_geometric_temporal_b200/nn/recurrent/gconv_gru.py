@@ -6,7 +6,9 @@ scaled Laplacian is a cached plan and T_k([X|H]) is computed once and shared by 
 
 Inside the fused envelope (K <= 2, out_channels = 32, in_channels <= 4, a graph that fits one SM) inference is one launch of the
 generic graph-GRU kernel, and training is that same launch plus a hand-written backward (ops.gru_seq_train): the gradients of the
-prepacked weights are handed to the parameters as blocks, so the cached fold needs no autograd graph."""
+prepacked weights are handed to the parameters as blocks, so the cached fold needs no autograd graph.  Graphs too large for one SM
+(K <= 2, out_channels = 32, in_channels <= 16, 2-D X) run the row-split cell kernels instead (ops.gru_rows_fwd / gru_rows_train):
+one launch with H = None, two with H given, and a hand-written backward of the same kind."""
 import torch
 
 from ... import ops
@@ -24,6 +26,7 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
             setattr(self, f"conv_h_{g}", ChebParams(out_channels, out_channels, K, bias))
         self._init_plans()
         self._pack = ops.PackCache()
+        self._rows_pack = ops.PackCache()
         self.fused_training = True      # False: op-for-op autograd path (tests compare the two)
 
     def _gate_weight(self, g, x_only=False, h_only=False):
@@ -60,16 +63,30 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
             return W, b, ops.gru_weight_image(W, b)
         return self._pack.get(list(self.parameters()), build)
 
-    def _param_spec(self):
-        """(spec, params) of ops.gru_seq_train: where each parameter's gradient sits in (dwcat, dbcat) -- the inverse of `_packed`.
-        Both ChebConvs of a gate add their biases, so both receive that gate's block of dbcat."""
+    def _rows_packed(self):
+        """(w [96, K(Ci+32)], b [96]) for stmp_gru_rows_fwd: columns [X | H] per Chebyshev order (one launch per weight update)."""
+        def build():
+            gates = [(getattr(self, f"conv_x_{g}"), getattr(self, f"conv_h_{g}")) for g in "zrh"]
+            wx = torch.stack([torch.stack([cx.lins[k].weight for k in range(self.K)]) for cx, _ in gates])
+            wh = torch.stack([torch.stack([ch.lins[k].weight for k in range(self.K)]) for _, ch in gates])
+            bx = bh = None
+            if self.bias:
+                bx, bh = torch.stack([cx.bias for cx, _ in gates]), torch.stack([ch.bias for _, ch in gates])
+            return ops.gru_rows_pack_weights(self.K - 1, self.in_channels, wx, wh, bx, bh)
+        return self._rows_pack.get(list(self.parameters()), build)
+
+    def _param_spec(self, rows=False):
+        """(spec, params) of ops.gru_seq_train (or, with `rows`, ops.gru_rows_train): where each parameter's gradient sits in the packed
+        weight / bias gradients -- the inverse of `_packed` (`_rows_packed`).  Both ChebConvs of a gate add their biases, so both receive
+        that gate's bias block."""
         spec, params = [], []
+        Ci = self.in_channels
         for gi, g in enumerate("zrh"):
             cx, ch = getattr(self, f"conv_x_{g}"), getattr(self, f"conv_h_{g}")
             for k in range(self.K):
-                spec.append(("w", 32 * gi, 32, 32 * k, 32))
+                spec.append(("w", 32 * gi, 32, k * (Ci + 32) + Ci if rows else 32 * k, 32))
                 params.append(ch.lins[k].weight)
-                spec.append(("w", 32 * gi, 32, 96 + 4 * k, self.in_channels))
+                spec.append(("w", 32 * gi, 32, k * (Ci + 32) if rows else 96 + 4 * k, Ci))
                 params.append(cx.lins[k].weight)
             if cx.bias is not None:
                 spec += [("b", 32 * gi, 32), ("b", 32 * gi, 32)]
@@ -97,6 +114,18 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
             return False
         return ops.gru_seq_supported(plan, 1 if self.K > 1 else 0, self.in_channels, self.out_channels)
 
+    def _rows_ok(self, plan, X, H, training):
+        """The row-split route: K <= 2, out_channels = 32, in_channels <= 16, 2-D float32 X, a graph the one-SM kernel cannot hold (checked
+        first, so graphs that fit one SM never consult the row-split entry); training calls also need `fused_training`."""
+        if self.K > 2 or self.out_channels != 32 or self.in_channels > 16 or X.dim() != 2 or X.dtype != torch.float32:
+            return False
+        if (training and not self.fused_training) or (H is not None and (H.shape != (X.size(0), 32) or H.dtype != torch.float32)):
+            return False
+        n_ops = self.K - 1
+        if ops.gru_seq_supported(plan, n_ops, 1, 32):
+            return False
+        return ops.gru_rows_supported(plan, n_ops, self.in_channels, 32)
+
     def forward(self, X: torch.FloatTensor, edge_index: torch.LongTensor, edge_weight: torch.FloatTensor = None,
                 H: torch.FloatTensor = None, lambda_max: torch.Tensor = None) -> torch.FloatTensor:
         _require_cuda(X, "X")
@@ -113,6 +142,14 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
             spec, params = self._param_spec()
             h0 = None if H_given is None else H_given.reshape(1, N, Co)      # None: zeros, and no dH
             return ops.gru_seq_train(plan, K - 1, X.reshape(1, 1, N, Ci), h0, W, b, img, spec, params)[0, 0]
+        training = torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters()) or X.requires_grad
+                                                 or (H_given is not None and H_given.requires_grad))
+        if self._rows_ok(plan, X, H_given, training):   # graphs larger than one SM: the row-split cell kernels (stmp_gru_rows_*)
+            w, b = self._rows_packed()
+            if training:
+                spec, params = self._param_spec(rows=True)
+                return ops.gru_rows_train(plan, K - 1, X, H_given, w, b, spec, params)
+            return ops.gru_rows_fwd(plan, K - 1, X, H_given, w, b)
         TU = cheb_basis(plan, torch.cat([X, H], dim=-1), K)              # K x (N, Ci+Co)
         S = torch.cat(TU, dim=-1)
         pre = torch.matmul(S, torch.cat([self._gate_weight("z"), self._gate_weight("r")], dim=1))

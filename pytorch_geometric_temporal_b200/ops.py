@@ -223,6 +223,20 @@ def gru_bwd_wgrad(n_ops: int, cin: int, S1, S2, dpzr_all, dph_all, has_bias: boo
     return dwcat, dbcat
 
 
+def _spec_grads(spec, dw, db):
+    """Parameter gradients as blocks of packed weight / bias gradients: ("w", row, n_rows, col, n_cols) -> dw[row:row+n_rows, col:col+n_cols],
+    ("b", row, n_rows) -> db[row:row+n_rows].  Parameters that share a block of db each get their own copy, so no two .grad tensors alias."""
+    grads, dbs = [None] * len(spec), None
+    for i, s in enumerate(spec):
+        if s[0] == "w":
+            grads[i] = dw[s[1]:s[1] + s[2], s[3]:s[3] + s[4]]
+        else:
+            if dbs is None:
+                dbs = db.expand(sum(1 for q in spec if q[0] == "b"), db.numel()).clone()
+            grads[i] = dbs[sum(1 for q in spec[:i] if q[0] == "b"), s[1]:s[1] + s[2]]
+    return grads
+
+
 class _GruSeqFn(torch.autograd.Function):
     """Training form of the generic fused graph-GRU recurrence.  forward = `stmp_gru_seq_fwd` with a stash: the same launch as inference,
     so the output is bit-identical to the `no_grad` one.  backward = pack -> basis -> reverse-time recurrence -> weight gradients
@@ -260,14 +274,7 @@ class _GruSeqFn(torch.autograd.Function):
         grads = [None] * len(ctx.spec)
         if any(ctx.needs_input_grad[8:]):
             dwcat, dbcat = gru_bwd_wgrad(n_ops, Ci, S1, S2, dpzr_all, dph_all, any(s[0] == "b" for s in ctx.spec))
-            db = None
-            for i, s in enumerate(ctx.spec):
-                if s[0] == "w":
-                    grads[i] = dwcat[s[1]:s[1] + s[2], s[3]:s[3] + s[4]]
-                else:
-                    if db is None:     # one copy per parameter that shares a dbcat block, so no two .grad tensors alias
-                        db = dbcat.expand(sum(1 for q in ctx.spec if q[0] == "b"), 96).clone()
-                    grads[i] = db[sum(1 for q in ctx.spec[:i] if q[0] == "b"), s[1]:s[1] + s[2]]
+            grads = _spec_grads(ctx.spec, dwcat, dbcat)
         gH0 = dH0 if (ctx.has_h0 and ctx.needs_input_grad[3]) else None
         return (None, None, dX, gH0, None, None, None, None, *grads)
 
@@ -275,6 +282,118 @@ class _GruSeqFn(torch.autograd.Function):
 def gru_seq_train(plan: GraphPlan, n_ops: int, x, h0, wcat, bcat, wimage, spec, params) -> torch.Tensor:
     """Differentiable (w.r.t. x, h0 and `params`, see _GruSeqFn) fused graph-GRU recurrence.  x (B,T,N,Cin), h0 (B,N,32) or None."""
     return _GruSeqFn.apply(plan, n_ops, x, h0, wcat, bcat, wimage, tuple(spec), *params)
+
+
+def gru_rows_supported(plan: GraphPlan, n_ops: int, cin: int, cout: int) -> bool:
+    return bool(_lib.lib().stmp_gru_rows_supported(plan.handle, n_ops, cin, cout))
+
+
+def gru_rows_basis_ld(n_ops: int, cin: int) -> int:
+    """Row pitch of the row-split cell's weight-gradient bases: (n_ops+1)(cin+32) rounded up to 8 floats."""
+    return ((n_ops + 1) * (cin + 32) + 7) // 8 * 8
+
+
+def gru_rows_pack_weights(n_ops: int, cin: int, wx, wh, bx=None, bh=None):
+    """(w (96, (n_ops+1)(cin+32)), b (96,)): the row-split cell's packed weights from the parameters' layout -- wx (3, n_ops+1, 32, cin),
+    wh (3, n_ops+1, 32, 32), bx / bh (3, 32) or None -- in one launch (stmp_gru_rows_pack_weights)."""
+    wx, wh = _f32c(wx, "wx"), _f32c(wh, "wh")
+    if wx.shape != (3, n_ops + 1, 32, cin) or wh.shape != (3, n_ops + 1, 32, 32):
+        raise RuntimeError("gru_rows_pack_weights: wx must be (3, n_ops+1, 32, cin) and wh (3, n_ops+1, 32, 32)")
+    bx = None if bx is None else _f32c(bx, "bx")
+    bh = None if bh is None else _f32c(bh, "bh")
+    w = torch.empty(96, (n_ops + 1) * (cin + 32), device=wx.device, dtype=torch.float32)
+    b = torch.empty(96, device=wx.device, dtype=torch.float32)
+    with torch.cuda.device(wx.device):
+        _lib.check(_lib.lib().stmp_gru_rows_pack_weights(n_ops, cin, _lib.ptr(wx), _lib.ptr(wh), _lib.ptr(bx), _lib.ptr(bh), _lib.ptr(w),
+                                                         _lib.ptr(b), _lib.stream_ptr()))
+    return w, b
+
+
+def gru_rows_fwd(plan: GraphPlan, n_ops: int, x: torch.Tensor, h: Optional[torch.Tensor], w: torch.Tensor, b: torch.Tensor,
+                 train: bool = False):
+    """Row-split graph-GRU cell (stmp_gru_rows_fwd) on one graph: x (N, cin), h (N, 32) or None -> H' (N, 32).  With `train`, returns
+    (H', stash (3, N, 32), S1, S2) -- the operands of gru_rows_bwd / gru_rows_wgrad; S2 is S1 when h is None."""
+    x, w, b = _f32c(x, "X"), _f32c(w, "w"), _f32c(b, "b")
+    N, cin = x.shape
+    f32 = dict(device=x.device, dtype=torch.float32)
+    out = torch.empty(N, 32, **f32)
+    hc = None if h is None else _f32c(h, "H")
+    scr = torch.empty(N, 96, **f32) if hc is not None else None
+    st = S1 = S2 = None
+    ld = gru_rows_basis_ld(n_ops, cin)
+    if train:
+        st = torch.empty(3, N, 32, **f32)
+        S1 = torch.empty(N, ld, **f32)
+        S2 = torch.empty(N, ld, **f32) if hc is not None else None
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.lib().stmp_gru_rows_fwd(plan.handle, n_ops, cin, _lib.ptr(x), _lib.ptr(hc), _lib.ptr(w), _lib.ptr(b), _lib.ptr(scr),
+                                                _lib.ptr(out), _lib.ptr(st), _lib.ptr(S1), _lib.ptr(S2), ld, _lib.stream_ptr()))
+    if not train:
+        return out
+    return out, st, S1, S1 if S2 is None else S2
+
+
+def gru_rows_bwd(plan: GraphPlan, n_ops: int, gout, h, stash, w, want_dx: bool, want_dh: bool, cin: int):
+    """(dph (N, 32), dpzr (N, 64), dx (N, cin) or None, dh (N, 32) or None) of the row-split cell (stmp_gru_rows_bwd)."""
+    gout = _f32c(gout, "gout")
+    N = gout.size(0)
+    f32 = dict(device=gout.device, dtype=torch.float32)
+    scr = torch.empty(int(_lib.lib().stmp_gru_rows_scratch_bytes(plan.handle)) // 4, **f32)
+    dph, dpzr = torch.empty(N, 32, **f32), torch.empty(N, 64, **f32)
+    dx = torch.empty(N, cin, **f32) if want_dx else None
+    dh = torch.empty(N, 32, **f32) if want_dh else None
+    with torch.cuda.device(gout.device):
+        _lib.check(_lib.lib().stmp_gru_rows_bwd(plan.handle, n_ops, cin, _lib.ptr(gout), _lib.ptr(h), _lib.ptr(stash), _lib.ptr(w),
+                                                _lib.ptr(scr), _lib.ptr(dph), _lib.ptr(dpzr), _lib.ptr(dx), _lib.ptr(dh), _lib.stream_ptr()))
+    return dph, dpzr, dx, dh
+
+
+def gru_rows_wgrad(n_ops: int, cin: int, S1, S2, dpzr, dph, has_bias: bool):
+    """(dw (96, (n_ops+1)(cin+32)), db (96,) or None): the packed weights' gradients of the row-split cell, two launches."""
+    dev = S1.device
+    key = (dev, torch.cuda.current_stream(dev).cuda_stream, "gru_rows", n_ops, cin)
+    ws = _WGRAD_WS.get(key)
+    if ws is None:
+        ws = torch.empty(int(_lib.lib().stmp_gru_rows_wgrad_workspace_bytes(n_ops, cin)), device=dev, dtype=torch.uint8)
+        _WGRAD_WS[key] = ws
+    dw = torch.empty(96, (n_ops + 1) * (cin + 32), device=dev, dtype=torch.float32)
+    db = torch.empty(96, device=dev, dtype=torch.float32) if has_bias else None
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().stmp_gru_rows_wgrad(n_ops, cin, S1.size(0), S1.size(1), _lib.ptr(S1), _lib.ptr(S2), _lib.ptr(dpzr), _lib.ptr(dph),
+                                                  _lib.ptr(ws), _lib.ptr(dw), _lib.ptr(db), _lib.stream_ptr()))
+    return dw, db
+
+
+class _GruRowsFn(torch.autograd.Function):
+    """Training form of the row-split graph-GRU cell, the twin of _GruSeqFn for graphs of any size.  forward = `stmp_gru_rows_fwd` with the
+    stash and the weight-gradient bases (the inference launches, so the output is bit-identical to the `no_grad` one); backward =
+    `stmp_gru_rows_bwd` + `stmp_gru_rows_wgrad`: dX (when x requires grad), dH (when h is given and requires grad) and the packed weights'
+    gradients, handed to `params` as blocks described by `spec` (see _spec_grads)."""
+
+    @staticmethod
+    def forward(ctx, plan, n_ops, x, h, w, b, spec, *params):
+        x = _f32c(x.detach(), "X")
+        hc = None if h is None else _f32c(h.detach(), "H")
+        out, stash, S1, S2 = gru_rows_fwd(plan, n_ops, x, hc, w, b, train=True)
+        ctx.plan, ctx.n_ops, ctx.spec, ctx.cin = plan, n_ops, spec, x.size(1)
+        ctx.save_for_backward(hc, stash, S1, S2, w)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        h, stash, S1, S2, w = ctx.saved_tensors
+        want_dh = h is not None and ctx.needs_input_grad[3]
+        dph, dpzr, dx, dh = gru_rows_bwd(ctx.plan, ctx.n_ops, gout, h, stash, w, ctx.needs_input_grad[2], want_dh, ctx.cin)
+        grads = [None] * len(ctx.spec)
+        if any(ctx.needs_input_grad[7:]):
+            dw, db = gru_rows_wgrad(ctx.n_ops, ctx.cin, S1, S2, dpzr, dph, any(s[0] == "b" for s in ctx.spec))
+            grads = _spec_grads(ctx.spec, dw, db)
+        return (None, None, dx, dh, None, None, None, *grads)
+
+
+def gru_rows_train(plan: GraphPlan, n_ops: int, x, h, w, b, spec, params) -> torch.Tensor:
+    """Differentiable (w.r.t. x, h and `params`, see _GruRowsFn) row-split graph-GRU cell.  x (N, cin), h (N, 32) or None (zeros, no dH)."""
+    return _GruRowsFn.apply(plan, n_ops, x, h, w, b, tuple(spec), *params)
 
 
 def tgcn_attn_fwd(plan: GraphPlan, x: torch.Tensor, A: torch.Tensor, Bm: torch.Tensor, c: torch.Tensor,

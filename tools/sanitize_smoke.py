@@ -49,6 +49,14 @@ with torch.enable_grad():
     for K in (1, 2):                                             # GConvGRU training: stashing forward, k_gru_pack_bwd_weights,
         gg = GConvGRU(2, 32, K).to(dev)                          # k_gru_bwd_basis, k_gru_bwd_seq (CTA pair), k_dcrnn_wgrad_tc, k_gru_wgrad_reduce
         gg(X[0, 0], ei_t, ew_t, torch.randn(207, 32, device=dev, requires_grad=True)).square().mean().backward()
+    ring = torch.arange(301, device=dev)
+    e_ring = torch.cat([torch.stack([ring, (ring + 1) % 301]), torch.stack([(ring + 5) % 301, ring])], dim=1)
+    gr = GConvGRU(14, 32, 2).to(dev)                             # 301 nodes: the row-split cell kernels (k_gru_rows_*), H given and None,
+    xr = torch.randn(301, 14, device=dev, requires_grad=True)    # X gradient: k_dcrnn_wgrad + k_gru_rows_wgrad_reduce
+    gr(xr, e_ring, None, torch.randn(301, 32, device=dev, requires_grad=True)).square().mean().backward()
+    gr(xr, e_ring, None).square().mean().backward()
+    with torch.no_grad():
+        gr(xr, e_ring, None, torch.randn(301, 32, device=dev))
 with torch.no_grad():
     e4 =torch.from_numpy(synthetic.pems04_like(0)).to(dev)
     ASTGCN(2, 1, 3, 64, 64, 1, 12, 12, 307, normalization="sym").to(dev)(torch.randn(2, 307, 1, 12, device=dev), e4)   # k_gemm_blocks x7
