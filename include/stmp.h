@@ -292,6 +292,47 @@ int64_t stmp_gru_rows_wgrad_workspace_bytes(int n_ops, int64_t cin);
 int stmp_gru_rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
                         const float* dph, void* workspace, float* dw, float* db, void* stream);
 
+/* ---- the peephole graph-LSTM cell on graphs of ANY size, split over CTAs by destination rows (lstm_rows.cu): GConvLSTM
+ * (gconv_lstm.py:168-238) and GCLSTM (gc_lstm.py:139-205) at K <= 2 on a Chebyshev plan, one graph and one step per call.  `variant`
+ * selects the basis: STMP_LSTM_GCONV [X | H | Op X | Op H], STMP_LSTM_GC [X | H | Op H] (X is not diffused); nb basis columns, X channels
+ * first; with n_ops = 0 both are [X | H].  Peepholes are the nullable `peep` (3, 32) = w_c_i | w_c_f | w_c_o (NULL: none, as GCLSTM).
+ * Envelope: cout = 32, cin 1..16, n_ops 0..1 and at most the plan's operators (stmp_lstm_rows_supported), any number of nodes and any
+ * degree.  Exact fp32 FFMA; deterministic (no atomics, every reduction in a fixed order); no host sync and no allocation: scratch and
+ * workspace come from the caller, so a call can be captured.
+ *   packed weights w [128][nb]: row gate*32 + o (gates i | f | c | o), column m of the basis; b [128] = the sum of every bias of a gate.
+ *   stmp_lstm_rows_pack_weights: w, b from the parameters' layout in one launch.  GConvLSTM: wx [4][n_ops+1][32][cin], wh
+ *                                [4][n_ops+1][32][32] (gate, Chebyshev order, out, in), bx / bh [4][32] (both or neither), bg [4][32];
+ *                                GCLSTM: wx [4][cin][32] (W_g, in x out), wh as above, bx NULL, bh [4][32] or NULL, bg [4][32].
+ *   stmp_lstm_rows_fwd:          x (N,cin), h and c (N,32) or NULL (zeros) -> hout, cout (N,32).  One launch.  Training adds (nullable)
+ *                                stash (4,N,32) = I | F | T | O and the weight-gradient basis S (N, ld), ld = nb rounded up to 8,
+ *                                16-byte aligned.  The outputs do not depend on which of them are given.
+ *   stmp_lstm_rows_bwd:          gh = dL/dH', gc = dL/dC' (N,32; either NULL), c, cn = C' and stash of the forward -> dpre (2,N,64) =
+ *                                [dpi | dpf], [dpc | dpo] (16-byte aligned), dx (N,cin), dh (N,32), dc (N,32) (nullable; dh / dc only
+ *                                with h / c given).  A rowwise launch (dpre, dC, dS = dpre W: own-row block -> dX, dH), then for n_ops = 1
+ *                                an Op^T gather of dS's operator block into dH (and dX for GConvLSTM) when one of them is asked for.
+ *                                scratch of stmp_lstm_rows_scratch_bytes(plan) bytes; with peep it also carries the per-CTA peephole sums
+ *                                to stmp_lstm_rows_wgrad.
+ *   stmp_lstm_rows_wgrad:        dw [128][nb] (the packed layout) = dpre^T S, db [128] = 1^T dpre and dpeep [96] = the sums of dpi*C,
+ *                                dpf*C and dpo*C' (db, dpeep nullable; dpeep reads the backward's scratch, rows = the plan's nodes):
+ *                                fp32 FFMA per-CTA partials + a fixed-order sum (two launches); workspace of
+ *                                stmp_lstm_rows_wgrad_workspace_bytes(variant, n_ops, cin) bytes, 16-byte aligned.
+ * STMP_EINVAL for NULL tensors or an unknown variant, STMP_ESHAPE for a bad pitch or alignment, STMP_EUNSUPPORTED for cin > 16,
+ * n_ops > 1, cout != 32 or n_ops above the plan's operators. */
+enum stmp_lstm_basis { STMP_LSTM_GCONV = 0, STMP_LSTM_GC = 1 };
+int stmp_lstm_rows_supported(const stmp_plan* plan, int variant, int n_ops, int64_t cin, int64_t cout);
+int stmp_lstm_rows_pack_weights(int variant, int n_ops, int64_t cin, const float* wx, const float* wh, const float* bx, const float* bh,
+                                const float* bg, float* w, float* b, void* stream);
+int stmp_lstm_rows_fwd(const stmp_plan* plan, int variant, int n_ops, int64_t cin, const float* x, const float* h, const float* c,
+                       const float* w, const float* b, const float* peep, float* hout, float* cout, float* stash, float* S, int64_t ld,
+                       void* stream);
+int64_t stmp_lstm_rows_scratch_bytes(const stmp_plan* plan);
+int stmp_lstm_rows_bwd(const stmp_plan* plan, int variant, int n_ops, int64_t cin, const float* gh, const float* gc, const float* c,
+                       const float* cn, const float* stash, const float* w, const float* peep, float* scratch, float* dpre, float* dx,
+                       float* dh, float* dc, void* stream);
+int64_t stmp_lstm_rows_wgrad_workspace_bytes(int variant, int n_ops, int64_t cin);
+int stmp_lstm_rows_wgrad(int variant, int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S, const float* dpre,
+                         const float* scratch, void* workspace, float* dw, float* db, float* dpeep, void* stream);
+
 /* ---- backward of the fused DCRNN sequence for narrow states (cout <= 4): the reference's training model BatchedDCRNN(F, F, K=3) ----
  * Served when stmp_dcrnn_narrow_bwd_supported(plan, cin, cout, K) != 0 (DCONV plan, cin and cout in 1..4, K in 1..4, graph and state
  * buffers fit one SM's shared memory: PEMS-BAY's 325 nodes at K = 3 do).  stmp_dcrnn_narrow_bwd_seq is the reverse-time recurrence in

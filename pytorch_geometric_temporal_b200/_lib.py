@@ -15,6 +15,7 @@ FLAVOR_DCONV, FLAVOR_CHEB, FLAVOR_GCN, FLAVOR_CHEB_ATT = range(4)
 NORM_NONE, NORM_SYM, NORM_RW = range(3)
 GCN_IMPROVED, GCN_NO_SELF_LOOPS, DCONV_ALLOW_DUPLICATES = 1, 2, 4
 NORM_CODE = {None: NORM_NONE, "sym": NORM_SYM, "rw": NORM_RW}
+LSTM_GCONV, LSTM_GC = range(2)                     # stmp_lstm_basis: the row-split LSTM cell's basis (GConvLSTM / GCLSTM)
 
 
 class StmpError(RuntimeError):
@@ -76,6 +77,13 @@ _SIGNATURES = {
     "stmp_gru_rows_bwd": (c_int, [_P, c_int, c_int64] + [_P] * 10),
     "stmp_gru_rows_wgrad_workspace_bytes": (c_int64, [c_int, c_int64]),
     "stmp_gru_rows_wgrad": (c_int, [c_int, c_int64, c_int64, c_int64] + [_P] * 8),
+    "stmp_lstm_rows_supported": (c_int, [_P, c_int, c_int, c_int64, c_int64]),
+    "stmp_lstm_rows_pack_weights": (c_int, [c_int, c_int, c_int64] + [_P] * 8),
+    "stmp_lstm_rows_fwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 10 + [c_int64, _P]),
+    "stmp_lstm_rows_scratch_bytes": (c_int64, [_P]),
+    "stmp_lstm_rows_bwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 13),
+    "stmp_lstm_rows_wgrad_workspace_bytes": (c_int64, [c_int, c_int, c_int64]),
+    "stmp_lstm_rows_wgrad": (c_int, [c_int, c_int, c_int64, c_int64, c_int64] + [_P] * 8),
     "stmp_tgcn_attn_bwd_workspace_bytes":(c_int64, [_P, c_int64]),
     "stmp_tgcn_attn_bwd": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "stmp_tgcn_cell_bwd_workspace_bytes": (c_int64, [_P, c_int64]),

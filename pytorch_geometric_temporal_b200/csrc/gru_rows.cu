@@ -14,62 +14,14 @@
 // broadcast with a shuffle and multiplied into the lane's column of the staged weights (pitch 97: the lane-indexed rows and the
 // lane-indexed columns are both free of bank conflicts).  Gathers walk the plan's CSR rows in entry order with separate multiply and
 // add, as stmp_spmm does.  No atomics anywhere; every result depends on its row alone, so repeated calls are bit-identical.
-#include "common.cuh"
+#include "rows.cuh"
 
 namespace stmp {
 namespace {
 
-constexpr int kCo = 32;
-constexpr int kRowsThreads = 256;
-constexpr int kRowsWarps = kRowsThreads / 32;
-constexpr int kRowTile = 16;                 // destination rows per CTA tile: two per warp
-constexpr int kWPitch = 97;                  // shared-memory pitch of a staged weight row (basis columns 0..95)
-constexpr int kMaxCin = 16;
+using namespace rows;
 constexpr int kScrPitch = 192;               // backward scratch row: dS2 (96) | Op^T operand Q (96)
 constexpr int kFwdScrPitch = 96;             // forward scratch row: H*R | X half of pre_h | Z
-
-// rows [r0, r0 + nr) of the packed weights w [96][nb] -> ws [nr][kWPitch] (columns >= nb zero)
-__device__ __forceinline__ void stage_w(float* ws, const float* __restrict__ w, int nb, int r0, int nr) {
-  for (int i = threadIdx.x; i < nr * kWPitch; i += kRowsThreads) {
-    const int r = i / kWPitch, m = i - r * kWPitch;
-    ws[i] = m < nb ? __ldg(w + (size_t)(r0 + r) * nb + m) : 0.f;
-  }
-  __syncthreads();
-}
-
-// ah = sum_e val_e * A[col_e][lane] (pitch lda), ax = sum_e val_e * B[col_e][lane] (pitch ldb, lanes < nx) over CSR row i, in entry order.
-template <bool WITH_A>
-__device__ __forceinline__ void gather_row(const int* __restrict__ rowptr, const int2* __restrict__ cv, int i, const float* __restrict__ A,
-                                           int lda, const float* __restrict__ Bx, int ldb, int nx, int lane, float& ah, float& ax) {
-  const int beg = __ldg(rowptr + i), end = __ldg(rowptr + i + 1);
-  const bool xl = lane < nx;
-  ah = 0.f;
-  ax = 0.f;
-  int k = beg;
-  for (; k + 4 <= end; k += 4) {
-    int2 e[4];
-    float av[4], bv[4];
-#pragma unroll
-    for (int u = 0; u < 4; ++u) e[u] = __ldg(cv + k + u);
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      av[u] = WITH_A ? __ldg(A + (size_t)e[u].x * lda + lane) : 0.f;
-      bv[u] = xl ? __ldg(Bx + (size_t)e[u].x * ldb + lane) : 0.f;
-    }
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const float w = __int_as_float(e[u].y);
-      if (WITH_A) ah = __fadd_rn(ah, __fmul_rn(w, av[u]));
-      if (xl) ax = __fadd_rn(ax, __fmul_rn(w, bv[u]));
-    }
-  }
-  for (; k < end; ++k) {
-    const int2 e = __ldg(cv + k);
-    const float w = __int_as_float(e.y);
-    if (WITH_A) ah = __fadd_rn(ah, __fmul_rn(w, __ldg(A + (size_t)e.x * lda + lane)));
-    if (xl) ax = __fadd_rn(ax, __fmul_rn(w, __ldg(Bx + (size_t)e.x * ldb + lane)));
-  }
-}
 
 struct RowsFwd {
   const int* rowptr; const int2* cv;         // operator 0 by destination (n_ops = 1)
@@ -320,18 +272,9 @@ __global__ void k_gru_rows_pack(int nops, int cin, const float* __restrict__ wx,
 
 using namespace stmp;
 
-static int rows_grid(int n) {
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int tiles = (n + kRowTile - 1) / kRowTile;
-  return tiles < 2 * sms ? (tiles > 0 ? tiles : 1) : 2 * sms;
-}
-
 static bool rows_supported(const stmp_plan* plan, int n_ops, int64_t cin, int64_t cout) {
   return plan && n_ops >= 0 && n_ops <= 1 && n_ops <= plan->n_ops && cout == kCo && cin >= 1 && cin <= kMaxCin;
 }
-
-static bool al4(const void* p) { return ((uintptr_t)p & 3u) == 0; }
 
 extern "C" int stmp_gru_rows_supported(const stmp_plan* plan, int n_ops, int64_t cin, int64_t cout) {
   return rows_supported(plan, n_ops, cin, cout) ? 1 : 0;

@@ -1,0 +1,77 @@
+// rows.cuh -- the pieces shared by the row-split recurrent cells (gru_rows.cu, lstm_rows.cu): one warp per destination row, lane = output
+// channel, CTAs owning grid-strided tiles of kRowTile rows, weights staged once per CTA at pitch kWPitch, and the entry-order CSR gather.
+#pragma once
+#include "common.cuh"
+
+namespace stmp {
+namespace rows {
+
+constexpr int kCo = 32;
+constexpr int kRowsThreads = 256;
+constexpr int kRowsWarps = kRowsThreads / 32;
+constexpr int kRowTile = 16;                 // destination rows per CTA tile: two per warp
+constexpr int kWPitch = 97;                  // shared-memory pitch of a staged weight row (basis columns 0..95)
+constexpr int kMaxCin = 16;
+
+// rows [r0, r0 + nr) of packed weights w [..][nb] -> ws [nr][kWPitch] (columns >= nb zero)
+__device__ __forceinline__ void stage_w(float* ws, const float* __restrict__ w, int nb, int r0, int nr) {
+  for (int i = threadIdx.x; i < nr * kWPitch; i += kRowsThreads) {
+    const int r = i / kWPitch, m = i - r * kWPitch;
+    ws[i] = m < nb ? __ldg(w + (size_t)(r0 + r) * nb + m) : 0.f;
+  }
+  __syncthreads();
+}
+
+// ah = sum_e val_e * A[col_e][lane] (pitch lda), ax = sum_e val_e * B[col_e][lane] (pitch ldb, lanes < nx) over CSR row i, in entry order.
+template <bool WITH_A>
+__device__ __forceinline__ void gather_row(const int* __restrict__ rowptr, const int2* __restrict__ cv, int i, const float* __restrict__ A,
+                                           int lda, const float* __restrict__ Bx, int ldb, int nx, int lane, float& ah, float& ax) {
+  const int beg = __ldg(rowptr + i), end = __ldg(rowptr + i + 1);
+  const bool xl = lane < nx;
+  ah = 0.f;
+  ax = 0.f;
+  int k = beg;
+  for (; k + 4 <= end; k += 4) {
+    int2 e[4];
+    float av[4], bv[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) e[u] = __ldg(cv + k + u);
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      av[u] = WITH_A ? __ldg(A + (size_t)e[u].x * lda + lane) : 0.f;
+      bv[u] = xl ? __ldg(Bx + (size_t)e[u].x * ldb + lane) : 0.f;
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const float w = __int_as_float(e[u].y);
+      if (WITH_A) ah = __fadd_rn(ah, __fmul_rn(w, av[u]));
+      if (xl) ax = __fadd_rn(ax, __fmul_rn(w, bv[u]));
+    }
+  }
+  for (; k < end; ++k) {
+    const int2 e = __ldg(cv + k);
+    const float w = __int_as_float(e.y);
+    if (WITH_A) ah = __fadd_rn(ah, __fmul_rn(w, __ldg(A + (size_t)e.x * lda + lane)));
+    if (xl) ax = __fadd_rn(ax, __fmul_rn(w, __ldg(Bx + (size_t)e.x * ldb + lane)));
+  }
+}
+
+// CTAs of a row-split launch over n rows: one per 16-row tile, at most two per SM (the tiles are grid-strided beyond that)
+inline int rows_grid(int n) {
+  int dev = 0, sms = 132;
+  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int tiles = (n + kRowTile - 1) / kRowTile;
+  return tiles < 2 * sms ? (tiles > 0 ? tiles : 1) : 2 * sms;
+}
+
+inline bool al4(const void* p) { return ((uintptr_t)p & 3u) == 0; }
+
+}  // namespace rows
+
+// The FFMA weight-gradient contraction of train.cu (k_dcrnn_wgrad<N2>): per-CTA partials [parts][MG*8*(64+N2) + 64+N2] of
+// S1^T A (A: rows x 64) and S2^T B (B: rows x N2, N2 = 32 or 64) and the column sums of A and B, over strided 16-row tiles.
+int wgrad_ffma_launch(int n2, long long rows, int ld, const float* S1, const float* S2, const float* A, const float* B, float* partial,
+                      cudaStream_t st, int* parts);
+int wgrad_ffma_max_parts();
+
+}  // namespace stmp

@@ -13,7 +13,7 @@
 //                               parameter / gradient buffer of distributed.FlatGradSync: one launch instead of the ~35 of the
 //                               capturable foreach implementation; the step counter lives on the device (CUDA-graph replay), the
 //                               gradient average over ranks and the zeroing of the gradient buffer are folded in.
-#include "common.cuh"
+#include "rows.cuh"
 
 namespace stmp {
 int wgrad_tc_launch(int c3, long long rows, int ld, const float* S1, const float* S2, const float* dpzr, const float* dph, float* partial,
@@ -29,15 +29,17 @@ struct WgradParams {
   const float* S1; const float* S2; const float* dpzr; const float* dph;
   long long rows;
   int ld, n_tiles, MG;
-  float* partial;                    // [grid][MG*8*96 + 96]
+  float* partial;                    // [grid][MG*8*(64+N2) + 64+N2]
 };
 
 __device__ __forceinline__ float4 ld4s(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
+// N2 = the column count of the second operand: 32 for the GRU cells (S2^T dph), 64 for the LSTM cell (S^T [dpc | dpo]).
+template <int N2>
 __global__ void __launch_bounds__(kWgThreads, 2) k_dcrnn_wgrad(WgradParams p) {
   extern __shared__ __align__(128) unsigned char smraw[];
   const int ld = p.ld, tid = threadIdx.x, MG = p.MG;
-  const int stage_floats = kWgTK * (2 * ld + 3 * kCo);
+  const int stage_floats = kWgTK * (2 * ld + 2 * kCo + N2);
   float* stages = reinterpret_cast<float*>(smraw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smraw + (size_t)kWgStages * stage_floats * 4);
   if (tid == 0) {
@@ -50,23 +52,25 @@ __global__ void __launch_bounds__(kWgThreads, 2) k_dcrnn_wgrad(WgradParams p) {
     const long long r0 = (long long)tile * kWgTK;
     const int nr = (int)((p.rows - r0) < kWgTK ? (p.rows - r0) : kWgTK);
     float* st = stages + (size_t)s * stage_floats;
-    const uint32_t bs = (uint32_t)nr * ld * 4u, bzr = (uint32_t)nr * 2 * kCo * 4u, bh = (uint32_t)nr * kCo * 4u;
+    const uint32_t bs = (uint32_t)nr * ld * 4u, bzr = (uint32_t)nr * 2 * kCo * 4u, bh = (uint32_t)nr * N2 * 4u;
     mbar_arrive_expect_tx(&bars[s], 2 * bs + bzr + bh);
     tma_bulk_g2s(st, p.S1 + r0 * ld, bs, &bars[s]);
     tma_bulk_g2s(st + kWgTK * ld, p.S2 + r0 * ld, bs, &bars[s]);
     tma_bulk_g2s(st + 2 * kWgTK * ld, p.dpzr + r0 * 2 * kCo, bzr, &bars[s]);
-    tma_bulk_g2s(st + 2 * kWgTK * ld + kWgTK * 2 * kCo, p.dph + r0 * kCo, bh, &bars[s]);
+    tma_bulk_g2s(st + 2 * kWgTK * ld + kWgTK * 2 * kCo, p.dph + r0 * N2, bh, &bars[s]);
   };
 
-  // roles: threads [0, 8 MG) own the 8x8 tiles of S1^T dpzr (MG x 8 tiles), threads [8 MG, 12 MG) those of S2^T dph (MG x 4)
-  const int n1 = 8 * MG, n2 = 4 * MG;
+  // roles: threads [0, 8 MG) own the 8x8 tiles of S1^T dpzr (MG x 8 tiles), threads [8 MG, (8 + N2/8) MG) those of S2^T dph (MG x N2/8)
+  constexpr int NG2 = N2 / 8;
+  const int n1 = 8 * MG, n2 = NG2 * MG;
   const bool prod = tid >= n1;
   const bool active = tid < n1 + n2;
   const int u = prod ? tid - n1 : tid;
-  const int mg = prod ? (u >> 2) : (u >> 3), ng = prod ? (u & 3) : (u & 7);
+  constexpr int LG2 = N2 == 64 ? 3 : 2;
+  const int mg = prod ? (u >> LG2) : (u >> 3), ng = prod ? (u & (NG2 - 1)) : (u & 7);
   const int a_off = (prod ? kWgTK * ld : 0) + 8 * mg;
   const int b_off = 2 * kWgTK * ld + (prod ? kWgTK * 2 * kCo : 0) + 8 * ng;
-  const int b_pitch = prod ? kCo : 2 * kCo;
+  const int b_pitch = prod ? N2 : 2 * kCo;
 
   float acc[8][8], bsum[8];
 #pragma unroll
@@ -109,7 +113,7 @@ __global__ void __launch_bounds__(kWgThreads, 2) k_dcrnn_wgrad(WgradParams p) {
     __syncthreads();
   }
   if (active) {
-    float* out = p.partial + (size_t)blockIdx.x * ((size_t)MG * 8 * 3 * kCo + 3 * kCo);
+    float* out = p.partial + (size_t)blockIdx.x * ((size_t)MG * 8 * (2 * kCo + N2) + 2 * kCo + N2);
     float* o = prod ? out + (size_t)MG * 8 * 2 * kCo : out;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -118,7 +122,7 @@ __global__ void __launch_bounds__(kWgThreads, 2) k_dcrnn_wgrad(WgradParams p) {
       q[1] = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
     }
     if (mg == 0) {
-      float4* q = reinterpret_cast<float4*>(out + (size_t)MG * 8 * 3 * kCo + (prod ? 2 * kCo : 0) + 8 * ng);
+      float4* q = reinterpret_cast<float4*>(out + (size_t)MG * 8 * (2 * kCo + N2) + (prod ? 2 * kCo : 0) + 8 * ng);
       q[0] = make_float4(bsum[0], bsum[1], bsum[2], bsum[3]);
       q[1] = make_float4(bsum[4], bsum[5], bsum[6], bsum[7]);
     }
@@ -329,8 +333,8 @@ extern "C" int stmp_dcrnn_bwd_wgrad(int64_t cin, int64_t cout, int64_t K, int64_
   } else {
     if (p.n_tiles < grid) grid = p.n_tiles > 0 ? p.n_tiles : 1;
     const int smem = kWgStages * kWgTK * (2 * (int)ld + 3 * kCo) * 4 + 64;
-    STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    k_dcrnn_wgrad<<<grid, kWgThreads, smem, st>>>(p);
+    STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_wgrad<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    k_dcrnn_wgrad<32><<<grid, kWgThreads, smem, st>>>(p);
     STMP_LAUNCH_OK("k_dcrnn_wgrad");
   }
   const int total = 3 * 4 * C * kCo + 3 * kCo;
@@ -393,14 +397,39 @@ extern "C" int stmp_gru_rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t
   int grid = wgrad_grid();
   if (p.n_tiles < grid) grid = p.n_tiles;
   const int smem = kWgStages * kWgTK * (2 * (int)ld + 3 * kCo) * 4 + 64;
-  STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  k_dcrnn_wgrad<<<grid, kWgThreads, smem, st>>>(p);
+  STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_wgrad<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  k_dcrnn_wgrad<32><<<grid, kWgThreads, smem, st>>>(p);
   STMP_LAUNCH_OK("k_dcrnn_wgrad");
   const int total = 96 * nb + 3 * kCo;
   k_gru_rows_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(grid, MG, nb, p.partial, dw, db);
   STMP_LAUNCH_OK("k_gru_rows_wgrad_reduce");
   return STMP_OK;
 }
+
+namespace stmp {
+int wgrad_ffma_max_parts() { return wgrad_grid(); }
+
+int wgrad_ffma_launch(int n2, long long rows, int ld, const float* S1, const float* S2, const float* A, const float* B, float* partial,
+                      cudaStream_t st, int* parts) {
+  WgradParams p;
+  p.S1 = S1; p.S2 = S2; p.dpzr = A; p.dph = B; p.rows = rows; p.ld = ld; p.MG = ld / 8;
+  p.n_tiles = (int)((rows + kWgTK - 1) / kWgTK);
+  p.partial = partial;
+  int grid = wgrad_grid();
+  if (p.n_tiles < grid) grid = p.n_tiles > 0 ? p.n_tiles : 1;
+  const int smem = kWgStages * kWgTK * (2 * ld + 2 * kCo + n2) * 4 + 64;
+  if (n2 == 64) {
+    STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_wgrad<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    k_dcrnn_wgrad<64><<<grid, kWgThreads, smem, st>>>(p);
+  } else {
+    STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_wgrad<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    k_dcrnn_wgrad<32><<<grid, kWgThreads, smem, st>>>(p);
+  }
+  STMP_LAUNCH_OK("k_dcrnn_wgrad");
+  *parts = grid;
+  return STMP_OK;
+}
+}  // namespace stmp
 
 extern "C" int stmp_adam_flat(int64_t n, float* param, float* grad, float* exp_avg, float* exp_avg_sq, float* step, void* ticket, float lr,
                               float beta1, float beta2, float eps, float weight_decay, float grad_scale, int zero_grad, void* stream) {

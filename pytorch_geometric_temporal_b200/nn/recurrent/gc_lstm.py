@@ -7,7 +7,11 @@ The reference runs four ChebConvs on the same H (4(K-1) propagations) and four `
 T_k(H) is computed once ((K-1) SpMMs on `out` channels, written in place into the basis buffer
 S = [X | T_0(H) | .. | T_{K-1}(H)]) and ONE GEMM produces all four gate pre-activations; without autograd that GEMM
 is the wgmma kernel with the LSTM gate chain in its epilogue (`stmp_gemm_lstm_f32`, zero peepholes -- GCLSTM has
-none, and its output gate therefore does not depend on the new cell state, gc_lstm.py:139-145)."""
+none, and its output gate therefore does not depend on the new cell state, gc_lstm.py:139-145).
+
+Inside the row-split envelope (K <= 2, out_channels = 32, in_channels <= 16, 2-D X; any graph) a step is one launch of the row-split
+LSTM cell kernel with the basis [X | H | Op H] and no peepholes, for inference and training alike; training adds its hand-written
+backward (ops.lstm_rows_train)."""
 import torch
 
 from ... import _lib, ops
@@ -34,6 +38,8 @@ class GCLSTM(torch.nn.Module, ChebPlanMixin):
         self.register_buffer("_no_peephole", torch.zeros(out_channels), persistent=False)
         self._init_plans()
         self._pack = ops.PackCache()
+        self._rows_pack = ops.PackCache()
+        self.fused_training = True      # False: op-for-op autograd path (tests compare the two)
 
     def _weight(self):
         """(in + K*out, 4*out): rows [W_g ; lins[0]^T ; .. ; lins[K-1]^T], gate columns i,f,c,o."""
@@ -51,17 +57,65 @@ class GCLSTM(torch.nn.Module, ChebPlanMixin):
             bs.append(b if cb is None else b + cb)
         return bs
 
+    def _rows_packed(self):
+        """(w [128, nb], b [128]) for stmp_lstm_rows_fwd: columns [X | H | Op H] (W_g transposed), b = conv_g.bias + b_g (one pack launch
+        per weight update)."""
+        def build():
+            convs = [getattr(self, f"conv_{g}") for g in "ifco"]
+            wx = torch.stack([getattr(self, f"W_{g}") for g in "ifco"])
+            wh = torch.stack([torch.stack([c.lins[k].weight for k in range(self.K)]) for c in convs])
+            bh = torch.stack([c.bias for c in convs]) if self.bias else None
+            bg = torch.cat([getattr(self, f"b_{g}") for g in "ifco"])
+            return ops.lstm_rows_pack_weights(_lib.LSTM_GC, self.K - 1, self.in_channels, wx, wh, None, bh, bg)
+        return self._rows_pack.get(list(self.parameters()), build)
+
+    def _rows_spec(self):
+        """(spec, params) of ops.lstm_rows_train: where each parameter's gradient sits in the packed weight gradient (128, nb) and the bias
+        gradient -- the inverse of `_rows_packed`.  W_g (in, out) receives its block transposed; both biases of a gate get the gate's block."""
+        spec, params = [], []
+        Ci = self.in_channels
+        for gi, g in enumerate("ifco"):
+            conv = getattr(self, f"conv_{g}")
+            spec.append(("wt", 32 * gi, 32, 0, Ci))
+            params.append(getattr(self, f"W_{g}"))
+            for k in range(self.K):
+                spec.append(("w", 32 * gi, 32, Ci + 32 * k, 32))
+                params.append(conv.lins[k].weight)
+            if conv.bias is not None:
+                spec.append(("b", 32 * gi, 32))
+                params.append(conv.bias)
+            spec.append(("b", 32 * gi, 32))
+            params.append(getattr(self, f"b_{g}"))
+        return spec, params
+
+    def _rows_ok(self, plan, X, H, C, training):
+        """The row-split route: K <= 2, out_channels = 32, in_channels <= 16, 2-D float32 X, H and C None or (N, 32) float32 (the module's
+        attributes are checked before the library is consulted); training calls also need `fused_training`."""
+        if self.K > 2 or self.out_channels != 32 or self.in_channels > 16 or X.dim() != 2 or X.dtype != torch.float32:
+            return False
+        if any(S is not None and (S.shape != (X.size(0), 32) or S.dtype != torch.float32) for S in (H, C)):
+            return False
+        if training and not self.fused_training:
+            return False
+        return ops.lstm_rows_supported(plan, _lib.LSTM_GC, self.K - 1, self.in_channels, 32)
+
     def forward(self, X: torch.FloatTensor, edge_index: torch.LongTensor, edge_weight: torch.FloatTensor = None,
                 H: torch.FloatTensor = None, C: torch.FloatTensor = None, lambda_max: torch.Tensor = None):
         _require_cuda(X, "X")
         N, Ci, Co, K = X.size(-2), self.in_channels, self.out_channels, self.K
+        plan = self._cheb_plan(edge_index, edge_weight, N, self.normalization, lambda_max)
+        needs_grad = torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters()) or X.requires_grad
+                                                  or (H is not None and H.requires_grad) or (C is not None and C.requires_grad))
+        if self._rows_ok(plan, X, H, C, needs_grad):    # the row-split cell kernel (stmp_lstm_rows_*): one launch per step
+            w, b = self._rows_packed()
+            if needs_grad:
+                spec, params = self._rows_spec()
+                return ops.lstm_rows_train(plan, _lib.LSTM_GC, K - 1, X, H, C, w, b, None, spec, params)
+            return ops.lstm_rows_fwd(plan, _lib.LSTM_GC, K - 1, X, H, C, w, b, None)
         if H is None:
             H = torch.zeros(*X.shape[:-1], Co, device=X.device, dtype=X.dtype)
         if C is None:
             C = torch.zeros(*X.shape[:-1], Co, device=X.device, dtype=X.dtype)
-        plan = self._cheb_plan(edge_index, edge_weight, N, self.normalization, lambda_max)
-        needs_grad = torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters()) or X.requires_grad
-                                                  or H.requires_grad or C.requires_grad)
         width = Ci + K * Co
         if not needs_grad:
             # the basis is built in place: T_k(H) lands in its column block of S straight from the SpMM kernel

@@ -3,7 +3,11 @@
 H, C, lambda_max) -> (H, C)`, state_dict keys `conv_{x,h}_{i,f,c,o}.lins.{k}.weight/.bias`,
 `w_c_{i,f,o} (1,out)` (glorot), `b_{i,f,c,o} (1,out)` (zeros).  Eight ChebConvs per step in the
 reference = 8(K-1) propagations; here T_k([X|H]) is computed once (K-1 SpMMs on Ci+Co channels) and one
-GEMM produces all four gate pre-activations."""
+GEMM produces all four gate pre-activations.
+
+Inside the row-split envelope (K <= 2, out_channels = 32, in_channels <= 16, 2-D X; any graph) a step is one launch of the row-split
+LSTM cell kernel for inference and training alike, and training adds a hand-written backward (ops.lstm_rows_train): the gradients of
+the packed weights are handed to the parameters as blocks, so the cached pack needs no autograd graph."""
 import torch
 
 from ... import _lib, ops
@@ -120,6 +124,7 @@ class GConvLSTM(torch.nn.Module, ChebPlanMixin):
             torch.nn.init.zeros_(getattr(self, f"b_{g}"))
         self._init_plans()
         self._pack = ops.PackCache()
+        self._rows_pack = ops.PackCache()
         self._train_cache = None
         self.fused_training = True      # False: op-for-op autograd path (tests compare the two)
 
@@ -156,17 +161,70 @@ class GConvLSTM(torch.nn.Module, ChebPlanMixin):
             return None
         return torch.cat([getattr(self, f"conv_x_{g}").bias + getattr(self, f"conv_h_{g}").bias for g in "ifco"])
 
+    def _rows_packed(self):
+        """(w [128, nb], b [128], peep [3, 32]) for stmp_lstm_rows_fwd: columns [X | H | Op X | Op H], b = the sum of a gate's three biases
+        (one pack launch per weight update)."""
+        def build():
+            cx = [getattr(self, f"conv_x_{g}") for g in "ifco"]
+            ch = [getattr(self, f"conv_h_{g}") for g in "ifco"]
+            wx = torch.stack([torch.stack([c.lins[k].weight for k in range(self.K)]) for c in cx])
+            wh = torch.stack([torch.stack([c.lins[k].weight for k in range(self.K)]) for c in ch])
+            bx = bh = None
+            if self.bias:
+                bx, bh = torch.stack([c.bias for c in cx]), torch.stack([c.bias for c in ch])
+            bg = torch.cat([getattr(self, f"b_{g}") for g in "ifco"])
+            w, b = ops.lstm_rows_pack_weights(_lib.LSTM_GCONV, self.K - 1, self.in_channels, wx, wh, bx, bh, bg)
+            return w, b, torch.cat([self.w_c_i, self.w_c_f, self.w_c_o])
+        return self._rows_pack.get(list(self.parameters()), build)
+
+    def _rows_spec(self):
+        """(spec, params) of ops.lstm_rows_train: where each parameter's gradient sits in the packed weight gradient (128, nb) and the
+        bias | peephole gradient (224,) -- the inverse of `_rows_packed`.  Every bias of a gate receives that gate's block."""
+        spec, params = [], []
+        Ci, C = self.in_channels, self.in_channels + 32
+        for gi, g in enumerate("ifco"):
+            cx, ch = getattr(self, f"conv_x_{g}"), getattr(self, f"conv_h_{g}")
+            for k in range(self.K):
+                spec += [("w", 32 * gi, 32, k * C, Ci), ("w", 32 * gi, 32, k * C + Ci, 32)]
+                params += [cx.lins[k].weight, ch.lins[k].weight]
+            if cx.bias is not None:
+                spec += [("b", 32 * gi, 32), ("b", 32 * gi, 32)]
+                params += [cx.bias, ch.bias]
+            spec.append(("b", 32 * gi, 32))
+            params.append(getattr(self, f"b_{g}"))
+        for j, g in enumerate("ifo"):
+            spec.append(("b", 128 + 32 * j, 32))
+            params.append(getattr(self, f"w_c_{g}"))
+        return spec, params
+
+    def _rows_ok(self, plan, X, H, C, training):
+        """The row-split route: K <= 2, out_channels = 32, in_channels <= 16, 2-D float32 X, H and C None or (N, 32) float32 (the module's
+        attributes are checked before the library is consulted); training calls also need `fused_training`."""
+        if self.K > 2 or self.out_channels != 32 or self.in_channels > 16 or X.dim() != 2 or X.dtype != torch.float32:
+            return False
+        if any(S is not None and (S.shape != (X.size(0), 32) or S.dtype != torch.float32) for S in (H, C)):
+            return False
+        if training and not self.fused_training:
+            return False
+        return ops.lstm_rows_supported(plan, _lib.LSTM_GCONV, self.K - 1, self.in_channels, 32)
+
     def forward(self, X: torch.FloatTensor, edge_index: torch.LongTensor, edge_weight: torch.FloatTensor = None,
                 H: torch.FloatTensor = None, C: torch.FloatTensor = None, lambda_max: torch.Tensor = None):
         _require_cuda(X, "X")
         N, Co = X.size(-2), self.out_channels
+        plan = self._cheb_plan(edge_index, edge_weight, N, self.normalization, lambda_max)
+        needs_grad = torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters()) or X.requires_grad
+                                                  or (H is not None and H.requires_grad) or (C is not None and C.requires_grad))
+        if self._rows_ok(plan, X, H, C, needs_grad):    # the row-split cell kernel (stmp_lstm_rows_*): one launch per step
+            w, b, peep = self._rows_packed()
+            if needs_grad:
+                spec, params = self._rows_spec()
+                return ops.lstm_rows_train(plan, _lib.LSTM_GCONV, self.K - 1, X, H, C, w, b, peep, spec, params)
+            return ops.lstm_rows_fwd(plan, _lib.LSTM_GCONV, self.K - 1, X, H, C, w, b, peep)
         if H is None:
             H = torch.zeros(*X.shape[:-1], Co, device=X.device, dtype=X.dtype)
         if C is None:
             C = torch.zeros(*X.shape[:-1], Co, device=X.device, dtype=X.dtype)
-        plan = self._cheb_plan(edge_index, edge_weight, N, self.normalization, lambda_max)
-        needs_grad = torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters()) or X.requires_grad
-                                                  or H.requires_grad or C.requires_grad)
         Cw = self.in_channels + Co
         if not needs_grad and Co in (32, 64) and (self.K * Cw) % 4 == 0 and Cw % 4 == 0:
             # large-graph inference: T_k written in place into S = [T_0|T_1|..] by the SpMM kernel, then ONE wgmma

@@ -224,12 +224,15 @@ def gru_bwd_wgrad(n_ops: int, cin: int, S1, S2, dpzr_all, dph_all, has_bias: boo
 
 
 def _spec_grads(spec, dw, db):
-    """Parameter gradients as blocks of packed weight / bias gradients: ("w", row, n_rows, col, n_cols) -> dw[row:row+n_rows, col:col+n_cols],
-    ("b", row, n_rows) -> db[row:row+n_rows].  Parameters that share a block of db each get their own copy, so no two .grad tensors alias."""
+    """Parameter gradients as blocks of packed weight / bias gradients: ("w", row, n_rows, col, n_cols) -> dw[row:row+n_rows, col:col+n_cols]
+    (("wt", ...) -> its transpose), ("b", row, n_rows) -> db[row:row+n_rows].  Parameters that share a block of db each get their own copy,
+    so no two .grad tensors alias."""
     grads, dbs = [None] * len(spec), None
     for i, s in enumerate(spec):
-        if s[0] == "w":
+        if s[0] in ("w", "wt"):
             grads[i] = dw[s[1]:s[1] + s[2], s[3]:s[3] + s[4]]
+            if s[0] == "wt":
+                grads[i] = grads[i].t()
         else:
             if dbs is None:
                 dbs = db.expand(sum(1 for q in spec if q[0] == "b"), db.numel()).clone()
@@ -394,6 +397,142 @@ class _GruRowsFn(torch.autograd.Function):
 def gru_rows_train(plan: GraphPlan, n_ops: int, x, h, w, b, spec, params) -> torch.Tensor:
     """Differentiable (w.r.t. x, h and `params`, see _GruRowsFn) row-split graph-GRU cell.  x (N, cin), h (N, 32) or None (zeros, no dH)."""
     return _GruRowsFn.apply(plan, n_ops, x, h, w, b, tuple(spec), *params)
+
+
+def lstm_rows_supported(plan: GraphPlan, variant: int, n_ops: int, cin: int, cout: int) -> bool:
+    return bool(_lib.lib().stmp_lstm_rows_supported(plan.handle, variant, n_ops, cin, cout))
+
+
+def lstm_rows_nb(variant: int, n_ops: int, cin: int) -> int:
+    """Basis columns of the row-split LSTM cell: (n_ops+1)(cin+32) for GConvLSTM ([X | H | Op X | Op H]), cin + 32(n_ops+1) for GCLSTM."""
+    return cin + 32 * (n_ops + 1) if variant == _lib.LSTM_GC else (n_ops + 1) * (cin + 32)
+
+
+def lstm_rows_basis_ld(variant: int, n_ops: int, cin: int) -> int:
+    """Row pitch of the row-split LSTM cell's weight-gradient basis: nb rounded up to 8 floats."""
+    return (lstm_rows_nb(variant, n_ops, cin) + 7) // 8 * 8
+
+
+def lstm_rows_pack_weights(variant: int, n_ops: int, cin: int, wx, wh, bx, bh, bg):
+    """(w (128, nb), b (128,)): the row-split LSTM cell's packed weights from the parameters' layout in one launch
+    (stmp_lstm_rows_pack_weights).  GConvLSTM: wx (4, n_ops+1, 32, cin), wh (4, n_ops+1, 32, 32), bx / bh (4, 32) or None;
+    GCLSTM: wx (4, cin, 32) (the dense W_g), wh as above, bx None, bh (4, 32) or None.  bg (4, 32): the gates' own biases b_g."""
+    wx, wh, bg = _f32c(wx, "wx"), _f32c(wh, "wh"), _f32c(bg, "bg")
+    want_x = (4, cin, 32) if variant == _lib.LSTM_GC else (4, n_ops + 1, 32, cin)
+    if wx.shape != want_x or wh.shape != (4, n_ops + 1, 32, 32) or bg.shape != (4, 32):
+        raise RuntimeError(f"lstm_rows_pack_weights: wx must be {want_x}, wh (4, n_ops+1, 32, 32) and bg (4, 32)")
+    bx = None if bx is None else _f32c(bx, "bx")
+    bh = None if bh is None else _f32c(bh, "bh")
+    w = torch.empty(128, lstm_rows_nb(variant, n_ops, cin), device=wx.device, dtype=torch.float32)
+    b = torch.empty(128, device=wx.device, dtype=torch.float32)
+    with torch.cuda.device(wx.device):
+        _lib.check(_lib.lib().stmp_lstm_rows_pack_weights(variant, n_ops, cin, _lib.ptr(wx), _lib.ptr(wh), _lib.ptr(bx), _lib.ptr(bh),
+                                                          _lib.ptr(bg), _lib.ptr(w), _lib.ptr(b), _lib.stream_ptr()))
+    return w, b
+
+
+def lstm_rows_fwd(plan: GraphPlan, variant: int, n_ops: int, x: torch.Tensor, h: Optional[torch.Tensor], c: Optional[torch.Tensor],
+                  w: torch.Tensor, b: torch.Tensor, peep: Optional[torch.Tensor], train: bool = False):
+    """Row-split peephole graph-LSTM cell (stmp_lstm_rows_fwd) on one graph: x (N, cin), h and c (N, 32) or None (zeros) -> (H', C').
+    peep (3, 32) = w_c_i | w_c_f | w_c_o, or None.  With `train`, returns (H', C', stash (4, N, 32), S) -- the operands of lstm_rows_bwd /
+    lstm_rows_wgrad."""
+    x, w, b = _f32c(x, "X"), _f32c(w, "w"), _f32c(b, "b")
+    N, cin = x.shape
+    f32 = dict(device=x.device, dtype=torch.float32)
+    hc = None if h is None else _f32c(h, "H")
+    cc = None if c is None else _f32c(c, "C")
+    pc = None if peep is None else _f32c(peep, "peep")
+    hout, cout = torch.empty(N, 32, **f32), torch.empty(N, 32, **f32)
+    st = S = None
+    ld = lstm_rows_basis_ld(variant, n_ops, cin)
+    if train:
+        st = torch.empty(4, N, 32, **f32)
+        S = torch.empty(N, ld, **f32)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.lib().stmp_lstm_rows_fwd(plan.handle, variant, n_ops, cin, _lib.ptr(x), _lib.ptr(hc), _lib.ptr(cc), _lib.ptr(w),
+                                                 _lib.ptr(b), _lib.ptr(pc), _lib.ptr(hout), _lib.ptr(cout), _lib.ptr(st), _lib.ptr(S), ld,
+                                                 _lib.stream_ptr()))
+    return (hout, cout, st, S) if train else (hout, cout)
+
+
+def lstm_rows_bwd(plan: GraphPlan, variant: int, n_ops: int, gh, gc, c, cn, stash, w, peep, want_dx: bool, want_dh: bool, want_dc: bool,
+                  cin: int):
+    """(dpre (2, N, 64), dx (N, cin) or None, dh or None, dc or None, scratch) of the row-split LSTM cell (stmp_lstm_rows_bwd); gh / gc
+    may be None.  The scratch carries the per-CTA peephole sums to lstm_rows_wgrad."""
+    N = cn.size(0)
+    f32 = dict(device=cn.device, dtype=torch.float32)
+    gh = None if gh is None else _f32c(gh, "gH")
+    gc = None if gc is None else _f32c(gc, "gC")
+    scr = torch.empty(int(_lib.lib().stmp_lstm_rows_scratch_bytes(plan.handle)) // 4, **f32)
+    dpre = torch.empty(2, N, 64, **f32)
+    dx = torch.empty(N, cin, **f32) if want_dx else None
+    dh = torch.empty(N, 32, **f32) if want_dh else None
+    dc = torch.empty(N, 32, **f32) if want_dc else None
+    with torch.cuda.device(cn.device):
+        _lib.check(_lib.lib().stmp_lstm_rows_bwd(plan.handle, variant, n_ops, cin, _lib.ptr(gh), _lib.ptr(gc), _lib.ptr(c), _lib.ptr(cn),
+                                                 _lib.ptr(stash), _lib.ptr(w), _lib.ptr(peep), _lib.ptr(scr), _lib.ptr(dpre), _lib.ptr(dx),
+                                                 _lib.ptr(dh), _lib.ptr(dc), _lib.stream_ptr()))
+    return dpre, dx, dh, dc, scr
+
+
+def lstm_rows_wgrad(variant: int, n_ops: int, cin: int, S, dpre, scratch, has_peep: bool):
+    """(dw (128, nb), dbp (224,)): the packed weights' gradient and, in one vector, the summed biases' gradient dbp[:128] and the
+    peepholes' dbp[128:] (left unwritten without peepholes) of the row-split LSTM cell, two launches."""
+    dev = S.device
+    key = (dev, torch.cuda.current_stream(dev).cuda_stream, "lstm_rows", variant, n_ops, cin)
+    ws = _WGRAD_WS.get(key)
+    if ws is None:
+        ws = torch.empty(int(_lib.lib().stmp_lstm_rows_wgrad_workspace_bytes(variant, n_ops, cin)), device=dev, dtype=torch.uint8)
+        _WGRAD_WS[key] = ws
+    dw = torch.empty(128, lstm_rows_nb(variant, n_ops, cin), device=dev, dtype=torch.float32)
+    dbp = torch.empty(128 + 96, device=dev, dtype=torch.float32)
+    dpeep = dbp[128:] if has_peep else None
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().stmp_lstm_rows_wgrad(variant, n_ops, cin, S.size(0), S.size(1), _lib.ptr(S), _lib.ptr(dpre), _lib.ptr(scratch),
+                                                   _lib.ptr(ws), _lib.ptr(dw), _lib.ptr(dbp), _lib.ptr(dpeep), _lib.stream_ptr()))
+    return dw, dbp
+
+
+class _LstmRowsFn(torch.autograd.Function):
+    """Training form of the row-split peephole graph-LSTM cell.  forward = `stmp_lstm_rows_fwd` with the stash and the weight-gradient basis
+    (the inference launch, so (H', C') are bit-identical to the `no_grad` ones); backward = `stmp_lstm_rows_bwd` + `stmp_lstm_rows_wgrad`:
+    dX (when x requires grad), dH / dC (when h / c are given and require grad) and the packed weights', summed biases' and peepholes'
+    gradients, handed to `params` as blocks described by `spec` (see _spec_grads; the peepholes sit in the bias vector after its 128
+    entries).  Either output's gradient may be None."""
+
+    @staticmethod
+    def forward(ctx, plan, variant, n_ops, x, h, c, w, b, peep, spec, *params):
+        ctx.set_materialize_grads(False)
+        x = _f32c(x.detach(), "X")
+        hc = None if h is None else _f32c(h.detach(), "H")
+        cc = None if c is None else _f32c(c.detach(), "C")
+        hout, cout, stash, S = lstm_rows_fwd(plan, variant, n_ops, x, hc, cc, w, b, peep, train=True)
+        ctx.plan, ctx.variant, ctx.n_ops, ctx.spec, ctx.cin = plan, variant, n_ops, spec, x.size(1)
+        ctx.has_h, ctx.shapes = hc is not None, [p.shape for p in params]
+        ctx.save_for_backward(cc, cout, stash, S, w, peep)
+        return hout, cout
+
+    @staticmethod
+    def backward(ctx, gH, gC):
+        c, cn, stash, S, w, peep = ctx.saved_tensors
+        nin = 10 + len(ctx.spec)
+        if gH is None and gC is None:
+            return (None,) * nin
+        want_dh = ctx.has_h and ctx.needs_input_grad[4]
+        want_dc = c is not None and ctx.needs_input_grad[5]
+        dpre, dx, dh, dc, scr = lstm_rows_bwd(ctx.plan, ctx.variant, ctx.n_ops, gH, gC, c, cn, stash, w, peep, ctx.needs_input_grad[3],
+                                              want_dh, want_dc, ctx.cin)
+        grads = [None] * len(ctx.spec)
+        if any(ctx.needs_input_grad[10:]):
+            dw, dbp = lstm_rows_wgrad(ctx.variant, ctx.n_ops, ctx.cin, S, dpre, scr, peep is not None)
+            grads = [g.reshape(shape) for g, shape in zip(_spec_grads(ctx.spec, dw, dbp), ctx.shapes)]
+        return (None, None, None, dx, dh, dc, None, None, None, None, *grads)
+
+
+def lstm_rows_train(plan: GraphPlan, variant: int, n_ops: int, x, h, c, w, b, peep, spec, params):
+    """Differentiable (w.r.t. x, h, c and `params`, see _LstmRowsFn) row-split peephole graph-LSTM cell -> (H', C').  x (N, cin); h, c
+    (N, 32) or None (zeros, no state gradient)."""
+    return _LstmRowsFn.apply(plan, variant, n_ops, x, h, c, w, b, peep, tuple(spec), *params)
 
 
 def tgcn_attn_fwd(plan: GraphPlan, x: torch.Tensor, A: torch.Tensor, Bm: torch.Tensor, c: torch.Tensor,

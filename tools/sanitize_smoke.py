@@ -9,7 +9,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from pytorch_geometric_temporal_b200 import _lib, ops                                        # noqa: E402
 from pytorch_geometric_temporal_b200.dataset import synthetic                               # noqa: E402
 from pytorch_geometric_temporal_b200.nn.attention import ASTGCN                              # noqa: E402
-from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, GConvGRU, GConvLSTM, TGCN2   # noqa: E402
+from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, GCLSTM, GConvGRU, GConvLSTM, TGCN2   # noqa: E402
 
 dev = torch.device("cuda")
 torch.manual_seed(0)
@@ -57,6 +57,14 @@ with torch.enable_grad():
     gr(xr, e_ring, None).square().mean().backward()
     with torch.no_grad():
         gr(xr, e_ring, None, torch.randn(301, 32, device=dev))
+    for cls in (GConvLSTM, GCLSTM):                              # the row-split LSTM cell (k_lstm_rows_*), both bases: n_ops 0 and 1,
+        for K in (1, 2):                                         # H / C given and None, k_dcrnn_wgrad<64> + k_lstm_rows_wgrad_reduce
+            gl = cls(14, 32, K).to(dev)
+            hc = [torch.randn(301, 32, device=dev, requires_grad=True) for _ in range(2)]
+            sum(t.square().mean() for t in gl(xr, e_ring, None, *hc)).backward()
+            sum(t.square().mean() for t in gl(xr, e_ring, None)).backward()
+            with torch.no_grad():
+                gl(xr, e_ring, None, hc[0].detach(), hc[1].detach())
 with torch.no_grad():
     e4 =torch.from_numpy(synthetic.pems04_like(0)).to(dev)
     ASTGCN(2, 1, 3, 64, 64, 1, 12, 12, 307, normalization="sym").to(dev)(torch.randn(2, 307, 1, 12, device=dev), e4)   # k_gemm_blocks x7
