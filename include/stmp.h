@@ -94,6 +94,12 @@ int64_t stmp_plan_nnz(const stmp_plan* plan, int op);
  * COO list, i.e. the order the reference's scatter_add_ visits it).  Any output may be NULL. */
 int stmp_plan_export(const stmp_plan* plan, int op, int transposed, int32_t* rowptr, int32_t* col,
                      float* val, int32_t* eid, void* stream);
+/* The compact shared-memory image of the first n_ops (1 or 2) forward operators that the wgmma graph-GRU kernel
+ * gathers from (layout: csrc/graph_image.cuh).  Returns its size in bytes, or 0 when the plan has none for n_ops
+ * (N > 207, a row of more than 508 entries, or too dense for the kernel's shared memory).  When dst is non-NULL and
+ * capacity >= that size, the image is copied to dst (host or device memory).  Setup path: synchronous.  A failed copy
+ * returns -STMP_ECUDA. */
+int64_t stmp_plan_graph_image(const stmp_plan* plan, int n_ops, void* dst, int64_t capacity);
 
 /* ---- K1/K3: gather -> weighted scatter-add (SpMM) with fused Chebyshev axpby -------------------
  * y[b,i,:] = alpha * sum_k val_k * x[b, col_k, :] + beta * z[b,i,:]        (z may be NULL)

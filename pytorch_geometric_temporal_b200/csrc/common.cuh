@@ -30,9 +30,11 @@ extern int g_narrow_pack;  // "dcrnn_narrow_pack": windows per CTA of the narrow
 #define STMP_CUDA_OK(expr)                                                                    \
   do {                                                                                        \
     cudaError_t _e = (expr);                                                                  \
-    if (_e != cudaSuccess)                                                                    \
+    if (_e != cudaSuccess) {                                                                  \
+      (void)cudaGetLastError();  /* consumed here, so the next STMP_LAUNCH_OK does not report it */ \
       return stmp::set_error(STMP_ECUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), \
                              __FILE__, __LINE__);                                             \
+    }                                                                                         \
   } while (0)
 
 #define STMP_LAUNCH_OK(name)                                                                  \

@@ -24,6 +24,9 @@ namespace {
 constexpr int kCo = 32;          // hidden size served by these kernels
 constexpr int kBwdThreads = 512;
 constexpr int kBatch = 4;        // vector slots per thread whose global operands are fetched together (latency paid once)
+// dynamic shared memory a k_dcrnn_bwd_seq block may request: the 227 KB opt-in limit covers static shared memory too, and the
+// cluster-pair variant's static mbarrier (dbar) takes 16 bytes (8, padded to the dynamic block's alignment; cuobjdump -res-usage)
+constexpr size_t kBwdSmemMax = 227 * 1024 - 16;
 
 // basis width [U | Op_0 U | .. | Op_{nops-1} U], U = [X | H], rounded up to whole 8-column groups
 __host__ __device__ constexpr int ncol_of(int cin, int nops = 2) { return ((nops + 1) * (cin + kCo) + 7) / 8 * 8; }
@@ -431,11 +434,11 @@ inline bool graph_in_smem(const stmp_plan* plan, int cin, int nops = 2) {
   if (nops == 0) return false;                   // nothing to stage
   for (int op = 0; op < nops; ++op)
     if (plan->bwd[op].nnz >= 65536) return false;
-  return plan->n <= 256 && seq_smem_base(plan->n, cin, nops) + seq_smem_graph(plan, nops) <= 227 * 1024;
+  return plan->n <= 256 && seq_smem_base(plan->n, cin, nops) + seq_smem_graph(plan, nops) <= kBwdSmemMax;
 }
 // the graph fits one SM: the GEMM tiles fit the block, the per-window buffers its shared memory, the basis kernel's [X|H] copies 100 KB
 inline bool fits_one_sm(const stmp_plan* plan, long long cin, int nops) {
-  return ((plan->n + 7) / 8) * (ncol_of((int)cin, nops) / 8) <= kBwdThreads && seq_smem_base(plan->n, (int)cin, nops) <= 227 * 1024 &&
+  return ((plan->n + 7) / 8) * (ncol_of((int)cin, nops) / 8) <= kBwdThreads && seq_smem_base(plan->n, (int)cin, nops) <= kBwdSmemMax &&
          2 * sizeof(float) * (size_t)plan->n * (cin + kCo) <= 100 * 1024;
 }
 inline bool bwd_supported(const stmp_plan* plan, long long cin, long long cout, long long K) {
@@ -528,7 +531,7 @@ int basis_impl(const stmp_plan* plan, int nops, int64_t B, int64_t T, int64_t ci
 
 int seq_impl(const stmp_plan* plan, int nops, int64_t B, int64_t T, int64_t cin, const float* gout, const float* out, const float* h0,
              const float* stash, const float* whsT, const float* wzrT, float* dph_all, float* dpzr_all, float* dx, float* dh0, cudaStream_t st,
-             int* split_out) {
+             int* split_out, bool* global_out) {
   BwdParams p;
   for (int o = 0; o < 2; ++o) {
     const bool on = o < nops;
@@ -544,6 +547,7 @@ int seq_impl(const stmp_plan* plan, int nops, int64_t B, int64_t T, int64_t cin,
   STMP_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int split = (g_bwd_split && 2 * B <= sms && plan->n >= 16) ? 2 : 1;      // small batches: two CTAs per window (cluster), rows halved
   *split_out = split;
+  *global_out = nops > 0 && !sg;          // the transposed operators are read from the global CSR, not a staged copy
   switch (nops) {
     case 0: return dispatch_seq<0>(p, (int)cin, sg, smem, split, st);
     case 1: return dispatch_seq<1>(p, (int)cin, sg, smem, split, st);
@@ -589,10 +593,13 @@ extern "C" int stmp_dcrnn_bwd_seq(const stmp_plan* plan, int64_t B, int64_t T, i
                "stmp_dcrnn_bwd_seq: operands must be 8-byte aligned");
   if (B == 0) return STMP_OK;
   int split = 1;
-  const int rc = seq_impl(plan, 2, B, T, cin, gout, out, h0, stash, whsT, wzrT, dph_all, dpzr_all, dx, dh0, (cudaStream_t)stream, &split);
+  bool global = false;
+  const int rc = seq_impl(plan, 2, B, T, cin, gout, out, h0, stash, whsT, wzrT, dph_all, dpzr_all, dx, dh0, (cudaStream_t)stream, &split,
+                          &global);
   if (rc != STMP_OK) return rc;
   STMP_LAUNCH_OK("k_dcrnn_bwd_seq");
   if (split == 2) { static const int slot2 = path_slot("k_dcrnn_bwd_seq[cluster2]"); count_path(slot2); }
+  if (global) { static const int slotg = path_slot("k_dcrnn_bwd_seq[graph-global]"); count_path(slotg); }
   return STMP_OK;
 }
 
@@ -636,10 +643,13 @@ extern "C" int stmp_gru_bwd_seq(const stmp_plan* plan, int n_ops, int64_t B, int
                "stmp_gru_bwd_seq: operands must be 8-byte aligned");
   if (B == 0) return STMP_OK;
   int split = 1;
-  const int rc = seq_impl(plan, n_ops, B, T, cin, gout, out, h0, stash, whsT, wzrT, dph_all, dpzr_all, dx, dh0, (cudaStream_t)stream, &split);
+  bool global = false;
+  const int rc = seq_impl(plan, n_ops, B, T, cin, gout, out, h0, stash, whsT, wzrT, dph_all, dpzr_all, dx, dh0, (cudaStream_t)stream, &split,
+                          &global);
   if (rc != STMP_OK) return rc;
   STMP_LAUNCH_OK("k_gru_bwd_seq");
   if (split == 2) { static const int slot2 = path_slot("k_gru_bwd_seq[cluster2]"); count_path(slot2); }
+  if (global) { static const int slotg = path_slot("k_gru_bwd_seq[graph-global]"); count_path(slotg); }
   return STMP_OK;
 }
 

@@ -624,6 +624,15 @@ bool tc_layout(const stmp_plan* plan, int n_ops, TcParams* p, int* smem_bytes) {
 
 }  // namespace
 
+// bytes of shared memory the kernel has left for a graph image: the plan builds no image larger than this (it could never be used)
+int tc_graph_image_budget() {
+  stmp_plan none;                           // no operators: tc_layout lays out everything but the image
+  TcParams p;
+  int smem = 0;
+  tc_layout(&none, 0, &p, &smem);
+  return kMaxSmemTc - smem;
+}
+
 int tc_ws_pitch(long long T, long long cin) { return (int)((T * cin + 7) / 8 * 8); }   // floats per (row, operator): whole 32-byte sectors
 
 long long tc_workspace_bytes(const stmp_plan* plan, long long T, long long cin) {

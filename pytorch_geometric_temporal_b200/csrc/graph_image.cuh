@@ -51,4 +51,7 @@ __host__ __device__ inline GraphImageLayout graph_image_layout(int n_tasks, int 
   return L;
 }
 
+// shared memory the wgmma kernel leaves for the image (dcrnn_seq_tc.cu); a plan keeps an image only if L.bytes fits it
+int tc_graph_image_budget();
+
 }  // namespace stmp

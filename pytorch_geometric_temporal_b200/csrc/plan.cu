@@ -722,7 +722,7 @@ int build_graph_images(Builder& b, stmp_plan* p) {
     int nnz = 0;
     for (int op = 0; op < n_ops; ++op) nnz += p->fwd[op].nnz;
     const GraphImageLayout L = graph_image_layout(n_ops * N, nnz);
-    if (L.bytes > 160 * 1024) continue;                       // cannot fit beside the operand panels anyway
+    if (L.bytes > tc_graph_image_budget()) continue;          // cannot fit beside the wgmma kernel's operand panels
     STMP_CUDA_OK(cudaMalloc(&p->gimg[n_ops], (size_t)L.bytes));
     STMP_CUDA_OK(cudaMemsetAsync(p->gimg[n_ops], 0, (size_t)L.bytes, b.st));
     const Csr& c1 = p->fwd[n_ops > 1 ? 1 : 0];
@@ -871,6 +871,16 @@ extern "C" int stmp_plan_export(const stmp_plan* p, int op, int transposed, int3
     STMP_LAUNCH_OK("k_export");
   }
   return STMP_OK;
+}
+
+extern "C" int64_t stmp_plan_graph_image(const stmp_plan* p, int n_ops, void* dst, int64_t capacity) {
+  if (!p || n_ops < 1 || n_ops > 2 || !p->gimg[n_ops]) return 0;
+  const int64_t bytes = p->gimg_bytes[n_ops];
+  if (dst && capacity >= bytes && cudaMemcpy(dst, p->gimg[n_ops], (size_t)bytes, cudaMemcpyDefault) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return -set_error(STMP_ECUDA, "stmp_plan_graph_image: copy of %lld bytes failed", (long long)bytes);
+  }
+  return bytes;
 }
 
 /* Test hook: select, at run time, the implementation or launch shape a test cross-checks against the default (common.cuh). */

@@ -74,6 +74,19 @@ class GraphPlan:
                                                    _lib.ptr(val), _lib.ptr(eid), _lib.stream_ptr()))
         return rowptr, col, val, eid
 
+    def graph_image(self, n_ops: int):
+        """The wgmma kernel's shared-memory image of the first `n_ops` operators as a CPU uint8 tensor, or None when the
+        plan has none -- test/introspection helper."""
+        size = int(_lib.lib().stmp_plan_graph_image(self._h, n_ops, None, 0))
+        if size <= 0:
+            return None
+        buf = torch.empty(size, dtype=torch.uint8)
+        with torch.cuda.device(self.device):
+            rc = int(_lib.lib().stmp_plan_graph_image(self._h, n_ops, ctypes.c_void_p(buf.data_ptr()), size))
+        if rc < 0:
+            _lib.check(-rc)
+        return buf
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h is not None and h.value:

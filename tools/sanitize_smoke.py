@@ -87,5 +87,19 @@ _lib.set_option("dcrnn_narrow_pack", 0)
 x = torch.randn(2, 2000, 64, device=dev, requires_grad=True)
 h, c = lstm(x, eg, wg)
 (h.sum() + c.sum()).backward()                                   # _LstmCellFn backward: k_gemm_split, k_lstm_gate_bwd, transposed SpMM
+# adversarial geometries (tests/test_gpu_graph_geometry.py): a 128-edge row in the second row tile, a backward that reads the global CSR,
+# the FFMA kernel's 7-rows-per-thread mapping
+r129 = torch.arange(129, device=dev)
+e_hub = torch.cat([torch.stack([r129, (r129 + 1) % 129]), torch.stack([r129[:-1], torch.full((128,), 128, device=dev)])], dim=1)
+mh = BatchedDCRNN(3, 32, 2).to(dev)
+mh(torch.randn(2, 4, 129, 3, device=dev), e_hub, torch.ones(e_hub.size(1), device=dev)).square().mean().backward()   # cluster pairs
+r207 = torch.arange(207, device=dev)
+pairs = torch.randperm(207 * 207, generator=torch.Generator().manual_seed(0))[:2107].to(dev)
+e_dense = torch.cat([torch.stack([r207, (r207 + 1) % 207]), torch.stack([pairs // 207, pairs % 207])], dim=1)
+m(X[:2], e_dense, torch.ones(e_dense.size(1), device=dev)).square().mean().backward()   # k_dcrnn_bwd_seq[graph-global]
+with torch.no_grad():
+    r225 = torch.arange(225, device=dev)
+    BatchedDCRNN(2, 32, 1).to(dev)(torch.randn(2, 12, 225, 2, device=dev), torch.stack([r225, (r225 + 1) % 225]),
+                                   torch.ones(225, device=dev))  # k_dcrnn_seq, RT 7
 torch.cuda.synchronize()
 print("sanitize_smoke ok:", {k: v for k, v in _lib.path_counters().items() if k.startswith("k_") and v})
