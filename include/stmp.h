@@ -100,6 +100,12 @@ int stmp_plan_export(const stmp_plan* plan, int op, int transposed, int32_t* row
  * capacity >= that size, the image is copied to dst (host or device memory).  Setup path: synchronous.  A failed copy
  * returns -STMP_ECUDA. */
 int64_t stmp_plan_graph_image(const stmp_plan* plan, int n_ops, void* dst, int64_t capacity);
+/* The row image the one-CTA wgmma graph-GRU kernel gathers from (layout: csrc/row_image.cuh), built on the host from host CSR
+ * arrays of n_ops (1 or 2) operators (rowptr [N+1], col / val [nnz]; the second set is ignored for n_ops = 1).  Returns its size
+ * in bytes, or 0 for a graph the format cannot hold (N outside 1..255, a column outside [0, N)).  When dst is non-NULL and
+ * capacity >= that size, the image is written to dst (host memory).  Needs no GPU. */
+int64_t stmp_row_image_build(int64_t num_nodes, int n_ops, const int32_t* rowptr0, const int32_t* col0, const float* val0,
+                             const int32_t* rowptr1, const int32_t* col1, const float* val1, void* dst, int64_t capacity);
 
 /* ---- K1/K3: gather -> weighted scatter-add (SpMM) with fused Chebyshev axpby -------------------
  * y[b,i,:] = alpha * sum_k val_k * x[b, col_k, :] + beta * z[b,i,:]        (z may be NULL)

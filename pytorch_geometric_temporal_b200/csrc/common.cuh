@@ -82,6 +82,10 @@ struct stmp_plan {
   // the kernel then fetches it with ONE TMA bulk copy instead of re-staging the CSR in every CTA.
   void* gimg[3] = {nullptr, nullptr, nullptr};   // index = n_ops (1, 2)
   int gimg_bytes[3] = {0, 0, 0};
+  // Row image of the first n_ops operators for the one-CTA kernel (row_image.cuh): nodes mapped onto the MMA rows, gather lists
+  // per (warp, operator, slot).  Its size follows from the number of group rows.
+  void* rimg[3] = {nullptr, nullptr, nullptr};
+  int rimg_groups[3] = {0, 0, 0};
 };
 
 namespace stmp {

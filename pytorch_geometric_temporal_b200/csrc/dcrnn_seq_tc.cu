@@ -2,6 +2,8 @@
 //
 // Same contract as k_dcrnn_seq (dcrnn_seq.cu) for K=2, Cout=32, Cin<=4, N<=255; what changes is WHERE the
 // S @ [Wz|Wr] and S @ Wh contractions run: warpgroup MMAs (wgmma, fp32 accumulators in registers) instead of FFMA.
+// Two kernels: k_dcrnn_seq_rf (one CTA per window, A operands gathered straight into registers; below, "the one-CTA kernel") and
+// k_dcrnn_seq_tc<CIN, 2> (a 2-CTA cluster per window for small batches, A operands in shared-memory panels; described first).
 //
 // fp32 accuracy on fp16 tensor cores: every fp32 operand v is split on the fly into hi = fp16(v) and
 // lo = fp16(v - hi) (22 mantissa bits together; products of fp16 pairs are exact in the fp32 accumulator) and
@@ -30,6 +32,7 @@
 #include "common.cuh"
 #include "dcrnn_common.cuh"
 #include "graph_image.cuh"
+#include "row_image.cuh"
 #include "tc_common.cuh"
 
 namespace stmp {
@@ -56,8 +59,10 @@ struct TcParams {
   const float* wcat;      // optional prepacked fp32 weights [96][112] in the kernel's k order (else: DConv weights p.w[])
   const float* bcat;      // with wcat: biases [96]
   int n_ops;              // 2: DConv (P_o, P_i); 1: single operator (ChebConv K=2 / GCN); 0: no propagation
-  const void* gimg;       // plan's prebuilt shared-memory graph image for n_ops operators (TMA bulk source)
+  const void* gimg;       // plan's prebuilt shared-memory graph image for n_ops operators (TMA bulk source; cluster pair)
   GraphImageLayout gl;    // its internal offsets
+  const void* rimg;       // plan's row image for n_ops operators (one-CTA kernel; null for n_ops = 0)
+  RowImageLayout rl;      // its offsets
   const void* wimage;     // prebuilt B-operand image (fp16 hi/lo, swizzled, + biases) or null
   float* out;
   float* stash;
@@ -606,7 +611,437 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
   }
 }
 
-// shared-memory layout for `n_ops` operators of `plan`
+// ---- the one-CTA kernel: A operands from registers ----------------------------------------------------------------------
+// Warpgroup wg owns MMA rows [64 wg, 64 wg + 64); the plan's row image (row_image.cuh) maps graph nodes onto these 256 positions so
+// that the gather work is balanced.  Thread (warp w, lane l; quad = l / 4, q = l % 4) owns positions 16 w + quad (slot 0) and +8
+// (slot 1) and, of every 32-channel block, the channels 8 jj + 2q (+1), jj = 0..3: exactly the (row, k) pairs of its m64nNk16 A
+// fragment and of its accumulator fragment.  So it gathers the diffusion of its own two rows straight into A fragments (split into fp16
+// hi / lo in registers) and applies the gates to the accumulators of the same rows; no operand goes through shared memory but B.
+//
+// Gather buffers U_H (H) and U_R (H*R): fp32 [256 positions][32], 128-byte rows without padding, channels permuted so that the 8
+// channels of quad lane q sit in 32 contiguous bytes (float 8q + 2jj + x = channel 8jj + 2q + x): a lane reads a source row with
+// two 16-byte loads, odd quads in the opposite order, so the two quads of a load phase touch disjoint banks whatever rows they read.
+//
+// Step:  round 1  gather P_o H of my rows -> issue the H | X and P_o k-steps -> gather P_i H while they run -> issue the P_i k-steps
+//                 -> wait -> r, H*R -> U_R                                                                            barrier
+//        round 2  the same over U_R (GEMM 2) -> z, candidate, H_t -> U_H, HBM                                         barrier
+// Between the two barriers a warpgroup depends only on itself.  The k-steps of a gemm are issued in the order of the cluster kernel
+// (k-steps 0, 1, 6, then 2, 3, then 4, 5, each pass-major lo*hi, hi*lo, hi*hi) and the gather sums the same entries in CSR order, so
+// the outputs are bit-identical to it.
+constexpr int RF_UBUF = kRiPos * 32;   // floats per gather buffer
+
+// 8 floats of a row in fragment order (v[2jj + x] = channel 8jj + 2q + x) <-> the two 16-byte chunks 2q, 2q+1 of the row; `par`
+// (quad parity) selects which chunk is touched first
+__device__ __forceinline__ void rf_ld_row(const float* row, int q, int par, float (&v)[8]) {
+  const float4 a = ld4(row + 4 * (2 * q + par)), b = ld4(row + 4 * (2 * q + 1 - par));
+  const float4 lo = par ? b : a, hi = par ? a : b;
+  v[0] = lo.x; v[1] = lo.y; v[2] = lo.z; v[3] = lo.w; v[4] = hi.x; v[5] = hi.y; v[6] = hi.z; v[7] = hi.w;
+}
+__device__ __forceinline__ void rf_st_row(float* row, int q, int par, const float (&v)[8]) {
+  const float4 lo = make_float4(v[0], v[1], v[2], v[3]), hi = make_float4(v[4], v[5], v[6], v[7]);
+  st4(row + 4 * (2 * q + par), par ? hi : lo);
+  st4(row + 4 * (2 * q + 1 - par), par ? lo : hi);
+}
+// fp16 hi / lo of a pair (as store_split2)
+__device__ __forceinline__ void rf_split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __half2 h = __floats2half2_rn(a, b);
+  const float2 f = __half22float2(h);
+  hi = pack_h2(h);
+  lo = pack_h2(__floats2half2_rn(a - f.x, b - f.y));
+}
+// A-fragment registers of the two k-steps of a 32-channel block that hold my fragment row e, from its values v in fragment order
+__device__ __forceinline__ void rf_split_row(const float (&v)[8], int e, uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
+#pragma unroll
+  for (int s = 0; s < 2; ++s) {
+    rf_split2(v[4 * s], v[4 * s + 1], hi[s][e], lo[s][e]);
+    rf_split2(v[4 * s + 2], v[4 * s + 3], hi[s][2 + e], lo[s][2 + e]);
+  }
+}
+// Weighted sum over one gather list (a (warp, operator, slot) of the row image) of the 8 floats of my quad lane: v in the order of
+// the row's chunks 2q, 2q+1.  Four entries per group as gather_groups, the next group's entries fetched while the current one's rows
+// are in flight; summation order = CSR order, products by FMA.
+__device__ __forceinline__ void rf_gather(const float* __restrict__ Ub, const uint32_t* __restrict__ idx, const float4* __restrict__ val,
+                                          int g0, int ng, int quad, int q, int par, float (&v)[8]) {
+  float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+  const int cf = 4 * (2 * q + par), cs = 4 * (2 * q + 1 - par);
+  const uint32_t* ix = idx + g0 * 8 + quad;
+  const float4* vx = val + g0 * 8 + quad;
+  uint32_t u = ix[0];
+  float4 w = vx[0];
+#pragma unroll 2
+  for (int g = 1; g <= ng; ++g) {
+    const uint32_t un = ix[8 * g];          // (one spare group row at the end of the arrays)
+    const float4 wn = vx[8 * g];
+    const float* r0 = Ub + (u & 0xffu) * 32;
+    const float* r1 = Ub + ((u >> 8) & 0xffu) * 32;
+    const float* r2 = Ub + ((u >> 16) & 0xffu) * 32;
+    const float* r3 = Ub + (u >> 24) * 32;
+    const float4 x0 = ld4(r0 + cf), y0 = ld4(r0 + cs);
+    const float4 x1 = ld4(r1 + cf), y1 = ld4(r1 + cs);
+    const float4 x2 = ld4(r2 + cf), y2 = ld4(r2 + cs);
+    const float4 x3 = ld4(r3 + cf), y3 = ld4(r3 + cs);
+    fma4(a, w.x, x0); fma4(b, w.x, y0);
+    fma4(a, w.y, x1); fma4(b, w.y, y1);
+    fma4(a, w.z, x2); fma4(b, w.z, y2);
+    fma4(a, w.w, x3); fma4(b, w.w, y3);
+    u = un;
+    w = wn;
+  }
+  const float4 lo = par ? b : a, hi = par ? a : b;
+  v[0] = lo.x; v[1] = lo.y; v[2] = lo.z; v[3] = lo.w; v[4] = hi.x; v[5] = hi.y; v[6] = hi.z; v[7] = hi.w;
+}
+
+template <int CIN>
+__global__ void __launch_bounds__(512, 1) k_dcrnn_seq_rf(const TcParams p) {
+  extern __shared__ __align__(1024) unsigned char smem[];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int N = p.N, T = p.T;
+  unsigned char* b_hi = smem + p.off_B;
+  unsigned char* b_lo = b_hi + 2 * TC_PANEL_B;
+  float* UH = reinterpret_cast<float*>(smem + p.off_U);
+  float* UR = UH + RF_UBUF;
+  unsigned char* img = smem + p.off_img;
+  int16_t* s_perm = reinterpret_cast<int16_t*>(img + kRiOffPerm);
+  const uint8_t* s_ipos = img + kRiOffIpos;
+  const uint16_t* s_gstart = reinterpret_cast<const uint16_t*>(img + kRiOffGstart);
+  const uint16_t* s_gcount = reinterpret_cast<const uint16_t*>(img + kRiOffGcount);
+  const uint32_t* s_idx = reinterpret_cast<const uint32_t*>(img + kRiOffIdx);
+  const float4* s_val = reinterpret_cast<const float4*>(img + p.rl.off_val);
+  float* Bs = reinterpret_cast<float*>(smem + p.off_bias);
+  uint64_t* tma_bar = reinterpret_cast<uint64_t*>(smem + p.off_bar);
+  if (blockIdx.x >= p.B) return;
+
+  // ---- one-time per CTA ------------------------------------------------------------------------------------
+  if (tid == 0) {
+    mbar_init(tma_bar, 1);
+    fence_mbar_init();
+    const uint32_t tx = (p.rimg ? (uint32_t)p.rl.bytes : 0u) + (p.wimage ? (uint32_t)TC_WIMAGE_BYTES : 0u);
+    if (tx) {
+      mbar_arrive_expect_tx(tma_bar, tx);
+      if (p.rimg) tma_bulk_g2s(img, p.rimg, (uint32_t)p.rl.bytes, tma_bar);
+      if (p.wimage) {
+        tma_bulk_g2s(b_hi, p.wimage, 4u * TC_PANEL_B, tma_bar);
+        tma_bulk_g2s(Bs, reinterpret_cast<const unsigned char*>(p.wimage) + 4 * TC_PANEL_B, 96u * 4u, tma_bar);
+      }
+    }
+  }
+  {  // zero both gather buffers (the rows of empty positions stay zero for good); B too unless the TMA image overwrites it
+    for (int i = tid; i < 2 * RF_UBUF; i += 512) UH[i] = 0.f;
+    if (!p.wimage) {
+      uint4* z = reinterpret_cast<uint4*>(b_hi);
+      for (int i = tid; i < 4 * TC_PANEL_B / 16; i += 512) z[i] = make_uint4(0, 0, 0, 0);
+    }
+    if (!p.rimg)   // no operator: the identity map
+      for (int i = tid; i < kRiPos; i += 512) s_perm[i] = (int16_t)(i < N ? i : -1);
+  }
+  __syncthreads();
+  if (!p.wimage) {
+    for (int idx = tid; idx < 96 * 112; idx += 512) {
+      const int n = idx / 112, kk = idx - n * 112;
+      const float v = tc_weight_value(p.wcat, p.w[0], p.w[1], p.w[2], CIN, n, kk);
+      const __half h = __float2half_rn(v);
+      const __half l = __float2half_rn(v - __half2float(h));
+      const int off = (kk >> 6) * TC_PANEL_B + sw128(n, kk & 63);
+      *reinterpret_cast<__half*>(b_hi + off) = h;
+      *reinterpret_cast<__half*>(b_lo + off) = l;
+    }
+    for (int idx = tid; idx < 96; idx += 512) {
+      const int gte = idx >> 5;
+      const float* bg = gte == 0 ? p.bias[0] : (gte == 1 ? p.bias[1] : p.bias[2]);
+      Bs[idx] = p.bcat ? p.bcat[idx] : (bg ? bg[idx & 31] : 0.f);
+    }
+  }
+  if (p.rimg || p.wimage) mbar_wait(tma_bar, 0);
+  fence_proxy_async();
+  __syncthreads();
+
+  const int quad = lane >> 2, q = lane & 3, par = quad & 1;
+  const int pos[2] = {16 * warp + quad, 16 * warp + quad + 8};   // my MMA rows (fragment slots 0, 1)
+  // graph node of my fragment row e (-1: empty), re-read where it is used: a register held across the step costs more
+  auto node_of = [&](int e) -> int { return s_perm[pos[e]]; };
+  const uint32_t b_hi_s = smem_u32(b_hi), b_lo_s = smem_u32(b_lo);
+
+  // Accumulators: GEMM 1 z in [0, 16), r in [16, 32); GEMM 2 the candidate.  Value of fragment row e, channel 8jj + 2q + x at
+  // 4jj + 2e + x (+16 for r).
+  float acc1[32], acc2[16];
+  // A fragments, [k-step of the block][register]: H | H*R (k-steps 0, 1), P_o (2, 3), P_i (4, 5); X (k-step 6)
+  uint32_t aH_hi[2][4], aH_lo[2][4], aO_hi[2][4], aO_lo[2][4], aI_hi[2][4], aI_lo[2][4], aX_hi[4], aX_lo[4];
+
+  auto mma = [&](int gm, int ks, int pass, const uint32_t (&a)[4]) {
+    const uint32_t bb = pass == 1 ? b_lo_s : b_hi_s;
+    const uint32_t bk = bb + (ks >> 2) * TC_PANEL_B + (ks & 3) * 32;
+    const bool first = ks == 0 && pass == 0;   // overwrites the accumulator
+    if (gm == 1) {
+      if (first) wgmma_f16_rs_n32_first(acc2, a, gmma_desc_sw128(bk + 64 * 128));
+      else wgmma_f16_rs_n32(acc2, a, gmma_desc_sw128(bk + 64 * 128), 1u);
+    } else {
+      if (first) wgmma_f16_rs_n64_first(acc1, a, gmma_desc_sw128(bk));
+      else wgmma_f16_rs_n64(acc1, a, gmma_desc_sw128(bk), 1u);
+    }
+  };
+  // k-steps 0, 1, 6 (H | H*R, X) and 2, 3 (P_o), each group pass-major: lo*hi, hi*lo, hi*hi
+  auto issue_hxo = [&](int gm) {
+    wgmma_fence();
+#pragma unroll
+    for (int pass = 0; pass < 3; ++pass) {
+      mma(gm, 0, pass, pass == 0 ? aH_lo[0] : aH_hi[0]);
+      mma(gm, 1, pass, pass == 0 ? aH_lo[1] : aH_hi[1]);
+      mma(gm, 6, pass, pass == 0 ? aX_lo : aX_hi);
+    }
+#pragma unroll
+    for (int pass = 0; pass < 3; ++pass) {
+      mma(gm, 2, pass, pass == 0 ? aO_lo[0] : aO_hi[0]);
+      mma(gm, 3, pass, pass == 0 ? aO_lo[1] : aO_hi[1]);
+    }
+    wgmma_commit();
+  };
+  auto issue_i = [&](int gm) {
+    wgmma_fence();
+#pragma unroll
+    for (int pass = 0; pass < 3; ++pass) {
+      mma(gm, 4, pass, pass == 0 ? aI_lo[0] : aI_hi[0]);
+      mma(gm, 5, pass, pass == 0 ? aI_lo[1] : aI_hi[1]);
+    }
+    wgmma_commit();
+  };
+  // diffusion by operator `op` of my two rows from gather buffer Ub -> A fragments (zero when the operator is absent)
+  auto gather_op = [&](const float* Ub, int op, uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float v[8];
+      if (p.n_ops > op) {
+        rf_gather(Ub, s_idx, s_val, s_gstart[ri_list(warp, op, e)], s_gcount[ri_list(warp, op, e)], quad, q, par, v);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = 0.f;
+      }
+      rf_split_row(v, e, hi, lo);
+    }
+  };
+
+  auto x_base = [&](long long b) -> const float* { return p.x + (p.win_start ? p.win_start[b] * p.x_tstride : b * p.x_bstride); };
+  // My values of the X k-step (k = X c0..3 | P_o X c0..3 | P_i X c0..3 | 0): k 2q, 2q+1 -> xr[4e], xr[4e+1]; k 8+2q, 9+2q ->
+  // xr[4e+2], xr[4e+3] (fragment row e).  Absent channels / operators and empty rows are 0 (the weights there are zero, the operand
+  // must be finite).
+  auto load_x = [&](const float* xb, long long b, int t, float (&xr)[8]) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int n = node_of(e);
+#pragma unroll
+      for (int x = 0; x < 2; ++x) {
+        const int c = 2 * (q & 1) + x;
+        float va = 0.f, vb = 0.f;
+        if (n >= 0 && c < CIN) {
+          auto ld_p = [&](int op) -> float {     // P_op X_t of row n, channel c: workspace or the parked output row
+            if (p.ws) return p.ws[(((long long)blockIdx.x * N + n) * 2 + op) * p.ws_pitch + t * CIN + c];
+            return p.out[((b * T + t) * (long long)N + n) * 32 + op * 4 + c];
+          };
+          if (q < 2) {
+            va = __ldg(xb + t * p.x_tstride + n * CIN + c);
+            if (p.n_ops >= 2) vb = ld_p(1);
+          } else if (p.n_ops >= 1) {
+            va = ld_p(0);
+          }
+        }
+        xr[4 * e + x] = va;
+        xr[4 * e + 2 + x] = vb;
+      }
+    }
+  };
+  auto split_x = [&](const float (&xr)[8]) {
+    rf_split2(xr[0], xr[1], aX_hi[0], aX_lo[0]);
+    rf_split2(xr[4], xr[5], aX_hi[1], aX_lo[1]);
+    rf_split2(xr[2], xr[3], aX_hi[2], aX_lo[2]);
+    rf_split2(xr[6], xr[7], aX_hi[3], aX_lo[3]);
+  };
+
+  for (long long b = blockIdx.x; b < p.B; b += gridDim.x) {
+    const float* xb = x_base(b);
+    // ---- window prologue A: P_o X_t, P_i X_t for every step of the window, TCH steps per gather pass (rows of T*Cin floats in U_R)
+    if (p.n_ops) {
+      constexpr int TCH = 32 / CIN;
+      for (int t0 = 0; t0 < T; t0 += TCH) {
+        const int tn = (T - t0) < TCH ? (T - t0) : TCH;
+        const int F = tn * CIN, NC = N * CIN;
+        for (int base = 0; base < tn * NC; base += 512 * 8) {
+          float xv8[8];
+#pragma unroll
+          for (int u = 0; u < 8; ++u) {
+            const int idx = base + u * 512 + tid;
+            xv8[u] = 0.f;
+            if (idx < tn * NC) {
+              const int tt = idx / NC, r = idx - tt * NC;
+              xv8[u] = __ldg(xb + (long long)(t0 + tt) * p.x_tstride + r);
+            }
+          }
+#pragma unroll
+          for (int u = 0; u < 8; ++u) {
+            const int idx = base + u * 512 + tid;
+            if (idx < tn * NC) {
+              const int tt = idx / NC, r = idx - tt * NC;
+              const int n = r / CIN, c = r - n * CIN;
+              UR[s_ipos[n] * 32 + tt * CIN + c] = xv8[u];
+            }
+          }
+        }
+        __syncthreads();
+        for (int op = 0; op < p.n_ops; ++op)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float v[8];   // floats 8q .. 8q+7 of the row = (t, c) pairs in order
+            rf_gather(UR, s_idx, s_val, s_gstart[ri_list(warp, op, e)], s_gcount[ri_list(warp, op, e)], quad, q, par, v);
+            const int n = node_of(e);
+            if (n < 0 || 8 * q >= F) continue;
+            if (p.ws) {
+              float* wrow = p.ws + (((long long)blockIdx.x * N + n) * 2 + op) * p.ws_pitch + t0 * CIN + 8 * q;
+              if (CIN != 3 && 8 * q + 8 <= F) {      // 16-byte aligned: t0 * CIN is a multiple of 32 for CIN = 1, 2, 4
+                st4(wrow, make_float4(v[0], v[1], v[2], v[3]));
+                st4(wrow + 4, make_float4(v[4], v[5], v[6], v[7]));
+              } else {
+#pragma unroll
+                for (int k = 0; k < 8; ++k)
+                  if (8 * q + k < F) wrow[k] = v[k];
+              }
+            } else {
+#pragma unroll
+              for (int k = 0; k < 8; ++k) {
+                const int f = 8 * q + k;
+                if (f < F) {
+                  const int tt = f / CIN, c = f - tt * CIN;
+                  p.out[((b * T + t0 + tt) * (long long)N + n) * 32 + op * 4 + c] = v[k];
+                }
+              }
+            }
+          }
+        __syncthreads();
+      }
+    }
+    // ---- window prologue B: H_0 into U_H and the A fragments; the X k-step of step 0 -----------------------------------------
+    {
+      float hv[2][8];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int n = node_of(e);
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          float2 h = make_float2(0.f, 0.f);
+          if (n >= 0 && p.h0) h = __ldg(reinterpret_cast<const float2*>(p.h0 + b * p.h0_bstride + n * 32 + 8 * jj + 2 * q));
+          hv[e][2 * jj] = h.x; hv[e][2 * jj + 1] = h.y;
+        }
+        if (n >= 0) rf_st_row(UH + pos[e] * 32, q, par, hv[e]);
+        rf_split_row(hv[e], e, aH_hi, aH_lo);
+      }
+      float xr[8];
+      load_x(xb, b, 0, xr);
+      split_x(xr);
+    }
+    __syncthreads();
+
+    for (int t = 0; t < T; ++t) {
+      const long long obase = (b * T + t) * (long long)N;
+      // ---- round 1: diffuse H (GEMM 1: z | r) -----------------------------------------------------------------------------
+      gather_op(UH, 0, aO_hi, aO_lo);
+      issue_hxo(0);
+      gather_op(UH, 1, aI_hi, aI_lo);
+      issue_i(0);
+      wgmma_wait<0>();
+      acc_fence(acc1);
+      // ---- epilogue 1: r gate; H*R -> U_R and the A fragments of round 2 --------------------------------------------------
+      {
+        float hr[2][8];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float h[8];
+          rf_ld_row(UH + pos[e] * 32, q, par, h);
+          float rv[8];
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+            for (int x = 0; x < 2; ++x) {
+              const float r = sigmoid_fast(acc1[16 + 4 * jj + 2 * e + x] + Bs[32 + 8 * jj + 2 * q + x]);
+              hr[e][2 * jj + x] = h[2 * jj + x] * r;
+              rv[2 * jj + x] = r;
+            }
+          const int n = node_of(e);
+          if (n >= 0) {
+            rf_st_row(UR + pos[e] * 32, q, par, hr[e]);
+            if (p.stash)
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj)
+                *reinterpret_cast<float2*>(p.stash + ((obase * 3) + n) * 32 + (long long)N * 32 + 8 * jj + 2 * q) =
+                    make_float2(rv[2 * jj], rv[2 * jj + 1]);
+          }
+          rf_split_row(hr[e], e, aH_hi, aH_lo);
+        }
+      }
+      __syncthreads();   // U_R complete
+      // ---- round 2: re-diffuse H*R (GEMM 2: candidate) ----------------------------------------------------------------------
+      gather_op(UR, 0, aO_hi, aO_lo);
+      issue_hxo(1);
+      gather_op(UR, 1, aI_hi, aI_lo);
+      issue_i(1);
+      wgmma_wait<0>();
+      acc_fence(acc2);
+      // ---- epilogue 2: candidate, H_t -> U_H, HBM and the A fragments of the next step ----------------------------------------
+      {
+        float hn[2][8];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float h[8], zv[8], ht[8];
+          rf_ld_row(UH + pos[e] * 32, q, par, h);
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+            for (int x = 0; x < 2; ++x) {
+              const int c = 8 * jj + 2 * q + x, a = 4 * jj + 2 * e + x;
+              const float z = sigmoid_fast(acc1[a] + Bs[c]);
+              const float hc = tanh_fast(acc2[a] + Bs[64 + c]);
+              zv[2 * jj + x] = z;
+              ht[2 * jj + x] = hc;
+              hn[e][2 * jj + x] = z * h[2 * jj + x] + (1.0f - z) * hc;   // dcrnn.py:190-192
+            }
+          const int n = node_of(e);
+          if (n >= 0) {
+            rf_st_row(UH + pos[e] * 32, q, par, hn[e]);
+            float* op = p.out + (obase + n) * 32;
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int c = 8 * jj + 2 * q;
+              *reinterpret_cast<float2*>(op + c) = make_float2(hn[e][2 * jj], hn[e][2 * jj + 1]);
+              if (p.stash) {
+                float* sp = p.stash + ((obase * 3) + n) * 32;
+                *reinterpret_cast<float2*>(sp + c) = make_float2(zv[2 * jj], zv[2 * jj + 1]);
+                *reinterpret_cast<float2*>(sp + 2 * (long long)N * 32 + c) = make_float2(ht[2 * jj], ht[2 * jj + 1]);
+              }
+            }
+          }
+          rf_split_row(hn[e], e, aH_hi, aH_lo);
+        }
+        if (t + 1 < T) {   // the X k-step of the next step (loaded here: held across the gate math, the values spill)
+          float xr[8];
+          load_x(xb, b, t + 1, xr);
+          split_x(xr);
+        }
+      }
+      __syncthreads();   // U_H complete
+    }
+  }
+}
+
+// shared-memory layout of the one-CTA kernel for `n_ops` operators of `plan`
+bool rf_layout(const stmp_plan* plan, int n_ops, TcParams* p, int* smem_bytes) {
+  int off = 0;
+  p->off_B = off; off += 4 * TC_PANEL_B;
+  p->off_U = off; off += 2 * RF_UBUF * 4;
+  p->rl = row_image_layout(n_ops && plan ? plan->rimg_groups[n_ops] : 0);
+  p->off_img = off; off += p->rl.bytes;
+  p->off_bias = off; off += 96 * 4;
+  p->off_bar = off; off += 8;
+  *smem_bytes = off;
+  return off <= kMaxSmemTc;
+}
+
+// shared-memory layout of the cluster-pair kernel for `n_ops` operators of `plan`
 bool tc_layout(const stmp_plan* plan, int n_ops, TcParams* p, int* smem_bytes) {
   int off = 0;
   p->off_A = off; off += 4 * TC_PANEL_A;
@@ -632,6 +1067,13 @@ int tc_graph_image_budget() {
   tc_layout(&none, 0, &p, &smem);
   return kMaxSmemTc - smem;
 }
+// the same for the row image of the one-CTA kernel
+int tc_row_image_budget() {
+  TcParams p;
+  int smem = 0;
+  rf_layout(nullptr, 0, &p, &smem);       // lays out the image of no group rows
+  return kMaxSmemTc - smem + p.rl.bytes;
+}
 
 int tc_ws_pitch(long long T, long long cin) { return (int)((T * cin + 7) / 8 * 8); }   // floats per (row, operator): whole 32-byte sectors
 
@@ -643,10 +1085,10 @@ long long tc_workspace_bytes(const stmp_plan* plan, long long T, long long cin) 
 
 static bool tc_fits(const stmp_plan* plan, int n_ops) {
   if (!plan || plan->n > kImgMaxN || plan->n < 1) return false;
-  if (n_ops > 0 && !plan->gimg[n_ops]) return false;      // no image: graph too large / too dense for the 8-bit format
+  if (n_ops > 0 && (!plan->gimg[n_ops] || !plan->rimg[n_ops])) return false;   // no image: graph too large / too dense
   TcParams p;
   int smem = 0;
-  return tc_layout(plan, n_ops, &p, &smem);
+  return tc_layout(plan, n_ops, &p, &smem) && rf_layout(plan, n_ops, &p, &smem);
 }
 
 bool gru_tc_supported(const stmp_plan* plan, long long cin, int n_ops) {
@@ -691,15 +1133,18 @@ int gru_tc_launch(const stmp_plan* plan, int n_ops, long long B, long long T, lo
 static int tc_launch_params(const stmp_plan* plan, TcParams& p, cudaStream_t st) {
   int smem = 0;
   const long long B = p.B;
-  if (!tc_layout(plan, p.n_ops, &p, &smem)) return set_error(STMP_EUNSUPPORTED, "tensor-core graph-GRU kernel needs %d B of shared memory", smem);
-  p.gimg = p.n_ops ? plan->gimg[p.n_ops] : nullptr;
-  if (p.n_ops && !p.gimg) return set_error(STMP_EUNSUPPORTED, "tensor-core graph-GRU kernel: the plan has no shared-memory graph image");
   int dev = 0, sms = 0;
   STMP_CUDA_OK(cudaGetDevice(&dev));
   STMP_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   // small batches: a CTA pair (thread-block cluster) per window when both tiles exist and 2 B CTAs fit the machine
   const bool split = g_fwd_split != 0 && plan->n > 128 && 2 * B <= sms;
   const int grid = split ? (int)(2 * B) : (int)(B < sms ? B : sms);
+  if (!(split ? tc_layout(plan, p.n_ops, &p, &smem) : rf_layout(plan, p.n_ops, &p, &smem)))
+    return set_error(STMP_EUNSUPPORTED, "tensor-core graph-GRU kernel needs %d B of shared memory", smem);
+  p.gimg = p.n_ops && split ? plan->gimg[p.n_ops] : nullptr;
+  p.rimg = p.n_ops && !split ? plan->rimg[p.n_ops] : nullptr;
+  if (p.n_ops && !(split ? p.gimg : p.rimg))
+    return set_error(STMP_EUNSUPPORTED, "tensor-core graph-GRU kernel: the plan has no shared-memory graph image");
   p.ws_pitch = tc_ws_pitch(p.T, p.CIN);
   switch (p.CIN) {
 #define STMP_TC_CASE(C)                                                                                              \
@@ -714,8 +1159,8 @@ static int tc_launch_params(const stmp_plan* plan, TcParams& p, cudaStream_t st)
       cfg.attrs = at; cfg.numAttrs = 1;                                                                              \
       STMP_CUDA_OK(cudaLaunchKernelEx(&cfg, k_dcrnn_seq_tc<C, 2>, p));                                               \
     } else {                                                                                                         \
-      STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_seq_tc<C, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));   \
-      k_dcrnn_seq_tc<C, 1><<<grid, 512, smem, st>>>(p);                                                              \
+      STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_seq_rf<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));      \
+      k_dcrnn_seq_rf<C><<<grid, 512, smem, st>>>(p);                                                                 \
     }                                                                                                                \
     break;
     STMP_TC_CASE(1) STMP_TC_CASE(2) STMP_TC_CASE(3) STMP_TC_CASE(4)

@@ -9,7 +9,9 @@
 // round-to-nearest intrinsics (no FMA contraction) so plan values are bit-identical to the oracle.
 #include <cub/cub.cuh>
 
+#include <algorithm>
 #include <cmath>
+#include <numeric>
 #include <vector>
 
 #include <cstring>
@@ -18,6 +20,7 @@
 #include "common.cuh"
 #include "dcrnn_common.cuh"
 #include "graph_image.cuh"
+#include "row_image.cuh"
 
 namespace stmp {
 
@@ -739,6 +742,32 @@ int build_graph_images(Builder& b, stmp_plan* p) {
       p->gimg[n_ops] = nullptr;
       p->gimg_bytes[n_ops] = 0;
     }
+  // the one-CTA kernel's row image, built on the host from the forward CSR
+  std::vector<int> rp[2], cl[2];
+  std::vector<float> vl[2];
+  for (int op = 0; op < p->n_ops; ++op) {
+    const Csr& c = p->fwd[op];
+    std::vector<int2> cv(c.nnz);
+    rp[op].resize(N + 1);
+    STMP_CUDA_OK(cudaMemcpyAsync(rp[op].data(), c.rowptr, (size_t)(N + 1) * sizeof(int), cudaMemcpyDeviceToHost, b.st));
+    if (c.nnz) STMP_CUDA_OK(cudaMemcpyAsync(cv.data(), c.cv, (size_t)c.nnz * sizeof(int2), cudaMemcpyDeviceToHost, b.st));
+    STMP_CUDA_OK(cudaStreamSynchronize(b.st));
+    cl[op].resize(c.nnz);
+    vl[op].resize(c.nnz);
+    for (int k = 0; k < c.nnz; ++k) { cl[op][k] = cv[k].x; std::memcpy(&vl[op][k], &cv[k].y, 4); }
+  }
+  const int* rps[2] = {rp[0].data(), rp[1].data()};
+  const int* cls[2] = {cl[0].data(), cl[1].data()};
+  const float* vls[2] = {vl[0].data(), vl[1].data()};
+  for (int n_ops = 1; n_ops <= p->n_ops; ++n_ops) {
+    const int64_t bytes = build_row_image(N, n_ops, rps, cls, vls, nullptr, 0);
+    if (bytes <= 0 || bytes > tc_row_image_budget()) continue;
+    std::vector<unsigned char> img((size_t)bytes);
+    build_row_image(N, n_ops, rps, cls, vls, img.data(), bytes);
+    STMP_CUDA_OK(cudaMalloc(&p->rimg[n_ops], (size_t)bytes));
+    STMP_CUDA_OK(cudaMemcpy(p->rimg[n_ops], img.data(), (size_t)bytes, cudaMemcpyHostToDevice));
+    p->rimg_groups[n_ops] = reinterpret_cast<const int*>(img.data())[0];
+  }
   return 0;
 }
 
@@ -750,6 +779,100 @@ void free_csr(Csr& c) {
 }
 
 }  // namespace
+
+// ---- row image for the one-CTA wgmma kernel (row_image.cuh) -------------------------------------------------------------
+int64_t build_row_image(int N, int n_ops, const int* const rowptr[2], const int* const col[2], const float* const val[2], void* dst,
+                        int64_t capacity) {
+  if (N < 1 || N > kRiMaxN || n_ops < 1 || n_ops > 2) return 0;
+  std::vector<int> ng(2 * N, 0);   // groups of 4 entries per (operator, row)
+  for (int op = 0; op < n_ops; ++op)
+    for (int i = 0; i < N; ++i) {
+      const int beg = rowptr[op][i], end = rowptr[op][i + 1];
+      if (end < beg) return 0;
+      for (int k = beg; k < end; ++k)
+        if (col[op][k] < 0 || col[op][k] >= N) return 0;
+      ng[op * N + i] = (end - beg + 3) / 4;
+    }
+  // nodes by descending group count over both operators (ties: node id), then the empty positions
+  std::vector<int> order(N);
+  std::iota(order.begin(), order.end(), 0);
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return ng[a] + ng[N + a] > ng[b] + ng[N + b]; });
+  order.resize(kRiPos, -1);
+  // bins of 8 consecutive nodes (one row per quad of a (warp, slot)); a bin's gather runs as long as its longest row per operator
+  constexpr int kBins = kRiPos / 8;
+  int bin_g[kBins][2] = {}, bin_cost[kBins];
+  for (int k = 0; k < kBins; ++k) {
+    for (int m = 0; m < 8; ++m) {
+      const int node = order[8 * k + m];
+      if (node >= 0)
+        for (int op = 0; op < 2; ++op) bin_g[k][op] = std::max(bin_g[k][op], ng[op * N + node]);
+    }
+    bin_cost[k] = bin_g[k][0] + bin_g[k][1];
+  }
+  // longest processing time first: every bin onto the least loaded warp that has a free slot
+  std::vector<int> bins(kBins);
+  std::iota(bins.begin(), bins.end(), 0);
+  std::stable_sort(bins.begin(), bins.end(), [&](int a, int b) { return bin_cost[a] > bin_cost[b]; });
+  int load[kRiWarps] = {}, used[kRiWarps] = {}, bin_at[kRiWarps][2];
+  for (int k : bins) {
+    int best = -1;
+    for (int w = 0; w < kRiWarps; ++w)
+      if (used[w] < 2 && (best < 0 || load[w] < load[best])) best = w;
+    bin_at[best][used[best]++] = k;
+    load[best] += bin_cost[k];
+  }
+  std::vector<int16_t> perm(kRiPos, -1);
+  std::vector<uint8_t> ipos(kRiPos, 0);
+  int n_groups = 0;
+  for (int w = 0; w < kRiWarps; ++w)
+    for (int s = 0; s < 2; ++s) {
+      for (int quad = 0; quad < 8; ++quad) {
+        const int node = order[8 * bin_at[w][s] + quad], pos = 16 * w + 8 * s + quad;
+        perm[pos] = (int16_t)node;
+        if (node >= 0) ipos[node] = (uint8_t)pos;
+      }
+      for (int op = 0; op < n_ops; ++op) n_groups += bin_g[bin_at[w][s]][op];
+    }
+  int zero_pos = 0;
+  while (perm[zero_pos] >= 0) ++zero_pos;   // N <= 255: there is an empty position
+  const RowImageLayout L = row_image_layout(n_groups);
+  if (!dst || capacity < L.bytes) return L.bytes;
+
+  unsigned char* img = static_cast<unsigned char*>(dst);
+  std::memset(img, 0, (size_t)L.bytes);
+  int* hdr = reinterpret_cast<int*>(img);
+  hdr[0] = n_groups; hdr[1] = zero_pos; hdr[2] = N; hdr[3] = n_ops;
+  std::memcpy(img + kRiOffPerm, perm.data(), 2 * kRiPos);
+  std::memcpy(img + kRiOffIpos, ipos.data(), kRiPos);
+  uint16_t* gstart = reinterpret_cast<uint16_t*>(img + kRiOffGstart);
+  uint16_t* gcount = reinterpret_cast<uint16_t*>(img + kRiOffGcount);
+  uint32_t* idx = reinterpret_cast<uint32_t*>(img + kRiOffIdx);
+  float* vals = reinterpret_cast<float*>(img + L.off_val);
+  int run = 0;
+  for (int w = 0; w < kRiWarps; ++w)
+    for (int op = 0; op < n_ops; ++op)
+      for (int s = 0; s < 2; ++s) {
+        const int G = bin_g[bin_at[w][s]][op];
+        gstart[ri_list(w, op, s)] = (uint16_t)run;
+        gcount[ri_list(w, op, s)] = (uint16_t)G;
+        for (int g = 0; g < G; ++g)
+          for (int quad = 0; quad < 8; ++quad) {
+            const int node = perm[16 * w + 8 * s + quad];
+            const int beg = node >= 0 ? rowptr[op][node] : 0, len = node >= 0 ? rowptr[op][node + 1] - beg : 0;
+            uint32_t u = 0;
+            for (int e = 0; e < 4; ++e) {
+              const int k = 4 * g + e;
+              u |= (uint32_t)(k < len ? ipos[col[op][beg + k]] : zero_pos) << (8 * e);
+              vals[((run + g) * 8 + quad) * 4 + e] = k < len ? val[op][beg + k] : 0.f;
+            }
+            idx[(run + g) * 8 + quad] = u;
+          }
+        run += G;
+      }
+  for (int quad = 0; quad < 8; ++quad) idx[run * 8 + quad] = (uint32_t)zero_pos * 0x01010101u;   // the spare group row
+  return L.bytes;
+}
+
 }  // namespace stmp
 
 using namespace stmp;
@@ -847,8 +970,10 @@ extern "C" void stmp_plan_destroy(stmp_plan* p) {
     free_csr(p->fwd[i]);
     free_csr(p->bwd[i]);
   }
-  for (int i = 0; i < 3; ++i)
+  for (int i = 0; i < 3; ++i) {
     if (p->gimg[i]) cudaFree(p->gimg[i]);
+    if (p->rimg[i]) cudaFree(p->rimg[i]);
+  }
   delete p;
 }
 
@@ -881,6 +1006,15 @@ extern "C" int64_t stmp_plan_graph_image(const stmp_plan* p, int n_ops, void* ds
     return -set_error(STMP_ECUDA, "stmp_plan_graph_image: copy of %lld bytes failed", (long long)bytes);
   }
   return bytes;
+}
+
+extern "C" int64_t stmp_row_image_build(int64_t num_nodes, int n_ops, const int32_t* rowptr0, const int32_t* col0, const float* val0,
+                                        const int32_t* rowptr1, const int32_t* col1, const float* val1, void* dst, int64_t capacity) {
+  if (num_nodes < 1 || num_nodes > kRiMaxN || n_ops < 1 || n_ops > 2 || !rowptr0 || (n_ops > 1 && !rowptr1)) return 0;
+  const int* rp[2] = {rowptr0, rowptr1};
+  const int* cl[2] = {col0, col1};
+  const float* vl[2] = {val0, val1};
+  return build_row_image((int)num_nodes, n_ops, rp, cl, vl, dst, capacity);
 }
 
 /* Test hook: select, at run time, the implementation or launch shape a test cross-checks against the default (common.cuh). */
