@@ -164,7 +164,7 @@ def launch_count() -> int:
 
 def path_counters() -> dict:
     """{kernel name: launches so far} -- lets tests and users assert which path (wgmma / FFMA / tiled) served a call."""
-    n = 96
+    n = lib().stmp_path_counters(None, None, 0)
     names = (c_char_p * n)()
     counts = (c_int64 * n)()
     k = lib().stmp_path_counters(ctypes.cast(names, c_void_p), ctypes.cast(counts, c_void_p), n)

@@ -70,13 +70,19 @@ __device__ __forceinline__ void gather_ax(const int* rowptr, const int2* cv, con
 }
 
 // Sum of column i of `parts` per-CTA partials (row length `width`) in a fixed association: warp w sums its contiguous share of the
-// partials, then the 8 sub-sums are added in warp order.  Valid in warp 0 only; i may depend on the lane only.
+// partials, then the 8 sub-sums are added in warp order.  Valid in warp 0 only; i may depend on the lane only.  A warp's share is
+// summed with Kahan compensation: at 65 535 batch rows a share is 8 192 partials, and a plain running sum lost ~3e-6 of the total.
 __device__ __forceinline__ float sum_partials(int parts, int width, const float* __restrict__ partial, int i, float (&sub)[8][32]) {
   const int x = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int per = (parts + 7) / 8, q0 = w * per, q1 = (q0 + per < parts) ? q0 + per : parts;
-  float s = 0.f;
+  float s = 0.f, comp = 0.f;
   if (i < width)
-    for (int q = q0; q < q1; ++q) s += partial[(size_t)q * width + i];
+    for (int q = q0; q < q1; ++q) {
+      const float y = __fsub_rn(partial[(size_t)q * width + i], comp);
+      const float t = __fadd_rn(s, y);
+      comp = __fsub_rn(__fsub_rn(t, s), y);
+      s = t;
+    }
   sub[w][x] = s;
   __syncthreads();
   float t = sub[0][x];
@@ -453,6 +459,7 @@ int launch_nq(const TgcnArgs& a, dim3 grid, size_t smem, cudaStream_t st) {
     k_tgcn_attn<NQ, false><<<grid, 256, smem, st>>>(a);
   }
   STMP_LAUNCH_OK("k_tgcn_attn");
+  if (!a.stage) { static const int slotg = path_slot("k_tgcn_attn[x-global]"); count_path(slotg); }
   return STMP_OK;
 }
 
@@ -532,6 +539,7 @@ extern "C" int stmp_tgcn_attn_bwd(const stmp_plan* plan, int64_t B, int64_t fin,
   }
 #undef STMP_TGCN_BWD
   STMP_LAUNCH_OK("k_tgcn_attn_bwd");
+  if (!a.stage) { static const int slotg = path_slot("k_tgcn_attn_bwd[x-global]"); count_path(slotg); }
   k_tgcn_attn_bwd_reduce<<<(kBwdPartial + 31) / 32, 256, 0, st>>>((int)(grid.x * grid.y), (int)fin, (int)periods, a.partial, dA, dc, dprobs);
   STMP_LAUNCH_OK("k_tgcn_attn_bwd_reduce");
   return STMP_OK;
@@ -565,6 +573,7 @@ extern "C" int stmp_tgcn_cell_bwd(const stmp_plan* plan, int64_t B, int64_t fin,
   STMP_CUDA_OK(cudaFuncSetAttribute(k_tgcn_cell_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k_tgcn_cell_bwd<<<grid, 256, smem, st>>>(a);
   STMP_LAUNCH_OK("k_tgcn_cell_bwd");
+  if (!a.stage) { static const int slotg = path_slot("k_tgcn_cell_bwd[x-global]"); count_path(slotg); }
   k_tgcn_cell_bwd_reduce<<<(kCellPartial + 31) / 32, 256, 0, st>>>((int)(grid.x * grid.y), (int)fin, a.partial, dA, dBm, dc);
   STMP_LAUNCH_OK("k_tgcn_cell_bwd_reduce");
   return STMP_OK;

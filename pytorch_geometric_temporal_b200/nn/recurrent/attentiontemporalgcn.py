@@ -2,6 +2,8 @@
 state_dict keys `_attention (periods)`, `_base_tgcn.*`.  The reference loops over the periods in Python
 (12 x 3 GCNConv chains, strided X[..., p] slices); the periods are independent (the SAME H enters each,
 :155), so all of them go through ONE batched SpMM + one set of GEMMs and the softmax-weighted sum."""
+import math
+
 import torch
 
 from ... import ops
@@ -14,7 +16,8 @@ class _A3Base(torch.nn.Module):
         _require_cuda(X, "X")
         base = self._base_tgcn
         P = X.shape[-1]
-        if base._attn_ok(X, H, P, self._attention):
+        rows = math.prod(X.shape[:-3])
+        if base._attn_ok(X, H, P, rows, self._attention):
             # ONE launch: gather A^X for all periods per node, the GRU gates of every period and the softmax-weighted sum
             N, F = X.shape[-3], X.shape[-2]
             plan = base._plan(edge_index, edge_weight, N)
@@ -23,7 +26,7 @@ class _A3Base(torch.nn.Module):
             if X.dim() == 3:                                        # A3TGCN: (N,F,P), H (N,out)
                 return ops.tgcn_attn_fwd(plan, X.unsqueeze(0), A, Bm, c, probs, H, h_shared=True)[0]
             return ops.tgcn_attn_fwd(plan, X, A, Bm, c, probs, H)   # A3TGCN2: (B,N,F,P), H (B,N,out)
-        if base._attn_train_ok(X, H, P):
+        if base._attn_train_ok(X, H, P, rows):
             # training without an incoming state: the same launch + a hand-written backward (gates recomputed, gradients of the folded
             # weights and of the attention probabilities reduced on the device)
             N, F = X.shape[-3], X.shape[-2]

@@ -2,6 +2,8 @@
 state_dict keys `conv_{z,r,h}.lin.weight (out,in)`, `conv_{z,r,h}.bias`, `linear_{z,r,h}.{weight,bias}`.
 The reference runs three GCNConvs (each: gcn_norm + lin + propagate of `out` channels); since
 A^(X W) = (A^ X) W, one SpMM on the `in` channels feeds all three gates."""
+import math
+
 import torch
 
 from ... import _lib, ops
@@ -100,18 +102,22 @@ class TGCN(torch.nn.Module):
             cs.append(L1 @ conv.bias + lin.bias)
         return torch.cat(As, dim=1), torch.cat(Bs, dim=1), torch.cat(cs)
 
-    def _attn_train_ok(self, X, H, periods):
+    # The fused kernels take the batch rows as the grid's y dimension, so at most 65 535 of them; a larger batch takes the op-for-op path.
+    _FUSED_MAX_ROWS = 65535
+
+    def _attn_train_ok(self, X, H, periods, rows):
         """The fused kernel pair (forward + hand-written backward) trains the configuration of the reference's examples: no incoming state,
-        no gradient w.r.t. X, out_channels == 32, in_channels <= 4, in_channels * periods <= 128."""
+        no gradient w.r.t. X, out_channels == 32, in_channels <= 4, in_channels * periods <= 128, `rows` <= 65 535 batch rows."""
         return (H is None and torch.is_grad_enabled() and not X.requires_grad and self.out_channels == 32 and self.in_channels <= 4
-                and self.in_channels * periods <= 128 and self.fused_training)
+                and self.in_channels * periods <= 128 and rows <= self._FUSED_MAX_ROWS and self.fused_training)
 
     def _cell_train_ok(self, X, H):
         """The steps after the first of a training loop that carries the state (the reference's BatchedTGCN, tgcn_example.py): the
         same forward launch with H + the hand-written cell backward (dH and the folded-weight gradients).  No gradient w.r.t. X,
-        out_channels == 32, in_channels <= 4, H of shape X.shape[:-1] + (32,)."""
+        out_channels == 32, in_channels <= 4, H of shape X.shape[:-1] + (32,), at most 65 535 batch rows."""
         return (H is not None and torch.is_grad_enabled() and not X.requires_grad and self.out_channels == 32 and self.in_channels <= 4
-                and tuple(H.shape) == tuple(X.shape[:-1]) + (32,) and self.fused_training)
+                and tuple(H.shape) == tuple(X.shape[:-1]) + (32,) and math.prod(X.shape[:-2]) <= self._FUSED_MAX_ROWS
+                and self.fused_training)
 
     fused_training = True     # False: train through autograd over SpMM + cuBLAS (tests compare the two)
 
@@ -121,11 +127,11 @@ class TGCN(torch.nn.Module):
         ts = list(self.parameters()) + [X] + ([] if H is None else [H]) + list(extra)
         return not any(t.requires_grad for t in ts)
 
-    def _attn_ok(self, X, H, periods, *extra):
-        """The fused temporal-attention + GCN kernel serves inference for out_channels == 32, in_channels <= 4 and
-        in_channels * periods <= 128 on graphs of any size."""
+    def _attn_ok(self, X, H, periods, rows, *extra):
+        """The fused temporal-attention + GCN kernel serves inference for out_channels == 32, in_channels <= 4,
+        in_channels * periods <= 128 and `rows` <= 65 535 batch rows on graphs of any size."""
         return (self.out_channels == 32 and self.in_channels <= 4 and self.in_channels * periods <= 128
-                and self._no_grad_needed(X, H, *extra))
+                and rows <= self._FUSED_MAX_ROWS and self._no_grad_needed(X, H, *extra))
 
     def _fused_ok(self, plan, X, H):
         if self.out_channels != 32:
@@ -139,13 +145,14 @@ class TGCN(torch.nn.Module):
                 H: torch.FloatTensor = None) -> torch.FloatTensor:
         _require_cuda(X, "X")
         plan = self._plan(edge_index, edge_weight, X.size(-2))
-        if self._attn_ok(X, H, 1):       # one period, weight 1: the cell itself
+        rows = math.prod(X.shape[:-2])
+        if self._attn_ok(X, H, 1, rows):       # one period, weight 1: the cell itself
             A, Bm, c = self._packed3()
             N, Ci = X.shape[-2], X.shape[-1]
             h = None if H is None else H.reshape(-1, N, self.out_channels)
             out = ops.tgcn_attn_fwd(plan, X.reshape(-1, N, Ci, 1), A, Bm, c, None, h)
             return out.reshape(*X.shape[:-1], self.out_channels)
-        if self._attn_train_ok(X, H, 1):
+        if self._attn_train_ok(X, H, 1, rows):
             A, Bm, c = self._fold3()
             N, Ci = X.shape[-2], X.shape[-1]
             out = ops.tgcn_attn_train(plan, X.reshape(-1, N, Ci, 1), A, Bm, c, None)

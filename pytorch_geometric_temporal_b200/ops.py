@@ -579,6 +579,8 @@ class _TgcnAttnFn(torch.autograd.Function):
         B, N, fin, P = x.shape
         gout = _f32c(gout, "gout")
         dev = x.device
+        if B == 0:                                  # nothing to launch (empty tensors have NULL data pointers)
+            return None, None, torch.zeros_like(A), None, torch.zeros_like(c), torch.zeros_like(probs) if ctx.has_probs else None
         ws = torch.empty(int(_lib.lib().stmp_tgcn_attn_bwd_workspace_bytes(plan.handle, B)), dtype=torch.uint8, device=dev)
         dA = torch.empty(fin, 96, dtype=torch.float32, device=dev)
         dc = torch.empty(96, dtype=torch.float32, device=dev)

@@ -129,22 +129,24 @@ def test_dcrnn_narrow_fused_backward():
 
 
 def test_a3tgcn2_fused_backward():
-    """A3TGCN2(2, 32, 12) without an incoming state under a Linear head: k_tgcn_attn_bwd."""
+    """A3TGCN2(2, 32, 12) and A3TGCN2(1, 32, 128) (four 32-period chunks per lane) without an incoming state under a Linear head:
+    k_tgcn_attn_bwd."""
     ei, ew = _graph(2)
-    m = _with_bias(A3TGCN2(2, 32, 12, 8), 2)
     head = torch.nn.Linear(32, 12).to(DEV)
-    X = torch.randn(8, 207, 2, 12, device=DEV)
     Y = _targets(8, 207, 12)
+    for fin, periods in ((2, 12), (1, 128)):
+        m = _with_bias(A3TGCN2(fin, 32, periods, 8), 2)
+        X = torch.randn(8, 207, fin, periods, device=DEV)
 
-    def run(scale):
-        m.zero_grad(set_to_none=True)
-        head.zero_grad(set_to_none=True)
-        c0 = _lib.path_counters()
-        (D.masked_mae_loss(head(torch.relu(m(X, ei, ew))), Y) * scale).backward()
-        ran = _ran(c0)
-        assert ran.get("k_tgcn_attn_bwd") == 1
-        return _grads(list(m.named_parameters()) + [("head." + k, p) for k, p in head.named_parameters()])
-    _assert_equivariant(run)
+        def run(scale):
+            m.zero_grad(set_to_none=True)
+            head.zero_grad(set_to_none=True)
+            c0 = _lib.path_counters()
+            (D.masked_mae_loss(head(torch.relu(m(X, ei, ew))), Y) * scale).backward()
+            ran = _ran(c0)
+            assert ran.get("k_tgcn_attn_bwd") == 1
+            return _grads(list(m.named_parameters()) + [("head." + k, p) for k, p in head.named_parameters()])
+        _assert_equivariant(run)
 
 
 def test_tgcn2_carried_state_fused_backward():
