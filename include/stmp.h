@@ -304,6 +304,33 @@ int64_t stmp_gru_rows_wgrad_workspace_bytes(int n_ops, int64_t cin);
 int stmp_gru_rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
                         const float* dph, void* workspace, float* dw, float* db, void* stream);
 
+/* ---- BatchedDCRNN at 32 hidden channels on graphs of ANY size, split over CTAs by destination rows (dcrnn_rows.cu): the reference's
+ * BatchedDCRNN (dcrnn.py:328-475) with H_0 = 0, all B windows of a step in each launch.  Envelope: a DConv plan, cout = 32, K = 2, cin 1..4
+ * (stmp_dcrnn_rows_supported), any number of nodes and any degree.  Exact fp32 FFMA; deterministic (no atomics, every sum in a fixed
+ * order); no host sync and no allocation: scratch comes from the caller, so a training step can be captured.
+ *   weights: wzrT (64, 3C) and whsT (32, 3C), C = cin + 32, from stmp_dcrnn_pack_bwd_weights (rows are outputs, columns the basis
+ *   [X | H | P_o X | P_o H | P_i X | P_i H]); bz / br / bh (32) each nullable.
+ *   stmp_dcrnn_rows_fwd:  x as stmp_dcrnn_seq_fwd (windows (B,T,N,cin) at strides x_bstride / x_tstride, or the resident series read at
+ *                         win_start) -> out (B,T,N,32).  2T - 1 launches: two per step, one for step 0 (a plan holding a non-finite
+ *                         operator value runs step 0 as two, so the non-finite values spread as in the reference).  Training adds
+ *                         stash (T,B,N,96) = Z | R | Ht and the weight-gradient bases S1 / S2 (T*B, N, ld), ld = 3C rounded up to 8,
+ *                         16-byte aligned (the layout stmp_dcrnn_bwd_wgrad reads); give all three or none.  The output does not depend
+ *                         on whether they are given.
+ *   stmp_dcrnn_rows_bwd:  gout = dL/dout (B,T,N,32), out and stash of the forward -> dph_all (T,B,N,32), dpzr_all (T,B,N,64) (the operands
+ *                         of stmp_dcrnn_bwd_wgrad) and dx (B,T,N,cin; nullable).  Reverse time: a rowwise launch, then per step t >= 1 the
+ *                         transposed gathers of dS2's and of dS1's operator blocks (the second also starts step t - 1), and one more
+ *                         gather for step 0's dX: 2T - 1 launches, 2T with dx.
+ *   Both take scratch of stmp_dcrnn_rows_scratch_bytes(plan, B) bytes.
+ * STMP_EINVAL for a NULL plan or tensor, a non-DConv plan or negative B / T, STMP_ESHAPE for a bad pitch, alignment or B * N >= 2^31,
+ * STMP_EUNSUPPORTED outside the envelope. */
+int stmp_dcrnn_rows_supported(const stmp_plan* plan, int64_t cin, int64_t cout, int64_t K);
+int64_t stmp_dcrnn_rows_scratch_bytes(const stmp_plan* plan, int64_t B);
+int stmp_dcrnn_rows_fwd(const stmp_plan* plan, int64_t B, int64_t T, int64_t cin, const float* x, const int64_t* win_start,
+                        int64_t x_bstride, int64_t x_tstride, const float* wzrT, const float* whsT, const float* bz, const float* br,
+                        const float* bh, float* scratch, float* out, float* stash, float* S1, float* S2, int64_t ld, void* stream);
+int stmp_dcrnn_rows_bwd(const stmp_plan* plan, int64_t B, int64_t T, int64_t cin, const float* gout, const float* out, const float* stash,
+                        const float* wzrT, const float* whsT, float* scratch, float* dph_all, float* dpzr_all, float* dx, void* stream);
+
 /* ---- the peephole graph-LSTM cell on graphs of ANY size, split over CTAs by destination rows (lstm_rows.cu): GConvLSTM
  * (gconv_lstm.py:168-238) and GCLSTM (gc_lstm.py:139-205) at K <= 2 on a Chebyshev plan, one graph and one step per call.  `variant`
  * selects the basis: STMP_LSTM_GCONV [X | H | Op X | Op H], STMP_LSTM_GC [X | H | Op H] (X is not diffused); nb basis columns, X channels

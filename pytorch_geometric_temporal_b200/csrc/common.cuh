@@ -74,6 +74,7 @@ struct stmp_plan {
   int normalization = 0;
   unsigned flags = 0;
   float lambda_max = 0.f;
+  bool nonfinite_vals = false;   // an operator holds a non-finite value (DConv: 1/deg_in = inf at a source of in-degree 0)
   stmp::Csr fwd[2];  // by destination
   stmp::Csr bwd[2];  // by source (transposed product)
   int device = 0;

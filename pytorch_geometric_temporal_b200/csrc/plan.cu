@@ -75,6 +75,7 @@ inline int blocks_for(long long n) { return (int)((n + kThreads - 1) / kThreads)
 // err flag bits
 constexpr int kErrRange = 1;
 constexpr int kErrDuplicate = 2;
+constexpr int kNonFinite = 4;   // not an error: an operator holds a non-finite value (stmp_plan::nonfinite_vals)
 
 struct Info {
   int err;
@@ -138,12 +139,13 @@ __global__ void k_segment_sum(int n, const int* __restrict__ rowptr, const int* 
 }
 
 __global__ void k_fill_csr(int nnz, const int* __restrict__ perm, const int* __restrict__ src,
-                           const float* __restrict__ val, int2* __restrict__ cv, int* __restrict__ eid) {
+                           const float* __restrict__ val, int2* __restrict__ cv, int* __restrict__ eid, Info* info) {
   int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= nnz) return;
   int p = perm[k];
   cv[k] = make_int2(src[p], __float_as_int(val[p]));
   eid[k] = p;
+  if (!isfinite(val[p])) atomicOr(&info->err, kNonFinite);
 }
 
 // ---- DCONV ------------------------------------------------------------------------------------------
@@ -382,7 +384,7 @@ struct Builder {
     k_rowptr<<<blocks_for(n + 1), kThreads, 0, st>>>(n, nnz, ks, out->rowptr);
     STMP_LAUNCH_OK("k_rowptr");
     if (nnz) {
-      k_fill_csr<<<blocks_for(nnz), kThreads, 0, st>>>(nnz, perm, src, val, out->cv, out->eid);
+      k_fill_csr<<<blocks_for(nnz), kThreads, 0, st>>>(nnz, perm, src, val, out->cv, out->eid, d_info);
       STMP_LAUNCH_OK("k_fill_csr");
     }
     k_max_row<<<blocks_for(n), kThreads, 0, st>>>(n, out->rowptr, &d_info->max_row[info_slot]);
@@ -949,6 +951,7 @@ static int plan_create_impl(int flavor, int64_t num_nodes, int64_t num_edges, co
                                   "on the norm/reverse-index length mismatch (dcrnn.py:59-77,87)");
       break;
     }
+    p->nonfinite_vals = (h.err & kNonFinite) != 0;
     for (int op = 0; op < p->n_ops; ++op) {
       p->fwd[op].max_row_nnz = h.max_row[op * 2];
       p->bwd[op].max_row_nnz = h.max_row[op * 2 + 1];

@@ -4,7 +4,9 @@ BatchedDCRNN :328-475).  Same constructor signatures, forward signatures and sta
 (`conv_x_{z,r,h}.weight (2,K,Cin+Cout,Cout)`, `.bias (Cout)`); the arithmetic runs in libstmp:
 
 * inference (no grad): the whole recurrence in ONE fused kernel (`stmp_dcrnn_seq_fwd`);
-* training / shapes the fused kernel cannot take: the tiled path = hand-written SpMM (`stmp_spmm`,
+* graphs too large for one SM (hidden 32, K = 2, Cin <= 4): BatchedDCRNN runs the row-split kernels (`stmp_dcrnn_rows_*`), two
+  launches per step for all windows, and a hand-written reverse-time backward (`ops._DcrnnRowsFn`);
+* training / shapes the fused kernels cannot take: the tiled path = hand-written SpMM (`stmp_spmm`,
   differentiable through its transposed product) + cuBLAS contraction, with the diffusion shared
   between the z and r gates.
 """
@@ -370,6 +372,27 @@ class BatchedDCRNN(DCRNN):
     _conv_cls = BatchedDConv
     _batched_semantics = True
 
+    def __init__(self, in_channels: int, out_channels: int, K: int, bias: bool = True):
+        super().__init__(in_channels, out_channels, K, bias)
+        self._rows_pack = ops.PackCache()
+
+    def _rows_ok(self, plan, X, training):
+        """The row-split route (stmp_dcrnn_rows_*): out_channels = 32, K = 2, in_channels 1..4, float32 X, a graph the one-SM kernels
+        cannot hold (checked after the module's own attributes, so other shapes never consult the library); training calls also need
+        `_fused_training`."""
+        if self.out_channels != 32 or self.K != 2 or not 1 <= self.in_channels <= 4 or X.dtype != torch.float32:
+            return False
+        if training and not self._fused_training:
+            return False
+        if ops.dcrnn_seq_supported(plan, self.in_channels, self.out_channels, self.K):
+            return False
+        return ops.dcrnn_rows_supported(plan, self.in_channels, self.out_channels, self.K)
+
+    def _rows_packed(self):
+        """(whsT, wzrT) of dcrnn_pack_bwd_weights for the row-split kernels, rebuilt only when a parameter changes."""
+        return self._rows_pack.get(list(self.parameters()),
+                                   lambda: ops.dcrnn_pack_bwd_weights(*self._params()[:3], self.in_channels, self.K))
+
     def forward(self, X, edge_index, edge_weight):
         _require_cuda(X, "X")
         B, T, N, F = X.size()
@@ -384,6 +407,12 @@ class BatchedDCRNN(DCRNN):
                 return _DcrnnSeqFn.apply(X, None, *self._params(), plan, self.K, self._weight_image())
             except _lib.StmpUnsupported:
                 pass
+        training = self._needs_grad(X)
+        if self._rows_ok(plan, X, training):    # graphs larger than one SM: the row-split kernels, all windows of a step per launch
+            if training:
+                return ops._DcrnnRowsFn.apply(X, *self._params(), plan, self._rows_packed())
+            whsT, wzrT = self._rows_packed()
+            return ops.dcrnn_rows_fwd(plan, X, wzrT, whsT, *self._params()[3:])
         H = torch.zeros(B, N, self.out_channels, device=X.device, dtype=X.dtype)
         outs = []
         for t in range(T):
@@ -402,5 +431,8 @@ class BatchedDCRNN(DCRNN):
                                          wimage=self._weight_image())
             except _lib.StmpUnsupported:      # e.g. a horizon whose shared-memory layout the FFMA kernel cannot hold
                 pass
+        if not self._needs_grad(series) and self._rows_ok(plan, series, False):     # windows read in place at win_start
+            whsT, wzrT = self._rows_packed()
+            return ops.dcrnn_rows_fwd(plan, series, wzrT, whsT, *self._params()[3:], win_start=win_start, horizon=horizon)
         X = ops.window_gather(series, win_start, horizon, with_target=False)
         return self.forward(X, edge_index, edge_weight)

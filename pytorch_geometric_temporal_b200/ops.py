@@ -955,6 +955,97 @@ def dcrnn_pack_bwd_weights(wz, wr, wh, cin: int, K: int):
     return whsT, wzrT
 
 
+def dcrnn_rows_supported(plan: GraphPlan, cin: int, cout: int, K: int) -> bool:
+    """The row-split DCRNN envelope (stmp_dcrnn_rows_supported): cout = 32, K = 2, cin 1..4 on a DConv plan, any graph size."""
+    if cout != 32 or K != 2 or not 1 <= cin <= 4:
+        return False
+    return bool(_lib.lib().stmp_dcrnn_rows_supported(plan.handle, cin, cout, K))
+
+
+def dcrnn_rows_fwd(plan: GraphPlan, x: torch.Tensor, wzrT: torch.Tensor, whsT: torch.Tensor, bz, br, bh,
+                   win_start: Optional[torch.Tensor] = None, horizon: Optional[int] = None, train: bool = False):
+    """Row-split BatchedDCRNN recurrence from H_0 = 0 (stmp_dcrnn_rows_fwd).  x: (B,T,N,cin) windows, or -- with win_start (int64 [B]) and
+    horizon -- the resident series (T_total,N,cin) read in place.  wzrT / whsT from dcrnn_pack_bwd_weights; biases (32,) or None.
+    Returns out (B,T,N,32); with `train`, (out, stash (T,B,N,96), S1, S2 (T*B, N, ld)) -- the operands of dcrnn_rows_bwd / dcrnn_bwd_wgrad."""
+    x = _f32c(x, "X")
+    N = plan.num_nodes
+    if win_start is None:
+        if x.dim() != 4 or x.size(2) != N:
+            raise RuntimeError(f"X must be (B,T,{N},Cin), got {tuple(x.shape)}")
+        B, T, _, cin = x.shape
+        bstride, tstride, ws = T * N * cin, N * cin, None
+    else:
+        if x.dim() != 3 or x.size(1) != N:
+            raise RuntimeError(f"series must be (T_total,{N},Cin), got {tuple(x.shape)}")
+        _require_cuda(win_start, "win_start")
+        ws = win_start.to(torch.int64).contiguous()
+        B, T, cin = ws.numel(), int(horizon), x.size(2)
+        bstride, tstride = 0, N * cin
+    nb = 3 * (cin + 32)
+    if wzrT.shape != (64, nb) or whsT.shape != (32, nb):
+        raise RuntimeError(f"dcrnn_rows_fwd: wzrT must be (64, {nb}) and whsT (32, {nb})")
+    f32 = dict(device=x.device, dtype=torch.float32)
+    ld = dcrnn_bwd_basis_ld(cin, 32, 2)
+    out = torch.empty(B, T, N, 32, **f32)
+    st = S1 = S2 = None
+    if train:
+        st = torch.empty(T, B, N, 96, **f32)
+        S1 = torch.empty(T * B, N, ld, **f32)
+        S2 = torch.empty(T * B, N, ld, **f32)
+    if B > 0 and T > 0:
+        scr = torch.empty(int(_lib.lib().stmp_dcrnn_rows_scratch_bytes(plan.handle, B)) // 4, **f32)
+        bs = [None if b is None else _f32c(b.detach(), "bias") for b in (bz, br, bh)]
+        with torch.cuda.device(x.device):
+            _lib.check(_lib.lib().stmp_dcrnn_rows_fwd(plan.handle, B, T, cin, _lib.ptr(x), _lib.ptr(ws), bstride, tstride,
+                                                      _lib.ptr(_f32c(wzrT, "wzrT")), _lib.ptr(_f32c(whsT, "whsT")), _lib.ptr(bs[0]),
+                                                      _lib.ptr(bs[1]), _lib.ptr(bs[2]), _lib.ptr(scr), _lib.ptr(out), _lib.ptr(st),
+                                                      _lib.ptr(S1), _lib.ptr(S2), ld, _lib.stream_ptr()))
+    return (out, st, S1, S2) if train else out
+
+
+def dcrnn_rows_bwd(plan: GraphPlan, cin: int, gout, out, stash, wzrT, whsT, want_dx: bool):
+    """(dph_all (T,B,N,32), dpzr_all (T,B,N,64), dx (B,T,N,cin) or None): the reverse-time backward of dcrnn_rows_fwd (stmp_dcrnn_rows_bwd)."""
+    gout = _f32c(gout, "gout")
+    B, T, N, _ = gout.shape
+    f32 = dict(device=gout.device, dtype=torch.float32)
+    dph, dpzr = torch.empty(T, B, N, 32, **f32), torch.empty(T, B, N, 64, **f32)
+    dx = torch.empty(B, T, N, cin, **f32) if want_dx else None
+    if B > 0 and T > 0:
+        scr = torch.empty(int(_lib.lib().stmp_dcrnn_rows_scratch_bytes(plan.handle, B)) // 4, **f32)
+        with torch.cuda.device(gout.device):
+            _lib.check(_lib.lib().stmp_dcrnn_rows_bwd(plan.handle, B, T, cin, _lib.ptr(gout), _lib.ptr(out), _lib.ptr(stash), _lib.ptr(wzrT),
+                                                      _lib.ptr(whsT), _lib.ptr(scr), _lib.ptr(dph), _lib.ptr(dpzr), _lib.ptr(dx),
+                                                      _lib.stream_ptr()))
+    return dph, dpzr, dx
+
+
+class _DcrnnRowsFn(torch.autograd.Function):
+    """Training form of the row-split BatchedDCRNN recurrence (H_0 = 0): forward = `stmp_dcrnn_rows_fwd` with the stash and the
+    weight-gradient bases (the inference launches, so the output is bit-identical to the `no_grad` one); backward = `stmp_dcrnn_rows_bwd`
+    + `stmp_dcrnn_bwd_wgrad`: dX (when X requires grad) and the gradients of the three gates' (2, 2, C, 32) weights and biases.
+    `packed` = (whsT, wzrT) of dcrnn_pack_bwd_weights for the current weights."""
+
+    @staticmethod
+    def forward(ctx, X, wz, wr, wh, bz, br, bh, plan, packed):
+        whsT, wzrT = packed
+        out, stash, S1, S2 = dcrnn_rows_fwd(plan, X.detach(), wzrT, whsT, bz, br, bh, train=True)
+        ctx.plan, ctx.cin, ctx.has_bias = plan, X.size(-1), bz is not None
+        ctx.save_for_backward(out, stash, S1, S2, whsT, wzrT)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        out, stash, S1, S2, whsT, wzrT = ctx.saved_tensors
+        dph, dpzr, dX = dcrnn_rows_bwd(ctx.plan, ctx.cin, gout, out, stash, wzrT, whsT, ctx.needs_input_grad[0])
+        g = [None] * 6
+        if any(ctx.needs_input_grad[1:7]) and S1.numel() == 0:              # no windows or no steps: nothing to contract
+            z = torch.zeros(2, 2, ctx.cin + 32, 32, device=gout.device)
+            g = [z, z.clone(), z.clone()] + ([torch.zeros(32, device=gout.device) for _ in range(3)] if ctx.has_bias else [None] * 3)
+        elif any(ctx.needs_input_grad[1:7]):
+            g = list(dcrnn_bwd_wgrad(ctx.cin, 2, S1, S2, dpzr, dph, ctx.has_bias))
+        return (dX, *g, None, None)
+
+
 class _MaskedMAE(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pred, target):

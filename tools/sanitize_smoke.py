@@ -65,6 +65,13 @@ with torch.enable_grad():
             sum(t.square().mean() for t in gl(xr, e_ring, None)).backward()
             with torch.no_grad():
                 gl(xr, e_ring, None, hc[0].detach(), hc[1].detach())
+    for cin, T in ((2, 3), (4, 1)):                              # 301 nodes: the row-split DCRNN (k_dcrnn_rows_*), T = 1 and T > 1, with and
+        dr = BatchedDCRNN(cin, 32, 2).to(dev)                    # without dX (k_dcrnn_rows_bwd_x), k_dcrnn_wgrad_tc + k_dcrnn_wgrad_reduce
+        xd = torch.randn(2, T, 301, cin, device=dev)
+        dr(xd.clone().requires_grad_(True), e_ring, None).square().mean().backward()
+        dr(xd, e_ring, None).square().mean().backward()
+        with torch.no_grad():
+            dr(xd, e_ring, None)
 with torch.no_grad():
     e4 =torch.from_numpy(synthetic.pems04_like(0)).to(dev)
     ASTGCN(2, 1, 3, 64, 64, 1, 12, 12, 307, normalization="sym").to(dev)(torch.randn(2, 307, 1, 12, device=dev), e4)   # k_gemm_blocks x7
