@@ -6,6 +6,9 @@ BatchedDCRNN :328-475).  Same constructor signatures, forward signatures and sta
 * inference (no grad): the whole recurrence in ONE fused kernel (`stmp_dcrnn_seq_fwd`);
 * graphs too large for one SM (hidden 32, K = 2, Cin <= 4): BatchedDCRNN runs the row-split kernels (`stmp_dcrnn_rows_*`), two
   launches per step for all windows, and a hand-written reverse-time backward (`ops._DcrnnRowsFn`);
+* graphs too large for one SM at narrow states (cout, Cin, K <= 4: the reference's BatchedDCRNN(F, F, K=3)): BatchedDCRNN runs the
+  narrow row-split kernels (`stmp_dcrnn_narrow_rows_*`), 2(K-1) launches per step for all windows after one hoisted diffusion of X, and
+  a hand-written reverse-time backward (`ops._DcrnnNarrowRowsFn`);
 * training / shapes the fused kernels cannot take: the tiled path = hand-written SpMM (`stmp_spmm`,
   differentiable through its transposed product) + cuBLAS contraction, with the diffusion shared
   between the z and r gates.
@@ -388,6 +391,18 @@ class BatchedDCRNN(DCRNN):
             return False
         return ops.dcrnn_rows_supported(plan, self.in_channels, self.out_channels, self.K)
 
+    def _nrows_ok(self, plan, X, training):
+        """The narrow row-split route (stmp_dcrnn_narrow_rows_*): out_channels, in_channels and K in 1..4, float32 X, a graph the one-SM
+        kernels cannot hold (checked after the module's own attributes, so other shapes never consult the library); training calls also
+        need `_fused_training`."""
+        if not (1 <= self.out_channels <= 4 and 1 <= self.in_channels <= 4 and 1 <= self.K <= 4) or X.dtype != torch.float32:
+            return False
+        if training and not self._fused_training:
+            return False
+        if ops.dcrnn_seq_supported(plan, self.in_channels, self.out_channels, self.K):
+            return False
+        return ops.dcrnn_narrow_rows_supported(plan, self.in_channels, self.out_channels, self.K)
+
     def _rows_packed(self):
         """(whsT, wzrT) of dcrnn_pack_bwd_weights for the row-split kernels, rebuilt only when a parameter changes."""
         return self._rows_pack.get(list(self.parameters()),
@@ -413,6 +428,11 @@ class BatchedDCRNN(DCRNN):
                 return ops._DcrnnRowsFn.apply(X, *self._params(), plan, self._rows_packed())
             whsT, wzrT = self._rows_packed()
             return ops.dcrnn_rows_fwd(plan, X, wzrT, whsT, *self._params()[3:])
+        if self._nrows_ok(plan, X, training):   # narrow states on graphs larger than one SM: the narrow row-split kernels
+            if training:
+                return ops._DcrnnNarrowRowsFn.apply(X, *self._params(), plan, self.K, self._rows_packed())
+            whsT, wzrT = self._rows_packed()
+            return ops.dcrnn_narrow_rows_fwd(plan, X, wzrT, whsT, *self._params()[3:], self.K)
         H = torch.zeros(B, N, self.out_channels, device=X.device, dtype=X.dtype)
         outs = []
         for t in range(T):

@@ -72,6 +72,14 @@ with torch.enable_grad():
         dr(xd, e_ring, None).square().mean().backward()
         with torch.no_grad():
             dr(xd, e_ring, None)
+    e_big = torch.stack([torch.arange(1100), (torch.arange(1100) + 1) % 1100]).to(dev)     # 1100 nodes: above the one-SM narrow kernels
+    for cin, cout, K, T in ((2, 2, 3, 3), (1, 3, 2, 1), (2, 1, 1, 2)):   # the narrow row-split DCRNN (k_dcrnn_nrows_*), with and without dX
+        dn = BatchedDCRNN(cin, cout, K).to(dev)
+        xn = torch.randn(3, T, 1100, cin, device=dev)
+        dn(xn.clone().requires_grad_(True), e_big, None).square().mean().backward()
+        dn(xn, e_big, None).square().mean().backward()
+        with torch.no_grad():
+            dn(xn, e_big, None)
 with torch.no_grad():
     e4 =torch.from_numpy(synthetic.pems04_like(0)).to(dev)
     ASTGCN(2, 1, 3, 64, 64, 1, 12, 12, 307, normalization="sym").to(dev)(torch.randn(2, 307, 1, 12, device=dev), e4)   # k_gemm_blocks x7
