@@ -363,6 +363,33 @@ int stmp_dcrnn_narrow_rows_bwd(const stmp_plan* plan, int64_t B, int64_t T, int6
                                const float* out, const float* stash, const float* wzrT, const float* whsT, float* scratch, float* dph_all,
                                float* dpzr_all, float* dsx, int64_t dsx_ld, void* stream);
 
+/* ---- BatchedDCRNN at 64 hidden channels on graphs of ANY size, split over CTAs by destination rows (dcrnn_wide_rows.cu): the reference's
+ * BatchedDCRNN (dcrnn.py:328-475) with H_0 = 0 at cout = 64, K = 2 or 3, cin 1..4 (stmp_dcrnn_wide_rows_supported) -- the DCRNN paper's
+ * 64 recurrent units with one or two diffusion steps, which no one-SM kernel holds.  All B windows of a step in each launch; rows are
+ * window-major (b N + n).  Exact fp32 FFMA; deterministic (no atomics, every sum in a fixed order); no host sync and no allocation: scratch
+ * comes from the caller, so a training step can be captured.  C = cin + 64, nbc = (2K-1) C.  Arguments as stmp_dcrnn_narrow_rows_*:
+ *   weights: wzrT (128, nbc) and whsT (64, nbc) from stmp_dcrnn_pack_bwd_weights; bz / br / bh (64) each nullable.
+ *   stmp_dcrnn_wide_rows_fwd: x = the X blocks of every (t, b) (block j of row n at x + t * x_tstride + b * x_bstride + n * x_ld +
+ *                         j * x_blk) -> out (B,T,N,64), 16-byte aligned.  One launch builds the kernels' weight image, then 2(K-1) launches
+ *                         per step and one for step 0 (a plan holding a non-finite operator value runs step 0 as 2(K-1) on a zero state).
+ *                         Training gives stash (T,B,N,192) = Z | R | Ht and the weight-gradient bases S1 / S2 (T*B, N, nbc) (all three or
+ *                         none); x is then NULL and the X blocks are read from S1's X columns (block j at column j C), which the caller
+ *                         has filled.  The output does not depend on whether they are given.
+ *   stmp_dcrnn_wide_rows_bwd: gout = dL/dout (B,T,N,64), out and stash of the forward -> dph_all (T,B,N,64), dpzr_all (T,B,N,128) and
+ *                         dsx (T*B, N, dsx_ld; nullable): the X columns of dS1 + dS2, block j at column j cin.  2 + 2(K-1)(T-1) launches.
+ *   Both take scratch of stmp_dcrnn_wide_rows_scratch_bytes(plan, B, cout, K) bytes, 16-byte aligned.
+ * STMP_EINVAL for a NULL plan or tensor, a non-DConv plan or negative B / T, STMP_ESHAPE for a bad stride or alignment or B N >= 2^40,
+ * STMP_EUNSUPPORTED outside the envelope. */
+int stmp_dcrnn_wide_rows_supported(const stmp_plan* plan, int64_t cin, int64_t cout, int64_t K);
+int64_t stmp_dcrnn_wide_rows_scratch_bytes(const stmp_plan* plan, int64_t B, int64_t cout, int64_t K);
+int stmp_dcrnn_wide_rows_fwd(const stmp_plan* plan, int64_t B, int64_t T, int64_t cin, int64_t cout, int64_t K, const float* x,
+                             int64_t x_bstride, int64_t x_tstride, int64_t x_ld, int64_t x_blk, const float* wzrT, const float* whsT,
+                             const float* bz, const float* br, const float* bh, float* scratch, float* out, float* stash, float* S1,
+                             float* S2, void* stream);
+int stmp_dcrnn_wide_rows_bwd(const stmp_plan* plan, int64_t B, int64_t T, int64_t cin, int64_t cout, int64_t K, const float* gout,
+                             const float* out, const float* stash, const float* wzrT, const float* whsT, float* scratch, float* dph_all,
+                             float* dpzr_all, float* dsx, int64_t dsx_ld, void* stream);
+
 /* ---- the peephole graph-LSTM cell on graphs of ANY size, split over CTAs by destination rows (lstm_rows.cu): GConvLSTM
  * (gconv_lstm.py:168-238) and GCLSTM (gc_lstm.py:139-205) at K <= 2 on a Chebyshev plan, one graph and one step per call.  `variant`
  * selects the basis: STMP_LSTM_GCONV [X | H | Op X | Op H], STMP_LSTM_GC [X | H | Op H] (X is not diffused); nb basis columns, X channels

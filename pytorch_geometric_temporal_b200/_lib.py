@@ -87,6 +87,10 @@ _SIGNATURES = {
     "stmp_dcrnn_narrow_rows_scratch_bytes": (c_int64, [_P, c_int64, c_int64, c_int64]),
     "stmp_dcrnn_narrow_rows_fwd": (c_int, [_P] + [c_int64] * 5 + [_P] + [c_int64] * 4 + [_P] * 10 + [_P]),
     "stmp_dcrnn_narrow_rows_bwd": (c_int, [_P] + [c_int64] * 5 + [_P] * 9 + [c_int64, _P]),
+    "stmp_dcrnn_wide_rows_supported": (c_int, [_P, c_int64, c_int64, c_int64]),
+    "stmp_dcrnn_wide_rows_scratch_bytes": (c_int64, [_P, c_int64, c_int64, c_int64]),
+    "stmp_dcrnn_wide_rows_fwd": (c_int, [_P] + [c_int64] * 5 + [_P] + [c_int64] * 4 + [_P] * 10 + [_P]),
+    "stmp_dcrnn_wide_rows_bwd": (c_int, [_P] + [c_int64] * 5 + [_P] * 9 + [c_int64, _P]),
     "stmp_lstm_rows_supported": (c_int, [_P, c_int, c_int, c_int64, c_int64]),
     "stmp_lstm_rows_pack_weights": (c_int, [c_int, c_int, c_int64] + [_P] * 8),
     "stmp_lstm_rows_fwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 10 + [c_int64, _P]),

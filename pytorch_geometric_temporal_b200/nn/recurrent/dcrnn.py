@@ -403,6 +403,16 @@ class BatchedDCRNN(DCRNN):
             return False
         return ops.dcrnn_narrow_rows_supported(plan, self.in_channels, self.out_channels, self.K)
 
+    def _wrows_ok(self, plan, X, training):
+        """The 64-wide row-split route (stmp_dcrnn_wide_rows_*): out_channels = 64, K = 2 or 3, in_channels 1..4, float32 X, any graph
+        (checked after the module's own attributes, so other shapes never consult the library); training calls also need
+        `_fused_training`."""
+        if self.out_channels != 64 or self.K not in (2, 3) or not 1 <= self.in_channels <= 4 or X.dtype != torch.float32:
+            return False
+        if training and not self._fused_training:
+            return False
+        return ops.dcrnn_wide_rows_supported(plan, self.in_channels, self.out_channels, self.K)
+
     def _rows_packed(self):
         """(whsT, wzrT) of dcrnn_pack_bwd_weights for the row-split kernels, rebuilt only when a parameter changes."""
         return self._rows_pack.get(list(self.parameters()),
@@ -433,6 +443,11 @@ class BatchedDCRNN(DCRNN):
                 return ops._DcrnnNarrowRowsFn.apply(X, *self._params(), plan, self.K, self._rows_packed())
             whsT, wzrT = self._rows_packed()
             return ops.dcrnn_narrow_rows_fwd(plan, X, wzrT, whsT, *self._params()[3:], self.K)
+        if self._wrows_ok(plan, X, training):   # 64 hidden channels, the DCRNN paper's width: the 64-wide row-split kernels
+            if training:
+                return ops._DcrnnWideRowsFn.apply(X, *self._params(), plan, self.K, self._rows_packed())
+            whsT, wzrT = self._rows_packed()
+            return ops.dcrnn_wide_rows_fwd(plan, X, wzrT, whsT, *self._params()[3:], self.K)
         H = torch.zeros(B, N, self.out_channels, device=X.device, dtype=X.dtype)
         outs = []
         for t in range(T):
@@ -454,5 +469,8 @@ class BatchedDCRNN(DCRNN):
         if not self._needs_grad(series) and self._rows_ok(plan, series, False):     # windows read in place at win_start
             whsT, wzrT = self._rows_packed()
             return ops.dcrnn_rows_fwd(plan, series, wzrT, whsT, *self._params()[3:], win_start=win_start, horizon=horizon)
+        if not self._needs_grad(series) and self._wrows_ok(plan, series, False):    # windows gathered into the hoisted X blocks
+            whsT, wzrT = self._rows_packed()
+            return ops.dcrnn_wide_rows_fwd(plan, series, wzrT, whsT, *self._params()[3:], self.K, win_start=win_start, horizon=horizon)
         X = ops.window_gather(series, win_start, horizon, with_target=False)
         return self.forward(X, edge_index, edge_weight)

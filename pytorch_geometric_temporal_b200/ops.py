@@ -1196,6 +1196,135 @@ class _DcrnnNarrowRowsFn(torch.autograd.Function):
         return (dX, *g, None, None, None)
 
 
+def dcrnn_wide_rows_supported(plan: GraphPlan, cin: int, cout: int, K: int) -> bool:
+    """The 64-wide row-split DCRNN envelope (stmp_dcrnn_wide_rows_supported): cout = 64, K = 2 or 3, cin 1..4 on a DConv plan, any graph
+    size."""
+    if cout != 64 or K not in (2, 3) or not 1 <= cin <= 4:
+        return False
+    return bool(_lib.lib().stmp_dcrnn_wide_rows_supported(plan.handle, cin, cout, K))
+
+
+def _wrows_scratch(plan: GraphPlan, B: int, K: int, device) -> torch.Tensor:
+    nbytes = int(_lib.lib().stmp_dcrnn_wide_rows_scratch_bytes(plan.handle, B, 64, K))
+    return torch.empty(nbytes // 4, device=device, dtype=torch.float32)
+
+
+def dcrnn_wide_rows_fwd(plan: GraphPlan, x: torch.Tensor, wzrT: torch.Tensor, whsT: torch.Tensor, bz, br, bh, K: int,
+                        win_start: Optional[torch.Tensor] = None, horizon: Optional[int] = None, train: bool = False):
+    """64-wide row-split BatchedDCRNN recurrence from H_0 = 0 (stmp_dcrnn_wide_rows_fwd).  x: (B,T,N,cin) windows, or -- with win_start
+    (int64 [B]) and horizon, inference only -- the resident series (T_total,N,cin), whose windows go straight into the hoisted X blocks.
+    wzrT / whsT from dcrnn_pack_bwd_weights; biases (64,) or None.  The X diffusion is hoisted out of the time loop.  Returns out
+    (B,T,N,64); with `train`, (out, stash (T,B,N,192), S1, S2 (T*B, N, (2K-1)C)) -- the operands of dcrnn_wide_rows_bwd and of the weight
+    gradients."""
+    x = _f32c(x, "X")
+    N = plan.num_nodes
+    if win_start is None:
+        if x.dim() != 4 or x.size(2) != N:
+            raise RuntimeError(f"X must be (B,T,{N},Cin), got {tuple(x.shape)}")
+        B, T, _, cin = x.shape
+    else:
+        if train:
+            raise RuntimeError("dcrnn_wide_rows_fwd: win_start is an inference entry")
+        if x.dim() != 3 or x.size(1) != N:
+            raise RuntimeError(f"series must be (T_total,{N},Cin), got {tuple(x.shape)}")
+        _require_cuda(win_start, "win_start")
+        win_start = win_start.to(torch.int64).contiguous()
+        B, T, cin = win_start.numel(), int(horizon), x.size(2)
+    C = cin + 64
+    nbc = (2 * K - 1) * C
+    if wzrT.shape != (128, nbc) or whsT.shape != (64, nbc):
+        raise RuntimeError(f"dcrnn_wide_rows_fwd: wzrT must be (128, {nbc}) and whsT (64, {nbc})")
+    f32 = dict(device=x.device, dtype=torch.float32)
+    wzrT, whsT = _f32c(wzrT, "wzrT"), _f32c(whsT, "whsT")
+    bs = [None if b is None else _f32c(b.detach(), "bias") for b in (bz, br, bh)]
+    out = torch.empty(B, T, N, 64, **f32)
+    L = _lib.lib()
+
+    def run(Bc, xp, strides, o, st, S1, S2, scr):
+        with torch.cuda.device(x.device):
+            _lib.check(L.stmp_dcrnn_wide_rows_fwd(plan.handle, Bc, T, cin, 64, K, _lib.ptr(xp), *strides, _lib.ptr(wzrT), _lib.ptr(whsT),
+                                                  _lib.ptr(bs[0]), _lib.ptr(bs[1]), _lib.ptr(bs[2]), _lib.ptr(scr), _lib.ptr(o), _lib.ptr(st),
+                                                  _lib.ptr(S1), _lib.ptr(S2), _lib.stream_ptr()))
+
+    if train:
+        st = torch.empty(T, B, N, 192, **f32)
+        S1 = torch.empty(T * B, N, nbc, **f32)
+        S2 = torch.empty(T * B, N, nbc, **f32)
+        if B > 0 and T > 0:
+            S1.view(T, B, N, nbc)[..., :cin] = x.transpose(0, 1)
+            _x_blocks(plan, S1, cin, C, K)
+            run(B, None, (0, 0, 0, 0), out, st, S1, S2, _wrows_scratch(plan, B, K, x.device))
+        return out, st, S1, S2
+    if B == 0 or T == 0:
+        return out
+    w = (2 * K - 1) * cin
+    Bc = max(1, min(B, _NROWS_XBUF_BYTES // (T * N * w * 4)))
+    scr = _wrows_scratch(plan, Bc, K, x.device)
+    buf = torch.empty(Bc * T, N, w, **f32)
+    for b0 in range(0, B, Bc):
+        nb = min(Bc, B - b0)
+        xb = buf[:nb * T]
+        if win_start is None:
+            xb.view(nb, T, N, w)[..., :cin] = x[b0:b0 + nb]
+        else:
+            xb.view(nb, T, N, w)[..., :cin] = window_gather(x, win_start[b0:b0 + nb], T, with_target=False)
+        _x_blocks(plan, xb, cin, cin, K)
+        run(nb, xb, (T * N * w, N * w, w, cin), out[b0:b0 + nb], None, None, None, scr)
+    return out
+
+
+def dcrnn_wide_rows_bwd(plan: GraphPlan, cin: int, K: int, gout, out, stash, wzrT, whsT, want_dx: bool):
+    """(dph_all (T,B,N,64), dpzr_all (T,B,N,128), dx (B,T,N,cin) or None): the reverse-time backward of dcrnn_wide_rows_fwd
+    (stmp_dcrnn_wide_rows_bwd), then dX from the X columns of dS1 + dS2 through one hoisted transposed basis adjoint."""
+    gout = _f32c(gout, "gout")
+    B, T, N, _ = gout.shape
+    f32 = dict(device=gout.device, dtype=torch.float32)
+    dph, dpzr = torch.empty(T, B, N, 64, **f32), torch.empty(T, B, N, 128, **f32)
+    w = (2 * K - 1) * cin
+    dsx = torch.empty(T * B, N, w, **f32) if want_dx else None
+    if B > 0 and T > 0:
+        scr = _wrows_scratch(plan, B, K, gout.device)
+        with torch.cuda.device(gout.device):
+            _lib.check(_lib.lib().stmp_dcrnn_wide_rows_bwd(plan.handle, B, T, cin, 64, K, _lib.ptr(gout), _lib.ptr(out), _lib.ptr(stash),
+                                                           _lib.ptr(wzrT), _lib.ptr(whsT), _lib.ptr(scr), _lib.ptr(dph), _lib.ptr(dpzr),
+                                                           _lib.ptr(dsx), w, _lib.stream_ptr()))
+    if not want_dx:
+        return dph, dpzr, None
+    if B == 0 or T == 0:
+        return dph, dpzr, torch.zeros(B, T, N, cin, **f32)
+    _x_blocks_adjoint(plan, dsx, cin, K)
+    return dph, dpzr, dsx.view(T, B, N, w)[..., :cin].transpose(0, 1).contiguous()
+
+
+class _DcrnnWideRowsFn(torch.autograd.Function):
+    """Training form of the 64-wide row-split BatchedDCRNN recurrence (H_0 = 0): forward = `stmp_dcrnn_wide_rows_fwd` with the stash and
+    the weight-gradient bases (the inference launches, so the output is bit-identical to the `no_grad` one); backward =
+    `stmp_dcrnn_wide_rows_bwd`, the hoisted dX adjoint when X requires grad, and the weight / bias gradients of `_DcrnnSeqFn._finish`.
+    `packed` = (whsT, wzrT) of dcrnn_pack_bwd_weights for the current weights."""
+
+    @staticmethod
+    def forward(ctx, X, wz, wr, wh, bz, br, bh, plan, K, packed):
+        whsT, wzrT = packed
+        out, stash, S1, S2 = dcrnn_wide_rows_fwd(plan, X.detach(), wzrT, whsT, bz, br, bh, K, train=True)
+        ctx.plan, ctx.K, ctx.cin, ctx.has_bias, ctx.has_h0 = plan, K, X.size(-1), bz is not None, False
+        ctx.save_for_backward(out, stash, S1, S2, whsT, wzrT)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        from .nn.recurrent.dcrnn import _DcrnnSeqFn
+        out, stash, S1, S2, whsT, wzrT = ctx.saved_tensors
+        K, cin = ctx.K, ctx.cin
+        dph, dpzr, dX = dcrnn_wide_rows_bwd(ctx.plan, cin, K, gout, out, stash, wzrT, whsT, ctx.needs_input_grad[0])
+        g = [None] * 6
+        if any(ctx.needs_input_grad[1:7]) and S1.numel() == 0:              # no windows or no steps: nothing to contract
+            z = torch.zeros(2, K, cin + 64, 64, device=gout.device)
+            g = [z, z.clone(), z.clone()] + ([torch.zeros(64, device=gout.device) for _ in range(3)] if ctx.has_bias else [None] * 3)
+        elif any(ctx.needs_input_grad[1:7]):
+            g = list(_DcrnnSeqFn._finish(ctx, S1, S2, dph, dpzr, None, None, K, cin + 64, 64)[2:8])
+        return (dX, *g, None, None, None)
+
+
 class _MaskedMAE(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pred, target):

@@ -80,6 +80,13 @@ with torch.enable_grad():
         dn(xn, e_big, None).square().mean().backward()
         with torch.no_grad():
             dn(xn, e_big, None)
+    for cin, K, T in ((2, 3, 3), (3, 2, 1)):                     # 301 nodes, 3 windows (a partial last warp): the 64-wide row-split DCRNN
+        dw = BatchedDCRNN(cin, 64, K).to(dev)                    # (k_dcrnn_wrows_*), T = 1 and T > 1, with and without dX
+        xw = torch.randn(3, T, 301, cin, device=dev)
+        dw(xw.clone().requires_grad_(True), e_ring, None).square().mean().backward()
+        dw(xw, e_ring, None).square().mean().backward()
+        with torch.no_grad():
+            dw(xw, e_ring, None)
 with torch.no_grad():
     e4 =torch.from_numpy(synthetic.pems04_like(0)).to(dev)
     ASTGCN(2, 1, 3, 64, 64, 1, 12, 12, 307, normalization="sym").to(dev)(torch.randn(2, 307, 1, 12, device=dev), e4)   # k_gemm_blocks x7
