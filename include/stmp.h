@@ -564,6 +564,19 @@ int stmp_gemm_blocks_f32(int64_t M, int64_t N, int64_t ncols, int64_t nblk, cons
                          const float* bias, int epilogue, const float* gamma, const float* beta, float eps, float* C, int64_t ldc, void* stream);
 int stmp_spatial_attention_fwd(int64_t B, int64_t n_nodes, int64_t n_steps, const float* lhs, const float* rhs, const float* bsT,
                                const void* vsT_packed, const void* vsT_image, float* st_out, int64_t ld_out, void* stream);
+/* stmp_spatial_attention_tiled_fwd:  the same st_out as stmp_spatial_attention_fwd, same inputs (vsT_packed only: no image), for
+ *   1 <= nodes <= 1024 (PeMS03 / PeMS07-sized graphs), T <= 12.  Two launches: k_spatt_tiles tiles the columns as well as the rows (<= 256
+ *   columns per CTA, the sigmoid operand regenerated per column tile), writes the unnormalised logits into st_out and one (max, sum) pair per
+ *   (row, column tile) into `workspace`; k_spatt_norm combines a row's pairs in a fixed order and normalises the row in place.
+ *   Deterministic (no atomics), no allocation, no host synchronisation: capturable into a CUDA graph.
+ *   workspace: >= stmp_spatial_attention_tiled_workspace_bytes(B, nodes) bytes, 8-byte aligned, given as `workspace_bytes`.
+ *   EUNSUPPORTED beyond 1024 nodes or 12 timesteps; ESHAPE for ld_out < nodes rounded up to 64, ld_out % 4 != 0 or st_out not 16-byte
+ *   aligned; EINVAL for NULL pointers (B > 0) or a short / misaligned workspace.  B == 0 launches nothing.
+ * stmp_spatial_attention_tiled_workspace_bytes: -1 outside the envelope. */
+int stmp_spatial_attention_tiled_fwd(int64_t B, int64_t n_nodes, int64_t n_steps, const float* lhs, const float* rhs, const float* bsT,
+                                     const void* vsT_packed, float* st_out, int64_t ld_out, void* workspace, int64_t workspace_bytes,
+                                     void* stream);
+int64_t stmp_spatial_attention_tiled_workspace_bytes(int64_t B, int64_t n_nodes);
 /* The small-matrix front of an ASTGCN block in one launch (astgcn.py:311-328 temporal attention, :427-430 X~ = X E, :245-256 the spatial
  * attention factors): x [B][nodes][T][F] channels-last; TemporalAttention parameters U1 [nodes], U2 [F][nodes], U3 [F], be [T][T],
  * Ve [T][T]; SpatialAttention parameters W1 [T], W2 [F][T], W3 [F]  ->  lhs_s [B][nodes][T] = (X~ W1) W2, rhs_s [B][T][nodes] = (W3 X~)^T

@@ -44,6 +44,8 @@ _SIGNATURES = {
     "stmp_gemm_blocks_f32": (c_int, [c_int64, c_int64, c_int64, c_int64, _P, _P, _P, _P, c_int64, _P, _P, _P, c_int, _P, _P, c_float, _P,
                                      c_int64, _P]),
     "stmp_spatial_attention_fwd": (c_int, [c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, _P, c_int64, _P]),
+    "stmp_spatial_attention_tiled_fwd": (c_int, [c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, c_int64, _P, c_int64, _P]),
+    "stmp_spatial_attention_tiled_workspace_bytes": (c_int64, [c_int64, c_int64]),
     "stmp_astgcn_factors_fwd": (c_int, [c_int64, c_int64, c_int64, c_int64] + [_P] * 13),
     "stmp_gemm_blocks_image_bytes": (c_int64, [c_int64, c_int64]),
     "stmp_gemm_blocks_image": (c_int, [_P, c_int64, c_int64, _P, _P]),

@@ -33,17 +33,32 @@ def pems_bay_like(seed: int = 0, t_total: int = 2048):
     return ei, ew, rng.standard_normal((t_total, 325, 2)).astype(np.float32)
 
 
-def pems04_like(seed: int = 0):
-    """N=307, 340 undirected links (E=680, symmetric, no loops), unweighted."""
+def _undirected_links(n: int, links: int, seed: int):
+    """`links` distinct undirected links between n nodes (uniform, without replacement), both directions, no loops, unweighted;
+    edge list in ROW-MAJOR order."""
     rng = np.random.RandomState(seed)
-    n = 307
     iu = np.stack(np.triu_indices(n, 1), axis=1)
-    pick = iu[rng.choice(len(iu), size=340, replace=False)]
+    pick = iu[rng.choice(len(iu), size=links, replace=False)]
     A = np.zeros((n, n), dtype=np.float32)
     A[pick[:, 0], pick[:, 1]] = 1
     A[pick[:, 1], pick[:, 0]] = 1
     row, col = np.nonzero(A)
     return np.stack([row, col]).astype(np.int64)
+
+
+def pems04_like(seed: int = 0):
+    """N=307, 340 undirected links (E=680, symmetric, no loops), unweighted."""
+    return _undirected_links(307, 340, seed)
+
+
+def pems03_like(seed: int = 0):
+    """N=358, 547 undirected links (E=1094, symmetric, no loops), unweighted: the PeMS03 sensor network's shape."""
+    return _undirected_links(358, 547, seed)
+
+
+def pems07_like(seed: int = 0):
+    """N=883, 866 undirected links (E=1732, symmetric, no loops), unweighted: the PeMS07 sensor network's shape."""
+    return _undirected_links(883, 866, seed)
 
 
 def large_graph(num_nodes=10000, num_edges=100000, seed=0):

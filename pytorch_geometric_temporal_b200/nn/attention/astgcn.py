@@ -11,10 +11,11 @@ What runs where
   (:442-450) is folded into the feature axis (the attention matrix is shared by all T timesteps), so one
   launch per hop covers every timestep; the dense `(I*S)^T @ x` used for a diagonal scale (:160-165) is
   a broadcast multiply;
-* inference on a static graph (N <= 320, T <= 12, 64 time filters, stride 1) keeps the activations channels-last
+* inference on a static graph (N <= 1024, T <= 12, 64 time filters, stride 1) keeps the activations channels-last
   (B, N, T, F) between blocks and runs every large product on wgmma with its neighbours fused (csrc/gemm_blocks.cu):
-  spatial attention `softmax(Vs @ sigmoid(LHS @ RHS + bs))` in ONE kernel (the N x N sigmoid is generated in the operand
-  stage, the softmax is the epilogue; the result is kept transposed and consumed so by `stmp_spmm_att_t`); the Chebyshev
+  spatial attention `softmax(Vs @ sigmoid(LHS @ RHS + bs))` in ONE kernel up to 320 nodes (the N x N sigmoid is generated in
+  the operand stage, the softmax is the epilogue; the result is kept transposed and consumed so by `stmp_spmm_att_t`), and
+  above that in a column-tiled pair whose second launch normalises the rows (csrc/spatial_attention_tiled.cu); the Chebyshev
   contraction + ReLU; time convolution + residual convolution + ReLU + LayerNorm; the final convolution; and the small-matrix
   front (temporal attention, X~ = X E, the (B,N,T) attention factors) in one launch (`stmp_astgcn_factors_fwd`).  No
   im2col, cat or permute of activations in HBM;
@@ -218,7 +219,7 @@ class ASTGCNBlock(nn.Module):
     def _native_ok(self, N, Fi, T):
         tc, rc = self._time_convolution, self._residual_convolution
         K = self._chebconv_attention._weight.size(0)
-        return (N <= 320 and T <= 12 and Fi <= 64 and K <= 12 and tc.out_channels == 64 and tc.in_channels == 64
+        return (N <= 1024 and T <= 12 and Fi <= 64 and K <= 12 and tc.out_channels == 64 and tc.in_channels == 64
                 and tc.stride[1] == 1 and rc.stride[1] == 1 and tc.kernel_size == (1, 3) and tc.padding == (0, 1))
 
     def _native_packs(self):

@@ -765,16 +765,39 @@ def spatial_attention_prepack(Vs: torch.Tensor) -> torch.Tensor:
     return packed, _weight_image(packed, P, P // 64)
 
 
+SPATT_ONE_TILE_MAX = 320     # widest padded node count stmp_spatial_attention_fwd holds in one CTA row tile
+
+
 def spatial_attention(lhs: torch.Tensor, rhs: torch.Tensor, bsT: torch.Tensor, vsT_packed: torch.Tensor) -> torch.Tensor:
-    """ST (B, N, P) with ST[b, j, i] = softmax_dim1(Vs @ sigmoid(lhs @ rhs + bs))[b, i, j]; columns >= N are zero."""
+    """ST (B, N, P) with ST[b, j, i] = softmax_dim1(Vs @ sigmoid(lhs @ rhs + bs))[b, i, j]; columns >= N are zero.
+    P = N rounded up to 64 <= 320: one kernel (stmp_spatial_attention_fwd); up to 1024 nodes: the column-tiled pair (spatial_attention_tiled)."""
+    P = (lhs.size(1) + 63) // 64 * 64
+    if P > SPATT_ONE_TILE_MAX:
+        return spatial_attention_tiled(lhs, rhs, bsT, vsT_packed)
     lhs, rhs, bsT = _f32c(lhs, "lhs"), _f32c(rhs, "rhs"), _f32c(bsT, "bsT")
     B, n, T = lhs.shape
-    P = (n + 63) // 64 * 64
     st = torch.empty((B, n, P), dtype=torch.float32, device=lhs.device)
     packed, image = vsT_packed if isinstance(vsT_packed, tuple) else (vsT_packed, None)
     with torch.cuda.device(lhs.device):
         _lib.check(_lib.lib().stmp_spatial_attention_fwd(B, n, T, _lib.ptr(lhs), _lib.ptr(rhs), _lib.ptr(bsT), _lib.ptr(packed),
                                                          _lib.ptr(image), _lib.ptr(st), P, _lib.stream_ptr()))
+    return st
+
+
+def spatial_attention_tiled(lhs: torch.Tensor, rhs: torch.Tensor, bsT: torch.Tensor, vsT_packed) -> torch.Tensor:
+    """`spatial_attention` on the column-tiled kernel pair (stmp_spatial_attention_tiled_fwd), any 1 <= N <= 1024; the per-row softmax
+    statistics go to a workspace from the caching allocator, so the call is capturable."""
+    lhs, rhs, bsT = _f32c(lhs, "lhs"), _f32c(rhs, "rhs"), _f32c(bsT, "bsT")
+    B, n, T = lhs.shape
+    P = (n + 63) // 64 * 64
+    st = torch.empty((B, n, P), dtype=torch.float32, device=lhs.device)
+    packed = vsT_packed[0] if isinstance(vsT_packed, tuple) else vsT_packed
+    l = _lib.lib()
+    nbytes = max(int(l.stmp_spatial_attention_tiled_workspace_bytes(B, n)), 0)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=lhs.device)
+    with torch.cuda.device(lhs.device):
+        _lib.check(l.stmp_spatial_attention_tiled_fwd(B, n, T, _lib.ptr(lhs), _lib.ptr(rhs), _lib.ptr(bsT), _lib.ptr(packed), _lib.ptr(st), P,
+                                                      _lib.ptr(ws), nbytes, _lib.stream_ptr()))
     return st
 
 

@@ -90,6 +90,10 @@ with torch.enable_grad():
 with torch.no_grad():
     e4 =torch.from_numpy(synthetic.pems04_like(0)).to(dev)
     ASTGCN(2, 1, 3, 64, 64, 1, 12, 12, 307, normalization="sym").to(dev)(torch.randn(2, 307, 1, 12, device=dev), e4)   # k_gemm_blocks x7
+    e7 = torch.from_numpy(synthetic.pems07_like(0)).to(dev)
+    ASTGCN(1, 1, 3, 64, 64, 1, 12, 12, 883, normalization="sym").to(dev)(torch.randn(2, 883, 1, 12, device=dev), e7)   # k_spatt_tiles x4 columns + k_spatt_norm
+    ops.spatial_attention_tiled(torch.randn(1, 70, 5, device=dev), torch.randn(1, 5, 70, device=dev), torch.randn(70, 70, device=dev),
+                                ops.spatial_attention_prepack(torch.randn(70, 70, device=dev)))   # one column tile, partial row tile, T < 12
     eg, wg = synthetic.large_graph(2000, 20000, 0)
     eg, wg = torch.from_numpy(eg).to(dev), torch.from_numpy(wg).to(dev)
     lstm = GConvLSTM(64, 64, 3).to(dev)
