@@ -5,10 +5,11 @@ BatchedDCRNN :328-475).  Same constructor signatures, forward signatures and sta
 
 * inference (no grad): the whole recurrence in ONE fused kernel (`stmp_dcrnn_seq_fwd`);
 * graphs too large for one SM (hidden 32, K = 2, Cin <= 4): BatchedDCRNN runs the row-split kernels (`stmp_dcrnn_rows_*`), two
-  launches per step for all windows, and a hand-written reverse-time backward (`ops._DcrnnRowsFn`);
-* graphs too large for one SM at narrow states (cout, Cin, K <= 4: the reference's BatchedDCRNN(F, F, K=3)): BatchedDCRNN runs the
-  narrow row-split kernels (`stmp_dcrnn_narrow_rows_*`), 2(K-1) launches per step for all windows after one hoisted diffusion of X, and
-  a hand-written reverse-time backward (`ops._DcrnnNarrowRowsFn`);
+  launches per step for all windows, and a hand-written reverse-time backward (`_DcrnnRowsFn`);
+* graphs too large for one SM at narrow states (cout, Cin, K <= 4: the reference's BatchedDCRNN(F, F, K=3)), and hidden 64 at K = 2, 3
+  on any graph: BatchedDCRNN runs the narrow / 64-wide row-split kernels (`stmp_dcrnn_narrow_rows_*`, `stmp_dcrnn_wide_rows_*`),
+  2(K-1) launches per step for all windows after one hoisted diffusion of X, and a hand-written reverse-time backward
+  (`_DcrnnHoistedRowsFn`);
 * training / shapes the fused kernels cannot take: the tiled path = hand-written SpMM (`stmp_spmm`,
   differentiable through its transposed product) + cuBLAS contraction, with the diffusion shared
   between the z and r gates.
@@ -17,6 +18,7 @@ import torch
 
 from ... import ops
 from ... import _lib
+from ...ops import _x_blocks, _x_blocks_adjoint
 from ...plan import PlanCache, _require_cuda
 
 
@@ -44,35 +46,6 @@ def _stack_weight(weight: torch.Tensor) -> torch.Tensor:
     return torch.cat(parts, dim=0)
 
 
-def _basis_raw(plan, U: torch.Tensor, K: int):
-    """no-autograd version of `_basis` (used inside the hand-written backward)."""
-    blocks = [U]
-    To = Ti = None
-    for k in range(1, K):
-        if k == 1:
-            To, Ti = ops.spmm_raw(plan, 0, U), ops.spmm_raw(plan, 1, U)
-        else:
-            To = ops.spmm_raw(plan, 0, To, alpha=2.0, z=U, beta=-1.0)
-            Ti = ops.spmm_raw(plan, 1, Ti, alpha=2.0, z=U, beta=-1.0)
-        blocks += [To, Ti]
-    return blocks
-
-
-def _basis_adjoint(plan, dS: torch.Tensor, C: int, K: int) -> torch.Tensor:
-    """Adjoint of U -> [U | P_o U | P_i U | 2 P_o T_1o - U | ...]: returns dU for dS (..., (2K-1)*C)."""
-    d = [dS[..., j * C:(j + 1) * C].contiguous() for j in range(2 * K - 1)]
-    d0 = d[0]
-    for k in range(K - 1, 1, -1):                      # T_k = 2 P T_{k-1} - U
-        for o in (0, 1):
-            dk = d[1 + 2 * (k - 1) + o]
-            d[1 + 2 * (k - 2) + o] = ops.spmm_raw(plan, o, dk, transposed=True, alpha=2.0, z=d[1 + 2 * (k - 2) + o], beta=1.0)
-            d0 = d0 - dk
-    if K > 1:                                          # T_1 = P U
-        d0 = ops.spmm_raw(plan, 0, d[1], transposed=True, z=d0, beta=1.0)
-        d0 = ops.spmm_raw(plan, 1, d[2], transposed=True, z=d0, beta=1.0)
-    return d0
-
-
 _UNSTACK_INDEX = {}
 _SIDE_STREAMS = {}
 
@@ -97,6 +70,40 @@ def _unstack_weight_grad(dWs: torch.Tensor, K: int, C: int) -> torch.Tensor:
     return dWs.reshape(2 * K - 1, C, O).index_select(0, idx).view(2, K, C, O)
 
 
+def _weight_grads(S1, S2, dph_all, dpzr_all, K, C, Co, has_bias):
+    """(gz, gr, gh, gbz, gbr, gbh): weight / bias gradients over all (t, b, n) rows.  A single (3C x rows) @ (rows x Co) GEMM has only a
+    handful of output tiles (cuBLAS runs it on 2 CTAs); chunking the row axis gives every SM a partial product to reduce."""
+    rows, nbC = S1.size(0) * S1.size(1), S1.size(-1)
+    chunks = 1
+    for c in (128, 96, 64, 48, 32, 16, 8, 4, 2):
+        if rows % c == 0:
+            chunks = c
+            break
+    per = rows // chunks
+    dWh = torch.bmm(S2.view(chunks, per, nbC).transpose(1, 2), dph_all.view(chunks, per, Co)).sum(0)
+    dWzr = torch.bmm(S1.view(chunks, per, nbC).transpose(1, 2), dpzr_all.view(chunks, per, 2 * Co)).sum(0)
+    gz = _unstack_weight_grad(dWzr[:, :Co], K, C)
+    gr = _unstack_weight_grad(dWzr[:, Co:], K, C)
+    gh = _unstack_weight_grad(dWh, K, C)
+    if not has_bias:
+        return gz, gr, gh, None, None, None
+    ones = S1.new_ones(chunks, 1, per)
+    dbzr = torch.bmm(ones, dpzr_all.view(chunks, per, 2 * Co)).sum(dim=(0, 1))
+    dbh = torch.bmm(ones, dph_all.view(chunks, per, Co)).sum(dim=(0, 1))
+    return gz, gr, gh, dbzr[:Co], dbzr[Co:], dbh
+
+
+def _rows_param_grads(ctx, S1, cout, grads):
+    """The six weight / bias gradients of a row-split Function (inputs 1..6): None when no parameter needs one, zeros when there are no
+    windows or no steps (nothing to contract), else `grads()`."""
+    if not any(ctx.needs_input_grad[1:7]):
+        return [None] * 6
+    if S1.numel() == 0:
+        z = torch.zeros(2, ctx.K, ctx.cin + cout, cout, device=S1.device)
+        return [z, z.clone(), z.clone()] + ([torch.zeros(cout, device=S1.device) for _ in range(3)] if ctx.has_bias else [None] * 3)
+    return list(grads())
+
+
 class _DcrnnSeqFn(torch.autograd.Function):
     """Training path of the recurrence: forward = ONE fused launch that also stashes (Z, R, H~) per step; backward =
     hand-written reverse-time loop over the stash (transposed SpMM for the diffusion adjoints, cuBLAS for the
@@ -119,7 +126,7 @@ class _DcrnnSeqFn(torch.autograd.Function):
         every step are built with 4 batched SpMMs straight into their column blocks, and the weight gradients are two
         large GEMMs over all (t, b, n) rows after the loop.  Two persistent kernels replace the loop where they apply: hidden 32 / K = 2
         (`dcrnn_bwd_seq`, with its own bases and weight-gradient kernels) and narrow states, cout <= 4 (`dcrnn_narrow_bwd_seq`, after the
-        same hoisted bases and before the same `_finish`)."""
+        same hoisted bases and before the same `_weight_grads`)."""
         X, H0, wz, wr, wh, out, stash = ctx.saved_tensors
         plan, K = ctx.plan, ctx.K
         B, T, N, Ci = X.shape
@@ -170,13 +177,7 @@ class _DcrnnSeqFn(torch.autograd.Function):
         S1[..., Ci:C] = Hp.view(T * B, N, Co)
         torch.mul(Hp, R.transpose(0, 1), out=S2.view(T, B, N, nb * C)[..., Ci:C])
         for S in (S1, S2):
-            for k in range(1, K):
-                for o in (0, 1):
-                    dst = (1 + 2 * (k - 1) + o) * C
-                    if k == 1:
-                        ops.spmm_cols(plan, o, S, 0, dst, C)
-                    else:
-                        ops.spmm_cols(plan, o, S, dst - 2 * C, dst, C, alpha=2.0, z_col=0, beta=-1.0)
+            _x_blocks(plan, S, C, C, K, ops.spmm_cols)
         dph_all = torch.empty(T, B, N, Co, **f32)
         dpzr_all = torch.empty(T, B, N, 2 * Co, **f32)
         if _DcrnnSeqFn.fused_backward and Co <= 4 and ops.dcrnn_narrow_bwd_supported(plan, Ci, Co, K):
@@ -184,24 +185,13 @@ class _DcrnnSeqFn(torch.autograd.Function):
             dX = torch.empty(X.shape, **f32) if ctx.needs_input_grad[0] else None
             dH0 = torch.empty(B, N, Co, **f32)
             ops.dcrnn_narrow_bwd_seq(plan, Ci, K, gout, out, H0, stash, WhsT, WzrT, dph_all, dpzr_all, dX, dH0)
-            return _DcrnnSeqFn._finish(ctx, S1, S2, dph_all, dpzr_all, dX, dH0, K, C, Co)
+            gH0 = dH0 if (ctx.has_h0 and ctx.needs_input_grad[1]) else None
+            return (dX, gH0, *_weight_grads(S1, S2, dph_all, dpzr_all, K, C, Co, ctx.has_bias), None, None, None)
         # ---- the recurrence ---------------------------------------------------------------------------------------------
         buf2 = torch.empty(B, N, nb * C, **f32)                                            # dL/dS2 -> (in place) dL/d[X | H*R]
         buf1 = torch.empty(B, N, nb * C, **f32)                                            # dL/dS1 -> (in place) dL/d[X | H_{t-1}]
         g = torch.empty(B, N, Co, **f32)
         dX = torch.empty(X.shape, **f32) if ctx.needs_input_grad[0] else None   # dense: the kernels write (B,T,N,Cin) row-major
-
-        def adjoint_inplace(buf):
-            """columns [0,C) of buf <- adjoint of U -> [U | P_o U | P_i U | 2 P_o T_1o - U | ..] applied to buf."""
-            for k in range(K - 1, 1, -1):                                                  # T_k = 2 P T_{k-1} - U
-                for o in (0, 1):
-                    src = (1 + 2 * (k - 1) + o) * C
-                    ops.spmm_cols(plan, o, buf, src, src - 2 * C, C, alpha=2.0, z_col=src - 2 * C, beta=1.0, transposed=True)
-                    buf[..., :C].sub_(buf[..., src:src + C])
-            if K > 1:                                                                      # T_1 = P U
-                ops.spmm_cols(plan, 0, buf, C, 0, C, z_col=0, beta=1.0, transposed=True)
-                ops.spmm_cols(plan, 1, buf, 2 * C, 0, C, z_col=0, beta=1.0, transposed=True)
-
         for t in range(T - 1, -1, -1):
             if t == T - 1:
                 ops.gru_bwd_carry(Ci, Co, buf2, buf1, gout=gout[:, t], z=Z[:, t], ht=Ht[:, t], g=g, dph=dph_all[t])
@@ -209,39 +199,59 @@ class _DcrnnSeqFn(torch.autograd.Function):
                 ops.gru_bwd_carry(Ci, Co, buf2, buf1, g_prev=g, z_prev=Z[:, t + 1], r_prev=R[:, t + 1],
                                   dx=None if dX is None else dX[:, t + 1], gout=gout[:, t], z=Z[:, t], ht=Ht[:, t], g=g, dph=dph_all[t])
             torch.matmul(dph_all[t].view(B * N, Co), WhsT, out=buf2.view(B * N, nb * C))
-            adjoint_inplace(buf2)
+            _x_blocks_adjoint(plan, buf2, C, C, K, ops.spmm_cols)
             ops.gru_bwd_zr(Ci, Co, g, Hp[t], Z[:, t], R[:, t], Ht[:, t], buf2, dpzr_all[t])
             torch.matmul(dpzr_all[t].view(B * N, 2 * Co), WzrT, out=buf1.view(B * N, nb * C))
-            adjoint_inplace(buf1)
+            _x_blocks_adjoint(plan, buf1, C, C, K, ops.spmm_cols)
         dH0 = torch.empty(B, N, Co, **f32)
         ops.gru_bwd_carry(Ci, Co, buf2, buf1, g_prev=g, z_prev=Z[:, 0], r_prev=R[:, 0], dx=None if dX is None else dX[:, 0], dh_out=dH0)
-        return _DcrnnSeqFn._finish(ctx, S1, S2, dph_all, dpzr_all, dX, dH0, K, C, Co)
+        gH0 = dH0 if (ctx.has_h0 and ctx.needs_input_grad[1]) else None
+        return (dX, gH0, *_weight_grads(S1, S2, dph_all, dpzr_all, K, C, Co, ctx.has_bias), None, None, None)
+
+
+class _DcrnnRowsFn(torch.autograd.Function):
+    """Training form of the row-split BatchedDCRNN recurrence at 32 hidden channels (H_0 = 0): forward = `stmp_dcrnn_rows_fwd` with the
+    stash and the weight-gradient bases (the inference launches, so the output is bit-identical to the `no_grad` one); backward =
+    `stmp_dcrnn_rows_bwd` + `stmp_dcrnn_bwd_wgrad`: dX (when X requires grad) and the gradients of the three gates' (2, 2, C, 32) weights
+    and biases.  `packed` = (whsT, wzrT) of dcrnn_pack_bwd_weights for the current weights."""
 
     @staticmethod
-    def _finish(ctx, S1, S2, dph_all, dpzr_all, dX, dH0, K, C, Co):
-        """weight / bias gradients over all (t, b, n) rows.  A single (3C x rows) @ (rows x Co) GEMM has only a handful of
-        output tiles (cuBLAS runs it on 2 CTAs); chunking the row axis gives every SM a partial product to reduce."""
-        rows, nbC = S1.size(0) * S1.size(1), S1.size(-1)
-        chunks = 1
-        for c in (128, 96, 64, 48, 32, 16, 8, 4, 2):
-            if rows % c == 0:
-                chunks = c
-                break
-        per = rows // chunks
-        dWh = torch.bmm(S2.view(chunks, per, nbC).transpose(1, 2), dph_all.view(chunks, per, Co)).sum(0)
-        dWzr = torch.bmm(S1.view(chunks, per, nbC).transpose(1, 2), dpzr_all.view(chunks, per, 2 * Co)).sum(0)
-        gz = _unstack_weight_grad(dWzr[:, :Co], K, C)
-        gr = _unstack_weight_grad(dWzr[:, Co:], K, C)
-        gh = _unstack_weight_grad(dWh, K, C)
-        if ctx.has_bias:
-            ones = S1.new_ones(chunks, 1, per)
-            dbzr = torch.bmm(ones, dpzr_all.view(chunks, per, 2 * Co)).sum(dim=(0, 1))
-            dbh = torch.bmm(ones, dph_all.view(chunks, per, Co)).sum(dim=(0, 1))
-            gb = (dbzr[:Co], dbzr[Co:], dbh)
-        else:
-            gb = (None, None, None)
-        gH0 = dH0 if (ctx.has_h0 and ctx.needs_input_grad[1]) else None
-        return dX, gH0, gz, gr, gh, gb[0], gb[1], gb[2], None, None, None
+    def forward(ctx, X, wz, wr, wh, bz, br, bh, plan, packed):
+        whsT, wzrT = packed
+        out, stash, S1, S2 = ops.dcrnn_rows_fwd(plan, X.detach(), wzrT, whsT, bz, br, bh, train=True)
+        ctx.plan, ctx.K, ctx.cin, ctx.has_bias = plan, 2, X.size(-1), bz is not None
+        ctx.save_for_backward(out, stash, S1, S2, whsT, wzrT)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        out, stash, S1, S2, whsT, wzrT = ctx.saved_tensors
+        dph, dpzr, dX = ops.dcrnn_rows_bwd(ctx.plan, ctx.cin, gout, out, stash, wzrT, whsT, ctx.needs_input_grad[0])
+        g = _rows_param_grads(ctx, S1, 32, lambda: ops.dcrnn_bwd_wgrad(ctx.cin, 2, S1, S2, dpzr, dph, ctx.has_bias))
+        return (dX, *g, None, None)
+
+
+class _DcrnnHoistedRowsFn(torch.autograd.Function):
+    """Training form of the narrow and 64-wide row-split BatchedDCRNN recurrences (H_0 = 0): forward = `ops.dcrnn_hoisted_rows_fwd` with
+    the stash and the weight-gradient bases (the inference launches, so the output is bit-identical to the `no_grad` one); backward =
+    `ops.dcrnn_hoisted_rows_bwd` (with the hoisted dX adjoint when X requires grad) and the weight / bias gradients of `_weight_grads`.
+    `packed` = (whsT, wzrT) of dcrnn_pack_bwd_weights for the current weights."""
+
+    @staticmethod
+    def forward(ctx, X, wz, wr, wh, bz, br, bh, plan, K, packed):
+        whsT, wzrT = packed
+        out, stash, S1, S2 = ops.dcrnn_hoisted_rows_fwd(plan, X.detach(), wzrT, whsT, bz, br, bh, K, train=True)
+        ctx.plan, ctx.K, ctx.cin, ctx.has_bias = plan, K, X.size(-1), bz is not None
+        ctx.save_for_backward(out, stash, S1, S2, whsT, wzrT)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        out, stash, S1, S2, whsT, wzrT = ctx.saved_tensors
+        K, cin, cout = ctx.K, ctx.cin, out.size(-1)
+        dph, dpzr, dX = ops.dcrnn_hoisted_rows_bwd(ctx.plan, cin, K, gout, out, stash, wzrT, whsT, ctx.needs_input_grad[0])
+        g = _rows_param_grads(ctx, S1, cout, lambda: _weight_grads(S1, S2, dph, dpzr, K, cin + cout, cout, ctx.has_bias))
+        return (dX, *g, None, None, None)
 
 
 class DConv(torch.nn.Module):
@@ -380,43 +390,26 @@ class BatchedDCRNN(DCRNN):
         self._rows_pack = ops.PackCache()
 
     def _rows_ok(self, plan, X, training):
-        """The row-split route (stmp_dcrnn_rows_*): out_channels = 32, K = 2, in_channels 1..4, float32 X, a graph the one-SM kernels
-        cannot hold (checked after the module's own attributes, so other shapes never consult the library); training calls also need
-        `_fused_training`."""
-        if self.out_channels != 32 or self.K != 2 or not 1 <= self.in_channels <= 4 or X.dtype != torch.float32:
+        """The row-split routes (`ops.dcrnn_rows_supported`: in_channels 1..4 and out_channels = 32 at K = 2, out_channels and K in 1..4, or
+        out_channels = 64 at K = 2 or 3): float32 X, `_fused_training` for training calls and a graph the one-SM kernels cannot hold.  The
+        envelope is checked on the module's attributes before the library is consulted, so other shapes never consult it."""
+        if X.dtype != torch.float32 or (training and not self._fused_training):
             return False
-        if training and not self._fused_training:
-            return False
-        if ops.dcrnn_seq_supported(plan, self.in_channels, self.out_channels, self.K):
-            return False
-        return ops.dcrnn_rows_supported(plan, self.in_channels, self.out_channels, self.K)
-
-    def _nrows_ok(self, plan, X, training):
-        """The narrow row-split route (stmp_dcrnn_narrow_rows_*): out_channels, in_channels and K in 1..4, float32 X, a graph the one-SM
-        kernels cannot hold (checked after the module's own attributes, so other shapes never consult the library); training calls also
-        need `_fused_training`."""
-        if not (1 <= self.out_channels <= 4 and 1 <= self.in_channels <= 4 and 1 <= self.K <= 4) or X.dtype != torch.float32:
-            return False
-        if training and not self._fused_training:
-            return False
-        if ops.dcrnn_seq_supported(plan, self.in_channels, self.out_channels, self.K):
-            return False
-        return ops.dcrnn_narrow_rows_supported(plan, self.in_channels, self.out_channels, self.K)
-
-    def _wrows_ok(self, plan, X, training):
-        """The 64-wide row-split route (stmp_dcrnn_wide_rows_*): out_channels = 64, K = 2 or 3, in_channels 1..4, float32 X, any graph
-        (checked after the module's own attributes, so other shapes never consult the library); training calls also need
-        `_fused_training`."""
-        if self.out_channels != 64 or self.K not in (2, 3) or not 1 <= self.in_channels <= 4 or X.dtype != torch.float32:
-            return False
-        if training and not self._fused_training:
-            return False
-        return ops.dcrnn_wide_rows_supported(plan, self.in_channels, self.out_channels, self.K)
+        cin, cout, K = self.in_channels, self.out_channels, self.K
+        return ops.dcrnn_rows_supported(plan, cin, cout, K) and not ops.dcrnn_seq_supported(plan, cin, cout, K)
 
     def _rows_packed(self):
         """(whsT, wzrT) of dcrnn_pack_bwd_weights for the row-split kernels, rebuilt only when a parameter changes."""
         return self._rows_pack.get(list(self.parameters()),
                                    lambda: ops.dcrnn_pack_bwd_weights(*self._params()[:3], self.in_channels, self.K))
+
+    def _rows_infer(self, plan, x, **window):
+        """A no_grad call on the row-split kernels: the 32-wide ones read the windows in place (also at `win_start`), the narrow and
+        64-wide ones diffuse X once up front (`ops.dcrnn_hoisted_rows_fwd`, windows at `win_start` gathered into the hoisted X blocks)."""
+        whsT, wzrT = self._rows_packed()
+        if self.out_channels == 32:
+            return ops.dcrnn_rows_fwd(plan, x, wzrT, whsT, *self._params()[3:], **window)
+        return ops.dcrnn_hoisted_rows_fwd(plan, x, wzrT, whsT, *self._params()[3:], self.K, **window)
 
     def forward(self, X, edge_index, edge_weight):
         _require_cuda(X, "X")
@@ -433,21 +426,12 @@ class BatchedDCRNN(DCRNN):
             except _lib.StmpUnsupported:
                 pass
         training = self._needs_grad(X)
-        if self._rows_ok(plan, X, training):    # graphs larger than one SM: the row-split kernels, all windows of a step per launch
-            if training:
-                return ops._DcrnnRowsFn.apply(X, *self._params(), plan, self._rows_packed())
-            whsT, wzrT = self._rows_packed()
-            return ops.dcrnn_rows_fwd(plan, X, wzrT, whsT, *self._params()[3:])
-        if self._nrows_ok(plan, X, training):   # narrow states on graphs larger than one SM: the narrow row-split kernels
-            if training:
-                return ops._DcrnnNarrowRowsFn.apply(X, *self._params(), plan, self.K, self._rows_packed())
-            whsT, wzrT = self._rows_packed()
-            return ops.dcrnn_narrow_rows_fwd(plan, X, wzrT, whsT, *self._params()[3:], self.K)
-        if self._wrows_ok(plan, X, training):   # 64 hidden channels, the DCRNN paper's width: the 64-wide row-split kernels
-            if training:
-                return ops._DcrnnWideRowsFn.apply(X, *self._params(), plan, self.K, self._rows_packed())
-            whsT, wzrT = self._rows_packed()
-            return ops.dcrnn_wide_rows_fwd(plan, X, wzrT, whsT, *self._params()[3:], self.K)
+        if self._rows_ok(plan, X, training):    # graphs larger than one SM, or 64 hidden channels: all windows of a step per launch
+            if not training:
+                return self._rows_infer(plan, X)
+            if self.out_channels == 32:
+                return _DcrnnRowsFn.apply(X, *self._params(), plan, self._rows_packed())
+            return _DcrnnHoistedRowsFn.apply(X, *self._params(), plan, self.K, self._rows_packed())
         H = torch.zeros(B, N, self.out_channels, device=X.device, dtype=X.dtype)
         outs = []
         for t in range(T):
@@ -466,11 +450,7 @@ class BatchedDCRNN(DCRNN):
                                          wimage=self._weight_image())
             except _lib.StmpUnsupported:      # e.g. a horizon whose shared-memory layout the FFMA kernel cannot hold
                 pass
-        if not self._needs_grad(series) and self._rows_ok(plan, series, False):     # windows read in place at win_start
-            whsT, wzrT = self._rows_packed()
-            return ops.dcrnn_rows_fwd(plan, series, wzrT, whsT, *self._params()[3:], win_start=win_start, horizon=horizon)
-        if not self._needs_grad(series) and self._wrows_ok(plan, series, False):    # windows gathered into the hoisted X blocks
-            whsT, wzrT = self._rows_packed()
-            return ops.dcrnn_wide_rows_fwd(plan, series, wzrT, whsT, *self._params()[3:], self.K, win_start=win_start, horizon=horizon)
+        if not self._needs_grad(series) and self._rows_ok(plan, series, False):
+            return self._rows_infer(plan, series, win_start=win_start, horizon=horizon)
         X = ops.window_gather(series, win_start, horizon, with_target=False)
         return self.forward(X, edge_index, edge_weight)

@@ -978,11 +978,34 @@ def dcrnn_pack_bwd_weights(wz, wr, wh, cin: int, K: int):
     return whsT, wzrT
 
 
+def _rows_entry(cin: int, cout: int, K: int) -> Optional[str]:
+    """Prefix of the row-split library entries that serve (cin, cout, K), from the attributes alone; None outside every envelope."""
+    if not 1 <= cin <= 4:
+        return None
+    if cout == 32 and K == 2:
+        return "stmp_dcrnn_rows"
+    if 1 <= cout <= 4 and 1 <= K <= 4:
+        return "stmp_dcrnn_narrow_rows"
+    if cout == 64 and K in (2, 3):
+        return "stmp_dcrnn_wide_rows"
+    return None
+
+
 def dcrnn_rows_supported(plan: GraphPlan, cin: int, cout: int, K: int) -> bool:
-    """The row-split DCRNN envelope (stmp_dcrnn_rows_supported): cout = 32, K = 2, cin 1..4 on a DConv plan, any graph size."""
-    if cout != 32 or K != 2 or not 1 <= cin <= 4:
-        return False
-    return bool(_lib.lib().stmp_dcrnn_rows_supported(plan.handle, cin, cout, K))
+    """The row-split DCRNN envelopes on a DConv plan, any graph size, cin 1..4: cout = 32 at K = 2 (stmp_dcrnn_rows_*), cout and K in
+    1..4 (stmp_dcrnn_narrow_rows_*), cout = 64 at K = 2 or 3 (stmp_dcrnn_wide_rows_*).  The plan is consulted only inside an envelope."""
+    entry = _rows_entry(cin, cout, K)
+    return entry is not None and bool(getattr(_lib.lib(), entry + "_supported")(plan.handle, cin, cout, K))
+
+
+def dcrnn_narrow_rows_supported(plan: GraphPlan, cin: int, cout: int, K: int) -> bool:
+    """dcrnn_rows_supported restricted to the narrow row-split kernels (cout 1..4)."""
+    return 1 <= cout <= 4 and dcrnn_rows_supported(plan, cin, cout, K)
+
+
+def dcrnn_wide_rows_supported(plan: GraphPlan, cin: int, cout: int, K: int) -> bool:
+    """dcrnn_rows_supported restricted to the 64-wide row-split kernels (cout = 64)."""
+    return cout == 64 and dcrnn_rows_supported(plan, cin, cout, K)
 
 
 def dcrnn_rows_fwd(plan: GraphPlan, x: torch.Tensor, wzrT: torch.Tensor, whsT: torch.Tensor, bz, br, bh,
@@ -1042,203 +1065,52 @@ def dcrnn_rows_bwd(plan: GraphPlan, cin: int, gout, out, stash, wzrT, whsT, want
     return dph, dpzr, dx
 
 
-class _DcrnnRowsFn(torch.autograd.Function):
-    """Training form of the row-split BatchedDCRNN recurrence (H_0 = 0): forward = `stmp_dcrnn_rows_fwd` with the stash and the
-    weight-gradient bases (the inference launches, so the output is bit-identical to the `no_grad` one); backward = `stmp_dcrnn_rows_bwd`
-    + `stmp_dcrnn_bwd_wgrad`: dX (when X requires grad) and the gradients of the three gates' (2, 2, C, 32) weights and biases.
-    `packed` = (whsT, wzrT) of dcrnn_pack_bwd_weights for the current weights."""
-
-    @staticmethod
-    def forward(ctx, X, wz, wr, wh, bz, br, bh, plan, packed):
-        whsT, wzrT = packed
-        out, stash, S1, S2 = dcrnn_rows_fwd(plan, X.detach(), wzrT, whsT, bz, br, bh, train=True)
-        ctx.plan, ctx.cin, ctx.has_bias = plan, X.size(-1), bz is not None
-        ctx.save_for_backward(out, stash, S1, S2, whsT, wzrT)
-        return out
-
-    @staticmethod
-    def backward(ctx, gout):
-        out, stash, S1, S2, whsT, wzrT = ctx.saved_tensors
-        dph, dpzr, dX = dcrnn_rows_bwd(ctx.plan, ctx.cin, gout, out, stash, wzrT, whsT, ctx.needs_input_grad[0])
-        g = [None] * 6
-        if any(ctx.needs_input_grad[1:7]) and S1.numel() == 0:              # no windows or no steps: nothing to contract
-            z = torch.zeros(2, 2, ctx.cin + 32, 32, device=gout.device)
-            g = [z, z.clone(), z.clone()] + ([torch.zeros(32, device=gout.device) for _ in range(3)] if ctx.has_bias else [None] * 3)
-        elif any(ctx.needs_input_grad[1:7]):
-            g = list(dcrnn_bwd_wgrad(ctx.cin, 2, S1, S2, dpzr, dph, ctx.has_bias))
-        return (dX, *g, None, None)
-
-
-def dcrnn_narrow_rows_supported(plan: GraphPlan, cin: int, cout: int, K: int) -> bool:
-    """The narrow row-split DCRNN envelope (stmp_dcrnn_narrow_rows_supported): cout, cin and K in 1..4 on a DConv plan, any graph size."""
-    if not (1 <= cout <= 4 and 1 <= cin <= 4 and 1 <= K <= 4):
-        return False
-    return bool(_lib.lib().stmp_dcrnn_narrow_rows_supported(plan.handle, cin, cout, K))
-
-
-def _nrows_cp(cout: int) -> int:
-    """floats per (row, window) of the narrow row-split kernels' node-major blocks: cout padded to 1, 2 or 4"""
-    return 4 if cout == 3 else cout
-
-
-def _nrows_scratch(plan: GraphPlan, B: int, cout: int, K: int, device) -> Optional[torch.Tensor]:
-    nbytes = int(_lib.lib().stmp_dcrnn_narrow_rows_scratch_bytes(plan.handle, B, cout, K))
-    return torch.empty(nbytes // 4, device=device, dtype=torch.float32) if nbytes else None
-
-
-def _x_blocks(plan: GraphPlan, buf: torch.Tensor, cin: int, pitch: int, K: int):
-    """In place in buf (rows, N, LD) holding X in columns [0, cin): the X blocks [X | P_o X | P_i X | 2 P_o T_1o - X | ...], block j at
-    column j * pitch (2(K-1) launches of stmp_spmm over all rows)."""
+def _x_blocks(plan: GraphPlan, buf: torch.Tensor, width: int, pitch: int, K: int, cols=spmm_cols):
+    """In place in buf (rows, N, LD) holding U in columns [0, width): the diffusion blocks [U | P_o U | P_i U | 2 P_o T_1o - U | ...],
+    block j at column j * pitch (2(K-1) launches of stmp_spmm over all rows).  `cols` is the column-block product, `spmm_cols`; the
+    DCRNN backward passes the one of the `ops` it runs against."""
     for k in range(1, K):
         for o in (0, 1):
             dst = (1 + 2 * (k - 1) + o) * pitch
             if k == 1:
-                spmm_cols(plan, o, buf, 0, dst, cin)
+                cols(plan, o, buf, 0, dst, width)
             else:
-                spmm_cols(plan, o, buf, dst - 2 * pitch, dst, cin, alpha=2.0, z_col=0, beta=-1.0)
+                cols(plan, o, buf, dst - 2 * pitch, dst, width, alpha=2.0, z_col=0, beta=-1.0)
 
 
-def _x_blocks_adjoint(plan: GraphPlan, buf: torch.Tensor, cin: int, K: int):
-    """In place: columns [0, cin) of buf (rows, N, (2K-1) cin) <- the transposed adjoint of X -> _x_blocks(X) applied to buf."""
-    for k in range(K - 1, 1, -1):                                                  # T_k = 2 P T_{k-1} - X
+def _x_blocks_adjoint(plan: GraphPlan, buf: torch.Tensor, width: int, pitch: int, K: int, cols=spmm_cols):
+    """In place: columns [0, width) of buf (rows, N, LD) <- the transposed adjoint of U -> _x_blocks(U) applied to the blocks of buf."""
+    for k in range(K - 1, 1, -1):                                                  # T_k = 2 P T_{k-1} - U
         for o in (0, 1):
-            src = (1 + 2 * (k - 1) + o) * cin
-            spmm_cols(plan, o, buf, src, src - 2 * cin, cin, alpha=2.0, z_col=src - 2 * cin, beta=1.0, transposed=True)
-            buf[..., :cin].sub_(buf[..., src:src + cin])
-    if K > 1:                                                                      # T_1 = P X
-        spmm_cols(plan, 0, buf, cin, 0, cin, z_col=0, beta=1.0, transposed=True)
-        spmm_cols(plan, 1, buf, 2 * cin, 0, cin, z_col=0, beta=1.0, transposed=True)
+            src = (1 + 2 * (k - 1) + o) * pitch
+            cols(plan, o, buf, src, src - 2 * pitch, width, alpha=2.0, z_col=src - 2 * pitch, beta=1.0, transposed=True)
+            buf[..., :width].sub_(buf[..., src:src + width])
+    if K > 1:                                                                      # T_1 = P U
+        cols(plan, 0, buf, pitch, 0, width, z_col=0, beta=1.0, transposed=True)
+        cols(plan, 1, buf, 2 * pitch, 0, width, z_col=0, beta=1.0, transposed=True)
+
+
+def _hoisted_entry(cout: int, what: str):
+    """stmp_dcrnn_wide_rows_<what> at 64 hidden channels, stmp_dcrnn_narrow_rows_<what> otherwise (its checks refuse all but cout 1..4);
+    the two families take the same arguments."""
+    return getattr(_lib.lib(), ("stmp_dcrnn_wide_rows_" if cout == 64 else "stmp_dcrnn_narrow_rows_") + what)
+
+
+def _hoisted_scratch(plan: GraphPlan, B: int, cout: int, K: int, device) -> Optional[torch.Tensor]:
+    nbytes = int(_hoisted_entry(cout, "scratch_bytes")(plan.handle, B, cout, K))
+    return torch.empty(nbytes // 4, device=device, dtype=torch.float32) if nbytes else None
 
 
 _NROWS_XBUF_BYTES = 256 << 20      # inference: windows are chunked so that the hoisted X blocks stay under this size
 
 
-def dcrnn_narrow_rows_fwd(plan: GraphPlan, x: torch.Tensor, wzrT: torch.Tensor, whsT: torch.Tensor, bz, br, bh, K: int, train: bool = False):
-    """Narrow-state row-split BatchedDCRNN recurrence from H_0 = 0 (stmp_dcrnn_narrow_rows_fwd).  x: (B,T,N,cin); wzrT / whsT from
-    dcrnn_pack_bwd_weights; biases (cout,) or None.  The X diffusion is hoisted out of the time loop.  Returns out (B,T,N,cout); with
-    `train`, (out, stash (T,N,B,3cp), S1, S2 (T*B, N, (2K-1)C)) -- the operands of dcrnn_narrow_rows_bwd and of the weight gradients."""
-    x = _f32c(x, "X")
-    N = plan.num_nodes
-    if x.dim() != 4 or x.size(2) != N:
-        raise RuntimeError(f"X must be (B,T,{N},Cin), got {tuple(x.shape)}")
-    B, T, _, cin = x.shape
-    cout = whsT.size(0)
-    C = cin + cout
-    nbc = (2 * K - 1) * C
-    if wzrT.shape != (2 * cout, nbc) or whsT.shape != (cout, nbc):
-        raise RuntimeError(f"dcrnn_narrow_rows_fwd: wzrT must be ({2 * cout}, {nbc}) and whsT ({cout}, {nbc})")
-    f32 = dict(device=x.device, dtype=torch.float32)
-    wzrT, whsT = _f32c(wzrT, "wzrT"), _f32c(whsT, "whsT")
-    bs = [None if b is None else _f32c(b.detach(), "bias") for b in (bz, br, bh)]
-    out = torch.empty(B, T, N, cout, **f32)
-    L = _lib.lib()
-
-    def run(Bc, xp, strides, o, st, S1, S2, scr):
-        with torch.cuda.device(x.device):
-            _lib.check(L.stmp_dcrnn_narrow_rows_fwd(plan.handle, Bc, T, cin, cout, K, _lib.ptr(xp), *strides, _lib.ptr(wzrT), _lib.ptr(whsT),
-                                                    _lib.ptr(bs[0]), _lib.ptr(bs[1]), _lib.ptr(bs[2]), _lib.ptr(scr), _lib.ptr(o), _lib.ptr(st),
-                                                    _lib.ptr(S1), _lib.ptr(S2), _lib.stream_ptr()))
-
-    if train:
-        st = torch.empty(T, N, B, 3 * _nrows_cp(cout), **f32)
-        S1 = torch.empty(T * B, N, nbc, **f32)
-        S2 = torch.empty(T * B, N, nbc, **f32)
-        if B > 0 and T > 0:
-            S1.view(T, B, N, nbc)[..., :cin] = x.transpose(0, 1)
-            _x_blocks(plan, S1, cin, C, K)
-            run(B, None, (0, 0, 0, 0), out, st, S1, S2, _nrows_scratch(plan, B, cout, K, x.device))
-        return out, st, S1, S2
-    if B == 0 or T == 0:
-        return out
-    w = (2 * K - 1) * cin
-    Bc = B if K == 1 else max(1, min(B, _NROWS_XBUF_BYTES // (T * N * w * 4)))
-    scr = _nrows_scratch(plan, Bc, cout, K, x.device)
-    buf = None if K == 1 else torch.empty(Bc * T, N, w, **f32)
-    for b0 in range(0, B, Bc):
-        xc = x[b0:b0 + Bc]
-        nb = xc.size(0)
-        if K == 1:                              # the X "blocks" are X itself, read in place
-            run(nb, xc, (T * N * cin, N * cin, cin, cin), out[b0:b0 + nb], None, None, None, scr)
-            continue
-        xb = buf[:nb * T]
-        xb.view(nb, T, N, w)[..., :cin] = xc
-        _x_blocks(plan, xb, cin, cin, K)
-        run(nb, xb, (T * N * w, N * w, w, cin), out[b0:b0 + nb], None, None, None, scr)
-    return out
-
-
-def dcrnn_narrow_rows_bwd(plan: GraphPlan, cin: int, K: int, gout, out, stash, wzrT, whsT, want_dx: bool):
-    """(dph_all (T,B,N,cout), dpzr_all (T,B,N,2cout), dx (B,T,N,cin) or None): the reverse-time backward of dcrnn_narrow_rows_fwd
-    (stmp_dcrnn_narrow_rows_bwd), then dX from the X columns of dS1 + dS2 through one hoisted transposed basis adjoint."""
-    gout = _f32c(gout, "gout")
-    B, T, N, cout = gout.shape
-    f32 = dict(device=gout.device, dtype=torch.float32)
-    dph, dpzr = torch.empty(T, B, N, cout, **f32), torch.empty(T, B, N, 2 * cout, **f32)
-    w = (2 * K - 1) * cin
-    dsx = torch.empty(T * B, N, w, **f32) if want_dx else None
-    if B > 0 and T > 0:
-        scr = _nrows_scratch(plan, B, cout, K, gout.device)
-        with torch.cuda.device(gout.device):
-            _lib.check(_lib.lib().stmp_dcrnn_narrow_rows_bwd(plan.handle, B, T, cin, cout, K, _lib.ptr(gout), _lib.ptr(out), _lib.ptr(stash),
-                                                             _lib.ptr(wzrT), _lib.ptr(whsT), _lib.ptr(scr), _lib.ptr(dph), _lib.ptr(dpzr),
-                                                             _lib.ptr(dsx), w, _lib.stream_ptr()))
-    if not want_dx:
-        return dph, dpzr, None
-    if B == 0 or T == 0:
-        return dph, dpzr, torch.zeros(B, T, N, cin, **f32)
-    _x_blocks_adjoint(plan, dsx, cin, K)
-    return dph, dpzr, dsx.view(T, B, N, w)[..., :cin].transpose(0, 1).contiguous()
-
-
-class _DcrnnNarrowRowsFn(torch.autograd.Function):
-    """Training form of the narrow-state row-split BatchedDCRNN recurrence (H_0 = 0): forward = `stmp_dcrnn_narrow_rows_fwd` with the stash
-    and the weight-gradient bases (the inference launches, so the output is bit-identical to the `no_grad` one); backward =
-    `stmp_dcrnn_narrow_rows_bwd`, the hoisted dX adjoint when X requires grad, and the weight / bias gradients of `_DcrnnSeqFn._finish`.
-    `packed` = (whsT, wzrT) of dcrnn_pack_bwd_weights for the current weights."""
-
-    @staticmethod
-    def forward(ctx, X, wz, wr, wh, bz, br, bh, plan, K, packed):
-        whsT, wzrT = packed
-        out, stash, S1, S2 = dcrnn_narrow_rows_fwd(plan, X.detach(), wzrT, whsT, bz, br, bh, K, train=True)
-        ctx.plan, ctx.K, ctx.cin, ctx.has_bias, ctx.has_h0 = plan, K, X.size(-1), bz is not None, False
-        ctx.save_for_backward(out, stash, S1, S2, whsT, wzrT)
-        return out
-
-    @staticmethod
-    def backward(ctx, gout):
-        from .nn.recurrent.dcrnn import _DcrnnSeqFn
-        out, stash, S1, S2, whsT, wzrT = ctx.saved_tensors
-        K, cin, cout = ctx.K, ctx.cin, out.size(-1)
-        dph, dpzr, dX = dcrnn_narrow_rows_bwd(ctx.plan, cin, K, gout, out, stash, wzrT, whsT, ctx.needs_input_grad[0])
-        g = [None] * 6
-        if any(ctx.needs_input_grad[1:7]) and S1.numel() == 0:              # no windows or no steps: nothing to contract
-            z = torch.zeros(2, K, cin + cout, cout, device=gout.device)
-            g = [z, z.clone(), z.clone()] + ([torch.zeros(cout, device=gout.device) for _ in range(3)] if ctx.has_bias else [None] * 3)
-        elif any(ctx.needs_input_grad[1:7]):
-            g = list(_DcrnnSeqFn._finish(ctx, S1, S2, dph, dpzr, None, None, K, cin + cout, cout)[2:8])
-        return (dX, *g, None, None, None)
-
-
-def dcrnn_wide_rows_supported(plan: GraphPlan, cin: int, cout: int, K: int) -> bool:
-    """The 64-wide row-split DCRNN envelope (stmp_dcrnn_wide_rows_supported): cout = 64, K = 2 or 3, cin 1..4 on a DConv plan, any graph
-    size."""
-    if cout != 64 or K not in (2, 3) or not 1 <= cin <= 4:
-        return False
-    return bool(_lib.lib().stmp_dcrnn_wide_rows_supported(plan.handle, cin, cout, K))
-
-
-def _wrows_scratch(plan: GraphPlan, B: int, K: int, device) -> torch.Tensor:
-    nbytes = int(_lib.lib().stmp_dcrnn_wide_rows_scratch_bytes(plan.handle, B, 64, K))
-    return torch.empty(nbytes // 4, device=device, dtype=torch.float32)
-
-
-def dcrnn_wide_rows_fwd(plan: GraphPlan, x: torch.Tensor, wzrT: torch.Tensor, whsT: torch.Tensor, bz, br, bh, K: int,
-                        win_start: Optional[torch.Tensor] = None, horizon: Optional[int] = None, train: bool = False):
-    """64-wide row-split BatchedDCRNN recurrence from H_0 = 0 (stmp_dcrnn_wide_rows_fwd).  x: (B,T,N,cin) windows, or -- with win_start
-    (int64 [B]) and horizon, inference only -- the resident series (T_total,N,cin), whose windows go straight into the hoisted X blocks.
-    wzrT / whsT from dcrnn_pack_bwd_weights; biases (64,) or None.  The X diffusion is hoisted out of the time loop.  Returns out
-    (B,T,N,64); with `train`, (out, stash (T,B,N,192), S1, S2 (T*B, N, (2K-1)C)) -- the operands of dcrnn_wide_rows_bwd and of the weight
-    gradients."""
+def dcrnn_hoisted_rows_fwd(plan: GraphPlan, x: torch.Tensor, wzrT: torch.Tensor, whsT: torch.Tensor, bz, br, bh, K: int,
+                           win_start: Optional[torch.Tensor] = None, horizon: Optional[int] = None, train: bool = False):
+    """Row-split BatchedDCRNN recurrence from H_0 = 0 with the X diffusion hoisted out of the time loop: stmp_dcrnn_narrow_rows_fwd for
+    cout 1..4, stmp_dcrnn_wide_rows_fwd for cout = 64 (cout = whsT.size(0)).  x: (B,T,N,cin) windows, or -- with win_start (int64 [B]) and
+    horizon, inference only -- the resident series (T_total,N,cin), whose windows are gathered into the hoisted X blocks.  wzrT / whsT from
+    dcrnn_pack_bwd_weights; biases (cout,) or None.  Returns out (B,T,N,cout); with `train`, (out, stash, S1, S2 (T*B, N, (2K-1)C)) -- the
+    operands of dcrnn_hoisted_rows_bwd and of the weight gradients."""
     x = _f32c(x, "X")
     N = plan.num_nodes
     if win_start is None:
@@ -1247,42 +1119,51 @@ def dcrnn_wide_rows_fwd(plan: GraphPlan, x: torch.Tensor, wzrT: torch.Tensor, wh
         B, T, _, cin = x.shape
     else:
         if train:
-            raise RuntimeError("dcrnn_wide_rows_fwd: win_start is an inference entry")
+            raise RuntimeError("dcrnn_hoisted_rows_fwd: win_start is an inference entry")
         if x.dim() != 3 or x.size(1) != N:
             raise RuntimeError(f"series must be (T_total,{N},Cin), got {tuple(x.shape)}")
         _require_cuda(win_start, "win_start")
         win_start = win_start.to(torch.int64).contiguous()
         B, T, cin = win_start.numel(), int(horizon), x.size(2)
-    C = cin + 64
+    cout = whsT.size(0)
+    C = cin + cout
     nbc = (2 * K - 1) * C
-    if wzrT.shape != (128, nbc) or whsT.shape != (64, nbc):
-        raise RuntimeError(f"dcrnn_wide_rows_fwd: wzrT must be (128, {nbc}) and whsT (64, {nbc})")
+    if wzrT.shape != (2 * cout, nbc) or whsT.shape != (cout, nbc):
+        raise RuntimeError(f"dcrnn_hoisted_rows_fwd: wzrT must be ({2 * cout}, {nbc}) and whsT ({cout}, {nbc})")
     f32 = dict(device=x.device, dtype=torch.float32)
     wzrT, whsT = _f32c(wzrT, "wzrT"), _f32c(whsT, "whsT")
     bs = [None if b is None else _f32c(b.detach(), "bias") for b in (bz, br, bh)]
-    out = torch.empty(B, T, N, 64, **f32)
-    L = _lib.lib()
+    out = torch.empty(B, T, N, cout, **f32)
+    fwd = _hoisted_entry(cout, "fwd")
 
     def run(Bc, xp, strides, o, st, S1, S2, scr):
         with torch.cuda.device(x.device):
-            _lib.check(L.stmp_dcrnn_wide_rows_fwd(plan.handle, Bc, T, cin, 64, K, _lib.ptr(xp), *strides, _lib.ptr(wzrT), _lib.ptr(whsT),
-                                                  _lib.ptr(bs[0]), _lib.ptr(bs[1]), _lib.ptr(bs[2]), _lib.ptr(scr), _lib.ptr(o), _lib.ptr(st),
-                                                  _lib.ptr(S1), _lib.ptr(S2), _lib.stream_ptr()))
+            _lib.check(fwd(plan.handle, Bc, T, cin, cout, K, _lib.ptr(xp), *strides, _lib.ptr(wzrT), _lib.ptr(whsT), _lib.ptr(bs[0]),
+                           _lib.ptr(bs[1]), _lib.ptr(bs[2]), _lib.ptr(scr), _lib.ptr(o), _lib.ptr(st), _lib.ptr(S1), _lib.ptr(S2),
+                           _lib.stream_ptr()))
 
     if train:
-        st = torch.empty(T, B, N, 192, **f32)
+        if cout == 64:
+            st = torch.empty(T, B, N, 192, **f32)
+        else:                               # node-major, the windows along the lanes; cout padded to 1, 2 or 4 floats
+            st = torch.empty(T, N, B, 3 * (4 if cout == 3 else cout), **f32)
         S1 = torch.empty(T * B, N, nbc, **f32)
         S2 = torch.empty(T * B, N, nbc, **f32)
         if B > 0 and T > 0:
             S1.view(T, B, N, nbc)[..., :cin] = x.transpose(0, 1)
             _x_blocks(plan, S1, cin, C, K)
-            run(B, None, (0, 0, 0, 0), out, st, S1, S2, _wrows_scratch(plan, B, K, x.device))
+            run(B, None, (0, 0, 0, 0), out, st, S1, S2, _hoisted_scratch(plan, B, cout, K, x.device))
         return out, st, S1, S2
     if B == 0 or T == 0:
         return out
+    if K == 1:                                  # the X "blocks" are X itself, read in place
+        if win_start is not None:
+            x = window_gather(x, win_start, T, with_target=False)
+        run(B, x, (T * N * cin, N * cin, cin, cin), out, None, None, None, _hoisted_scratch(plan, B, cout, K, x.device))
+        return out
     w = (2 * K - 1) * cin
     Bc = max(1, min(B, _NROWS_XBUF_BYTES // (T * N * w * 4)))
-    scr = _wrows_scratch(plan, Bc, K, x.device)
+    scr = _hoisted_scratch(plan, Bc, cout, K, x.device)
     buf = torch.empty(Bc * T, N, w, **f32)
     for b0 in range(0, B, Bc):
         nb = min(Bc, B - b0)
@@ -1296,56 +1177,28 @@ def dcrnn_wide_rows_fwd(plan: GraphPlan, x: torch.Tensor, wzrT: torch.Tensor, wh
     return out
 
 
-def dcrnn_wide_rows_bwd(plan: GraphPlan, cin: int, K: int, gout, out, stash, wzrT, whsT, want_dx: bool):
-    """(dph_all (T,B,N,64), dpzr_all (T,B,N,128), dx (B,T,N,cin) or None): the reverse-time backward of dcrnn_wide_rows_fwd
-    (stmp_dcrnn_wide_rows_bwd), then dX from the X columns of dS1 + dS2 through one hoisted transposed basis adjoint."""
+def dcrnn_hoisted_rows_bwd(plan: GraphPlan, cin: int, K: int, gout, out, stash, wzrT, whsT, want_dx: bool):
+    """(dph_all (T,B,N,cout), dpzr_all (T,B,N,2cout), dx (B,T,N,cin) or None): the reverse-time backward of dcrnn_hoisted_rows_fwd
+    (stmp_dcrnn_narrow_rows_bwd or stmp_dcrnn_wide_rows_bwd), then dX from the X columns of dS1 + dS2 through one hoisted transposed
+    basis adjoint."""
     gout = _f32c(gout, "gout")
-    B, T, N, _ = gout.shape
+    B, T, N, cout = gout.shape
     f32 = dict(device=gout.device, dtype=torch.float32)
-    dph, dpzr = torch.empty(T, B, N, 64, **f32), torch.empty(T, B, N, 128, **f32)
+    dph, dpzr = torch.empty(T, B, N, cout, **f32), torch.empty(T, B, N, 2 * cout, **f32)
     w = (2 * K - 1) * cin
     dsx = torch.empty(T * B, N, w, **f32) if want_dx else None
     if B > 0 and T > 0:
-        scr = _wrows_scratch(plan, B, K, gout.device)
+        scr = _hoisted_scratch(plan, B, cout, K, gout.device)
         with torch.cuda.device(gout.device):
-            _lib.check(_lib.lib().stmp_dcrnn_wide_rows_bwd(plan.handle, B, T, cin, 64, K, _lib.ptr(gout), _lib.ptr(out), _lib.ptr(stash),
-                                                           _lib.ptr(wzrT), _lib.ptr(whsT), _lib.ptr(scr), _lib.ptr(dph), _lib.ptr(dpzr),
-                                                           _lib.ptr(dsx), w, _lib.stream_ptr()))
+            _lib.check(_hoisted_entry(cout, "bwd")(plan.handle, B, T, cin, cout, K, _lib.ptr(gout), _lib.ptr(out), _lib.ptr(stash),
+                                                   _lib.ptr(wzrT), _lib.ptr(whsT), _lib.ptr(scr), _lib.ptr(dph), _lib.ptr(dpzr),
+                                                   _lib.ptr(dsx), w, _lib.stream_ptr()))
     if not want_dx:
         return dph, dpzr, None
     if B == 0 or T == 0:
         return dph, dpzr, torch.zeros(B, T, N, cin, **f32)
-    _x_blocks_adjoint(plan, dsx, cin, K)
+    _x_blocks_adjoint(plan, dsx, cin, cin, K)
     return dph, dpzr, dsx.view(T, B, N, w)[..., :cin].transpose(0, 1).contiguous()
-
-
-class _DcrnnWideRowsFn(torch.autograd.Function):
-    """Training form of the 64-wide row-split BatchedDCRNN recurrence (H_0 = 0): forward = `stmp_dcrnn_wide_rows_fwd` with the stash and
-    the weight-gradient bases (the inference launches, so the output is bit-identical to the `no_grad` one); backward =
-    `stmp_dcrnn_wide_rows_bwd`, the hoisted dX adjoint when X requires grad, and the weight / bias gradients of `_DcrnnSeqFn._finish`.
-    `packed` = (whsT, wzrT) of dcrnn_pack_bwd_weights for the current weights."""
-
-    @staticmethod
-    def forward(ctx, X, wz, wr, wh, bz, br, bh, plan, K, packed):
-        whsT, wzrT = packed
-        out, stash, S1, S2 = dcrnn_wide_rows_fwd(plan, X.detach(), wzrT, whsT, bz, br, bh, K, train=True)
-        ctx.plan, ctx.K, ctx.cin, ctx.has_bias, ctx.has_h0 = plan, K, X.size(-1), bz is not None, False
-        ctx.save_for_backward(out, stash, S1, S2, whsT, wzrT)
-        return out
-
-    @staticmethod
-    def backward(ctx, gout):
-        from .nn.recurrent.dcrnn import _DcrnnSeqFn
-        out, stash, S1, S2, whsT, wzrT = ctx.saved_tensors
-        K, cin = ctx.K, ctx.cin
-        dph, dpzr, dX = dcrnn_wide_rows_bwd(ctx.plan, cin, K, gout, out, stash, wzrT, whsT, ctx.needs_input_grad[0])
-        g = [None] * 6
-        if any(ctx.needs_input_grad[1:7]) and S1.numel() == 0:              # no windows or no steps: nothing to contract
-            z = torch.zeros(2, K, cin + 64, 64, device=gout.device)
-            g = [z, z.clone(), z.clone()] + ([torch.zeros(64, device=gout.device) for _ in range(3)] if ctx.has_bias else [None] * 3)
-        elif any(ctx.needs_input_grad[1:7]):
-            g = list(_DcrnnSeqFn._finish(ctx, S1, S2, dph, dpzr, None, None, K, cin + 64, 64)[2:8])
-        return (dX, *g, None, None, None)
 
 
 class _MaskedMAE(torch.autograd.Function):

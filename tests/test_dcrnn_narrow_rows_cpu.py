@@ -1,5 +1,5 @@
-"""Host side of BatchedDCRNN on the narrow row-split kernels (stmp_dcrnn_narrow_rows_*): the routing of a call (`BatchedDCRNN._nrows_ok`),
-the weight pack, the autograd Function `ops._DcrnnNarrowRowsFn` and the hand-off of its operands to `_DcrnnSeqFn._finish`, with every
+"""Host side of BatchedDCRNN on the narrow row-split kernels (stmp_dcrnn_narrow_rows_*): the routing of a call (`BatchedDCRNN._rows_ok`),
+the weight pack, the autograd Function `_DcrnnHoistedRowsFn` and the hand-off of its operands to `_weight_grads`, with every
 library call replaced by a dense torch restatement of its contract on the dense DConv operators -- the output, gX and EVERY parameter
 gradient against the unmodified reference (tests/golden/make_goldens_dcrnn_narrow_rows.py: BatchedDCRNN(2, 2, 3) on 2 000 nodes)."""
 import gzip
@@ -12,6 +12,7 @@ import torch
 from pytorch_geometric_temporal_b200 import ops
 from pytorch_geometric_temporal_b200.nn.recurrent import BatchedDCRNN
 from pytorch_geometric_temporal_b200.nn.recurrent import dcrnn as dcrnn_mod
+from test_dcrnn_rows_cpu import fake_rows_library
 from test_modules_host_logic_cpu import dense_dconv_gcn_ops  # noqa: F401  (dense DConv operators + SpMM, one-SM kernels off)
 
 
@@ -89,11 +90,12 @@ def make_fake_bwd(state):
     return fake_bwd
 
 
-@pytest.fixture()
-def dense_nrows(dense_dconv_gcn_ops, monkeypatch):   # noqa: F811
+def fake_hoisted_rows(monkeypatch, served):
+    """ops.dcrnn_hoisted_rows_fwd / _bwd replaced by the dense fakes, the library by `fake_rows_library(served)`; returns the call log"""
     calls, state = [], {}
 
-    def fwd(plan, x, wzrT, whsT, bz, br, bh, K, train=False):
+    def fwd(plan, x, wzrT, whsT, bz, br, bh, K, win_start=None, horizon=None, train=False):
+        assert win_start is None
         calls.append("fwd")
         state["x"], state["b"] = x, (bz, br, bh)
         return fake_fwd(plan, x, wzrT, whsT, bz, br, bh, K, train)
@@ -101,12 +103,16 @@ def dense_nrows(dense_dconv_gcn_ops, monkeypatch):   # noqa: F811
     def bwd(*a, **k):
         calls.append("bwd")
         return make_fake_bwd(state)(*a, **k)
-    monkeypatch.setattr(ops, "dcrnn_narrow_rows_supported", lambda plan, cin, cout, K: 1 <= cin <= 4 and 1 <= cout <= 4 and 1 <= K <= 4)
-    monkeypatch.setattr(ops, "dcrnn_rows_supported", lambda *a, **k: pytest.fail("32-wide row-split entry consulted"))
+    fake_rows_library(monkeypatch, served)
     monkeypatch.setattr(ops, "dcrnn_pack_bwd_weights", fake_pack)
-    monkeypatch.setattr(ops, "dcrnn_narrow_rows_fwd", fwd)
-    monkeypatch.setattr(ops, "dcrnn_narrow_rows_bwd", bwd)
+    monkeypatch.setattr(ops, "dcrnn_hoisted_rows_fwd", fwd)
+    monkeypatch.setattr(ops, "dcrnn_hoisted_rows_bwd", bwd)
     return calls
+
+
+@pytest.fixture()
+def dense_nrows(dense_dconv_gcn_ops, monkeypatch):   # noqa: F811
+    return fake_hoisted_rows(monkeypatch, "stmp_dcrnn_narrow_rows_supported")
 
 
 def _close(got, want, rtol=1e-4, atol=1e-5):
@@ -118,7 +124,7 @@ def _grad_close(got, ref):
     _close(got, ref, 1e-3, 1e-3 * max(ref.abs().max().item(), 1e-12))
 
 
-def test_training_and_inference_route_to_the_narrow_rows_path_and_match_the_golden(golden_dir, dense_nrows):
+def test_narrow_states_route_to_the_hoisted_rows_path_and_match_the_golden(golden_dir, dense_nrows):
     g = _load(golden_dir)
     m = BatchedDCRNN(2, 2, 3)
     m.load_state_dict(g["state"])
@@ -137,7 +143,7 @@ def test_training_and_inference_route_to_the_narrow_rows_path_and_match_the_gold
         _grad_close(p.grad, g["grads"][k])
 
 
-def test_fused_training_off_and_shapes_outside_the_envelope_keep_the_tiled_path(golden_dir, dense_nrows):
+def test_narrow_fused_training_off_and_shapes_outside_the_envelope_keep_the_tiled_path(golden_dir, dense_nrows):
     g = _load(golden_dir)
     m = BatchedDCRNN(2, 2, 3)
     m.load_state_dict(g["state"])

@@ -1,5 +1,5 @@
-"""Host side of BatchedDCRNN on the row-split kernels (stmp_dcrnn_rows_*): the routing of a call (`BatchedDCRNN._rows_ok`), the weight pack
-(`BatchedDCRNN._rows_packed`), the autograd Function `ops._DcrnnRowsFn` and the hand-off of the weight-gradient contraction to the
+"""Host side of BatchedDCRNN on the row-split kernels (stmp_dcrnn_rows_*): the routing of a call (`BatchedDCRNN._rows_ok` and the envelope
+of `ops.dcrnn_rows_supported`), the weight pack (`BatchedDCRNN._rows_packed`), the autograd Function `_DcrnnRowsFn` and the hand-off of the weight-gradient contraction to the
 parameters, with every library call replaced by a dense torch restatement of its contract on the dense DConv operators -- the output, gX
 and EVERY parameter gradient against the unmodified reference on the PEMS-BAY shape (tests/golden/make_goldens_dcrnn_rows.py; the output at steps 0, 1 and 11)."""
 import gzip
@@ -8,10 +8,25 @@ import os
 import pytest
 import torch
 
-from pytorch_geometric_temporal_b200 import ops
+from pytorch_geometric_temporal_b200 import _lib, ops
 from pytorch_geometric_temporal_b200.nn.recurrent import DCRNN, BatchedDCRNN
 from pytorch_geometric_temporal_b200.nn.recurrent import dcrnn as dcrnn_mod
-from test_modules_host_logic_cpu import dense_dconv_gcn_ops  # noqa: F401  (dense DConv operators + SpMM, one-SM kernels off)
+from test_modules_host_logic_cpu import _DensePair, dense_dconv_gcn_ops  # noqa: F401  (dense DConv operators + SpMM, one-SM kernels off)
+
+
+def fake_rows_library(monkeypatch, served):
+    """The library as the row-split routing sees it: the entry `served` (e.g. "stmp_dcrnn_rows_supported") admits every plan, and any other
+    library call -- the other widths' entries included -- fails the test."""
+    class Lib(object):
+        def __getattr__(self, name):
+            if name == served:
+                return lambda handle, cin, cout, K: 1
+
+            def refuse(*a):
+                pytest.fail(f"{name} consulted")
+            return refuse
+    monkeypatch.setattr(_lib, "lib", Lib)
+    monkeypatch.setattr(_DensePair, "handle", None, raising=False)
 
 
 def _load(golden_dir):
@@ -104,7 +119,7 @@ def dense_rows(dense_dconv_gcn_ops, monkeypatch):   # noqa: F811
             calls.append(name)
             return fn(*a, **k)
         return f
-    monkeypatch.setattr(ops, "dcrnn_rows_supported", lambda plan, cin, cout, K: cout == 32 and K == 2 and 1 <= cin <= 4)
+    fake_rows_library(monkeypatch, "stmp_dcrnn_rows_supported")
     monkeypatch.setattr(ops, "dcrnn_pack_bwd_weights", counted("pack", fake_pack))
     monkeypatch.setattr(ops, "dcrnn_rows_fwd", counted("fwd", fake_fwd))
     monkeypatch.setattr(ops, "dcrnn_rows_bwd", counted("bwd", fake_bwd))
@@ -209,5 +224,7 @@ def test_routing_outside_the_envelope(dense_rows):
 
 
 def test_envelope_is_checked_before_the_plan():
-    for cin, cout, K in ((0, 32, 2), (5, 32, 2), (2, 16, 2), (2, 32, 1), (2, 32, 3)):
+    """outside all three row-split envelopes the plan (None here) is never consulted"""
+    for cin, cout, K in ((0, 32, 2), (5, 32, 2), (2, 16, 2), (2, 32, 1), (2, 32, 3), (2, 5, 3), (5, 2, 3), (2, 2, 5), (2, 0, 2),
+                         (2, 2, 0), (2, 64, 1), (2, 64, 4), (5, 64, 2), (2, 16, 3)):
         assert ops.dcrnn_rows_supported(None, cin, cout, K) is False

@@ -1,18 +1,18 @@
-"""Host side of BatchedDCRNN on the 64-wide row-split kernels (stmp_dcrnn_wide_rows_*): the routing of a call (`BatchedDCRNN._wrows_ok`,
-which checks the module's attributes before it consults the library), the autograd Function `ops._DcrnnWideRowsFn` and the hand-off of its
-operands to `_DcrnnSeqFn._finish`, with every library call replaced by a dense torch restatement of its contract on the dense DConv
+"""Host side of BatchedDCRNN on the 64-wide row-split kernels (stmp_dcrnn_wide_rows_*): the routing of a call (`BatchedDCRNN._rows_ok`,
+which checks the module's attributes before it consults the library), the autograd Function `_DcrnnHoistedRowsFn` and the hand-off of its
+operands to `_weight_grads`, with every library call replaced by a dense torch restatement of its contract on the dense DConv
 operators -- the output, gX and EVERY parameter gradient against the tiled path on the golden's models and graphs
 (tests/golden/make_goldens_dcrnn_wide_rows.py: BatchedDCRNN(2, 64, 3) on the METR-LA shape and (2, 64, 2) on the PEMS-BAY shape)."""
 import gzip
 import importlib.util
 import os
+import types
 
 import pytest
 import torch
 
-from pytorch_geometric_temporal_b200 import ops
 from pytorch_geometric_temporal_b200.nn.recurrent import BatchedDCRNN
-from test_dcrnn_narrow_rows_cpu import fake_fwd, fake_pack, make_fake_bwd
+from test_dcrnn_narrow_rows_cpu import fake_hoisted_rows
 from test_modules_host_logic_cpu import dense_dconv_gcn_ops  # noqa: F401  (dense DConv operators + SpMM, one-SM kernels off)
 
 
@@ -30,24 +30,7 @@ def _load(golden_dir, name):
 
 @pytest.fixture()
 def dense_wrows(dense_dconv_gcn_ops, monkeypatch):   # noqa: F811
-    calls, state = [], {}
-
-    def fwd(plan, x, wzrT, whsT, bz, br, bh, K, win_start=None, horizon=None, train=False):
-        assert win_start is None
-        calls.append("fwd")
-        state["x"], state["b"] = x, (bz, br, bh)
-        return fake_fwd(plan, x, wzrT, whsT, bz, br, bh, K, train)
-
-    def bwd(*a, **k):
-        calls.append("bwd")
-        return make_fake_bwd(state)(*a, **k)
-    monkeypatch.setattr(ops, "dcrnn_wide_rows_supported", lambda plan, cin, cout, K: 1 <= cin <= 4 and cout == 64 and K in (2, 3))
-    monkeypatch.setattr(ops, "dcrnn_rows_supported", lambda *a, **k: pytest.fail("32-wide row-split entry consulted"))
-    monkeypatch.setattr(ops, "dcrnn_narrow_rows_supported", lambda *a, **k: pytest.fail("narrow row-split entry consulted"))
-    monkeypatch.setattr(ops, "dcrnn_pack_bwd_weights", fake_pack)
-    monkeypatch.setattr(ops, "dcrnn_wide_rows_fwd", fwd)
-    monkeypatch.setattr(ops, "dcrnn_wide_rows_bwd", bwd)
-    return calls
+    return fake_hoisted_rows(monkeypatch, "stmp_dcrnn_wide_rows_supported")
 
 
 def _close(got, want, rtol=1e-4, atol=1e-5):
@@ -60,9 +43,9 @@ def _grad_close(got, ref):
 
 
 @pytest.mark.parametrize("name", ["metr_la", "pems_bay"])
-def test_training_and_inference_route_to_the_wide_rows_path_and_match_the_tiled_path(golden_dir, dense_wrows, name):
+def test_64_channels_route_to_the_hoisted_rows_path_and_match_the_tiled_path(golden_dir, dense_wrows, name):
     """The fused route (fakes) against the tiled path on the same dense operators: the output, gX and every parameter gradient, so the
-    Function's hand-off to `_DcrnnSeqFn._finish` (layouts of S1 / S2 / dph / dpzr, the gradient order) is checked on the golden's shapes."""
+    Function's hand-off to `_weight_grads` (layouts of S1 / S2 / dph / dpzr, the gradient order) is checked on the golden's shapes."""
     g, m = _load(golden_dir, name)
     ei, ew, X0 = g["edge_index"], g["edge_weight"], g["X"][:, :3]
     with torch.no_grad():
@@ -83,7 +66,7 @@ def test_training_and_inference_route_to_the_wide_rows_path_and_match_the_tiled_
         _grad_close(a, b)
 
 
-def test_no_bias_and_no_x_grad_bookkeeping(golden_dir, dense_wrows):
+def test_hoisted_rows_no_bias_and_no_x_grad_bookkeeping(golden_dir, dense_wrows):
     """Without biases the Function returns no bias gradients; without an X gradient it asks the backward for no dX."""
     g, _ = _load(golden_dir, "metr_la")
     m = BatchedDCRNN(2, 64, 3, bias=False)
@@ -93,21 +76,24 @@ def test_no_bias_and_no_x_grad_bookkeeping(golden_dir, dense_wrows):
     assert all(p.grad is not None and p.grad.shape == p.shape for p in m.parameters())
 
 
-def test_envelope_is_checked_before_the_plan(dense_wrows):
-    """Shapes outside the envelope are refused from the module's attributes alone: the plan is never consulted."""
+def test_rows_ok_checks_the_envelope_before_the_plan(dense_wrows):
+    """Shapes outside every row-split envelope are refused from the module's attributes alone: the plan is never consulted.  (2, 32, 2)
+    is inside the 32-wide envelope; that it never reaches the 64-wide entry is checked by the fixture's library."""
     class NoPlan:
         def __getattr__(self, k):
             raise AssertionError("plan consulted")
     X = torch.zeros(1, 1, 3, 2)
-    for cin, cout, K in ((2, 32, 2), (2, 64, 1), (2, 64, 4), (5, 64, 2), (2, 16, 3)):
-        assert not BatchedDCRNN(cin, cout, K)._wrows_ok(NoPlan(), X, False)
-    assert not BatchedDCRNN(2, 64, 3)._wrows_ok(NoPlan(), X.double(), False)
+    for cin, cout, K in ((2, 64, 1), (2, 64, 4), (5, 64, 2), (2, 16, 3)):
+        assert not BatchedDCRNN(cin, cout, K)._rows_ok(NoPlan(), X, False)
+    assert not BatchedDCRNN(2, 64, 3)._rows_ok(NoPlan(), X.double(), False)
     m = BatchedDCRNN(2, 64, 3)
     m._fused_training = False
-    assert not m._wrows_ok(NoPlan(), X, True)
+    assert not m._rows_ok(NoPlan(), X, True)
+    with pytest.raises(pytest.fail.Exception, match="stmp_dcrnn_rows_supported consulted"):
+        BatchedDCRNN(2, 32, 2)._rows_ok(types.SimpleNamespace(handle=None), X, False)
 
 
-def test_fused_training_off_and_shapes_outside_the_envelope_keep_the_tiled_path(golden_dir, dense_wrows):
+def test_wide_fused_training_off_and_shapes_outside_the_envelope_keep_the_tiled_path(golden_dir, dense_wrows):
     g, m = _load(golden_dir, "metr_la")
     X = g["X"][:, :2]
     m._fused_training = False

@@ -307,6 +307,21 @@ def test_forward_indexed_equals_materialised_windows_and_empty_calls():
         m.zero_grad(set_to_none=True)
 
 
+def test_forward_indexed_at_k1_reads_the_gathered_windows_in_place():
+    """K = 1 has no X diffusion to hoist: the windows are gathered once and the kernel reads them in place."""
+    n = 2000
+    ei, ew = _banded(n, 3)
+    s = torch.randn(300, n, 2, device=DEV)
+    m = _model(2, 2, 1, 1)
+    starts = torch.randint(0, 300 - 12, (64,), generator=torch.Generator().manual_seed(0)).to(DEV)
+    X = torch.stack([s[i:i + 12] for i in starts.tolist()])
+    with torch.no_grad():
+        with _counted() as c:
+            a = m.forward_indexed(s, starts, 12, ei, ew)
+        assert c["k_window_gather"] == 1 and c["k_dcrnn_nrows_seq1"] == 1 and _nrows(c) == 1 and "k_spmm" not in c
+        assert torch.equal(a, m(X, ei, ew))
+
+
 # ---- the reference's full-PeMS size ---------------------------------------------------------------------------------------------------
 def test_pems_like_size_training_step_vs_tiled():
     n, B, T = 11160, 64, 12
