@@ -2,9 +2,14 @@
 the kernels against float64.
 
 Every kernel that keeps a whole graph on one SM reads it from a compact format the plan builds:
-  * the shared-memory graph image (csrc/graph_image.cuh) of the wgmma forward `k_dcrnn_seq_tc` -- 8-bit rows, pad entries that point
-    at zero row 207, edges in groups of four with a 7-bit group count per task, tasks cut into segments by 128-row tile and operator
-    and dealt to 16 warps longest-first.  It exists only if it fits the kernel's shared memory;
+  * the wgmma forward reads two images.  The CTA-pair kernel `k_dcrnn_seq_tc` (small batches, the `[cluster2]` counter) reads the
+    shared-memory graph image (csrc/graph_image.cuh) -- 8-bit rows, pad entries that point at zero row 207, edges in groups of four
+    with a 7-bit group count per task, tasks cut into segments by 128-row tile and operator and dealt to 16 warps longest-first.
+    Windows not served by a CTA pair (the B = 200 cases here) run the one-CTA kernel `k_dcrnn_seq_rf`, which gathers straight into
+    wgmma register fragments from the row image (csrc/row_image.cuh).  Each image exists only if it fits its kernel's shared memory,
+    and the wgmma path takes a plan only when it has both (`tc_fits`).  This file decodes the graph image only; the
+    `ops.gru_seq_supported(...) == image_fits(...)` assertions below therefore hold because on these graphs the row image is never
+    the tighter limit, and the B = 200 cases check the row-image kernel numerically;
   * the persistent backward (csrc/dcrnn_bwd.cu) reads the transposed operators from a compressed shared-memory copy when it fits
     beside the per-window buffers (`graph_in_smem`), otherwise from the global CSR (path counter `k_*_bwd_seq[graph-global]`);
   * the FFMA forward `k_dcrnn_seq` picks one of five row mappings by N.

@@ -127,5 +127,25 @@ with torch.no_grad():
     r225 = torch.arange(225, device=dev)
     BatchedDCRNN(2, 32, 1).to(dev)(torch.randn(2, 12, 225, 2, device=dev), torch.stack([r225, (r225 + 1) % 225]),
                                    torch.ones(225, device=dev))  # k_dcrnn_seq, RT 7
+# the row-split kernels below the modules' routing (tests/test_gpu_rows_envelope.py): 17 nodes, 3 windows -- 16-row tiles and 8-row
+# warps that straddle windows, a partial last tile and warp, a partial lane group
+from pytorch_geometric_temporal_b200.nn.recurrent.dcrnn import _DcrnnHoistedRowsFn, _DcrnnRowsFn   # noqa: E402
+r17 = torch.arange(17, device=dev)
+e17 = torch.cat([torch.stack([r17, (r17 + 1) % 17]), torch.stack([r17, (r17 + 5) % 17])], dim=1)
+for cin, cout, K in ((3, 32, 2), (3, 64, 3), (2, 3, 3)):
+    d17 = BatchedDCRNN(cin, cout, K).to(dev)
+    p17 = d17._plan(e17, torch.ones(34, device=dev), 17)
+    x17 = torch.randn(3, 3, 17, cin, device=dev, requires_grad=True)
+    if cout == 32:
+        _DcrnnRowsFn.apply(x17, *d17._params(), p17, d17._rows_packed()).square().mean().backward()
+    else:
+        _DcrnnHoistedRowsFn.apply(x17, *d17._params(), p17, K, d17._rows_packed()).square().mean().backward()
+    with torch.no_grad():
+        d17._rows_infer(p17, x17.detach())
+g17 = GConvGRU(5, 32, 2).to(dev)
+xg, hg = torch.randn(17, 5, device=dev, requires_grad=True), torch.randn(17, 32, device=dev, requires_grad=True)
+ops.gru_rows_train(g17._cheb_plan(e17, None, 17, "sym", None), 1, xg, hg, *g17._rows_packed(), *g17._param_spec(rows=True)).square().mean().backward()
+for cls in (GConvLSTM, GCLSTM):
+    sum(t.square().mean() for t in cls(5, 32, 2).to(dev)(xg, e17, None, hg, torch.randn(17, 32, device=dev, requires_grad=True))).backward()
 torch.cuda.synchronize()
 print("sanitize_smoke ok:", {k: v for k, v in _lib.path_counters().items() if k.startswith("k_") and v})
