@@ -555,7 +555,8 @@ int stmp_gemm_lstm_f32(const float* A, int64_t lda, int64_t M, int64_t K, int64_
  *   lhs [B][nodes][T] = (X~ W1) W2, rhs [B][T][nodes] = (W3 X~)^T, bsT [nodes][nodes] = bs^T, vsT_packed = stmp_gemm_prepack of Vs^T
  *   zero-padded to [P][P], P = nodes rounded up to 64 (<= 320).  The N x N sigmoid is generated inside the GEMM's operand stage and the
  *   softmax is the GEMM epilogue: neither ever reaches HBM.
- *   nodes <= 320, T <= 12.
+ *   nodes <= 320, T <= 12.  At T == 12 lhs must be 16-byte aligned (its rows are read as float4): EINVAL otherwise.  NULL pointers are
+ *   EINVAL when B > 0; B == 0 launches nothing.
  * Optional weight IMAGE (both entries; NULL = the kernel swizzles the packed weights itself): stmp_gemm_blocks_image rewrites a packed weight
  * into the per-k-block shared-memory image (hi | lo tile, SWIZZLE_128B) of stmp_gemm_blocks_image_bytes(N, nblk) bytes, which every CTA then
  * fetches with ONE TMA bulk copy per k-block while it loads / generates its A tile. */
@@ -580,7 +581,9 @@ int64_t stmp_spatial_attention_tiled_workspace_bytes(int64_t B, int64_t n_nodes)
 /* The small-matrix front of an ASTGCN block in one launch (astgcn.py:311-328 temporal attention, :427-430 X~ = X E, :245-256 the spatial
  * attention factors): x [B][nodes][T][F] channels-last; TemporalAttention parameters U1 [nodes], U2 [F][nodes], U3 [F], be [T][T],
  * Ve [T][T]; SpatialAttention parameters W1 [T], W2 [F][T], W3 [F]  ->  lhs_s [B][nodes][T] = (X~ W1) W2, rhs_s [B][T][nodes] = (W3 X~)^T
- * (the inputs of stmp_spatial_attention_fwd) and optionally E [B][T][T].  X~ is never materialised.  T <= 12, F in {1,2,4,...,64}. */
+ * (the inputs of stmp_spatial_attention_fwd) and optionally E [B][T][T].  X~ is never materialised.  T <= 12, F in {1,2,4,...,64}
+ * (F >= 32 needs x 16-byte aligned), B <= 65535 and 4 (3 nodes T + T F + 2 T^2 + T + 16) <= 200 KB: EUNSUPPORTED otherwise.  B == 0
+ * launches nothing. */
 int stmp_astgcn_factors_fwd(int64_t B, int64_t n_nodes, int64_t n_steps, int64_t f_in, const float* x, const float* U1, const float* U2,
                             const float* U3, const float* be, const float* Ve, const float* W1, const float* W2, const float* W3,
                             float* lhs_s, float* rhs_s, float* E_out, void* stream);

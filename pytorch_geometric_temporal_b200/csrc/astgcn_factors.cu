@@ -252,7 +252,6 @@ using namespace stmp;
 extern "C" int stmp_astgcn_factors_fwd(int64_t B, int64_t n_nodes, int64_t n_steps, int64_t f_in, const float* x, const float* U1,
                                        const float* U2, const float* U3, const float* be, const float* Ve, const float* W1, const float* W2,
                                        const float* W3, float* lhs_s, float* rhs_s, float* E_out, void* stream) {
-  STMP_REQUIRE(x && U1 && U2 && U3 && be && Ve && W1 && W2 && W3 && lhs_s && rhs_s, STMP_EINVAL, "stmp_astgcn_factors_fwd: NULL pointer");
   STMP_REQUIRE(B >= 0 && n_nodes >= 1 && n_steps >= 1 && f_in >= 1, STMP_EINVAL, "stmp_astgcn_factors_fwd: bad sizes");
   const bool vec4 = f_in % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
   const int lpr = (int)(vec4 ? f_in / 4 : f_in);
@@ -261,6 +260,7 @@ extern "C" int stmp_astgcn_factors_fwd(int64_t B, int64_t n_nodes, int64_t n_ste
     return set_error(STMP_EUNSUPPORTED, "fused ASTGCN factors: T <= 12, F in {1,2,4,8,16,32,64} (got T=%lld F=%lld N=%lld)", (long long)n_steps,
                      (long long)f_in, (long long)n_nodes);
   if (B == 0) return STMP_OK;
+  STMP_REQUIRE(x && U1 && U2 && U3 && be && Ve && W1 && W2 && W3 && lhs_s && rhs_s, STMP_EINVAL, "stmp_astgcn_factors_fwd: NULL pointer");
   FactorArgs a;
   a.N = (int)n_nodes; a.T = (int)n_steps; a.F = (int)f_in; a.x = x; a.U1 = U1; a.U2 = U2; a.U3 = U3; a.be = be; a.Ve = Ve;
   a.W1 = W1; a.W2 = W2; a.W3 = W3; a.lhs_s = lhs_s; a.rhs_s = rhs_s; a.E_out = E_out;

@@ -445,7 +445,7 @@ using namespace stmp;
 extern "C" int stmp_gemm_blocks_f32(int64_t M, int64_t N, int64_t ncols, int64_t nblk, const float* const* blk_ptr, const int64_t* blk_ld,
                                     const int32_t* blk_width, const int32_t* blk_shift, int64_t seq, const void* packed, const void* image,
                                     const float* bias, int epilogue, const float* gamma, const float* beta, float eps, float* C, int64_t ldc, void* stream) {
-  STMP_REQUIRE(blk_ptr && blk_ld && blk_width && blk_shift && packed && C, STMP_EINVAL, "stmp_gemm_blocks_f32: NULL pointer");
+  STMP_REQUIRE(blk_ptr && blk_ld && blk_width && blk_shift && packed, STMP_EINVAL, "stmp_gemm_blocks_f32: NULL pointer");
   STMP_REQUIRE(M >= 0 && nblk >= 1 && seq >= 1, STMP_EINVAL, "stmp_gemm_blocks_f32: bad sizes");
   if (nblk > GB_MAXBLK || N > 320 || N % 16 != 0 || N < 16 || ncols > N || ncols < 1 || M >= (1ll << 31) - 128)
     return set_error(STMP_EUNSUPPORTED, "blocked GEMM takes <= %d k-blocks, N <= 320, N %% 16 == 0 (nblk=%lld N=%lld)", GB_MAXBLK,
@@ -454,6 +454,7 @@ extern "C" int stmp_gemm_blocks_f32(int64_t M, int64_t N, int64_t ncols, int64_t
     return set_error(STMP_EUNSUPPORTED, "blocked GEMM: the LayerNorm epilogue needs N == 64, gamma/beta and 16-byte aligned rows");
   if (epilogue == EPI_SOFTMAX) return set_error(STMP_EINVAL, "blocked GEMM: the softmax epilogue belongs to stmp_spatial_attention_fwd");
   if (M == 0) return STMP_OK;
+  STMP_REQUIRE(C != nullptr, STMP_EINVAL, "stmp_gemm_blocks_f32: NULL pointer");
   GbParams p = {};
   for (int i = 0; i < nblk; ++i) {
     STMP_REQUIRE(blk_ptr[i] != nullptr && blk_width[i] >= 1 && blk_width[i] <= 64, STMP_EINVAL, "stmp_gemm_blocks_f32: bad block %d", i);
@@ -480,13 +481,15 @@ extern "C" int stmp_gemm_blocks_image(const void* packed, int64_t N, int64_t nbl
 
 extern "C" int stmp_spatial_attention_fwd(int64_t B, int64_t n_nodes, int64_t n_steps, const float* lhs, const float* rhs, const float* bsT,
                                           const void* vsT_packed, const void* vsT_image, float* st_out, int64_t ld_out, void* stream) {
-  STMP_REQUIRE(lhs && rhs && bsT && vsT_packed && st_out, STMP_EINVAL, "stmp_spatial_attention_fwd: NULL pointer");
   STMP_REQUIRE(B >= 0 && n_nodes >= 1 && n_steps >= 1, STMP_EINVAL, "stmp_spatial_attention_fwd: bad sizes");
   const int64_t Npad = (n_nodes + 63) / 64 * 64;
   if (Npad > 320 || n_steps > 12 || ld_out < Npad || ld_out % 4 != 0 || (reinterpret_cast<uintptr_t>(st_out) & 15))
     return set_error(STMP_EUNSUPPORTED, "fused spatial attention takes <= 320 nodes, <= 12 timesteps and 16-byte aligned rows of >= %lld floats "
                                         "(nodes=%lld steps=%lld ld=%lld)", (long long)Npad, (long long)n_nodes, (long long)n_steps, (long long)ld_out);
   if (B == 0) return STMP_OK;
+  STMP_REQUIRE(lhs && rhs && bsT && vsT_packed && st_out, STMP_EINVAL, "stmp_spatial_attention_fwd: NULL pointer");
+  // at T == 12 the operand generator reads each 48-byte LHS row as three float4
+  STMP_REQUIRE(n_steps != 12 || (reinterpret_cast<uintptr_t>(lhs) & 15) == 0, STMP_EINVAL, "stmp_spatial_attention_fwd: lhs must be 16-byte aligned");
   GbParams p = {};
   p.nblk = (int)(Npad / 64); p.M = (int)(B * n_nodes); p.N = (int)Npad; p.seq = 1; p.ncols = (int)n_nodes;
   p.w_hi = reinterpret_cast<const __half*>(vsT_packed); p.w_lo = p.w_hi + Npad * Npad;

@@ -167,7 +167,7 @@ extern "C" int stmp_spmm(const stmp_plan* plan, int op, int transposed, int64_t 
 extern "C" int stmp_spmm_att_t(const stmp_plan* plan, int op, int64_t batch, int64_t f, const float* x, int64_t ldx, int64_t bsx,
                               float* y, int64_t ldy, int64_t bsy, float alpha, const float* z, int64_t ldz, int64_t bsz, float beta,
                               const float* attT, int64_t att_ld, void* stream) {
-  STMP_REQUIRE(attT != nullptr, STMP_EINVAL, "stmp_spmm_att_t: attT is NULL");
+  STMP_REQUIRE(attT != nullptr || batch == 0 || f == 0, STMP_EINVAL, "stmp_spmm_att_t: attT is NULL");
   STMP_REQUIRE(plan == nullptr || att_ld >= plan->n, STMP_ESHAPE, "stmp_spmm_att_t: att_ld smaller than the node count");
   return spmm_impl(plan, op, 0, batch, f, x, ldx, bsx, y, ldy, bsy, alpha, z, ldz, bsz, beta, attT, att_ld, 1, stream);
 }
@@ -177,11 +177,11 @@ static int spmm_impl(const stmp_plan* plan, int op, int transposed, int64_t batc
                      int64_t ldz, int64_t bsz, float beta, const float* att, int64_t att_ld, int att_is_transposed, void* stream) {
   STMP_REQUIRE(plan != nullptr, STMP_EINVAL, "stmp_spmm: plan is NULL");
   STMP_REQUIRE(op >= 0 && op < plan->n_ops, STMP_EINVAL, "stmp_spmm: op %d out of range", op);
-  STMP_REQUIRE(x && y, STMP_EINVAL, "stmp_spmm: x/y is NULL");
   STMP_REQUIRE(batch >= 0 && f >= 0, STMP_EINVAL, "stmp_spmm: negative size");
   STMP_REQUIRE(ldx >= f && ldy >= f && (!z || ldz >= f), STMP_ESHAPE, "stmp_spmm: row stride smaller than f");
+  if (batch == 0 || f == 0) return STMP_OK;     // empty tensors may come with NULL data pointers
+  STMP_REQUIRE(x && y, STMP_EINVAL, "stmp_spmm: x/y is NULL");
   STMP_REQUIRE(x != y, STMP_EINVAL, "stmp_spmm: in-place product is not supported");
-  if (batch == 0 || f == 0) return STMP_OK;
   const Csr& c = transposed ? plan->bwd[op] : plan->fwd[op];
   SpmmArgs a;
   a.rowptr = c.rowptr; a.cv = c.cv; a.n = c.n; a.batch = batch; a.f = (int)f;

@@ -218,8 +218,12 @@ class ASTGCNBlock(nn.Module):
     # ---- native inference path: channels-last activations, fused wgmma products ------------------------------------
     def _native_ok(self, N, Fi, T):
         tc, rc = self._time_convolution, self._residual_convolution
+        ta, sa = self._temporal_attention, self._spatial_attention
         K = self._chebconv_attention._weight.size(0)
-        return (N <= 1024 and T <= 12 and Fi <= 64 and K <= 12 and tc.out_channels == 64 and tc.in_channels == 64
+        # the kernels take N, Fi and T from X and index the parameters with them: an X of another shape goes to the op-for-op path,
+        # which raises the reference's shape error
+        shapes_match = (ta._U1.shape == (N,) and ta._U3.shape == (Fi,) and ta._be.shape == (1, T, T) and sa._Vs.shape == (N, N))
+        return (shapes_match and N <= 1024 and T <= 12 and Fi <= 64 and K <= 12 and tc.out_channels == 64 and tc.in_channels == 64
                 and tc.stride[1] == 1 and rc.stride[1] == 1 and tc.kernel_size == (1, 3) and tc.padding == (0, 1))
 
     def _native_packs(self):
@@ -329,8 +333,9 @@ class ASTGCN(nn.Module):
         _require_cuda(X, "X")
         B, N, Fi, T = X.shape
         fc = self._final_conv
+        # the final convolution is one blocked GEMM of num_for_predict (rounded up to 16) <= 320 output columns
         if (not isinstance(edge_index, list) and not _needs_grad(self, X) and fc.in_channels <= 12 and fc.kernel_size[1] == 64
-                and all(b._native_ok(N, Fi if i == 0 else 64, T) for i, b in enumerate(self._blocklist))):
+                and fc.out_channels <= 320 and all(b._native_ok(N, Fi if i == 0 else 64, T) for i, b in enumerate(self._blocklist))):
             # inference: channels-last (B,N,T,F) all the way, one layout change at the input
             Xc = X.permute(0, 1, 3, 2).contiguous()
             for block in self._blocklist:

@@ -768,13 +768,21 @@ def spatial_attention_prepack(Vs: torch.Tensor) -> torch.Tensor:
 SPATT_ONE_TILE_MAX = 320     # widest padded node count stmp_spatial_attention_fwd holds in one CTA row tile
 
 
+def _spatt_factors(lhs, rhs, bsT):
+    """Contiguous fp32 factors; an lhs view that does not start on 16 bytes is copied (both kernels read its 48-byte rows as float4 at T = 12)."""
+    lhs, rhs, bsT = _f32c(lhs, "lhs"), _f32c(rhs, "rhs"), _f32c(bsT, "bsT")
+    if lhs.data_ptr() % 16:
+        lhs = lhs.clone()
+    return lhs, rhs, bsT
+
+
 def spatial_attention(lhs: torch.Tensor, rhs: torch.Tensor, bsT: torch.Tensor, vsT_packed: torch.Tensor) -> torch.Tensor:
     """ST (B, N, P) with ST[b, j, i] = softmax_dim1(Vs @ sigmoid(lhs @ rhs + bs))[b, i, j]; columns >= N are zero.
     P = N rounded up to 64 <= 320: one kernel (stmp_spatial_attention_fwd); up to 1024 nodes: the column-tiled pair (spatial_attention_tiled)."""
     P = (lhs.size(1) + 63) // 64 * 64
     if P > SPATT_ONE_TILE_MAX:
         return spatial_attention_tiled(lhs, rhs, bsT, vsT_packed)
-    lhs, rhs, bsT = _f32c(lhs, "lhs"), _f32c(rhs, "rhs"), _f32c(bsT, "bsT")
+    lhs, rhs, bsT = _spatt_factors(lhs, rhs, bsT)
     B, n, T = lhs.shape
     st = torch.empty((B, n, P), dtype=torch.float32, device=lhs.device)
     packed, image = vsT_packed if isinstance(vsT_packed, tuple) else (vsT_packed, None)
@@ -787,7 +795,7 @@ def spatial_attention(lhs: torch.Tensor, rhs: torch.Tensor, bsT: torch.Tensor, v
 def spatial_attention_tiled(lhs: torch.Tensor, rhs: torch.Tensor, bsT: torch.Tensor, vsT_packed) -> torch.Tensor:
     """`spatial_attention` on the column-tiled kernel pair (stmp_spatial_attention_tiled_fwd), any 1 <= N <= 1024; the per-row softmax
     statistics go to a workspace from the caching allocator, so the call is capturable."""
-    lhs, rhs, bsT = _f32c(lhs, "lhs"), _f32c(rhs, "rhs"), _f32c(bsT, "bsT")
+    lhs, rhs, bsT = _spatt_factors(lhs, rhs, bsT)
     B, n, T = lhs.shape
     P = (n + 63) // 64 * 64
     st = torch.empty((B, n, P), dtype=torch.float32, device=lhs.device)

@@ -94,6 +94,15 @@ with torch.no_grad():
     ASTGCN(1, 1, 3, 64, 64, 1, 12, 12, 883, normalization="sym").to(dev)(torch.randn(2, 883, 1, 12, device=dev), e7)   # k_spatt_tiles x4 columns + k_spatt_norm
     ops.spatial_attention_tiled(torch.randn(1, 70, 5, device=dev), torch.randn(1, 5, 70, device=dev), torch.randn(70, 70, device=dev),
                                 ops.spatial_attention_prepack(torch.randn(70, 70, device=dev)))   # one column tile, partial row tile, T < 12
+    # the ASTGCN envelope (tests/test_gpu_astgcn_envelope.py): a scalar factors instance (F = 2), the 8-chunk one-tile attention
+    # (100 nodes, T = 7), and a forward at in_channels 3 (torch factors), K = 1, T = 1 with 129 outputs (the 20-chunk EPI_BIAS instance)
+    ops.astgcn_factors(torch.randn(2, 40, 7, 2, device=dev), *[torch.randn(*s, device=dev) for s in ((40,), (2, 40), (2,), (7, 7), (7, 7),
+                                                                                                      (7,), (2, 7), (2,))])
+    ops.spatial_attention(torch.randn(2, 100, 7, device=dev), torch.randn(2, 7, 100, device=dev), torch.randn(100, 100, device=dev),
+                          ops.spatial_attention_prepack(torch.randn(100, 100, device=dev)))
+    r50 = torch.arange(50, device=dev)
+    ASTGCN(1, 3, 1, 64, 64, 1, 129, 1, 50, normalization="sym").to(dev)(torch.randn(2, 50, 3, 1, device=dev),
+                                                                         torch.stack([r50, (r50 + 1) % 50]))
     eg, wg = synthetic.large_graph(2000, 20000, 0)
     eg, wg = torch.from_numpy(eg).to(dev), torch.from_numpy(wg).to(dev)
     lstm = GConvLSTM(64, 64, 3).to(dev)
