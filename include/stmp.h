@@ -291,7 +291,7 @@ int stmp_gru_bwd_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const f
  *                               over `rows` rows: fp32 FFMA per-CTA partials + a fixed-order sum (two launches); workspace of
  *                               stmp_gru_rows_wgrad_workspace_bytes(n_ops, cin) bytes, 16-byte aligned operands.
  * STMP_EINVAL for NULL tensors, STMP_ESHAPE for bad sizes, pitches or alignment, STMP_EUNSUPPORTED for cin > 16, n_ops > 1, cout != 32
- * or n_ops above the plan's operators. */
+ * or n_ops above the plan's operators.  stmp_gru_rows_supported also answers 1 for cout = 64 (the stmp_gru_wide_rows_* entries below). */
 int stmp_gru_rows_supported(const stmp_plan* plan, int n_ops, int64_t cin, int64_t cout);
 int stmp_gru_rows_pack_weights(int n_ops, int64_t cin, const float* wx, const float* wh, const float* bx, const float* bh, float* w,
                                float* b, void* stream);
@@ -303,6 +303,31 @@ int stmp_gru_rows_bwd(const stmp_plan* plan, int n_ops, int64_t cin, const float
 int64_t stmp_gru_rows_wgrad_workspace_bytes(int n_ops, int64_t cin);
 int stmp_gru_rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
                         const float* dph, void* workspace, float* dw, float* db, void* stream);
+
+/* ---- the same cell at 64 hidden channels (gru_rows.cu, the width-2 instance of its kernels): GConvGRU(cin, 64, K <= 2).  Envelope: cout =
+ * 64, cin 1..16, n_ops 0..1 and at most the plan's operators (stmp_gru_rows_supported(plan, n_ops, cin, 64)), any number of nodes and any
+ * degree.  Same argument lists, launch chain and guarantees as the stmp_gru_rows_* entries, with 32 -> 64 throughout:
+ *   packed weights w [192][nb], nb = (n_ops+1)(cin+64): row gate*64 + o, column m of the basis [X | H | Op X | Op H]; b [192].
+ *   stmp_gru_wide_rows_pack_weights: wx [3][n_ops+1][64][cin], wh [3][n_ops+1][64][64], bx / bh [3][64] (both or neither).
+ *   stmp_gru_wide_rows_fwd:          x (N,cin), h (N,64) or NULL -> out (N,64); scratch of N*192 floats when h is given; stash (3,N,64);
+ *                                    S1 / S2 (N, ld), ld = nb rounded up to 8, 16-byte aligned.
+ *   stmp_gru_wide_rows_bwd:          gout (N,64) -> dph (N,64), dpzr (N,128), dx (N,cin), dh (N,64); scratch of
+ *                                    stmp_gru_wide_rows_scratch_bytes(plan) bytes (N*320 floats).
+ *   stmp_gru_wide_rows_wgrad:        dw [192][nb], db [192] (nullable): fp32 FFMA per-CTA partials of each gate's product over strided
+ *                                    32-row tiles + a fixed-order sum (two launches); workspace of
+ *                                    stmp_gru_wide_rows_wgrad_workspace_bytes(n_ops, cin) bytes, 16-byte aligned operands.
+ * STMP_EINVAL for NULL tensors, STMP_ESHAPE for bad sizes, pitches or alignment, STMP_EUNSUPPORTED for cin > 16, n_ops > 1 or n_ops above
+ * the plan's operators. */
+int stmp_gru_wide_rows_pack_weights(int n_ops, int64_t cin, const float* wx, const float* wh, const float* bx, const float* bh, float* w,
+                                    float* b, void* stream);
+int stmp_gru_wide_rows_fwd(const stmp_plan* plan, int n_ops, int64_t cin, const float* x, const float* h, const float* w, const float* b,
+                           float* scratch, float* out, float* stash, float* S1, float* S2, int64_t ld, void* stream);
+int64_t stmp_gru_wide_rows_scratch_bytes(const stmp_plan* plan);
+int stmp_gru_wide_rows_bwd(const stmp_plan* plan, int n_ops, int64_t cin, const float* gout, const float* h, const float* stash,
+                           const float* w, float* scratch, float* dph, float* dpzr, float* dx, float* dh, void* stream);
+int64_t stmp_gru_wide_rows_wgrad_workspace_bytes(int n_ops, int64_t cin);
+int stmp_gru_wide_rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
+                             const float* dph, void* workspace, float* dw, float* db, void* stream);
 
 /* ---- BatchedDCRNN at 32 hidden channels on graphs of ANY size, split over CTAs by destination rows (dcrnn_rows.cu): the reference's
  * BatchedDCRNN (dcrnn.py:328-475) with H_0 = 0, all B windows of a step in each launch.  Envelope: a DConv plan, cout = 32, K = 2, cin 1..4

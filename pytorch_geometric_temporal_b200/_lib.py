@@ -81,6 +81,12 @@ _SIGNATURES = {
     "stmp_gru_rows_bwd": (c_int, [_P, c_int, c_int64] + [_P] * 10),
     "stmp_gru_rows_wgrad_workspace_bytes": (c_int64, [c_int, c_int64]),
     "stmp_gru_rows_wgrad": (c_int, [c_int, c_int64, c_int64, c_int64] + [_P] * 8),
+    "stmp_gru_wide_rows_pack_weights": (c_int, [c_int, c_int64] + [_P] * 7),
+    "stmp_gru_wide_rows_fwd": (c_int, [_P, c_int, c_int64] + [_P] * 9 + [c_int64, _P]),
+    "stmp_gru_wide_rows_scratch_bytes": (c_int64, [_P]),
+    "stmp_gru_wide_rows_bwd": (c_int, [_P, c_int, c_int64] + [_P] * 10),
+    "stmp_gru_wide_rows_wgrad_workspace_bytes": (c_int64, [c_int, c_int64]),
+    "stmp_gru_wide_rows_wgrad": (c_int, [c_int, c_int64, c_int64, c_int64] + [_P] * 8),
     "stmp_dcrnn_rows_supported": (c_int, [_P, c_int64, c_int64, c_int64]),
     "stmp_dcrnn_rows_scratch_bytes": (c_int64, [_P, c_int64]),
     "stmp_dcrnn_rows_fwd": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, c_int64, c_int64] + [_P] * 10 + [c_int64, _P]),

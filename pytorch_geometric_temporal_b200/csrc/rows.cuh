@@ -1,5 +1,5 @@
 // rows.cuh -- the pieces shared by the row-split recurrent cells (gru_rows.cu, lstm_rows.cu): one warp per destination row, lane = output
-// channel, CTAs owning grid-strided tiles of kRowTile rows, weights staged once per CTA at pitch kWPitch, and the entry-order CSR gather.
+// channel (lane + 32 j for j < NC in gru_rows.cu's 64-wide instance), CTAs owning grid-strided tiles of kRowTile rows, weights staged once per CTA at pitch kWPitch, and the entry-order CSR gather.
 #pragma once
 #include "common.cuh"
 
@@ -13,47 +13,64 @@ constexpr int kRowTile = 16;                 // destination rows per CTA tile: t
 constexpr int kWPitch = 97;                  // shared-memory pitch of a staged weight row (basis columns 0..95)
 constexpr int kMaxCin = 16;
 
-// rows [r0, r0 + nr) of packed weights w [..][nb] -> ws [nr][kWPitch] (columns >= nb zero)
+// rows [r0, r0 + nr) of packed weights w [..][nb] -> ws [nr][P] (columns >= nb zero)
+template <int P = kWPitch>
 __device__ __forceinline__ void stage_w(float* ws, const float* __restrict__ w, int nb, int r0, int nr) {
-  for (int i = threadIdx.x; i < nr * kWPitch; i += kRowsThreads) {
-    const int r = i / kWPitch, m = i - r * kWPitch;
+  for (int i = threadIdx.x; i < nr * P; i += kRowsThreads) {
+    const int r = i / P, m = i - r * P;
     ws[i] = m < nb ? __ldg(w + (size_t)(r0 + r) * nb + m) : 0.f;
   }
   __syncthreads();
 }
 
-// ah = sum_e val_e * A[col_e][lane] (pitch lda), ax = sum_e val_e * B[col_e][lane] (pitch ldb, lanes < nx) over CSR row i, in entry order.
-template <bool WITH_A>
-__device__ __forceinline__ void gather_row(const int* __restrict__ rowptr, const int2* __restrict__ cv, int i, const float* __restrict__ A,
-                                           int lda, const float* __restrict__ Bx, int ldb, int nx, int lane, float& ah, float& ax) {
+// ah[j] = sum_e val_e * A[col_e][lane + 32 j] (pitch lda, j < NC), ax = sum_e val_e * B[col_e][lane] (pitch ldb, lanes < nx) over CSR row
+// i, in entry order.
+template <int NC, bool WITH_A>
+__device__ __forceinline__ void gather_rows(const int* __restrict__ rowptr, const int2* __restrict__ cv, int i, const float* __restrict__ A,
+                                            int lda, const float* __restrict__ Bx, int ldb, int nx, int lane, float (&ah)[NC], float& ax) {
   const int beg = __ldg(rowptr + i), end = __ldg(rowptr + i + 1);
   const bool xl = lane < nx;
-  ah = 0.f;
+#pragma unroll
+  for (int j = 0; j < NC; ++j) ah[j] = 0.f;
   ax = 0.f;
   int k = beg;
   for (; k + 4 <= end; k += 4) {
     int2 e[4];
-    float av[4], bv[4];
+    float av[4][NC], bv[4];
 #pragma unroll
     for (int u = 0; u < 4; ++u) e[u] = __ldg(cv + k + u);
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
-      av[u] = WITH_A ? __ldg(A + (size_t)e[u].x * lda + lane) : 0.f;
+#pragma unroll
+      for (int j = 0; j < NC; ++j) av[u][j] = WITH_A ? __ldg(A + (size_t)e[u].x * lda + lane + 32 * j) : 0.f;
       bv[u] = xl ? __ldg(Bx + (size_t)e[u].x * ldb + lane) : 0.f;
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const float w = __int_as_float(e[u].y);
-      if (WITH_A) ah = __fadd_rn(ah, __fmul_rn(w, av[u]));
+#pragma unroll
+      for (int j = 0; j < NC; ++j)
+        if (WITH_A) ah[j] = __fadd_rn(ah[j], __fmul_rn(w, av[u][j]));
       if (xl) ax = __fadd_rn(ax, __fmul_rn(w, bv[u]));
     }
   }
   for (; k < end; ++k) {
     const int2 e = __ldg(cv + k);
     const float w = __int_as_float(e.y);
-    if (WITH_A) ah = __fadd_rn(ah, __fmul_rn(w, __ldg(A + (size_t)e.x * lda + lane)));
+#pragma unroll
+    for (int j = 0; j < NC; ++j)
+      if (WITH_A) ah[j] = __fadd_rn(ah[j], __fmul_rn(w, __ldg(A + (size_t)e.x * lda + lane + 32 * j)));
     if (xl) ax = __fadd_rn(ax, __fmul_rn(w, __ldg(Bx + (size_t)e.x * ldb + lane)));
   }
+}
+
+// gather_rows for one channel per lane
+template <bool WITH_A>
+__device__ __forceinline__ void gather_row(const int* __restrict__ rowptr, const int2* __restrict__ cv, int i, const float* __restrict__ A,
+                                           int lda, const float* __restrict__ Bx, int ldb, int nx, int lane, float& ah, float& ax) {
+  float a[1];
+  gather_rows<1, WITH_A>(rowptr, cv, i, A, lda, Bx, ldb, nx, lane, a, ax);
+  ah = a[0];
 }
 
 // CTAs of a row-split launch over n rows: one per 16-row tile, at most two per SM (the tiles are grid-strided beyond that)

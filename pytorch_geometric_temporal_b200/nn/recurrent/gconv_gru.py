@@ -8,7 +8,9 @@ Inside the fused envelope (K <= 2, out_channels = 32, in_channels <= 4, a graph 
 generic graph-GRU kernel, and training is that same launch plus a hand-written backward (ops.gru_seq_train): the gradients of the
 prepacked weights are handed to the parameters as blocks, so the cached fold needs no autograd graph.  Graphs too large for one SM
 (K <= 2, out_channels = 32, in_channels <= 16, 2-D X) run the row-split cell kernels instead (ops.gru_rows_fwd / gru_rows_train):
-one launch with H = None, two with H given, and a hand-written backward of the same kind."""
+one launch with H = None, two with H given, and a hand-written backward of the same kind.  At out_channels = 64 (K <= 2, in_channels <=
+16, 2-D X) every graph, small or large, runs the 64-wide instance of those kernels (stmp_gru_wide_rows_*): no one-SM kernel holds that
+width."""
 import torch
 
 from ... import ops
@@ -64,7 +66,8 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
         return self._pack.get(list(self.parameters()), build)
 
     def _rows_packed(self):
-        """(w [96, K(Ci+32)], b [96]) for stmp_gru_rows_fwd: columns [X | H] per Chebyshev order (one launch per weight update)."""
+        """(w [3 Co, K(Ci+Co)], b [3 Co]) for stmp_gru_rows_fwd / stmp_gru_wide_rows_fwd: columns [X | H] per Chebyshev order (one launch per
+        weight update)."""
         def build():
             gates = [(getattr(self, f"conv_x_{g}"), getattr(self, f"conv_h_{g}")) for g in "zrh"]
             wx = torch.stack([torch.stack([cx.lins[k].weight for k in range(self.K)]) for cx, _ in gates])
@@ -80,16 +83,16 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
         weight / bias gradients -- the inverse of `_packed` (`_rows_packed`).  Both ChebConvs of a gate add their biases, so both receive
         that gate's bias block."""
         spec, params = [], []
-        Ci = self.in_channels
+        Ci, Co = self.in_channels, (self.out_channels if rows else 32)
         for gi, g in enumerate("zrh"):
             cx, ch = getattr(self, f"conv_x_{g}"), getattr(self, f"conv_h_{g}")
             for k in range(self.K):
-                spec.append(("w", 32 * gi, 32, k * (Ci + 32) + Ci if rows else 32 * k, 32))
+                spec.append(("w", Co * gi, Co, k * (Ci + Co) + Ci if rows else 32 * k, Co))
                 params.append(ch.lins[k].weight)
-                spec.append(("w", 32 * gi, 32, k * (Ci + 32) if rows else 96 + 4 * k, Ci))
+                spec.append(("w", Co * gi, Co, k * (Ci + Co) if rows else 96 + 4 * k, Ci))
                 params.append(cx.lins[k].weight)
             if cx.bias is not None:
-                spec += [("b", 32 * gi, 32), ("b", 32 * gi, 32)]
+                spec += [("b", Co * gi, Co), ("b", Co * gi, Co)]
                 params += [cx.bias, ch.bias]
         return spec, params
 
@@ -115,16 +118,18 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
         return ops.gru_seq_supported(plan, 1 if self.K > 1 else 0, self.in_channels, self.out_channels)
 
     def _rows_ok(self, plan, X, H, training):
-        """The row-split route: K <= 2, out_channels = 32, in_channels <= 16, 2-D float32 X, a graph the one-SM kernel cannot hold (checked
-        first, so graphs that fit one SM never consult the row-split entry); training calls also need `fused_training`."""
-        if self.K > 2 or self.out_channels != 32 or self.in_channels > 16 or X.dim() != 2 or X.dtype != torch.float32:
+        """The row-split route: K <= 2, out_channels 32 or 64, in_channels <= 16, 2-D float32 X; at 32 only a graph the one-SM kernel
+        cannot hold (checked first, so graphs that fit one SM never consult the row-split entry), at 64 any graph; training calls also need
+        `fused_training`."""
+        Co = self.out_channels
+        if self.K > 2 or Co not in (32, 64) or self.in_channels > 16 or X.dim() != 2 or X.dtype != torch.float32:
             return False
-        if (training and not self.fused_training) or (H is not None and (H.shape != (X.size(0), 32) or H.dtype != torch.float32)):
+        if (training and not self.fused_training) or (H is not None and (H.shape != (X.size(0), Co) or H.dtype != torch.float32)):
             return False
         n_ops = self.K - 1
-        if ops.gru_seq_supported(plan, n_ops, 1, 32):
+        if Co == 32 and ops.gru_seq_supported(plan, n_ops, 1, 32):
             return False
-        return ops.gru_rows_supported(plan, n_ops, self.in_channels, 32)
+        return ops.gru_rows_supported(plan, n_ops, self.in_channels, Co)
 
     def forward(self, X: torch.FloatTensor, edge_index: torch.LongTensor, edge_weight: torch.FloatTensor = None,
                 H: torch.FloatTensor = None, lambda_max: torch.Tensor = None) -> torch.FloatTensor:
@@ -144,7 +149,7 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
             return ops.gru_seq_train(plan, K - 1, X.reshape(1, 1, N, Ci), h0, W, b, img, spec, params)[0, 0]
         training = torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters()) or X.requires_grad
                                                  or (H_given is not None and H_given.requires_grad))
-        if self._rows_ok(plan, X, H_given, training):   # graphs larger than one SM: the row-split cell kernels (stmp_gru_rows_*)
+        if self._rows_ok(plan, X, H_given, training):   # graphs larger than one SM, or 64 channels: the row-split cell kernels
             w, b = self._rows_packed()
             if training:
                 spec, params = self._param_spec(rows=True)

@@ -291,45 +291,56 @@ def gru_rows_supported(plan: GraphPlan, n_ops: int, cin: int, cout: int) -> bool
     return bool(_lib.lib().stmp_gru_rows_supported(plan.handle, n_ops, cin, cout))
 
 
-def gru_rows_basis_ld(n_ops: int, cin: int) -> int:
-    """Row pitch of the row-split cell's weight-gradient bases: (n_ops+1)(cin+32) rounded up to 8 floats."""
-    return ((n_ops + 1) * (cin + 32) + 7) // 8 * 8
+def gru_rows_basis_ld(n_ops: int, cin: int, cout: int = 32) -> int:
+    """Row pitch of the row-split cell's weight-gradient bases: (n_ops+1)(cin+cout) rounded up to 8 floats."""
+    return ((n_ops + 1) * (cin + cout) + 7) // 8 * 8
+
+
+def _gru_rows_entry(cout: int, what: str):
+    """stmp_gru_rows_<what> at 32 hidden channels, stmp_gru_wide_rows_<what> at 64; the two families take the same arguments."""
+    if cout not in (32, 64):
+        raise RuntimeError(f"the row-split graph-GRU cell serves 32 or 64 hidden channels, not {cout}")
+    return getattr(_lib.lib(), ("stmp_gru_wide_rows_" if cout == 64 else "stmp_gru_rows_") + what)
 
 
 def gru_rows_pack_weights(n_ops: int, cin: int, wx, wh, bx=None, bh=None):
-    """(w (96, (n_ops+1)(cin+32)), b (96,)): the row-split cell's packed weights from the parameters' layout -- wx (3, n_ops+1, 32, cin),
-    wh (3, n_ops+1, 32, 32), bx / bh (3, 32) or None -- in one launch (stmp_gru_rows_pack_weights)."""
+    """(w (3 cout, (n_ops+1)(cin+cout)), b (3 cout,)): the row-split cell's packed weights from the parameters' layout -- wx (3, n_ops+1, cout,
+    cin), wh (3, n_ops+1, cout, cout), bx / bh (3, cout) or None, cout = 32 or 64 -- in one launch (stmp_gru_rows_pack_weights or
+    stmp_gru_wide_rows_pack_weights)."""
     wx, wh = _f32c(wx, "wx"), _f32c(wh, "wh")
-    if wx.shape != (3, n_ops + 1, 32, cin) or wh.shape != (3, n_ops + 1, 32, 32):
-        raise RuntimeError("gru_rows_pack_weights: wx must be (3, n_ops+1, 32, cin) and wh (3, n_ops+1, 32, 32)")
+    cout = wh.size(-1) if wh.dim() == 4 else 32
+    if wx.shape != (3, n_ops + 1, cout, cin) or wh.shape != (3, n_ops + 1, cout, cout):
+        raise RuntimeError("gru_rows_pack_weights: wx must be (3, n_ops+1, cout, cin) and wh (3, n_ops+1, cout, cout)")
     bx = None if bx is None else _f32c(bx, "bx")
     bh = None if bh is None else _f32c(bh, "bh")
-    w = torch.empty(96, (n_ops + 1) * (cin + 32), device=wx.device, dtype=torch.float32)
-    b = torch.empty(96, device=wx.device, dtype=torch.float32)
+    w = torch.empty(3 * cout, (n_ops + 1) * (cin + cout), device=wx.device, dtype=torch.float32)
+    b = torch.empty(3 * cout, device=wx.device, dtype=torch.float32)
     with torch.cuda.device(wx.device):
-        _lib.check(_lib.lib().stmp_gru_rows_pack_weights(n_ops, cin, _lib.ptr(wx), _lib.ptr(wh), _lib.ptr(bx), _lib.ptr(bh), _lib.ptr(w),
+        _lib.check(_gru_rows_entry(cout, "pack_weights")(n_ops, cin, _lib.ptr(wx), _lib.ptr(wh), _lib.ptr(bx), _lib.ptr(bh), _lib.ptr(w),
                                                          _lib.ptr(b), _lib.stream_ptr()))
     return w, b
 
 
 def gru_rows_fwd(plan: GraphPlan, n_ops: int, x: torch.Tensor, h: Optional[torch.Tensor], w: torch.Tensor, b: torch.Tensor,
                  train: bool = False):
-    """Row-split graph-GRU cell (stmp_gru_rows_fwd) on one graph: x (N, cin), h (N, 32) or None -> H' (N, 32).  With `train`, returns
-    (H', stash (3, N, 32), S1, S2) -- the operands of gru_rows_bwd / gru_rows_wgrad; S2 is S1 when h is None."""
+    """Row-split graph-GRU cell (stmp_gru_rows_fwd, or stmp_gru_wide_rows_fwd for packed weights of 192 rows) on one graph: x (N, cin),
+    h (N, cout) or None -> H' (N, cout), cout = w.size(0) / 3.  With `train`, returns (H', stash (3, N, cout), S1, S2) -- the operands of
+    gru_rows_bwd / gru_rows_wgrad; S2 is S1 when h is None."""
     x, w, b = _f32c(x, "X"), _f32c(w, "w"), _f32c(b, "b")
     N, cin = x.shape
+    cout = w.size(0) // 3
     f32 = dict(device=x.device, dtype=torch.float32)
-    out = torch.empty(N, 32, **f32)
+    out = torch.empty(N, cout, **f32)
     hc = None if h is None else _f32c(h, "H")
-    scr = torch.empty(N, 96, **f32) if hc is not None else None
+    scr = torch.empty(N, 3 * cout, **f32) if hc is not None else None
     st = S1 = S2 = None
-    ld = gru_rows_basis_ld(n_ops, cin)
+    ld = gru_rows_basis_ld(n_ops, cin, cout)
     if train:
-        st = torch.empty(3, N, 32, **f32)
+        st = torch.empty(3, N, cout, **f32)
         S1 = torch.empty(N, ld, **f32)
         S2 = torch.empty(N, ld, **f32) if hc is not None else None
     with torch.cuda.device(x.device):
-        _lib.check(_lib.lib().stmp_gru_rows_fwd(plan.handle, n_ops, cin, _lib.ptr(x), _lib.ptr(hc), _lib.ptr(w), _lib.ptr(b), _lib.ptr(scr),
+        _lib.check(_gru_rows_entry(cout, "fwd")(plan.handle, n_ops, cin, _lib.ptr(x), _lib.ptr(hc), _lib.ptr(w), _lib.ptr(b), _lib.ptr(scr),
                                                 _lib.ptr(out), _lib.ptr(st), _lib.ptr(S1), _lib.ptr(S2), ld, _lib.stream_ptr()))
     if not train:
         return out
@@ -337,38 +348,42 @@ def gru_rows_fwd(plan: GraphPlan, n_ops: int, x: torch.Tensor, h: Optional[torch
 
 
 def gru_rows_bwd(plan: GraphPlan, n_ops: int, gout, h, stash, w, want_dx: bool, want_dh: bool, cin: int):
-    """(dph (N, 32), dpzr (N, 64), dx (N, cin) or None, dh (N, 32) or None) of the row-split cell (stmp_gru_rows_bwd)."""
+    """(dph (N, cout), dpzr (N, 2 cout), dx (N, cin) or None, dh (N, cout) or None) of the row-split cell (stmp_gru_rows_bwd, or
+    stmp_gru_wide_rows_bwd when gout has 64 channels)."""
     gout = _f32c(gout, "gout")
-    N = gout.size(0)
+    N, cout = gout.shape
     f32 = dict(device=gout.device, dtype=torch.float32)
-    scr = torch.empty(int(_lib.lib().stmp_gru_rows_scratch_bytes(plan.handle)) // 4, **f32)
-    dph, dpzr = torch.empty(N, 32, **f32), torch.empty(N, 64, **f32)
+    scr = torch.empty(int(_gru_rows_entry(cout, "scratch_bytes")(plan.handle)) // 4, **f32)
+    dph, dpzr = torch.empty(N, cout, **f32), torch.empty(N, 2 * cout, **f32)
     dx = torch.empty(N, cin, **f32) if want_dx else None
-    dh = torch.empty(N, 32, **f32) if want_dh else None
+    dh = torch.empty(N, cout, **f32) if want_dh else None
     with torch.cuda.device(gout.device):
-        _lib.check(_lib.lib().stmp_gru_rows_bwd(plan.handle, n_ops, cin, _lib.ptr(gout), _lib.ptr(h), _lib.ptr(stash), _lib.ptr(w),
+        _lib.check(_gru_rows_entry(cout, "bwd")(plan.handle, n_ops, cin, _lib.ptr(gout), _lib.ptr(h), _lib.ptr(stash), _lib.ptr(w),
                                                 _lib.ptr(scr), _lib.ptr(dph), _lib.ptr(dpzr), _lib.ptr(dx), _lib.ptr(dh), _lib.stream_ptr()))
     return dph, dpzr, dx, dh
 
 
 def gru_rows_wgrad(n_ops: int, cin: int, S1, S2, dpzr, dph, has_bias: bool):
-    """(dw (96, (n_ops+1)(cin+32)), db (96,) or None): the packed weights' gradients of the row-split cell, two launches."""
+    """(dw (3 cout, (n_ops+1)(cin+cout)), db (3 cout,) or None): the packed weights' gradients of the row-split cell, two launches; cout =
+    dph.size(1)."""
     dev = S1.device
-    key = (dev, torch.cuda.current_stream(dev).cuda_stream, "gru_rows", n_ops, cin)
+    cout = dph.size(1)
+    key = (dev, torch.cuda.current_stream(dev).cuda_stream, "gru_rows", n_ops, cin, cout)
     ws = _WGRAD_WS.get(key)
     if ws is None:
-        ws = torch.empty(int(_lib.lib().stmp_gru_rows_wgrad_workspace_bytes(n_ops, cin)), device=dev, dtype=torch.uint8)
+        ws = torch.empty(int(_gru_rows_entry(cout, "wgrad_workspace_bytes")(n_ops, cin)), device=dev, dtype=torch.uint8)
         _WGRAD_WS[key] = ws
-    dw = torch.empty(96, (n_ops + 1) * (cin + 32), device=dev, dtype=torch.float32)
-    db = torch.empty(96, device=dev, dtype=torch.float32) if has_bias else None
+    dw = torch.empty(3 * cout, (n_ops + 1) * (cin + cout), device=dev, dtype=torch.float32)
+    db = torch.empty(3 * cout, device=dev, dtype=torch.float32) if has_bias else None
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().stmp_gru_rows_wgrad(n_ops, cin, S1.size(0), S1.size(1), _lib.ptr(S1), _lib.ptr(S2), _lib.ptr(dpzr), _lib.ptr(dph),
+        _lib.check(_gru_rows_entry(cout, "wgrad")(n_ops, cin, S1.size(0), S1.size(1), _lib.ptr(S1), _lib.ptr(S2), _lib.ptr(dpzr), _lib.ptr(dph),
                                                   _lib.ptr(ws), _lib.ptr(dw), _lib.ptr(db), _lib.stream_ptr()))
     return dw, db
 
 
 class _GruRowsFn(torch.autograd.Function):
-    """Training form of the row-split graph-GRU cell, the twin of _GruSeqFn for graphs of any size.  forward = `stmp_gru_rows_fwd` with the
+    """Training form of the row-split graph-GRU cell (32 or 64 hidden channels, from the packed weights), the twin of _GruSeqFn for graphs
+    of any size.  forward = `stmp_gru_rows_fwd` (`stmp_gru_wide_rows_fwd`) with the
     stash and the weight-gradient bases (the inference launches, so the output is bit-identical to the `no_grad` one); backward =
     `stmp_gru_rows_bwd` + `stmp_gru_rows_wgrad`: dX (when x requires grad), dH (when h is given and requires grad) and the packed weights'
     gradients, handed to `params` as blocks described by `spec` (see _spec_grads)."""
@@ -395,7 +410,7 @@ class _GruRowsFn(torch.autograd.Function):
 
 
 def gru_rows_train(plan: GraphPlan, n_ops: int, x, h, w, b, spec, params) -> torch.Tensor:
-    """Differentiable (w.r.t. x, h and `params`, see _GruRowsFn) row-split graph-GRU cell.  x (N, cin), h (N, 32) or None (zeros, no dH)."""
+    """Differentiable (w.r.t. x, h and `params`, see _GruRowsFn) row-split graph-GRU cell.  x (N, cin), h (N, cout) or None (zeros, no dH)."""
     return _GruRowsFn.apply(plan, n_ops, x, h, w, b, tuple(spec), *params)
 
 

@@ -154,6 +154,11 @@ for cin, cout, K in ((3, 32, 2), (3, 64, 3), (2, 3, 3)):
 g17 = GConvGRU(5, 32, 2).to(dev)
 xg, hg = torch.randn(17, 5, device=dev, requires_grad=True), torch.randn(17, 32, device=dev, requires_grad=True)
 ops.gru_rows_train(g17._cheb_plan(e17, None, 17, "sym", None), 1, xg, hg, *g17._rows_packed(), *g17._param_spec(rows=True)).square().mean().backward()
+g64 = GConvGRU(5, 64, 2).to(dev)                                # the 64-wide cell at 17 nodes: partial last tile, every launch
+xw, hw = torch.randn(17, 5, device=dev, requires_grad=True), torch.randn(17, 64, device=dev, requires_grad=True)
+g64(xw, e17, None, hw).square().mean().backward()
+with torch.no_grad():
+    g64(xw, e17, None)
 for cls in (GConvLSTM, GCLSTM):
     sum(t.square().mean() for t in cls(5, 32, 2).to(dev)(xg, e17, None, hg, torch.randn(17, 32, device=dev, requires_grad=True))).backward()
 torch.cuda.synchronize()
