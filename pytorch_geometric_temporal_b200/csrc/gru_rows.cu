@@ -424,8 +424,31 @@ __global__ void __launch_bounds__(kWgThreads, 1) k_gru_wide_rows_wgrad(long long
   }
 }
 
-// dw [192][nb] (row g*64 + o, column m) and db [192] (nullable): the partials summed in a fixed order -- each of a block's 8 warps sums a
-// contiguous eighth of the parts, then thread (0, x) adds the 8 sub-sums in warp order.
+// The fixed-order sums (fixed_order_sum, rows.cuh) of the 32-wide cell's k_dcrnn_wgrad<32> partials [part][ld*96 + 96] into its packed
+// layout dw [96][nb] (row gate*32 + o, column m of the basis [X | H | Op X | Op H]) and db [96] (nullable).
+__global__ void __launch_bounds__(256) k_gru_rows_wgrad_reduce(int parts, int MG, int nb, const float* __restrict__ partial,
+                                                               float* __restrict__ dw, float* __restrict__ db) {
+  __shared__ float sub[8][32];
+  const int x = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int i = blockIdx.x * 32 + x;
+  const size_t stride = (size_t)MG * 8 * 3 * kCo + 3 * kCo;
+  size_t src = 0;
+  float* dst = nullptr;
+  if (i < 96 * nb) {
+    const int row = i / nb, m = i - row * nb, gate = row >> 5, o = row & 31;
+    src = gate == 2 ? (size_t)MG * 8 * 2 * kCo + (size_t)m * kCo + o : (size_t)m * 2 * kCo + gate * kCo + o;
+    dst = dw + i;
+  } else if (i < 96 * nb + 3 * kCo) {
+    const int b = i - 96 * nb;                                   // bias sums are stored z | r | h
+    src = (size_t)MG * 8 * 3 * kCo + b;
+    dst = db ? db + b : nullptr;
+  }
+  const float t = fixed_order_sum(partial + src, stride, parts, dst != nullptr, sub);
+  if (w == 0 && dst) *dst = t;
+}
+
+// ... and of the 64-wide cell's k_gru_wide_rows_wgrad partials [gate][part][ld*64 + 64] into dw [192][nb] (row g*64 + o, column m) and
+// db [192] (nullable).
 __global__ void __launch_bounds__(256) k_gru_wide_rows_wgrad_reduce(int parts, int ld, int nb, const float* __restrict__ partial,
                                                                     float* __restrict__ dw, float* __restrict__ db) {
   __shared__ float sub[8][32];
@@ -446,25 +469,8 @@ __global__ void __launch_bounds__(256) k_gru_wide_rows_wgrad_reduce(int parts, i
     src = (size_t)ld * 64 + (r & 63);
     dst = db ? db + r : nullptr;
   }
-  const float* pg = partial + (size_t)g * parts * stride + src;
-  const int per = (parts + 7) / 8, q0 = w * per, q1 = (q0 + per < parts) ? q0 + per : parts;
-  float s0 = 0.f, s1 = 0.f;
-  if (dst) {
-    int q = q0;
-    for (; q + 2 <= q1; q += 2) {
-      s0 += pg[(size_t)q * stride];
-      s1 += pg[(size_t)(q + 1) * stride];
-    }
-    if (q < q1) s0 += pg[(size_t)q * stride];
-  }
-  sub[w][x] = s0 + s1;
-  __syncthreads();
-  if (w == 0 && dst) {
-    float t = sub[0][x];
-#pragma unroll
-    for (int k = 1; k < 8; ++k) t += sub[k][x];
-    *dst = t;
-  }
+  const float t = fixed_order_sum(partial + (size_t)g * parts * stride + src, stride, parts, dst != nullptr, sub);
+  if (w == 0 && dst) *dst = t;
 }
 
 }  // namespace
@@ -492,6 +498,8 @@ template <> struct Names<1> {
   static constexpr const char* bwd_b = "k_gru_rows_bwd_b";
   static constexpr const char* bwd_c = "k_gru_rows_bwd_c";
   static constexpr const char* kpack = "k_gru_rows_pack";
+  static constexpr const char* wgrad = "stmp_gru_rows_wgrad";
+  static constexpr const char* wgrad_reduce = "k_gru_rows_wgrad_reduce";
 };
 template <> struct Names<2> {
   static constexpr const char* pack = "stmp_gru_wide_rows_pack_weights";
@@ -503,6 +511,8 @@ template <> struct Names<2> {
   static constexpr const char* bwd_b = "k_gru_wide_rows_bwd_b";
   static constexpr const char* bwd_c = "k_gru_wide_rows_bwd_c";
   static constexpr const char* kpack = "k_gru_wide_rows_pack";
+  static constexpr const char* wgrad = "stmp_gru_wide_rows_wgrad";
+  static constexpr const char* wgrad_reduce = "k_gru_wide_rows_wgrad_reduce";
 };
 
 template <int NC>
@@ -596,6 +606,52 @@ static int rows_bwd(const stmp_plan* plan, int n_ops, int64_t cin, const float* 
   return STMP_OK;
 }
 
+// the weight-gradient workspace: wgrad_ffma_max_parts() partials of (ld + 1) * 3 CO floats (at 64 wide, one of (ld + 1) * CO per gate)
+template <int NC>
+static int64_t rows_wgrad_workspace_bytes(int n_ops, int64_t cin) {
+  constexpr int CO = Wd<NC>::CO;
+  const int64_t ld = ((n_ops + 1) * (cin + CO) + 7) / 8 * 8;
+  return (int64_t)wgrad_ffma_max_parts() * (ld + 1) * 3 * CO * 4;
+}
+
+// Exact fp32: per-CTA FFMA partials over strided row tiles, then a fixed-order sum into the packed layout dw [3 CO][nb], db [3 CO].  The
+// 32-wide cell contracts with train.cu's k_dcrnn_wgrad<32> (16-row tiles), the 64-wide one with k_gru_wide_rows_wgrad (32-row tiles, one
+// partial per gate and CTA).
+template <int NC>
+static int rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr, const float* dph,
+                      void* workspace, float* dw, float* db, void* stream) {
+  using N = Names<NC>;
+  constexpr int CO = Wd<NC>::CO;
+  STMP_REQUIRE(S1 && S2 && dpzr && dph && workspace && dw && rows >= 0, STMP_EINVAL, "%s: bad argument", N::wgrad);
+  STMP_REQUIRE(n_ops >= 0 && n_ops <= 1 && cin >= 1 && cin <= kMaxCin, STMP_EUNSUPPORTED, "%s: n_ops <= 1, cin 1..16 only", N::wgrad);
+  const int nb = (n_ops + 1) * ((int)cin + CO);
+  STMP_REQUIRE(ld == (nb + 7) / 8 * 8, STMP_ESHAPE, "%s: the basis row pitch must be (n_ops+1)(cin+%d) rounded up to 8", N::wgrad, CO);
+  STMP_REQUIRE((((uintptr_t)S1 | (uintptr_t)S2 | (uintptr_t)dpzr | (uintptr_t)dph | (uintptr_t)workspace) & 15u) == 0, STMP_ESHAPE,
+               "%s: S1, S2, dpzr, dph and the workspace must be 16-byte aligned", N::wgrad);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rows == 0) {
+    STMP_CUDA_OK(cudaMemsetAsync(dw, 0, (size_t)3 * CO * nb * 4, st));
+    if (db) STMP_CUDA_OK(cudaMemsetAsync(db, 0, (size_t)3 * CO * 4, st));
+    return STMP_OK;
+  }
+  float* partial = reinterpret_cast<float*>(workspace);
+  const int reduce_grid = (3 * CO * nb + 3 * CO + 31) / 32;
+  if constexpr (NC == 1) {
+    int parts = 0;
+    const int rc = wgrad_ffma_launch(CO, rows, (int)ld, S1, S2, dpzr, dph, partial, st, &parts);
+    if (rc != STMP_OK) return rc;
+    k_gru_rows_wgrad_reduce<<<reduce_grid, 256, 0, st>>>(parts, (int)ld / 8, nb, partial, dw, db);
+  } else {
+    const long long tiles = (rows + kWgRows - 1) / kWgRows, max_parts = wgrad_ffma_max_parts();
+    const int parts = (int)(tiles < max_parts ? tiles : max_parts);
+    k_gru_wide_rows_wgrad<<<dim3(parts, 3), kWgThreads, 0, st>>>(rows, (int)ld, S1, S2, dpzr, dph, partial);
+    STMP_LAUNCH_OK("k_gru_wide_rows_wgrad");
+    k_gru_wide_rows_wgrad_reduce<<<reduce_grid, 256, 0, st>>>(parts, (int)ld, nb, partial, dw, db);
+  }
+  STMP_LAUNCH_OK(N::wgrad_reduce);
+  return STMP_OK;
+}
+
 extern "C" int stmp_gru_rows_pack_weights(int n_ops, int64_t cin, const float* wx, const float* wh, const float* bx, const float* bh,
                                           float* w, float* b, void* stream) {
   return pack_weights<1>(n_ops, cin, wx, wh, bx, bh, w, b, stream);
@@ -613,6 +669,13 @@ extern "C" int64_t stmp_gru_rows_scratch_bytes(const stmp_plan* plan) {
 extern "C" int stmp_gru_rows_bwd(const stmp_plan* plan, int n_ops, int64_t cin, const float* gout, const float* h, const float* stash,
                                  const float* w, float* scratch, float* dph, float* dpzr, float* dx, float* dh, void* stream) {
   return rows_bwd<1>(plan, n_ops, cin, gout, h, stash, w, scratch, dph, dpzr, dx, dh, stream);
+}
+
+extern "C" int64_t stmp_gru_rows_wgrad_workspace_bytes(int n_ops, int64_t cin) { return rows_wgrad_workspace_bytes<1>(n_ops, cin); }
+
+extern "C" int stmp_gru_rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
+                                   const float* dph, void* workspace, float* dw, float* db, void* stream) {
+  return rows_wgrad<1>(n_ops, cin, rows, ld, S1, S2, dpzr, dph, workspace, dw, db, stream);
 }
 
 extern "C" int stmp_gru_wide_rows_pack_weights(int n_ops, int64_t cin, const float* wx, const float* wh, const float* bx, const float* bh,
@@ -634,40 +697,9 @@ extern "C" int stmp_gru_wide_rows_bwd(const stmp_plan* plan, int n_ops, int64_t 
   return rows_bwd<2>(plan, n_ops, cin, gout, h, stash, w, scratch, dph, dpzr, dx, dh, stream);
 }
 
-static int wide_wgrad_parts() {
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return 2 * sms;
-}
+extern "C" int64_t stmp_gru_wide_rows_wgrad_workspace_bytes(int n_ops, int64_t cin) { return rows_wgrad_workspace_bytes<2>(n_ops, cin); }
 
-extern "C" int64_t stmp_gru_wide_rows_wgrad_workspace_bytes(int n_ops, int64_t cin) {
-  const int64_t ld = ((n_ops + 1) * (cin + 64) + 7) / 8 * 8;
-  return (int64_t)3 * wide_wgrad_parts() * (ld * 64 + 64) * 4;
-}
-
-// Exact fp32: per-CTA FFMA partials of each gate's product over strided 32-row tiles (k_gru_wide_rows_wgrad), then a fixed-order sum
-// (k_gru_wide_rows_wgrad_reduce).
 extern "C" int stmp_gru_wide_rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
                                         const float* dph, void* workspace, float* dw, float* db, void* stream) {
-  STMP_REQUIRE(S1 && S2 && dpzr && dph && workspace && dw && rows >= 0, STMP_EINVAL, "stmp_gru_wide_rows_wgrad: bad argument");
-  STMP_REQUIRE(n_ops >= 0 && n_ops <= 1 && cin >= 1 && cin <= kMaxCin, STMP_EUNSUPPORTED, "stmp_gru_wide_rows_wgrad: n_ops <= 1, cin 1..16 only");
-  const int nb = (n_ops + 1) * ((int)cin + 64);
-  STMP_REQUIRE(ld == (nb + 7) / 8 * 8, STMP_ESHAPE, "stmp_gru_wide_rows_wgrad: the basis row pitch must be (n_ops+1)(cin+64) rounded up to 8");
-  STMP_REQUIRE((((uintptr_t)S1 | (uintptr_t)S2 | (uintptr_t)dpzr | (uintptr_t)dph | (uintptr_t)workspace) & 15u) == 0, STMP_ESHAPE,
-               "stmp_gru_wide_rows_wgrad: S1, S2, dpzr, dph and the workspace must be 16-byte aligned");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (rows == 0) {
-    STMP_CUDA_OK(cudaMemsetAsync(dw, 0, (size_t)192 * nb * 4, st));
-    if (db) STMP_CUDA_OK(cudaMemsetAsync(db, 0, (size_t)192 * 4, st));
-    return STMP_OK;
-  }
-  const long long tiles = (rows + kWgRows - 1) / kWgRows;
-  const int parts = (int)(tiles < wide_wgrad_parts() ? tiles : wide_wgrad_parts());
-  float* partial = reinterpret_cast<float*>(workspace);
-  k_gru_wide_rows_wgrad<<<dim3(parts, 3), kWgThreads, 0, st>>>(rows, (int)ld, S1, S2, dpzr, dph, partial);
-  STMP_LAUNCH_OK("k_gru_wide_rows_wgrad");
-  const int total = 192 * nb + 192;
-  k_gru_wide_rows_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(parts, (int)ld, nb, partial, dw, db);
-  STMP_LAUNCH_OK("k_gru_wide_rows_wgrad_reduce");
-  return STMP_OK;
+  return rows_wgrad<2>(n_ops, cin, rows, ld, S1, S2, dpzr, dph, workspace, dw, db, stream);
 }

@@ -223,10 +223,9 @@ __global__ void k_lstm_rows_pack(int nops, int cin, const float* __restrict__ wx
   }
 }
 
-// Fixed-order sums of the per-CTA partials into dw [128][nb] (the packed layout), db [128] and dpeep [96] (both nullable).  The weight
-// partials are k_dcrnn_wgrad<64>'s: S^T [dpi | dpf] (m*64 + row), then S^T [dpc | dpo], then the column sums of dpre; the peephole
-// partials are k_lstm_rows_bwd_a's.  A block covers 32 outputs; its 8 warps each sum a contiguous eighth of the partials and thread (0, x)
-// adds the 8 sub-sums in warp order, as k_dcrnn_wgrad_reduce does.
+// Fixed-order sums (fixed_order_sum, rows.cuh) of the per-CTA partials into dw [128][nb] (the packed layout), db [128] and dpeep [96]
+// (both nullable).  The weight partials are k_dcrnn_wgrad<64>'s: S^T [dpi | dpf] (m*64 + row), then S^T [dpc | dpo], then the column sums
+// of dpre; the peephole partials are k_lstm_rows_bwd_a's, with their own base, stride and count.
 __global__ void __launch_bounds__(256) k_lstm_rows_wgrad_reduce(int parts, int MG, int nb, const float* __restrict__ partial, int pparts,
                                                                 const float* __restrict__ pp, float* __restrict__ dw, float* __restrict__ db,
                                                                 float* __restrict__ dpeep) {
@@ -253,24 +252,8 @@ __global__ void __launch_bounds__(256) k_lstm_rows_wgrad_reduce(int parts, int M
     n = pparts;
     dst = dpeep ? dpeep + src : nullptr;
   }
-  const int per = (n + 7) / 8, q0 = w * per, q1 = (q0 + per < n) ? q0 + per : n;
-  float s0 = 0.f, s1 = 0.f;
-  if (dst) {
-    int q = q0;
-    for (; q + 2 <= q1; q += 2) {
-      s0 += base[(size_t)q * stride + src];
-      s1 += base[(size_t)(q + 1) * stride + src];
-    }
-    if (q < q1) s0 += base[(size_t)q * stride + src];
-  }
-  sub[w][x] = s0 + s1;
-  __syncthreads();
-  if (w == 0 && dst) {
-    float t = sub[0][x];
-#pragma unroll
-    for (int k = 1; k < 8; ++k) t += sub[k][x];
-    *dst = t;
-  }
+  const float t = fixed_order_sum(base + src, stride, n, dst != nullptr, sub);
+  if (w == 0 && dst) *dst = t;
 }
 
 }  // namespace

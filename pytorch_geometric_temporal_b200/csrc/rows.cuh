@@ -1,5 +1,7 @@
 // rows.cuh -- the pieces shared by the row-split recurrent cells (gru_rows.cu, lstm_rows.cu): one warp per destination row, lane = output
 // channel (lane + 32 j for j < NC in gru_rows.cu's 64-wide instance), CTAs owning grid-strided tiles of kRowTile rows, weights staged once per CTA at pitch kWPitch, and the entry-order CSR gather.
+// Also the weight-gradient pieces of train.cu, gru_rows.cu and lstm_rows.cu: the FFMA contraction's launch, the part count of every
+// weight-gradient contraction, and the fixed-order sum every reduce kernel adds the partials with.
 #pragma once
 #include "common.cuh"
 
@@ -89,6 +91,35 @@ inline bool al4(const void* p) { return ((uintptr_t)p & 3u) == 0; }
 // S1^T A (A: rows x 64) and S2^T B (B: rows x N2, N2 = 32 or 64) and the column sums of A and B, over strided 16-row tiles.
 int wgrad_ffma_launch(int n2, long long rows, int ld, const float* S1, const float* S2, const float* A, const float* B, float* partial,
                       cudaStream_t st, int* parts);
+// 2 x SMs: the most partials any weight-gradient contraction writes (per gate in gru_rows.cu's 64-wide one), which sizes every workspace
 int wgrad_ffma_max_parts();
+
+// The sum of p[q * stride] over the n parts q < n in the one fixed association every weight-gradient reduce kernel uses: warp w of the
+// 256-thread block adds the contiguous parts [w per, (w + 1) per), per = ceil(n / 8), in two interleaved accumulators (the odd tail into
+// the first), and the 8 warp sums are added in warp order.  The association depends on n alone, never on the launch, so the gradients are
+// bit-reproducible.  Lane x of each warp sums its own output in column x of `sub`; a thread with nothing to sum passes live = false.
+// It holds a __syncthreads, so every thread of the block must call it.  The result is valid in warp 0 only.
+__device__ __forceinline__ float fixed_order_sum(const float* p, size_t stride, int n, bool live, float (&sub)[8][32]) {
+  const int x = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int per = (n + 7) / 8, q0 = w * per, q1 = (q0 + per < n) ? q0 + per : n;
+  float s0 = 0.f, s1 = 0.f;
+  if (live) {
+    int q = q0;
+    for (; q + 2 <= q1; q += 2) {
+      s0 += p[(size_t)q * stride];
+      s1 += p[(size_t)(q + 1) * stride];
+    }
+    if (q < q1) s0 += p[(size_t)q * stride];
+  }
+  sub[w][x] = s0 + s1;
+  __syncthreads();
+  float t = 0.f;
+  if (w == 0) {
+    t = sub[0][x];
+#pragma unroll
+    for (int k = 1; k < 8; ++k) t += sub[k][x];
+  }
+  return t;
+}
 
 }  // namespace stmp

@@ -129,9 +129,8 @@ __global__ void __launch_bounds__(kWgThreads, 2) k_dcrnn_wgrad(WgradParams p) {
   }
 }
 
-// Sum the partials in a fixed order and scatter: gate weights W (2, 2, C, Co) <- stacked rows (block 0 -> W[0,0] and W[1,0]; block 1 + o -> W[o,1]).
-// A block covers 32 consecutive outputs; its 8 warps each sum a contiguous eighth of the partials, then thread (0, x) adds the 8 sub-sums
-// in warp order -- the same association whatever the launch, hence bit-reproducible.
+// Sum the partials in a fixed order (fixed_order_sum, rows.cuh; a block covers 32 consecutive outputs) and scatter: gate weights
+// W (2, 2, C, Co) <- stacked rows (block 0 -> W[0,0] and W[1,0]; block 1 + o -> W[o,1]).
 __global__ void __launch_bounds__(256) k_dcrnn_wgrad_reduce(int parts, int MG, int C, const float* __restrict__ partial, float* __restrict__ gz,
                                                             float* __restrict__ gr, float* __restrict__ gh, float* __restrict__ gbz,
                                                             float* __restrict__ gbr, float* __restrict__ gbh) {
@@ -154,24 +153,8 @@ __global__ void __launch_bounds__(256) k_dcrnn_wgrad_reduce(int parts, int MG, i
     float* base = b < kCo ? gbz : (b < 2 * kCo ? gbr : gbh);
     dst = base ? base + (b & (kCo - 1)) : nullptr;
   }
-  const int per = (parts + 7) / 8, q0 = w * per, q1 = (q0 + per < parts) ? q0 + per : parts;
-  float s0 = 0.f, s1 = 0.f;
-  if (dst) {
-    int q = q0;
-    for (; q + 2 <= q1; q += 2) {
-      s0 += partial[(size_t)q * stride + src];
-      s1 += partial[(size_t)(q + 1) * stride + src];
-    }
-    if (q < q1) s0 += partial[(size_t)q * stride + src];
-  }
-  sub[w][x] = s0 + s1;
-  __syncthreads();
-  if (w == 0 && dst) {
-    float t = sub[0][x];
-#pragma unroll
-    for (int k = 1; k < 8; ++k) t += sub[k][x];
-    *dst = t;
-  }
+  const float t = fixed_order_sum(partial + src, stride, parts, dst != nullptr, sub);
+  if (w == 0 && dst) *dst = t;
 }
 
 // The same fixed-order sum for the generic graph-GRU (bases [U | Op_0 U | ..] of nb = n_ops + 1 blocks), scattered straight into the layout
@@ -199,63 +182,8 @@ __global__ void __launch_bounds__(256) k_gru_wgrad_reduce(int parts, int MG, int
     src = (size_t)MG * 8 * 3 * kCo + b;
     dst = dbcat ? dbcat + b : nullptr;
   }
-  const int per = (parts + 7) / 8, q0 = w * per, q1 = (q0 + per < parts) ? q0 + per : parts;
-  float s0 = 0.f, s1 = 0.f;
-  if (dst && !zero) {
-    int q = q0;
-    for (; q + 2 <= q1; q += 2) {
-      s0 += partial[(size_t)q * stride + src];
-      s1 += partial[(size_t)(q + 1) * stride + src];
-    }
-    if (q < q1) s0 += partial[(size_t)q * stride + src];
-  }
-  sub[w][x] = s0 + s1;
-  __syncthreads();
-  if (w == 0 && dst) {
-    float t = sub[0][x];
-#pragma unroll
-    for (int k = 1; k < 8; ++k) t += sub[k][x];
-    *dst = zero ? 0.f : t;
-  }
-}
-
-// The same fixed-order sum for the row-split graph-GRU cell (gru_rows.cu), scattered into its packed layout dw [96][nb] (row gate*32 + o,
-// column m of the basis [X | H | Op X | Op H]) and db [96] (nullable).
-__global__ void __launch_bounds__(256) k_gru_rows_wgrad_reduce(int parts, int MG, int nb, const float* __restrict__ partial,
-                                                               float* __restrict__ dw, float* __restrict__ db) {
-  __shared__ float sub[8][32];
-  const int x = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int i = blockIdx.x * 32 + x;
-  const size_t stride = (size_t)MG * 8 * 3 * kCo + 3 * kCo;
-  size_t src = 0;
-  float* dst = nullptr;
-  if (i < 96 * nb) {
-    const int row = i / nb, m = i - row * nb, gate = row >> 5, o = row & 31;
-    src = gate == 2 ? (size_t)MG * 8 * 2 * kCo + (size_t)m * kCo + o : (size_t)m * 2 * kCo + gate * kCo + o;
-    dst = dw + i;
-  } else if (i < 96 * nb + 3 * kCo) {
-    const int b = i - 96 * nb;                                   // bias sums are stored z | r | h
-    src = (size_t)MG * 8 * 3 * kCo + b;
-    dst = db ? db + b : nullptr;
-  }
-  const int per = (parts + 7) / 8, q0 = w * per, q1 = (q0 + per < parts) ? q0 + per : parts;
-  float s0 = 0.f, s1 = 0.f;
-  if (dst) {
-    int q = q0;
-    for (; q + 2 <= q1; q += 2) {
-      s0 += partial[(size_t)q * stride + src];
-      s1 += partial[(size_t)(q + 1) * stride + src];
-    }
-    if (q < q1) s0 += partial[(size_t)q * stride + src];
-  }
-  sub[w][x] = s0 + s1;
-  __syncthreads();
-  if (w == 0 && dst) {
-    float t = sub[0][x];
-#pragma unroll
-    for (int k = 1; k < 8; ++k) t += sub[k][x];
-    *dst = t;
-  }
+  const float t = fixed_order_sum(partial + src, stride, parts, dst && !zero, sub);
+  if (w == 0 && dst) *dst = zero ? 0.f : t;
 }
 
 // ---- Adam over one flat buffer -------------------------------------------------------------------------------------------------
@@ -293,15 +221,9 @@ __global__ void __launch_bounds__(256) k_adam_flat(long long n, float* __restric
 
 using namespace stmp;
 
-static int wgrad_grid() {
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return 2 * sms;
-}
-
 extern "C" int64_t stmp_dcrnn_bwd_wgrad_workspace_bytes(int64_t cin) {
   const int64_t MG = (3 * (cin + kCo) + 7) / 8;
-  return (int64_t)wgrad_grid() * (MG * 8 * 3 * kCo + 3 * kCo) * 4;
+  return (int64_t)wgrad_ffma_max_parts() * (MG * 8 * 3 * kCo + 3 * kCo) * 4;
 }
 
 extern "C" int stmp_dcrnn_bwd_wgrad(int64_t cin, int64_t cout, int64_t K, int64_t rows, int64_t ld, const float* S1, const float* S2,
@@ -322,30 +244,20 @@ extern "C" int stmp_dcrnn_bwd_wgrad(int64_t cin, int64_t cout, int64_t K, int64_
     if (gbh) STMP_CUDA_OK(cudaMemsetAsync(gbh, 0, kCo * 4, st));
     return STMP_OK;
   }
-  WgradParams p;
-  p.S1 = S1; p.S2 = S2; p.dpzr = dpzr; p.dph = dph; p.rows = rows; p.ld = (int)ld; p.MG = MG;
-  p.n_tiles = (int)((rows + kWgTK - 1) / kWgTK);
-  p.partial = reinterpret_cast<float*>(workspace);
-  int grid = wgrad_grid();
-  if (g_wgrad_tc) {
-    const int rc = wgrad_tc_launch(3 * (int)(cin + kCo), rows, (int)ld, S1, S2, dpzr, dph, p.partial, grid, st, &grid);
-    if (rc != STMP_OK) return rc;
-  } else {
-    if (p.n_tiles < grid) grid = p.n_tiles > 0 ? p.n_tiles : 1;
-    const int smem = kWgStages * kWgTK * (2 * (int)ld + 3 * kCo) * 4 + 64;
-    STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_wgrad<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    k_dcrnn_wgrad<32><<<grid, kWgThreads, smem, st>>>(p);
-    STMP_LAUNCH_OK("k_dcrnn_wgrad");
-  }
+  float* partial = reinterpret_cast<float*>(workspace);
+  int parts = 0;
+  const int rc = g_wgrad_tc ? wgrad_tc_launch(3 * C, rows, (int)ld, S1, S2, dpzr, dph, partial, wgrad_ffma_max_parts(), st, &parts)
+                            : wgrad_ffma_launch(kCo, rows, (int)ld, S1, S2, dpzr, dph, partial, st, &parts);
+  if (rc != STMP_OK) return rc;
   const int total = 3 * 4 * C * kCo + 3 * kCo;
-  k_dcrnn_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(grid, MG, C, p.partial, gz, gr, gh, gbz, gbr, gbh);
+  k_dcrnn_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(parts, MG, C, partial, gz, gr, gh, gbz, gbr, gbh);
   STMP_LAUNCH_OK("k_dcrnn_wgrad_reduce");
   return STMP_OK;
 }
 
 extern "C" int64_t stmp_gru_bwd_wgrad_workspace_bytes(int n_ops, int64_t cin) {
   const int64_t MG = ((n_ops + 1) * (cin + kCo) + 7) / 8;
-  return (int64_t)wgrad_grid() * (MG * 8 * 3 * kCo + 3 * kCo) * 4;
+  return (int64_t)wgrad_ffma_max_parts() * (MG * 8 * 3 * kCo + 3 * kCo) * 4;
 }
 
 extern "C" int stmp_gru_bwd_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
@@ -361,53 +273,21 @@ extern "C" int stmp_gru_bwd_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t 
     return STMP_OK;
   }
   float* partial = reinterpret_cast<float*>(workspace);
-  int grid = wgrad_grid();
-  const int rc = wgrad_tc_launch(C3, rows, (int)ld, S1, S2, dpzr, dph, partial, grid, st, &grid);
+  int parts = 0;
+  const int rc = wgrad_tc_launch(C3, rows, (int)ld, S1, S2, dpzr, dph, partial, wgrad_ffma_max_parts(), st, &parts);
   if (rc != STMP_OK) return rc;
   const int total = 96 * 112 + 3 * kCo;
-  k_gru_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(grid, MG, (int)cin, n_ops + 1, partial, dwcat, dbcat);
+  k_gru_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(parts, MG, (int)cin, n_ops + 1, partial, dwcat, dbcat);
   STMP_LAUNCH_OK("k_gru_wgrad_reduce");
   return STMP_OK;
 }
 
-extern "C" int64_t stmp_gru_rows_wgrad_workspace_bytes(int n_ops, int64_t cin) {
-  const int64_t MG = ((n_ops + 1) * (cin + kCo) + 7) / 8;
-  return (int64_t)wgrad_grid() * (MG * 8 * 3 * kCo + 3 * kCo) * 4;
-}
-
-// Exact fp32: the FFMA contraction k_dcrnn_wgrad (per-CTA partials over strided 16-row tiles) and k_gru_rows_wgrad_reduce.
-extern "C" int stmp_gru_rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr,
-                                   const float* dph, void* workspace, float* dw, float* db, void* stream) {
-  STMP_REQUIRE(S1 && S2 && dpzr && dph && workspace && dw && rows >= 0, STMP_EINVAL, "stmp_gru_rows_wgrad: bad argument");
-  STMP_REQUIRE(n_ops >= 0 && n_ops <= 1 && cin >= 1 && cin <= 16, STMP_EUNSUPPORTED, "stmp_gru_rows_wgrad: n_ops <= 1, cin 1..16 only");
-  const int nb = (n_ops + 1) * ((int)cin + kCo), MG = (nb + 7) / 8;
-  STMP_REQUIRE(ld == 8 * MG, STMP_ESHAPE, "stmp_gru_rows_wgrad: the basis row pitch must be (n_ops+1)(cin+32) rounded up to 8");
-  STMP_REQUIRE((((uintptr_t)S1 | (uintptr_t)S2 | (uintptr_t)dpzr | (uintptr_t)dph | (uintptr_t)workspace) & 15u) == 0, STMP_ESHAPE,
-               "stmp_gru_rows_wgrad: S1, S2, dpzr, dph and the workspace must be 16-byte aligned");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (rows == 0) {
-    STMP_CUDA_OK(cudaMemsetAsync(dw, 0, (size_t)96 * nb * 4, st));
-    if (db) STMP_CUDA_OK(cudaMemsetAsync(db, 0, (size_t)96 * 4, st));
-    return STMP_OK;
-  }
-  WgradParams p;
-  p.S1 = S1; p.S2 = S2; p.dpzr = dpzr; p.dph = dph; p.rows = rows; p.ld = (int)ld; p.MG = MG;
-  p.n_tiles = (int)((rows + kWgTK - 1) / kWgTK);
-  p.partial = reinterpret_cast<float*>(workspace);
-  int grid = wgrad_grid();
-  if (p.n_tiles < grid) grid = p.n_tiles;
-  const int smem = kWgStages * kWgTK * (2 * (int)ld + 3 * kCo) * 4 + 64;
-  STMP_CUDA_OK(cudaFuncSetAttribute(k_dcrnn_wgrad<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  k_dcrnn_wgrad<32><<<grid, kWgThreads, smem, st>>>(p);
-  STMP_LAUNCH_OK("k_dcrnn_wgrad");
-  const int total = 96 * nb + 3 * kCo;
-  k_gru_rows_wgrad_reduce<<<(total + 31) / 32, 256, 0, st>>>(grid, MG, nb, p.partial, dw, db);
-  STMP_LAUNCH_OK("k_gru_rows_wgrad_reduce");
-  return STMP_OK;
-}
-
 namespace stmp {
-int wgrad_ffma_max_parts() { return wgrad_grid(); }
+int wgrad_ffma_max_parts() {
+  int dev = 0, sms = 132;
+  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return 2 * sms;
+}
 
 int wgrad_ffma_launch(int n2, long long rows, int ld, const float* S1, const float* S2, const float* A, const float* B, float* partial,
                       cudaStream_t st, int* parts) {
@@ -415,7 +295,7 @@ int wgrad_ffma_launch(int n2, long long rows, int ld, const float* S1, const flo
   p.S1 = S1; p.S2 = S2; p.dpzr = A; p.dph = B; p.rows = rows; p.ld = ld; p.MG = ld / 8;
   p.n_tiles = (int)((rows + kWgTK - 1) / kWgTK);
   p.partial = partial;
-  int grid = wgrad_grid();
+  int grid = wgrad_ffma_max_parts();
   if (p.n_tiles < grid) grid = p.n_tiles > 0 ? p.n_tiles : 1;
   const int smem = kWgStages * kWgTK * (2 * ld + 2 * kCo + n2) * 4 + 64;
   if (n2 == 64) {

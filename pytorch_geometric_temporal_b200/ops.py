@@ -78,6 +78,7 @@ def spmm(plan: GraphPlan, op: int, x: torch.Tensor, alpha: float = 1.0, z: Optio
 
 
 _SEQ_WS = {}
+_WGRAD_WS = {}
 
 
 def _seq_workspace(plan: GraphPlan, T: int, cin: int, device) -> torch.Tensor:
@@ -89,6 +90,16 @@ def _seq_workspace(plan: GraphPlan, T: int, cin: int, device) -> torch.Tensor:
     if buf is None or buf.numel() < need:
         buf = torch.empty(max(need, 1), dtype=torch.uint8, device=device)
         _SEQ_WS[key] = buf
+    return buf
+
+
+def _wgrad_workspace(device, bytes_entry, *shape) -> torch.Tensor:
+    """Per-(device, stream, entry, shape) workspace of a weight-gradient entry, `bytes_entry(*shape)` bytes (its *_wgrad_workspace_bytes,
+    asked on the first call only) and then reused as it is: launches on one stream are ordered, so consecutive calls may share it."""
+    key = (device, torch.cuda.current_stream(device).cuda_stream, bytes_entry.__name__, *shape)
+    buf = _WGRAD_WS.get(key)
+    if buf is None:
+        buf = _WGRAD_WS[key] = torch.empty(int(bytes_entry(*shape)), device=device, dtype=torch.uint8)
     return buf
 
 
@@ -209,11 +220,7 @@ def gru_bwd_seq(plan: GraphPlan, n_ops: int, cin: int, gout, out, h0, stash, whs
 def gru_bwd_wgrad(n_ops: int, cin: int, S1, S2, dpzr_all, dph_all, has_bias: bool):
     """(dwcat (96, 112), dbcat (96,) or None): gradients of the forward's prepacked weights over all (t, b, n) rows, two launches."""
     dev = S1.device
-    key = (dev, torch.cuda.current_stream(dev).cuda_stream, "gru", n_ops, cin)
-    ws = _WGRAD_WS.get(key)
-    if ws is None:
-        ws = torch.empty(int(_lib.lib().stmp_gru_bwd_wgrad_workspace_bytes(n_ops, cin)), device=dev, dtype=torch.uint8)
-        _WGRAD_WS[key] = ws
+    ws = _wgrad_workspace(dev, _lib.lib().stmp_gru_bwd_wgrad_workspace_bytes, n_ops, cin)
     dwcat = torch.empty(96, 112, device=dev, dtype=torch.float32)
     dbcat = torch.empty(96, device=dev, dtype=torch.float32) if has_bias else None
     with torch.cuda.device(dev):
@@ -368,11 +375,7 @@ def gru_rows_wgrad(n_ops: int, cin: int, S1, S2, dpzr, dph, has_bias: bool):
     dph.size(1)."""
     dev = S1.device
     cout = dph.size(1)
-    key = (dev, torch.cuda.current_stream(dev).cuda_stream, "gru_rows", n_ops, cin, cout)
-    ws = _WGRAD_WS.get(key)
-    if ws is None:
-        ws = torch.empty(int(_gru_rows_entry(cout, "wgrad_workspace_bytes")(n_ops, cin)), device=dev, dtype=torch.uint8)
-        _WGRAD_WS[key] = ws
+    ws = _wgrad_workspace(dev, _gru_rows_entry(cout, "wgrad_workspace_bytes"), n_ops, cin)
     dw = torch.empty(3 * cout, (n_ops + 1) * (cin + cout), device=dev, dtype=torch.float32)
     db = torch.empty(3 * cout, device=dev, dtype=torch.float32) if has_bias else None
     with torch.cuda.device(dev):
@@ -494,11 +497,7 @@ def lstm_rows_wgrad(variant: int, n_ops: int, cin: int, S, dpre, scratch, has_pe
     """(dw (128, nb), dbp (224,)): the packed weights' gradient and, in one vector, the summed biases' gradient dbp[:128] and the
     peepholes' dbp[128:] (left unwritten without peepholes) of the row-split LSTM cell, two launches."""
     dev = S.device
-    key = (dev, torch.cuda.current_stream(dev).cuda_stream, "lstm_rows", variant, n_ops, cin)
-    ws = _WGRAD_WS.get(key)
-    if ws is None:
-        ws = torch.empty(int(_lib.lib().stmp_lstm_rows_wgrad_workspace_bytes(variant, n_ops, cin)), device=dev, dtype=torch.uint8)
-        _WGRAD_WS[key] = ws
+    ws = _wgrad_workspace(dev, _lib.lib().stmp_lstm_rows_wgrad_workspace_bytes, variant, n_ops, cin)
     dw = torch.empty(128, lstm_rows_nb(variant, n_ops, cin), device=dev, dtype=torch.float32)
     dbp = torch.empty(128 + 96, device=dev, dtype=torch.float32)
     dpeep = dbp[128:] if has_peep else None
@@ -951,9 +950,6 @@ def dcrnn_bwd_basis_ld(cin: int, cout: int, K: int) -> int:
     return ((2 * K - 1) * (cin + cout) + 7) // 8 * 8
 
 
-_WGRAD_WS = {}
-
-
 def dcrnn_bwd_wgrad(cin: int, K: int, S1, S2, dpzr_all, dph_all, has_bias: bool):
     """(gz, gr, gh, gbz, gbr, gbh): weight / bias gradients of the three gates over all (t, b, n) rows in two launches
     (`stmp_dcrnn_bwd_wgrad`); S1 / S2 (T*B, N, ld) from dcrnn_bwd_basis with ld = dcrnn_bwd_basis_ld(...)."""
@@ -961,11 +957,7 @@ def dcrnn_bwd_wgrad(cin: int, K: int, S1, S2, dpzr_all, dph_all, has_bias: bool)
     C = cin + Co
     dev = S1.device
     rows = S1.size(0) * S1.size(1)
-    key = (dev, torch.cuda.current_stream(dev).cuda_stream, cin)
-    ws = _WGRAD_WS.get(key)
-    if ws is None:
-        ws = torch.empty(int(_lib.lib().stmp_dcrnn_bwd_wgrad_workspace_bytes(cin)), device=dev, dtype=torch.uint8)
-        _WGRAD_WS[key] = ws
+    ws = _wgrad_workspace(dev, _lib.lib().stmp_dcrnn_bwd_wgrad_workspace_bytes, cin)
     g = torch.empty(3, 2, K, C, Co, device=dev, dtype=torch.float32)
     gb = torch.empty(3, Co, device=dev, dtype=torch.float32) if has_bias else None
     with torch.cuda.device(dev):
