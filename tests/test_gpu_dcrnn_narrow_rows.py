@@ -211,7 +211,12 @@ def test_forward_vs_float64_oracle(case):
     assert _nrows(c) == ch * _fwd_launches(K, T) and c.get("k_spmm", 0) == ch * 2 * (K - 1)
     sd = {k: v.detach() for k, v in m.state_dict().items()}
     with torch.no_grad():
-        ref32 = R.batched_dcrnn(sd, X, ei, ew)
+        if graph.startswith("hub"):
+            # the float32 oracle of a hub graph runs on the CPU, where scatter_add_ sums each row in edge order every time; on the GPU its
+            # atomics pick the order per run, and on a 400-entry hub row that moved e32 enough for one run to measure 9.5x and another 4.6x
+            ref32 = R.batched_dcrnn({k: v.cpu() for k, v in sd.items()}, X.cpu(), ei.cpu(), ew.cpu()).to(DEV)
+        else:
+            ref32 = R.batched_dcrnn(sd, X, ei, ew)
         with _float64():
             ref64 = R.batched_dcrnn({k: v.double() for k, v in sd.items()}, X.double(), ei, ew.double())
     got = out.double()

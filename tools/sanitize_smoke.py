@@ -117,8 +117,11 @@ _lib.set_option("dcrnn_narrow_pack", 2)
 e8 = torch.stack([torch.arange(40), (torch.arange(40) * 7 + 1) % 40]).to(dev)
 nm8 = BatchedDCRNN(4, 4, 3).to(dev)
 _lib.set_option("dcrnn_narrow_pack", 8)
-(nm8(torch.randn(10, 3, 40, 4, device=dev), e8, torch.ones(40, device=dev)) ** 2).sum().backward()   # CP = 8, 8 windows per CTA, tail group
+(nm8(torch.randn(10, 3, 40, 4, device=dev), e8, torch.ones(40, device=dev)) ** 2).sum().backward()   # CP = 8, 8 windows per CTA, tail group, 320 tasks: the backward at 2 per thread
 _lib.set_option("dcrnn_narrow_pack", 0)
+with torch.no_grad():
+    r600 = torch.arange(600, device=dev)
+    nm8(torch.randn(2, 3, 600, 4, device=dev), torch.stack([r600, (r600 * 7 + 1) % 600]), torch.ones(600, device=dev))   # CP = 8, 4 tasks per thread
 x = torch.randn(2, 2000, 64, device=dev, requires_grad=True)
 h, c = lstm(x, eg, wg)
 (h.sum() + c.sum()).backward()                                   # _LstmCellFn backward: k_gemm_split, k_lstm_gate_bwd, transposed SpMM
