@@ -440,7 +440,8 @@ int stmp_dcrnn_wide_rows_bwd(const stmp_plan* plan, int64_t B, int64_t T, int64_
  *                                fp32 FFMA per-CTA partials + a fixed-order sum (two launches); workspace of
  *                                stmp_lstm_rows_wgrad_workspace_bytes(variant, n_ops, cin) bytes, 16-byte aligned.
  * STMP_EINVAL for NULL tensors or an unknown variant, STMP_ESHAPE for a bad pitch or alignment, STMP_EUNSUPPORTED for cin > 16,
- * n_ops > 1, cout != 32 or n_ops above the plan's operators. */
+ * n_ops > 1, cout != 32 or n_ops above the plan's operators.  stmp_lstm_rows_supported also answers 1 for cout = 64 (the
+ * stmp_lstm_wide_rows_* entries below). */
 enum stmp_lstm_basis { STMP_LSTM_GCONV = 0, STMP_LSTM_GC = 1 };
 int stmp_lstm_rows_supported(const stmp_plan* plan, int variant, int n_ops, int64_t cin, int64_t cout);
 int stmp_lstm_rows_pack_weights(int variant, int n_ops, int64_t cin, const float* wx, const float* wh, const float* bx, const float* bh,
@@ -455,6 +456,35 @@ int stmp_lstm_rows_bwd(const stmp_plan* plan, int variant, int n_ops, int64_t ci
 int64_t stmp_lstm_rows_wgrad_workspace_bytes(int variant, int n_ops, int64_t cin);
 int stmp_lstm_rows_wgrad(int variant, int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S, const float* dpre,
                          const float* scratch, void* workspace, float* dw, float* db, float* dpeep, void* stream);
+
+/* ---- the same cell at 64 hidden channels (lstm_rows.cu, the width-2 instance of its kernels): GConvLSTM / GCLSTM(cin, 64, K <= 2).
+ * Envelope: cout = 64, cin 1..16, n_ops 0..1 and at most the plan's operators (stmp_lstm_rows_supported(plan, variant, n_ops, cin, 64)),
+ * any number of nodes and any degree.  Same argument lists, launch chain and guarantees as the stmp_lstm_rows_* entries, with 32 -> 64
+ * throughout:
+ *   packed weights w [256][nb]: row gate*64 + o, column m of the basis; nb = (n_ops+1)(cin+64) (GConvLSTM) or cin + 64(n_ops+1) (GCLSTM);
+ *                                     b [256]; peep (3, 64) or NULL.
+ *   stmp_lstm_wide_rows_pack_weights: wx [4][n_ops+1][64][cin] (GCLSTM: [4][cin][64]), wh [4][n_ops+1][64][64], bx / bh / bg [4][64].
+ *   stmp_lstm_wide_rows_fwd:          x (N,cin), h and c (N,64) or NULL -> hout, cout (N,64); stash (4,N,64); S (N, ld), ld = nb
+ *                                     rounded up to 8, 16-byte aligned.
+ *   stmp_lstm_wide_rows_bwd:          gh, gc (N,64) -> dpre (2,N,128) = [dpi | dpf], [dpc | dpo], dx (N,cin), dh (N,64), dc (N,64);
+ *                                     scratch of stmp_lstm_wide_rows_scratch_bytes(plan) bytes (N*80 floats + 192 per CTA).
+ *   stmp_lstm_wide_rows_wgrad:        dw [256][nb], db [256], dpeep [192] (db, dpeep nullable): fp32 FFMA per-CTA partials of each gate's
+ *                                     product over strided 32-row tiles + a fixed-order sum (two launches); workspace of
+ *                                     stmp_lstm_wide_rows_wgrad_workspace_bytes(variant, n_ops, cin) bytes, 16-byte aligned operands.
+ * STMP_EINVAL for NULL tensors or an unknown variant, STMP_ESHAPE for a bad pitch or alignment, STMP_EUNSUPPORTED for cin > 16,
+ * n_ops > 1 or n_ops above the plan's operators. */
+int stmp_lstm_wide_rows_pack_weights(int variant, int n_ops, int64_t cin, const float* wx, const float* wh, const float* bx,
+                                     const float* bh, const float* bg, float* w, float* b, void* stream);
+int stmp_lstm_wide_rows_fwd(const stmp_plan* plan, int variant, int n_ops, int64_t cin, const float* x, const float* h, const float* c,
+                            const float* w, const float* b, const float* peep, float* hout, float* cout, float* stash, float* S,
+                            int64_t ld, void* stream);
+int64_t stmp_lstm_wide_rows_scratch_bytes(const stmp_plan* plan);
+int stmp_lstm_wide_rows_bwd(const stmp_plan* plan, int variant, int n_ops, int64_t cin, const float* gh, const float* gc, const float* c,
+                            const float* cn, const float* stash, const float* w, const float* peep, float* scratch, float* dpre,
+                            float* dx, float* dh, float* dc, void* stream);
+int64_t stmp_lstm_wide_rows_wgrad_workspace_bytes(int variant, int n_ops, int64_t cin);
+int stmp_lstm_wide_rows_wgrad(int variant, int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S, const float* dpre,
+                              const float* scratch, void* workspace, float* dw, float* db, float* dpeep, void* stream);
 
 /* ---- backward of the fused DCRNN sequence for narrow states (cout <= 4): the reference's training model BatchedDCRNN(F, F, K=3) ----
  * Served when stmp_dcrnn_narrow_bwd_supported(plan, cin, cout, K) != 0 (DCONV plan, cin and cout in 1..4, K in 1..4, graph and state

@@ -106,6 +106,12 @@ _SIGNATURES = {
     "stmp_lstm_rows_bwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 13),
     "stmp_lstm_rows_wgrad_workspace_bytes": (c_int64, [c_int, c_int, c_int64]),
     "stmp_lstm_rows_wgrad": (c_int, [c_int, c_int, c_int64, c_int64, c_int64] + [_P] * 8),
+    "stmp_lstm_wide_rows_pack_weights": (c_int, [c_int, c_int, c_int64] + [_P] * 8),
+    "stmp_lstm_wide_rows_fwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 10 + [c_int64, _P]),
+    "stmp_lstm_wide_rows_scratch_bytes": (c_int64, [_P]),
+    "stmp_lstm_wide_rows_bwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 13),
+    "stmp_lstm_wide_rows_wgrad_workspace_bytes": (c_int64, [c_int, c_int, c_int64]),
+    "stmp_lstm_wide_rows_wgrad": (c_int, [c_int, c_int, c_int64, c_int64, c_int64] + [_P] * 8),
     "stmp_tgcn_attn_bwd_workspace_bytes":(c_int64, [_P, c_int64]),
     "stmp_tgcn_attn_bwd": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "stmp_tgcn_cell_bwd_workspace_bytes": (c_int64, [_P, c_int64]),

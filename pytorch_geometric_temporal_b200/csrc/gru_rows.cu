@@ -16,7 +16,7 @@
 // Gathers walk the plan's CSR rows in entry order with separate multiply and add, as stmp_spmm does.  No atomics anywhere; every result
 // depends on its row alone, so repeated calls are bit-identical.  The 64-wide instance (stmp_gru_wide_rows_*) keeps the per-launch staging of
 // the 32-wide one: at the graph sizes the cell serves, a step has fewer 16-row tiles than the H100 has SMs, so the one CTA per SM that
-// 123 KB of staged weights allows costs nothing there; its weight gradients come from k_gru_wide_rows_wgrad below.
+// 123 KB of staged weights allows costs nothing there; its weight gradients come from k_wide_rows_wgrad<3> (rows.cuh).
 #include "rows.cuh"
 
 namespace stmp {
@@ -353,77 +353,6 @@ __global__ void k_gru_rows_pack(int nops, int cin, const float* __restrict__ wx,
   }
 }
 
-// ---- weight gradients of the 64-wide cell ---------------------------------------------------------------------------------------------
-// Per-CTA partials of one gate's product over strided tiles of kWgRows rows: blockIdx.y = gate g, S = S1 (z, r) or S2 (h), A = the gate's
-// 64 columns of dpzr (pitch 128) or dph (pitch 64); partial [g][part][ld*64 + 64] = S^T A and the column sums of A.  Thread (mg, ng) owns
-// the 8 x 8 register tile of basis columns 8 mg.. and gate channels 8 ng..; a second launch sums the partials in a fixed order.
-constexpr int kWgRows = 32, kWgThreads = 160;            // 8 * ceil(160 / 8) tiles: the widest basis, n_ops = 1 and cin = 16
-
-__global__ void __launch_bounds__(kWgThreads, 1) k_gru_wide_rows_wgrad(long long rows, int ld, const float* __restrict__ S1,
-                                                                    const float* __restrict__ S2, const float* __restrict__ dpzr,
-                                                                    const float* __restrict__ dph, float* __restrict__ partial) {
-  __shared__ __align__(16) float ss[kWgRows * 160];
-  __shared__ __align__(16) float sa[kWgRows * 64];
-  const int g = blockIdx.y, tid = threadIdx.x, MG = ld / 8;
-  const float* S = g == 2 ? S2 : S1;
-  const float* A = g == 2 ? dph : dpzr + 64 * g;
-  const int apitch = g == 2 ? 64 : 128;
-  const bool active = tid < 8 * MG;
-  const int mg = tid >> 3, ng = tid & 7;
-  float acc[8][8], cs[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    cs[i] = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-  }
-  const long long n_tiles = (rows + kWgRows - 1) / kWgRows;
-  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const long long r0 = tile * kWgRows;
-    const int nr = (int)min((long long)kWgRows, rows - r0);
-    for (int e = tid; e < nr * (ld / 4); e += kWgThreads) {
-      const int r = e / (ld / 4), c4 = e - r * (ld / 4);
-      reinterpret_cast<float4*>(ss + r * ld)[c4] = __ldg(reinterpret_cast<const float4*>(S + (r0 + r) * ld) + c4);
-    }
-    for (int e = tid; e < nr * 16; e += kWgThreads) {
-      const int r = e >> 4, c4 = e & 15;
-      reinterpret_cast<float4*>(sa + r * 64)[c4] = __ldg(reinterpret_cast<const float4*>(A + (r0 + r) * apitch) + c4);
-    }
-    __syncthreads();
-    if (active) {
-#pragma unroll 4
-      for (int k = 0; k < nr; ++k) {
-        const float4 a0 = *reinterpret_cast<const float4*>(ss + k * ld + 8 * mg), a1 = *reinterpret_cast<const float4*>(ss + k * ld + 8 * mg + 4);
-        const float4 b0 = *reinterpret_cast<const float4*>(sa + k * 64 + 8 * ng), b1 = *reinterpret_cast<const float4*>(sa + k * 64 + 8 * ng + 4);
-        const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-        const float bv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) acc[i][jj] = fmaf(av[i], bv[jj], acc[i][jj]);
-        if (mg == 0) {
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) cs[jj] += bv[jj];
-        }
-      }
-    }
-    __syncthreads();
-  }
-  if (!active) return;
-  float* out = partial + ((size_t)g * gridDim.x + blockIdx.x) * ((size_t)ld * 64 + 64);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    float4* q = reinterpret_cast<float4*>(out + (size_t)(8 * mg + i) * 64 + 8 * ng);
-    q[0] = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-    q[1] = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
-  }
-  if (mg == 0) {
-    float4* q = reinterpret_cast<float4*>(out + (size_t)ld * 64 + 8 * ng);
-    q[0] = make_float4(cs[0], cs[1], cs[2], cs[3]);
-    q[1] = make_float4(cs[4], cs[5], cs[6], cs[7]);
-  }
-}
-
 // The fixed-order sums (fixed_order_sum, rows.cuh) of the 32-wide cell's k_dcrnn_wgrad<32> partials [part][ld*96 + 96] into its packed
 // layout dw [96][nb] (row gate*32 + o, column m of the basis [X | H | Op X | Op H]) and db [96] (nullable).
 __global__ void __launch_bounds__(256) k_gru_rows_wgrad_reduce(int parts, int MG, int nb, const float* __restrict__ partial,
@@ -444,32 +373,6 @@ __global__ void __launch_bounds__(256) k_gru_rows_wgrad_reduce(int parts, int MG
     dst = db ? db + b : nullptr;
   }
   const float t = fixed_order_sum(partial + src, stride, parts, dst != nullptr, sub);
-  if (w == 0 && dst) *dst = t;
-}
-
-// ... and of the 64-wide cell's k_gru_wide_rows_wgrad partials [gate][part][ld*64 + 64] into dw [192][nb] (row g*64 + o, column m) and
-// db [192] (nullable).
-__global__ void __launch_bounds__(256) k_gru_wide_rows_wgrad_reduce(int parts, int ld, int nb, const float* __restrict__ partial,
-                                                                    float* __restrict__ dw, float* __restrict__ db) {
-  __shared__ float sub[8][32];
-  const int x = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int i = blockIdx.x * 32 + x;
-  const size_t stride = (size_t)ld * 64 + 64;
-  size_t src = 0;
-  float* dst = nullptr;
-  int g = 0;
-  if (i < 192 * nb) {
-    const int row = i / nb, m = i - row * nb, o = row & 63;
-    g = row >> 6;
-    src = (size_t)m * 64 + o;
-    dst = dw + i;
-  } else if (i < 192 * nb + 192) {
-    const int r = i - 192 * nb;
-    g = r >> 6;
-    src = (size_t)ld * 64 + (r & 63);
-    dst = db ? db + r : nullptr;
-  }
-  const float t = fixed_order_sum(partial + (size_t)g * parts * stride + src, stride, parts, dst != nullptr, sub);
   if (w == 0 && dst) *dst = t;
 }
 
@@ -615,8 +518,8 @@ static int64_t rows_wgrad_workspace_bytes(int n_ops, int64_t cin) {
 }
 
 // Exact fp32: per-CTA FFMA partials over strided row tiles, then a fixed-order sum into the packed layout dw [3 CO][nb], db [3 CO].  The
-// 32-wide cell contracts with train.cu's k_dcrnn_wgrad<32> (16-row tiles), the 64-wide one with k_gru_wide_rows_wgrad (32-row tiles, one
-// partial per gate and CTA).
+// 32-wide cell contracts with train.cu's k_dcrnn_wgrad<32> (16-row tiles), the 64-wide one with k_wide_rows_wgrad<3> (rows.cuh; 32-row tiles,
+// one partial per gate and CTA).
 template <int NC>
 static int rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S1, const float* S2, const float* dpzr, const float* dph,
                       void* workspace, float* dw, float* db, void* stream) {
@@ -642,11 +545,11 @@ static int rows_wgrad(int n_ops, int64_t cin, int64_t rows, int64_t ld, const fl
     if (rc != STMP_OK) return rc;
     k_gru_rows_wgrad_reduce<<<reduce_grid, 256, 0, st>>>(parts, (int)ld / 8, nb, partial, dw, db);
   } else {
-    const long long tiles = (rows + kWgRows - 1) / kWgRows, max_parts = wgrad_ffma_max_parts();
-    const int parts = (int)(tiles < max_parts ? tiles : max_parts);
-    k_gru_wide_rows_wgrad<<<dim3(parts, 3), kWgThreads, 0, st>>>(rows, (int)ld, S1, S2, dpzr, dph, partial);
+    const int parts = wide_wgrad_parts(rows);
+    const WideWgradOps<3> op = {{S1, S1, S2}, {dpzr, dpzr + CO, dph}, {2 * CO, 2 * CO, CO}};
+    k_wide_rows_wgrad<3><<<dim3(parts, 3), kWideWgThreads, 0, st>>>(rows, (int)ld, op, partial);
     STMP_LAUNCH_OK("k_gru_wide_rows_wgrad");
-    k_gru_wide_rows_wgrad_reduce<<<reduce_grid, 256, 0, st>>>(parts, (int)ld, nb, partial, dw, db);
+    k_wide_rows_wgrad_reduce<3><<<reduce_grid, 256, 0, st>>>(parts, (int)ld, nb, partial, 0, 0, nullptr, dw, db, nullptr);
   }
   STMP_LAUNCH_OK(N::wgrad_reduce);
   return STMP_OK;

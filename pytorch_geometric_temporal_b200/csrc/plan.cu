@@ -37,7 +37,7 @@ int g_wgrad_tc = 1;
 int g_narrow_pack = 0;
 
 // ---- per-kernel launch counters (stmp_path_counters) ----------------------------------------------------
-constexpr int kMaxPaths = 128;
+constexpr int kMaxPaths = 256;  // more than the library's distinct launch names: past the last slot, names would share one counter
 static const char* g_path_names[kMaxPaths];
 static std::atomic<long long> g_path_counts[kMaxPaths];
 static std::atomic<int> g_n_paths{0};

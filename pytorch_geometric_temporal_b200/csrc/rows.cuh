@@ -1,7 +1,8 @@
 // rows.cuh -- the pieces shared by the row-split recurrent cells (gru_rows.cu, lstm_rows.cu): one warp per destination row, lane = output
-// channel (lane + 32 j for j < NC in gru_rows.cu's 64-wide instance), CTAs owning grid-strided tiles of kRowTile rows, weights staged once per CTA at pitch kWPitch, and the entry-order CSR gather.
+// channel (lane + 32 j for j < NC in the 64-wide instances), CTAs owning grid-strided tiles of kRowTile rows, weights staged once per CTA at pitch kWPitch, and the entry-order CSR gather.
 // Also the weight-gradient pieces of train.cu, gru_rows.cu and lstm_rows.cu: the FFMA contraction's launch, the part count of every
-// weight-gradient contraction, and the fixed-order sum every reduce kernel adds the partials with.
+// weight-gradient contraction, the fixed-order sum every reduce kernel adds the partials with, and the per-gate contraction and reduce of
+// the 64-wide cells.
 #pragma once
 #include "common.cuh"
 
@@ -120,6 +121,128 @@ __device__ __forceinline__ float fixed_order_sum(const float* p, size_t stride, 
     for (int k = 1; k < 8; ++k) t += sub[k][x];
   }
   return t;
+}
+
+// ---- weight gradients of the 64-wide row-split cells (gru_rows.cu: G = 3 gates, lstm_rows.cu: G = 4) -------------------------------------
+// Per-CTA partials of one gate's product over strided tiles of kWideWgRows rows: blockIdx.y = gate g, partial [g][part][ld*64 + 64] =
+// S_g^T A_g and the column sums of A_g, A_g = the gate's 64 columns of its pre-activation gradient at pitch apitch_g.  Thread (mg, ng) owns
+// the 8 x 8 register tile of basis columns 8 mg.. and gate channels 8 ng..; a second launch sums the partials in a fixed order.
+constexpr int kWideWgRows = 32, kWideMaxLd = 160;          // the widest basis of either cell: 2 (16 + 64) columns
+constexpr int kWideWgThreads = kWideMaxLd;                 // 8 * ceil(kWideMaxLd / 8) tiles
+
+template <int G>
+struct WideWgradOps {
+  const float* S[G];                         // (rows, ld) basis of gate g
+  const float* A[G];                         // (rows, apitch[g]): gate g's 64 columns
+  int apitch[G];
+};
+
+// partials of the contraction over `rows` rows: one per 32-row tile, at most wgrad_ffma_max_parts()
+inline int wide_wgrad_parts(long long rows) {
+  const long long tiles = (rows + kWideWgRows - 1) / kWideWgRows, max_parts = wgrad_ffma_max_parts();
+  return (int)(tiles < max_parts ? tiles : max_parts);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kWideWgThreads, 1) k_wide_rows_wgrad(long long rows, int ld, WideWgradOps<G> op, float* __restrict__ partial) {
+  __shared__ __align__(16) float ss[kWideWgRows * kWideMaxLd];
+  __shared__ __align__(16) float sa[kWideWgRows * 64];
+  const int g = blockIdx.y, tid = threadIdx.x, MG = ld / 8;
+  const float* S = op.S[0];                  // gate g's operands, selected without indexing the parameter arrays (no local copy)
+  const float* A = op.A[0];
+  int apitch = op.apitch[0];
+#pragma unroll
+  for (int k = 1; k < G; ++k)
+    if (g == k) { S = op.S[k]; A = op.A[k]; apitch = op.apitch[k]; }
+  const bool active = tid < 8 * MG;
+  const int mg = tid >> 3, ng = tid & 7;
+  float acc[8][8], cs[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    cs[i] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
+  }
+  const long long n_tiles = (rows + kWideWgRows - 1) / kWideWgRows;
+  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const long long r0 = tile * kWideWgRows;
+    const int nr = (int)min((long long)kWideWgRows, rows - r0);
+    for (int e = tid; e < nr * (ld / 4); e += kWideWgThreads) {
+      const int r = e / (ld / 4), c4 = e - r * (ld / 4);
+      reinterpret_cast<float4*>(ss + r * ld)[c4] = __ldg(reinterpret_cast<const float4*>(S + (r0 + r) * ld) + c4);
+    }
+    for (int e = tid; e < nr * 16; e += kWideWgThreads) {
+      const int r = e >> 4, c4 = e & 15;
+      reinterpret_cast<float4*>(sa + r * 64)[c4] = __ldg(reinterpret_cast<const float4*>(A + (r0 + r) * apitch) + c4);
+    }
+    __syncthreads();
+    if (active) {
+#pragma unroll 4
+      for (int k = 0; k < nr; ++k) {
+        const float4 a0 = *reinterpret_cast<const float4*>(ss + k * ld + 8 * mg), a1 = *reinterpret_cast<const float4*>(ss + k * ld + 8 * mg + 4);
+        const float4 b0 = *reinterpret_cast<const float4*>(sa + k * 64 + 8 * ng), b1 = *reinterpret_cast<const float4*>(sa + k * 64 + 8 * ng + 4);
+        const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+        const float bv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) acc[i][jj] = fmaf(av[i], bv[jj], acc[i][jj]);
+        if (mg == 0) {
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) cs[jj] += bv[jj];
+        }
+      }
+    }
+    __syncthreads();
+  }
+  if (!active) return;
+  float* out = partial + ((size_t)g * gridDim.x + blockIdx.x) * ((size_t)ld * 64 + 64);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    float4* q = reinterpret_cast<float4*>(out + (size_t)(8 * mg + i) * 64 + 8 * ng);
+    q[0] = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+    q[1] = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
+  }
+  if (mg == 0) {
+    float4* q = reinterpret_cast<float4*>(out + (size_t)ld * 64 + 8 * ng);
+    q[0] = make_float4(cs[0], cs[1], cs[2], cs[3]);
+    q[1] = make_float4(cs[4], cs[5], cs[6], cs[7]);
+  }
+}
+
+// The fixed-order sums of k_wide_rows_wgrad<G>'s partials [gate][part][ld*64 + 64] into dw [64 G][nb] (row g*64 + o, column m of the basis)
+// and db [64 G] (nullable), and of `pparts` per-CTA partials pp [pparts][npeep] into dpeep [npeep] (the LSTM's peephole sums; npeep = 0
+// without them, dpeep nullable).
+template <int G>
+__global__ void __launch_bounds__(256) k_wide_rows_wgrad_reduce(int parts, int ld, int nb, const float* __restrict__ partial, int npeep,
+                                                                int pparts, const float* __restrict__ pp, float* __restrict__ dw,
+                                                                float* __restrict__ db, float* __restrict__ dpeep) {
+  constexpr int R = 64 * G;
+  __shared__ float sub[8][32];
+  const int x = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int i = blockIdx.x * 32 + x;
+  const size_t wstride = (size_t)ld * 64 + 64;
+  const float* base = partial;
+  size_t src = 0, stride = wstride;
+  int n = parts;
+  float* dst = nullptr;
+  if (i < R * nb) {
+    const int row = i / nb, m = i - row * nb;
+    src = (size_t)(row >> 6) * parts * wstride + (size_t)m * 64 + (row & 63);
+    dst = dw + i;
+  } else if (i < R * nb + R) {
+    const int r = i - R * nb;
+    src = (size_t)(r >> 6) * parts * wstride + (size_t)ld * 64 + (r & 63);
+    dst = db ? db + r : nullptr;
+  } else if (i < R * nb + R + npeep) {
+    src = i - R * nb - R;
+    base = pp;
+    stride = npeep;
+    n = pparts;
+    dst = dpeep ? dpeep + src : nullptr;
+  }
+  const float t = fixed_order_sum(base + src, stride, n, dst != nullptr, sub);
+  if (w == 0 && dst) *dst = t;
 }
 
 }  // namespace stmp

@@ -9,9 +9,10 @@ S = [X | T_0(H) | .. | T_{K-1}(H)]) and ONE GEMM produces all four gate pre-acti
 is the wgmma kernel with the LSTM gate chain in its epilogue (`stmp_gemm_lstm_f32`, zero peepholes -- GCLSTM has
 none, and its output gate therefore does not depend on the new cell state, gc_lstm.py:139-145).
 
-Inside the row-split envelope (K <= 2, out_channels = 32, in_channels <= 16, 2-D X; any graph) a step is one launch of the row-split
-LSTM cell kernel with the basis [X | H | Op H] and no peepholes, for inference and training alike; training adds its hand-written
-backward (ops.lstm_rows_train)."""
+Inside the row-split envelope (K <= 2, out_channels 32 or 64, in_channels <= 16, 2-D X; any graph) a step is one launch of the
+row-split LSTM cell kernel with the basis [X | H | Op H] and no peepholes, for inference and training alike; training adds its
+hand-written backward (ops.lstm_rows_train).  At 64 channels, inference with in_channels % 4 == 0 on graphs of
+ops.LSTM_WIDE_ROWS_GEMM_NODES nodes or more keeps the SpMM + wgmma route, which is faster there (DESIGN §4o)."""
 import torch
 
 from ... import _lib, ops
@@ -58,8 +59,8 @@ class GCLSTM(torch.nn.Module, ChebPlanMixin):
         return bs
 
     def _rows_packed(self):
-        """(w [128, nb], b [128]) for stmp_lstm_rows_fwd: columns [X | H | Op H] (W_g transposed), b = conv_g.bias + b_g (one pack launch
-        per weight update)."""
+        """(w [4 Co, nb], b [4 Co]) for stmp_lstm_rows_fwd / stmp_lstm_wide_rows_fwd: columns [X | H | Op H] (W_g transposed), b =
+        conv_g.bias + b_g (one pack launch per weight update)."""
         def build():
             convs = [getattr(self, f"conv_{g}") for g in "ifco"]
             wx = torch.stack([getattr(self, f"W_{g}") for g in "ifco"])
@@ -70,34 +71,39 @@ class GCLSTM(torch.nn.Module, ChebPlanMixin):
         return self._rows_pack.get(list(self.parameters()), build)
 
     def _rows_spec(self):
-        """(spec, params) of ops.lstm_rows_train: where each parameter's gradient sits in the packed weight gradient (128, nb) and the bias
-        gradient -- the inverse of `_rows_packed`.  W_g (in, out) receives its block transposed; both biases of a gate get the gate's block."""
+        """(spec, params) of ops.lstm_rows_train: where each parameter's gradient sits in the packed weight gradient (4 Co, nb) and the
+        bias gradient -- the inverse of `_rows_packed`.  W_g (in, out) receives its block transposed; both biases of a gate get the gate's
+        block."""
         spec, params = [], []
-        Ci = self.in_channels
+        Ci, Co = self.in_channels, self.out_channels
         for gi, g in enumerate("ifco"):
             conv = getattr(self, f"conv_{g}")
-            spec.append(("wt", 32 * gi, 32, 0, Ci))
+            spec.append(("wt", Co * gi, Co, 0, Ci))
             params.append(getattr(self, f"W_{g}"))
             for k in range(self.K):
-                spec.append(("w", 32 * gi, 32, Ci + 32 * k, 32))
+                spec.append(("w", Co * gi, Co, Ci + Co * k, Co))
                 params.append(conv.lins[k].weight)
             if conv.bias is not None:
-                spec.append(("b", 32 * gi, 32))
+                spec.append(("b", Co * gi, Co))
                 params.append(conv.bias)
-            spec.append(("b", 32 * gi, 32))
+            spec.append(("b", Co * gi, Co))
             params.append(getattr(self, f"b_{g}"))
         return spec, params
 
     def _rows_ok(self, plan, X, H, C, training):
-        """The row-split route: K <= 2, out_channels = 32, in_channels <= 16, 2-D float32 X, H and C None or (N, 32) float32 (the module's
-        attributes are checked before the library is consulted); training calls also need `fused_training`."""
-        if self.K > 2 or self.out_channels != 32 or self.in_channels > 16 or X.dim() != 2 or X.dtype != torch.float32:
+        """The row-split route: K <= 2, out_channels 32 or 64, in_channels <= 16, 2-D float32 X, H and C None or (N, out_channels) float32
+        (the module's attributes are checked before the library is consulted); training calls also need `fused_training`.  At 64 channels,
+        inference that the SpMM + wgmma route serves stays there on large graphs (ops.lstm_rows_for_no_grad)."""
+        Co = self.out_channels
+        if self.K > 2 or Co not in (32, 64) or self.in_channels > 16 or X.dim() != 2 or X.dtype != torch.float32:
             return False
-        if any(S is not None and (S.shape != (X.size(0), 32) or S.dtype != torch.float32) for S in (H, C)):
+        if any(S is not None and (S.shape != (X.size(0), Co) or S.dtype != torch.float32) for S in (H, C)):
             return False
         if training and not self.fused_training:
             return False
-        return ops.lstm_rows_supported(plan, _lib.LSTM_GC, self.K - 1, self.in_channels, 32)
+        if not training and not ops.lstm_rows_for_no_grad(plan, self.in_channels, Co):
+            return False
+        return ops.lstm_rows_supported(plan, _lib.LSTM_GC, self.K - 1, self.in_channels, Co)
 
     def forward(self, X: torch.FloatTensor, edge_index: torch.LongTensor, edge_weight: torch.FloatTensor = None,
                 H: torch.FloatTensor = None, C: torch.FloatTensor = None, lambda_max: torch.Tensor = None):

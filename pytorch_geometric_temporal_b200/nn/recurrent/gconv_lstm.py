@@ -5,9 +5,11 @@ H, C, lambda_max) -> (H, C)`, state_dict keys `conv_{x,h}_{i,f,c,o}.lins.{k}.wei
 reference = 8(K-1) propagations; here T_k([X|H]) is computed once (K-1 SpMMs on Ci+Co channels) and one
 GEMM produces all four gate pre-activations.
 
-Inside the row-split envelope (K <= 2, out_channels = 32, in_channels <= 16, 2-D X; any graph) a step is one launch of the row-split
-LSTM cell kernel for inference and training alike, and training adds a hand-written backward (ops.lstm_rows_train): the gradients of
-the packed weights are handed to the parameters as blocks, so the cached pack needs no autograd graph."""
+Inside the row-split envelope (K <= 2, out_channels 32 or 64, in_channels <= 16, 2-D X; any graph) a step is one launch of the
+row-split LSTM cell kernel for inference and training alike, and training adds a hand-written backward (ops.lstm_rows_train): the
+gradients of the packed weights are handed to the parameters as blocks, so the cached pack needs no autograd graph.  At 64 channels,
+inference with in_channels % 4 == 0 on graphs of ops.LSTM_WIDE_ROWS_GEMM_NODES nodes or more keeps the SpMM + wgmma route, which is
+faster there (DESIGN §4o)."""
 import torch
 
 from ... import _lib, ops
@@ -162,8 +164,8 @@ class GConvLSTM(torch.nn.Module, ChebPlanMixin):
         return torch.cat([getattr(self, f"conv_x_{g}").bias + getattr(self, f"conv_h_{g}").bias for g in "ifco"])
 
     def _rows_packed(self):
-        """(w [128, nb], b [128], peep [3, 32]) for stmp_lstm_rows_fwd: columns [X | H | Op X | Op H], b = the sum of a gate's three biases
-        (one pack launch per weight update)."""
+        """(w [4 Co, nb], b [4 Co], peep [3, Co]) for stmp_lstm_rows_fwd / stmp_lstm_wide_rows_fwd: columns [X | H | Op X | Op H], b = the
+        sum of a gate's three biases (one pack launch per weight update)."""
         def build():
             cx = [getattr(self, f"conv_x_{g}") for g in "ifco"]
             ch = [getattr(self, f"conv_h_{g}") for g in "ifco"]
@@ -178,35 +180,40 @@ class GConvLSTM(torch.nn.Module, ChebPlanMixin):
         return self._rows_pack.get(list(self.parameters()), build)
 
     def _rows_spec(self):
-        """(spec, params) of ops.lstm_rows_train: where each parameter's gradient sits in the packed weight gradient (128, nb) and the
-        bias | peephole gradient (224,) -- the inverse of `_rows_packed`.  Every bias of a gate receives that gate's block."""
+        """(spec, params) of ops.lstm_rows_train: where each parameter's gradient sits in the packed weight gradient (4 Co, nb) and the
+        bias | peephole gradient (7 Co,) -- the inverse of `_rows_packed`.  Every bias of a gate receives that gate's block."""
         spec, params = [], []
-        Ci, C = self.in_channels, self.in_channels + 32
+        Ci, Co = self.in_channels, self.out_channels
+        C = Ci + Co
         for gi, g in enumerate("ifco"):
             cx, ch = getattr(self, f"conv_x_{g}"), getattr(self, f"conv_h_{g}")
             for k in range(self.K):
-                spec += [("w", 32 * gi, 32, k * C, Ci), ("w", 32 * gi, 32, k * C + Ci, 32)]
+                spec += [("w", Co * gi, Co, k * C, Ci), ("w", Co * gi, Co, k * C + Ci, Co)]
                 params += [cx.lins[k].weight, ch.lins[k].weight]
             if cx.bias is not None:
-                spec += [("b", 32 * gi, 32), ("b", 32 * gi, 32)]
+                spec += [("b", Co * gi, Co), ("b", Co * gi, Co)]
                 params += [cx.bias, ch.bias]
-            spec.append(("b", 32 * gi, 32))
+            spec.append(("b", Co * gi, Co))
             params.append(getattr(self, f"b_{g}"))
         for j, g in enumerate("ifo"):
-            spec.append(("b", 128 + 32 * j, 32))
+            spec.append(("b", 4 * Co + Co * j, Co))
             params.append(getattr(self, f"w_c_{g}"))
         return spec, params
 
     def _rows_ok(self, plan, X, H, C, training):
-        """The row-split route: K <= 2, out_channels = 32, in_channels <= 16, 2-D float32 X, H and C None or (N, 32) float32 (the module's
-        attributes are checked before the library is consulted); training calls also need `fused_training`."""
-        if self.K > 2 or self.out_channels != 32 or self.in_channels > 16 or X.dim() != 2 or X.dtype != torch.float32:
+        """The row-split route: K <= 2, out_channels 32 or 64, in_channels <= 16, 2-D float32 X, H and C None or (N, out_channels) float32
+        (the module's attributes are checked before the library is consulted); training calls also need `fused_training`.  At 64 channels,
+        inference that the SpMM + wgmma route serves stays there on large graphs (ops.lstm_rows_for_no_grad)."""
+        Co = self.out_channels
+        if self.K > 2 or Co not in (32, 64) or self.in_channels > 16 or X.dim() != 2 or X.dtype != torch.float32:
             return False
-        if any(S is not None and (S.shape != (X.size(0), 32) or S.dtype != torch.float32) for S in (H, C)):
+        if any(S is not None and (S.shape != (X.size(0), Co) or S.dtype != torch.float32) for S in (H, C)):
             return False
         if training and not self.fused_training:
             return False
-        return ops.lstm_rows_supported(plan, _lib.LSTM_GCONV, self.K - 1, self.in_channels, 32)
+        if not training and not ops.lstm_rows_for_no_grad(plan, self.in_channels, Co):
+            return False
+        return ops.lstm_rows_supported(plan, _lib.LSTM_GCONV, self.K - 1, self.in_channels, Co)
 
     def forward(self, X: torch.FloatTensor, edge_index: torch.LongTensor, edge_weight: torch.FloatTensor = None,
                 H: torch.FloatTensor = None, C: torch.FloatTensor = None, lambda_max: torch.Tensor = None):

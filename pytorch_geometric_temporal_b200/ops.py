@@ -417,101 +417,127 @@ def gru_rows_train(plan: GraphPlan, n_ops: int, x, h, w, b, spec, params) -> tor
     return _GruRowsFn.apply(plan, n_ops, x, h, w, b, tuple(spec), *params)
 
 
+# GConvLSTM / GCLSTM at 64 hidden channels: from this many nodes on, inference with in_channels % 4 == 0 takes the SpMM + wgmma route
+# (gemm_lstm).  Below it the 64-wide row-split cell's one launch is faster; above it, its 16-row tiles need a second wave of CTAs on an
+# H100 (132 SMs, one CTA per SM) and the wgmma route is faster on the device (DESIGN §4o, tests/perf/bench_lstm64.py).
+LSTM_WIDE_ROWS_GEMM_NODES = 2048
+
+
+def lstm_rows_for_no_grad(plan: GraphPlan, cin: int, cout: int) -> bool:
+    """Whether a `no_grad` call inside the row-split envelope takes the row-split LSTM cell: always at 32 channels; at 64 unless the SpMM
+    + wgmma route serves it (cin % 4 == 0) on a graph of LSTM_WIDE_ROWS_GEMM_NODES nodes or more."""
+    return cout != 64 or cin % 4 != 0 or plan.num_nodes < LSTM_WIDE_ROWS_GEMM_NODES
+
+
 def lstm_rows_supported(plan: GraphPlan, variant: int, n_ops: int, cin: int, cout: int) -> bool:
     return bool(_lib.lib().stmp_lstm_rows_supported(plan.handle, variant, n_ops, cin, cout))
 
 
-def lstm_rows_nb(variant: int, n_ops: int, cin: int) -> int:
-    """Basis columns of the row-split LSTM cell: (n_ops+1)(cin+32) for GConvLSTM ([X | H | Op X | Op H]), cin + 32(n_ops+1) for GCLSTM."""
-    return cin + 32 * (n_ops + 1) if variant == _lib.LSTM_GC else (n_ops + 1) * (cin + 32)
+def lstm_rows_nb(variant: int, n_ops: int, cin: int, cout: int = 32) -> int:
+    """Basis columns of the row-split LSTM cell: (n_ops+1)(cin+cout) for GConvLSTM ([X | H | Op X | Op H]), cin + cout(n_ops+1) for
+    GCLSTM."""
+    return cin + cout * (n_ops + 1) if variant == _lib.LSTM_GC else (n_ops + 1) * (cin + cout)
 
 
-def lstm_rows_basis_ld(variant: int, n_ops: int, cin: int) -> int:
+def lstm_rows_basis_ld(variant: int, n_ops: int, cin: int, cout: int = 32) -> int:
     """Row pitch of the row-split LSTM cell's weight-gradient basis: nb rounded up to 8 floats."""
-    return (lstm_rows_nb(variant, n_ops, cin) + 7) // 8 * 8
+    return (lstm_rows_nb(variant, n_ops, cin, cout) + 7) // 8 * 8
+
+
+def _lstm_rows_entry(cout: int, what: str):
+    """stmp_lstm_rows_<what> at 32 hidden channels, stmp_lstm_wide_rows_<what> at 64; the two families take the same arguments."""
+    if cout not in (32, 64):
+        raise RuntimeError(f"the row-split graph-LSTM cell serves 32 or 64 hidden channels, not {cout}")
+    return getattr(_lib.lib(), ("stmp_lstm_wide_rows_" if cout == 64 else "stmp_lstm_rows_") + what)
 
 
 def lstm_rows_pack_weights(variant: int, n_ops: int, cin: int, wx, wh, bx, bh, bg):
-    """(w (128, nb), b (128,)): the row-split LSTM cell's packed weights from the parameters' layout in one launch
-    (stmp_lstm_rows_pack_weights).  GConvLSTM: wx (4, n_ops+1, 32, cin), wh (4, n_ops+1, 32, 32), bx / bh (4, 32) or None;
-    GCLSTM: wx (4, cin, 32) (the dense W_g), wh as above, bx None, bh (4, 32) or None.  bg (4, 32): the gates' own biases b_g."""
+    """(w (4 cout, nb), b (4 cout,)): the row-split LSTM cell's packed weights from the parameters' layout in one launch
+    (stmp_lstm_rows_pack_weights, or stmp_lstm_wide_rows_pack_weights at cout = 64; cout = wh.size(-1)).  GConvLSTM: wx (4, n_ops+1, cout,
+    cin), wh (4, n_ops+1, cout, cout), bx / bh (4, cout) or None; GCLSTM: wx (4, cin, cout) (the dense W_g), wh as above, bx None, bh
+    (4, cout) or None.  bg (4, cout): the gates' own biases b_g."""
     wx, wh, bg = _f32c(wx, "wx"), _f32c(wh, "wh"), _f32c(bg, "bg")
-    want_x = (4, cin, 32) if variant == _lib.LSTM_GC else (4, n_ops + 1, 32, cin)
-    if wx.shape != want_x or wh.shape != (4, n_ops + 1, 32, 32) or bg.shape != (4, 32):
-        raise RuntimeError(f"lstm_rows_pack_weights: wx must be {want_x}, wh (4, n_ops+1, 32, 32) and bg (4, 32)")
+    cout = wh.size(-1)
+    want_x = (4, cin, cout) if variant == _lib.LSTM_GC else (4, n_ops + 1, cout, cin)
+    if wx.shape != want_x or wh.shape != (4, n_ops + 1, cout, cout) or bg.shape != (4, cout):
+        raise RuntimeError(f"lstm_rows_pack_weights: wx must be {want_x}, wh (4, n_ops+1, {cout}, {cout}) and bg (4, {cout})")
     bx = None if bx is None else _f32c(bx, "bx")
     bh = None if bh is None else _f32c(bh, "bh")
-    w = torch.empty(128, lstm_rows_nb(variant, n_ops, cin), device=wx.device, dtype=torch.float32)
-    b = torch.empty(128, device=wx.device, dtype=torch.float32)
+    w = torch.empty(4 * cout, lstm_rows_nb(variant, n_ops, cin, cout), device=wx.device, dtype=torch.float32)
+    b = torch.empty(4 * cout, device=wx.device, dtype=torch.float32)
     with torch.cuda.device(wx.device):
-        _lib.check(_lib.lib().stmp_lstm_rows_pack_weights(variant, n_ops, cin, _lib.ptr(wx), _lib.ptr(wh), _lib.ptr(bx), _lib.ptr(bh),
+        _lib.check(_lstm_rows_entry(cout, "pack_weights")(variant, n_ops, cin, _lib.ptr(wx), _lib.ptr(wh), _lib.ptr(bx), _lib.ptr(bh),
                                                           _lib.ptr(bg), _lib.ptr(w), _lib.ptr(b), _lib.stream_ptr()))
     return w, b
 
 
 def lstm_rows_fwd(plan: GraphPlan, variant: int, n_ops: int, x: torch.Tensor, h: Optional[torch.Tensor], c: Optional[torch.Tensor],
                   w: torch.Tensor, b: torch.Tensor, peep: Optional[torch.Tensor], train: bool = False):
-    """Row-split peephole graph-LSTM cell (stmp_lstm_rows_fwd) on one graph: x (N, cin), h and c (N, 32) or None (zeros) -> (H', C').
-    peep (3, 32) = w_c_i | w_c_f | w_c_o, or None.  With `train`, returns (H', C', stash (4, N, 32), S) -- the operands of lstm_rows_bwd /
-    lstm_rows_wgrad."""
+    """Row-split peephole graph-LSTM cell (stmp_lstm_rows_fwd, or stmp_lstm_wide_rows_fwd for packed weights of 256 rows) on one graph:
+    x (N, cin), h and c (N, cout) or None (zeros) -> (H', C'), cout = w.size(0) / 4.  peep (3, cout) = w_c_i | w_c_f | w_c_o, or None.
+    With `train`, returns (H', C', stash (4, N, cout), S) -- the operands of lstm_rows_bwd / lstm_rows_wgrad."""
     x, w, b = _f32c(x, "X"), _f32c(w, "w"), _f32c(b, "b")
     N, cin = x.shape
+    co = w.size(0) // 4
     f32 = dict(device=x.device, dtype=torch.float32)
     hc = None if h is None else _f32c(h, "H")
     cc = None if c is None else _f32c(c, "C")
     pc = None if peep is None else _f32c(peep, "peep")
-    hout, cout = torch.empty(N, 32, **f32), torch.empty(N, 32, **f32)
+    hout, cout = torch.empty(N, co, **f32), torch.empty(N, co, **f32)
     st = S = None
-    ld = lstm_rows_basis_ld(variant, n_ops, cin)
+    ld = lstm_rows_basis_ld(variant, n_ops, cin, co)
     if train:
-        st = torch.empty(4, N, 32, **f32)
+        st = torch.empty(4, N, co, **f32)
         S = torch.empty(N, ld, **f32)
     with torch.cuda.device(x.device):
-        _lib.check(_lib.lib().stmp_lstm_rows_fwd(plan.handle, variant, n_ops, cin, _lib.ptr(x), _lib.ptr(hc), _lib.ptr(cc), _lib.ptr(w),
-                                                 _lib.ptr(b), _lib.ptr(pc), _lib.ptr(hout), _lib.ptr(cout), _lib.ptr(st), _lib.ptr(S), ld,
-                                                 _lib.stream_ptr()))
+        _lib.check(_lstm_rows_entry(co, "fwd")(plan.handle, variant, n_ops, cin, _lib.ptr(x), _lib.ptr(hc), _lib.ptr(cc), _lib.ptr(w),
+                                               _lib.ptr(b), _lib.ptr(pc), _lib.ptr(hout), _lib.ptr(cout), _lib.ptr(st), _lib.ptr(S), ld,
+                                               _lib.stream_ptr()))
     return (hout, cout, st, S) if train else (hout, cout)
 
 
 def lstm_rows_bwd(plan: GraphPlan, variant: int, n_ops: int, gh, gc, c, cn, stash, w, peep, want_dx: bool, want_dh: bool, want_dc: bool,
                   cin: int):
-    """(dpre (2, N, 64), dx (N, cin) or None, dh or None, dc or None, scratch) of the row-split LSTM cell (stmp_lstm_rows_bwd); gh / gc
-    may be None.  The scratch carries the per-CTA peephole sums to lstm_rows_wgrad."""
-    N = cn.size(0)
+    """(dpre (2, N, 2 cout), dx (N, cin) or None, dh or None, dc or None, scratch) of the row-split LSTM cell (stmp_lstm_rows_bwd, or
+    stmp_lstm_wide_rows_bwd when cn has 64 channels); gh / gc may be None.  The scratch carries the per-CTA peephole sums to
+    lstm_rows_wgrad."""
+    N, co = cn.shape
     f32 = dict(device=cn.device, dtype=torch.float32)
     gh = None if gh is None else _f32c(gh, "gH")
     gc = None if gc is None else _f32c(gc, "gC")
-    scr = torch.empty(int(_lib.lib().stmp_lstm_rows_scratch_bytes(plan.handle)) // 4, **f32)
-    dpre = torch.empty(2, N, 64, **f32)
+    scr = torch.empty(int(_lstm_rows_entry(co, "scratch_bytes")(plan.handle)) // 4, **f32)
+    dpre = torch.empty(2, N, 2 * co, **f32)
     dx = torch.empty(N, cin, **f32) if want_dx else None
-    dh = torch.empty(N, 32, **f32) if want_dh else None
-    dc = torch.empty(N, 32, **f32) if want_dc else None
+    dh = torch.empty(N, co, **f32) if want_dh else None
+    dc = torch.empty(N, co, **f32) if want_dc else None
     with torch.cuda.device(cn.device):
-        _lib.check(_lib.lib().stmp_lstm_rows_bwd(plan.handle, variant, n_ops, cin, _lib.ptr(gh), _lib.ptr(gc), _lib.ptr(c), _lib.ptr(cn),
-                                                 _lib.ptr(stash), _lib.ptr(w), _lib.ptr(peep), _lib.ptr(scr), _lib.ptr(dpre), _lib.ptr(dx),
-                                                 _lib.ptr(dh), _lib.ptr(dc), _lib.stream_ptr()))
+        _lib.check(_lstm_rows_entry(co, "bwd")(plan.handle, variant, n_ops, cin, _lib.ptr(gh), _lib.ptr(gc), _lib.ptr(c), _lib.ptr(cn),
+                                               _lib.ptr(stash), _lib.ptr(w), _lib.ptr(peep), _lib.ptr(scr), _lib.ptr(dpre), _lib.ptr(dx),
+                                               _lib.ptr(dh), _lib.ptr(dc), _lib.stream_ptr()))
     return dpre, dx, dh, dc, scr
 
 
 def lstm_rows_wgrad(variant: int, n_ops: int, cin: int, S, dpre, scratch, has_peep: bool):
-    """(dw (128, nb), dbp (224,)): the packed weights' gradient and, in one vector, the summed biases' gradient dbp[:128] and the
-    peepholes' dbp[128:] (left unwritten without peepholes) of the row-split LSTM cell, two launches."""
+    """(dw (4 cout, nb), dbp (7 cout,)): the packed weights' gradient and, in one vector, the summed biases' gradient dbp[:4 cout] and the
+    peepholes' dbp[4 cout:] (left unwritten without peepholes) of the row-split LSTM cell, two launches; cout = dpre.size(2) / 2."""
     dev = S.device
-    ws = _wgrad_workspace(dev, _lib.lib().stmp_lstm_rows_wgrad_workspace_bytes, variant, n_ops, cin)
-    dw = torch.empty(128, lstm_rows_nb(variant, n_ops, cin), device=dev, dtype=torch.float32)
-    dbp = torch.empty(128 + 96, device=dev, dtype=torch.float32)
-    dpeep = dbp[128:] if has_peep else None
+    co = dpre.size(2) // 2
+    ws = _wgrad_workspace(dev, _lstm_rows_entry(co, "wgrad_workspace_bytes"), variant, n_ops, cin)
+    dw = torch.empty(4 * co, lstm_rows_nb(variant, n_ops, cin, co), device=dev, dtype=torch.float32)
+    dbp = torch.empty(7 * co, device=dev, dtype=torch.float32)
+    dpeep = dbp[4 * co:] if has_peep else None
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().stmp_lstm_rows_wgrad(variant, n_ops, cin, S.size(0), S.size(1), _lib.ptr(S), _lib.ptr(dpre), _lib.ptr(scratch),
-                                                   _lib.ptr(ws), _lib.ptr(dw), _lib.ptr(dbp), _lib.ptr(dpeep), _lib.stream_ptr()))
+        _lib.check(_lstm_rows_entry(co, "wgrad")(variant, n_ops, cin, S.size(0), S.size(1), _lib.ptr(S), _lib.ptr(dpre), _lib.ptr(scratch),
+                                                 _lib.ptr(ws), _lib.ptr(dw), _lib.ptr(dbp), _lib.ptr(dpeep), _lib.stream_ptr()))
     return dw, dbp
 
 
 class _LstmRowsFn(torch.autograd.Function):
-    """Training form of the row-split peephole graph-LSTM cell.  forward = `stmp_lstm_rows_fwd` with the stash and the weight-gradient basis
+    """Training form of the row-split peephole graph-LSTM cell (32 or 64 hidden channels, from the packed weights).  forward =
+    `stmp_lstm_rows_fwd` (`stmp_lstm_wide_rows_fwd`) with the stash and the weight-gradient basis
     (the inference launch, so (H', C') are bit-identical to the `no_grad` ones); backward = `stmp_lstm_rows_bwd` + `stmp_lstm_rows_wgrad`:
     dX (when x requires grad), dH / dC (when h / c are given and require grad) and the packed weights', summed biases' and peepholes'
-    gradients, handed to `params` as blocks described by `spec` (see _spec_grads; the peepholes sit in the bias vector after its 128
+    gradients, handed to `params` as blocks described by `spec` (see _spec_grads; the peepholes sit in the bias vector after its 4 cout
     entries).  Either output's gradient may be None."""
 
     @staticmethod
@@ -545,7 +571,7 @@ class _LstmRowsFn(torch.autograd.Function):
 
 def lstm_rows_train(plan: GraphPlan, variant: int, n_ops: int, x, h, c, w, b, peep, spec, params):
     """Differentiable (w.r.t. x, h, c and `params`, see _LstmRowsFn) row-split peephole graph-LSTM cell -> (H', C').  x (N, cin); h, c
-    (N, 32) or None (zeros, no state gradient)."""
+    (N, cout) or None (zeros, no state gradient)."""
     return _LstmRowsFn.apply(plan, variant, n_ops, x, h, c, w, b, peep, tuple(spec), *params)
 
 

@@ -164,5 +164,10 @@ with torch.no_grad():
     g64(xw, e17, None)
 for cls in (GConvLSTM, GCLSTM):
     sum(t.square().mean() for t in cls(5, 32, 2).to(dev)(xg, e17, None, hg, torch.randn(17, 32, device=dev, requires_grad=True))).backward()
+    l64 = cls(5, 64, 2).to(dev)                                 # the 64-wide LSTM cell at 17 nodes, H given and not
+    sum(t.square().mean() for t in l64(xw, e17, None, hw, torch.randn(17, 64, device=dev, requires_grad=True))).backward()
+    sum(t.square().mean() for t in l64(xw, e17, None)).backward()
+    with torch.no_grad():
+        l64(xw, e17, None, hw, hw)
 torch.cuda.synchronize()
 print("sanitize_smoke ok:", {k: v for k, v in _lib.path_counters().items() if k.startswith("k_") and v})
