@@ -521,6 +521,23 @@ int stmp_tgcn_cell_bwd(const stmp_plan* plan, int64_t B, int64_t fin, const floa
                        const float* Bm, const float* c, const float* gout, void* workspace, float* dh, float* dA, float* dBm, float* dc,
                        void* stream);
 
+/* The three entries above at out_channels = 64, with the same argument lists and answers: A (fin, 192), Bm (64, 192), c (192) in
+ * columns z | r | h of 64 each; h, out, gout and dh (B, N, 64); dA (fin, 192), dBm (64, 192), dc (192).  The forward stages Bm in shared
+ * memory next to X[b].  stmp_tgcn_wide_cell_bwd writes dH, the per-row gate gradients and the bases [A^X | H], [A^X | H*R] into the
+ * workspace, contracts them with the 64-wide weight-gradient kernels of the row-split GConvGRU cell (fixed-order sums, no atomics) and
+ * unpacks the result into dA and dBm: four launches, deterministic; the workspace (16-byte aligned) grows with B * N. */
+int stmp_tgcn_wide_attn_fwd(const stmp_plan* plan, int64_t B, int64_t fin, int64_t periods, const float* x, const float* h,
+                            int64_t h_bstride, const float* A, const float* Bm, const float* c, const float* probs, float* out,
+                            void* stream);
+int64_t stmp_tgcn_wide_attn_bwd_workspace_bytes(const stmp_plan* plan, int64_t B);
+int stmp_tgcn_wide_attn_bwd(const stmp_plan* plan, int64_t B, int64_t fin, int64_t periods, const float* x, const float* A,
+                            const float* c, const float* probs, const float* gout, void* workspace, float* dA, float* dc,
+                            float* dprobs, void* stream);
+int64_t stmp_tgcn_wide_cell_bwd_workspace_bytes(const stmp_plan* plan, int64_t B);
+int stmp_tgcn_wide_cell_bwd(const stmp_plan* plan, int64_t B, int64_t fin, const float* x, const float* h, int64_t h_bstride,
+                            const float* A, const float* Bm, const float* c, const float* gout, void* workspace, float* dh, float* dA,
+                            float* dBm, float* dc, void* stream);
+
 /* Weight / bias gradients of the three DCRNN gates over all (t, b, n) rows (what autograd accumulates for the `matmul(basis, W)` and
  * `+ bias` of dcrnn.py:86-111 across steps, gates and hops): S1 / S2 (rows, ld) are stmp_dcrnn_bwd_basis' bases (ld = 3(cin+cout) rounded
  * up to 8), dpzr (rows, 2cout) / dph (rows, cout) stmp_dcrnn_bwd_seq's d pre-activations.  Writes gz / gr / gh in the module's

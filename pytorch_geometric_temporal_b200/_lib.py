@@ -116,6 +116,11 @@ _SIGNATURES = {
     "stmp_tgcn_attn_bwd": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "stmp_tgcn_cell_bwd_workspace_bytes": (c_int64, [_P, c_int64]),
     "stmp_tgcn_cell_bwd": (c_int, [_P, c_int64, c_int64, _P, _P, c_int64] + [_P] * 10),
+    "stmp_tgcn_wide_attn_fwd": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, c_int64, _P, _P, _P, _P, _P, _P]),
+    "stmp_tgcn_wide_attn_bwd_workspace_bytes": (c_int64, [_P, c_int64]),
+    "stmp_tgcn_wide_attn_bwd": (c_int, [_P, c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "stmp_tgcn_wide_cell_bwd_workspace_bytes": (c_int64, [_P, c_int64]),
+    "stmp_tgcn_wide_cell_bwd": (c_int, [_P, c_int64, c_int64, _P, _P, c_int64] + [_P] * 10),
     "stmp_dcrnn_bwd_wgrad_workspace_bytes": (c_int64, [c_int64]),
     "stmp_dcrnn_bwd_wgrad": (c_int, [c_int64, c_int64, c_int64, c_int64, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "stmp_adam_flat": (c_int, [c_int64, _P, _P, _P, _P, _P, _P, c_float, c_float, c_float, c_float, c_float, c_float, c_int, _P]),

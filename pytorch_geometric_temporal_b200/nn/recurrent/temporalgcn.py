@@ -71,16 +71,18 @@ class TGCN(torch.nn.Module):
 
     def _packed3(self):
         """The same folding for `stmp_tgcn_attn_fwd` (any graph size):  pre_g = (A^X) A[:, g] + H' Bm[:, g] + c[g]
-        with A = (L1 W)^T (in x out), Bm = L2^T (out x out), c = L1 b + l;  columns z | r | h."""
+        with A = (L1 W)^T (in x out), Bm = L2^T (out x out), c = L1 b + l;  columns z | r | h, each a block of the kernel's width:
+        64 columns at out_channels = 64 (the *_wide_* entries), 32 otherwise."""
         def build():
             Ci, Co, dev = self.in_channels, self.out_channels, self.conv_z.lin.weight.device
-            A = torch.zeros(Ci, 96, device=dev)
-            Bm = torch.zeros(32, 96, device=dev)
-            c = torch.zeros(96, device=dev)
+            w = 64 if Co == 64 else 32
+            A = torch.zeros(Ci, 3 * w, device=dev)
+            Bm = torch.zeros(w, 3 * w, device=dev)
+            c = torch.zeros(3 * w, device=dev)
             for gi, g in enumerate("zrh"):
                 conv, lin = getattr(self, f"conv_{g}"), getattr(self, f"linear_{g}")
                 L1, L2 = lin.weight[:, :Co], lin.weight[:, Co:]
-                r = slice(32 * gi, 32 * gi + Co)
+                r = slice(w * gi, w * gi + Co)
                 A[:, r] = (L1 @ conv.lin.weight).t()
                 Bm[:Co, r] = L2.t()
                 c[r] = L1 @ conv.bias + lin.bias
@@ -104,20 +106,22 @@ class TGCN(torch.nn.Module):
 
     # The fused kernels take the batch rows as the grid's y dimension, so at most 65 535 of them; a larger batch takes the op-for-op path.
     _FUSED_MAX_ROWS = 65535
+    # hidden widths the fused temporal-attention kernels and their backwards serve
+    _ATTN_WIDTHS = (32, 64)
 
     def _attn_train_ok(self, X, H, periods, rows):
         """The fused kernel pair (forward + hand-written backward) trains the configuration of the reference's examples: no incoming state,
-        no gradient w.r.t. X, out_channels == 32, in_channels <= 4, in_channels * periods <= 128, `rows` <= 65 535 batch rows."""
-        return (H is None and torch.is_grad_enabled() and not X.requires_grad and self.out_channels == 32 and self.in_channels <= 4
-                and self.in_channels * periods <= 128 and rows <= self._FUSED_MAX_ROWS and self.fused_training)
+        no gradient w.r.t. X, out_channels 32 or 64, in_channels <= 4, in_channels * periods <= 128, `rows` <= 65 535 batch rows."""
+        return (H is None and torch.is_grad_enabled() and not X.requires_grad and self.out_channels in self._ATTN_WIDTHS
+                and self.in_channels <= 4 and self.in_channels * periods <= 128 and rows <= self._FUSED_MAX_ROWS and self.fused_training)
 
     def _cell_train_ok(self, X, H):
         """The steps after the first of a training loop that carries the state (the reference's BatchedTGCN, tgcn_example.py): the
         same forward launch with H + the hand-written cell backward (dH and the folded-weight gradients).  No gradient w.r.t. X,
-        out_channels == 32, in_channels <= 4, H of shape X.shape[:-1] + (32,), at most 65 535 batch rows."""
-        return (H is not None and torch.is_grad_enabled() and not X.requires_grad and self.out_channels == 32 and self.in_channels <= 4
-                and tuple(H.shape) == tuple(X.shape[:-1]) + (32,) and math.prod(X.shape[:-2]) <= self._FUSED_MAX_ROWS
-                and self.fused_training)
+        out_channels 32 or 64, in_channels <= 4, H of shape X.shape[:-1] + (out_channels,), at most 65 535 batch rows."""
+        return (H is not None and torch.is_grad_enabled() and not X.requires_grad and self.out_channels in self._ATTN_WIDTHS
+                and self.in_channels <= 4 and tuple(H.shape) == tuple(X.shape[:-1]) + (self.out_channels,)
+                and math.prod(X.shape[:-2]) <= self._FUSED_MAX_ROWS and self.fused_training)
 
     fused_training = True     # False: train through autograd over SpMM + cuBLAS (tests compare the two)
 
@@ -128,9 +132,9 @@ class TGCN(torch.nn.Module):
         return not any(t.requires_grad for t in ts)
 
     def _attn_ok(self, X, H, periods, rows, *extra):
-        """The fused temporal-attention + GCN kernel serves inference for out_channels == 32, in_channels <= 4,
+        """The fused temporal-attention + GCN kernel serves inference for out_channels 32 or 64, in_channels <= 4,
         in_channels * periods <= 128 and `rows` <= 65 535 batch rows on graphs of any size."""
-        return (self.out_channels == 32 and self.in_channels <= 4 and self.in_channels * periods <= 128
+        return (self.out_channels in self._ATTN_WIDTHS and self.in_channels <= 4 and self.in_channels * periods <= 128
                 and rows <= self._FUSED_MAX_ROWS and self._no_grad_needed(X, H, *extra))
 
     def _fused_ok(self, plan, X, H):
@@ -160,7 +164,7 @@ class TGCN(torch.nn.Module):
         if self._cell_train_ok(X, H):
             A, Bm, c = self._fold3()
             N, Ci = X.shape[-2], X.shape[-1]
-            out = ops.tgcn_cell_train(plan, X.reshape(-1, N, Ci, 1), H.reshape(-1, N, 32), A, Bm, c)
+            out = ops.tgcn_cell_train(plan, X.reshape(-1, N, Ci, 1), H.reshape(-1, N, self.out_channels), A, Bm, c)
             return out.reshape(*X.shape[:-1], self.out_channels)
         if H is None:
             H = torch.zeros(*X.shape[:-1], self.out_channels, device=X.device, dtype=X.dtype)

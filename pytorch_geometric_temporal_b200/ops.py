@@ -575,60 +575,71 @@ def lstm_rows_train(plan: GraphPlan, variant: int, n_ops: int, x, h, c, w, b, pe
     return _LstmRowsFn.apply(plan, variant, n_ops, x, h, c, w, b, peep, tuple(spec), *params)
 
 
+def _tgcn_entry(co: int, name: str):
+    """The library entry `name` of the fused TGCN kernels at hidden width `co`: stmp_tgcn_<name> at 32, stmp_tgcn_wide_<name> at 64."""
+    if co not in (32, 64):
+        raise RuntimeError(f"the fused TGCN kernels take 32 or 64 hidden channels, got {co}")
+    return getattr(_lib.lib(), ("stmp_tgcn_" if co == 32 else "stmp_tgcn_wide_") + name)
+
+
 def tgcn_attn_fwd(plan: GraphPlan, x: torch.Tensor, A: torch.Tensor, Bm: torch.Tensor, c: torch.Tensor,
                   probs: Optional[torch.Tensor] = None, h: Optional[torch.Tensor] = None, h_shared: bool = False) -> torch.Tensor:
-    """Fused A3TGCN(2) / TGCN(2) forward (stmp_tgcn_attn_fwd).  x (B,N,Fin,P) -> (B,N,32); h (B,N,32), or (N,32) with
-    h_shared=True (the same state for every batch row), or None (zeros)."""
+    """Fused A3TGCN(2) / TGCN(2) forward (stmp_tgcn_attn_fwd at 32 hidden channels, stmp_tgcn_wide_attn_fwd at 64; the width Co is
+    Bm.shape[0]).  x (B,N,Fin,P) -> (B,N,Co); h (B,N,Co), or (N,Co) with h_shared=True (the same state for every batch row), or None
+    (zeros)."""
     x = _f32c(x, "X")
     if x.dim() != 4 or x.size(1) != plan.num_nodes:
         raise RuntimeError(f"X must be (B,{plan.num_nodes},Fin,P), got {tuple(x.shape)}")
     B, N, fin, P = x.shape
     A, Bm, c = _f32c(A, "A"), _f32c(Bm, "Bm"), _f32c(c, "c")
-    if A.shape != (fin, 96) or Bm.shape != (32, 96) or c.numel() != 96:
-        raise RuntimeError("folded weights must be A (Fin,96), Bm (32,96), c (96,)")
-    out = torch.empty((B, N, 32), dtype=torch.float32, device=x.device)
+    co = Bm.shape[0]
+    entry = _tgcn_entry(co, "attn_fwd")
+    if A.shape != (fin, 3 * co) or Bm.shape != (co, 3 * co) or c.numel() != 3 * co:
+        raise RuntimeError(f"folded weights must be A (Fin,{3 * co}), Bm ({co},{3 * co}), c ({3 * co},)")
+    out = torch.empty((B, N, co), dtype=torch.float32, device=x.device)
     if B == 0:
         return out
     hc, hs = None, 0
     if h is not None:
         hc = _f32c(h, "H")
-        hs = 0 if h_shared else N * 32
+        hs = 0 if h_shared else N * co
     pr = None if probs is None else _f32c(probs.detach(), "probs")
     with torch.cuda.device(x.device):
-        _lib.check(_lib.lib().stmp_tgcn_attn_fwd(plan.handle, B, fin, P, _lib.ptr(x), _lib.ptr(hc), hs, _lib.ptr(A), _lib.ptr(Bm),
-                                                 _lib.ptr(c), _lib.ptr(pr), _lib.ptr(out), _lib.stream_ptr()))
+        _lib.check(entry(plan.handle, B, fin, P, _lib.ptr(x), _lib.ptr(hc), hs, _lib.ptr(A), _lib.ptr(Bm), _lib.ptr(c), _lib.ptr(pr),
+                         _lib.ptr(out), _lib.stream_ptr()))
     return out
 
 
 class _TgcnAttnFn(torch.autograd.Function):
     """Training form of the fused A3TGCN(2) / TGCN(2) forward for H = None: forward = `stmp_tgcn_attn_fwd`, backward =
     `stmp_tgcn_attn_bwd` (gates recomputed, gradients of the folded weights A, c and of the attention probabilities reduced on the
-    device).  No gradient w.r.t. X."""
+    device; the *_wide_* entries at 64 hidden channels).  No gradient w.r.t. X."""
 
     @staticmethod
     def forward(ctx, plan, x, A, Bm, c, probs):
         out = tgcn_attn_fwd(plan, x, A.detach(), Bm.detach(), c.detach(), None if probs is None else probs.detach(), None)
-        ctx.plan, ctx.has_probs = plan, probs is not None
+        ctx.plan, ctx.has_probs, ctx.co = plan, probs is not None, Bm.shape[0]
         ctx.save_for_backward(x, A.detach(), c.detach(), probs.detach() if probs is not None else x.new_empty(0))
         return out
 
     @staticmethod
     def backward(ctx, gout):
         x, A, c, probs = ctx.saved_tensors
-        plan = ctx.plan
+        plan, co = ctx.plan, ctx.co
         B, N, fin, P = x.shape
         gout = _f32c(gout, "gout")
         dev = x.device
         if B == 0:                                  # nothing to launch (empty tensors have NULL data pointers)
             return None, None, torch.zeros_like(A), None, torch.zeros_like(c), torch.zeros_like(probs) if ctx.has_probs else None
-        ws = torch.empty(int(_lib.lib().stmp_tgcn_attn_bwd_workspace_bytes(plan.handle, B)), dtype=torch.uint8, device=dev)
-        dA = torch.empty(fin, 96, dtype=torch.float32, device=dev)
-        dc = torch.empty(96, dtype=torch.float32, device=dev)
+        ws = torch.empty(int(_tgcn_entry(co, "attn_bwd_workspace_bytes")(plan.handle, B)), dtype=torch.uint8, device=dev)
+        dA = torch.empty(fin, 3 * co, dtype=torch.float32, device=dev)
+        dc = torch.empty(3 * co, dtype=torch.float32, device=dev)
         dprobs = torch.empty(P, dtype=torch.float32, device=dev) if ctx.has_probs else None
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().stmp_tgcn_attn_bwd(plan.handle, B, fin, P, _lib.ptr(_f32c(x, "X")), _lib.ptr(_f32c(A, "A")), _lib.ptr(_f32c(c, "c")),
-                                                     _lib.ptr(_f32c(probs, "probs")) if ctx.has_probs else None, _lib.ptr(gout), _lib.ptr(ws),
-                                                     _lib.ptr(dA), _lib.ptr(dc), _lib.ptr(dprobs), _lib.stream_ptr()))
+            _lib.check(_tgcn_entry(co, "attn_bwd")(plan.handle, B, fin, P, _lib.ptr(_f32c(x, "X")), _lib.ptr(_f32c(A, "A")),
+                                                   _lib.ptr(_f32c(c, "c")), _lib.ptr(_f32c(probs, "probs")) if ctx.has_probs else None,
+                                                   _lib.ptr(gout), _lib.ptr(ws), _lib.ptr(dA), _lib.ptr(dc), _lib.ptr(dprobs),
+                                                   _lib.stream_ptr()))
         return None, None, dA, None, dc, dprobs
 
 
@@ -640,7 +651,7 @@ def tgcn_attn_train(plan: GraphPlan, x, A, Bm, c, probs=None) -> torch.Tensor:
 class _TgcnCellFn(torch.autograd.Function):
     """Training form of one TGCN / TGCN2 cell step with an incoming state: forward = `stmp_tgcn_attn_fwd` (periods = 1, H given; the
     same launch as inference, so the output is bit-identical to it), backward = `stmp_tgcn_cell_bwd` (gates recomputed; dH and the
-    gradients of the folded weights A, Bm, c).  No gradient w.r.t. X."""
+    gradients of the folded weights A, Bm, c; the *_wide_* entries at 64 hidden channels).  No gradient w.r.t. X."""
 
     @staticmethod
     def forward(ctx, plan, x, h, A, Bm, c):
@@ -654,26 +665,28 @@ class _TgcnCellFn(torch.autograd.Function):
     def backward(ctx, gout):
         x, h, A, Bm, c = ctx.saved_tensors
         B, N, fin = x.shape[:3]
+        co = Bm.shape[0]
         dev = x.device
         want_dh = ctx.needs_input_grad[2]
-        dh = torch.empty(B, N, 32, dtype=torch.float32, device=dev) if want_dh else None
+        dh = torch.empty(B, N, co, dtype=torch.float32, device=dev) if want_dh else None
         if B == 0:                                  # nothing to launch (empty tensors have NULL data pointers)
             return None, None, dh, torch.zeros_like(A), torch.zeros_like(Bm), torch.zeros_like(c)
-        dA = torch.empty(fin, 96, dtype=torch.float32, device=dev)
-        dBm = torch.empty(32, 96, dtype=torch.float32, device=dev)
-        dc = torch.empty(96, dtype=torch.float32, device=dev)
+        dA = torch.empty(fin, 3 * co, dtype=torch.float32, device=dev)
+        dBm = torch.empty(co, 3 * co, dtype=torch.float32, device=dev)
+        dc = torch.empty(3 * co, dtype=torch.float32, device=dev)
         gout = _f32c(gout, "gout")
         handle = ctx.plan.handle
-        ws = torch.empty(int(_lib.lib().stmp_tgcn_cell_bwd_workspace_bytes(handle, B)), dtype=torch.uint8, device=dev)
+        ws = torch.empty(int(_tgcn_entry(co, "cell_bwd_workspace_bytes")(handle, B)), dtype=torch.uint8, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().stmp_tgcn_cell_bwd(handle, B, fin, _lib.ptr(_f32c(x, "X")), _lib.ptr(h), N * 32, _lib.ptr(A),
-                                                     _lib.ptr(Bm), _lib.ptr(c), _lib.ptr(gout), _lib.ptr(ws), _lib.ptr(dh), _lib.ptr(dA),
-                                                     _lib.ptr(dBm), _lib.ptr(dc), _lib.stream_ptr()))
+            _lib.check(_tgcn_entry(co, "cell_bwd")(handle, B, fin, _lib.ptr(_f32c(x, "X")), _lib.ptr(h), N * co, _lib.ptr(A), _lib.ptr(Bm),
+                                                   _lib.ptr(c), _lib.ptr(gout), _lib.ptr(ws), _lib.ptr(dh), _lib.ptr(dA), _lib.ptr(dBm),
+                                                   _lib.ptr(dc), _lib.stream_ptr()))
         return None, None, dh, dA, dBm, dc
 
 
 def tgcn_cell_train(plan: GraphPlan, x, h, A, Bm, c) -> torch.Tensor:
-    """Differentiable (w.r.t. h, A, Bm, c) fused TGCN(2) cell step with an incoming state.  x (B,N,Fin,1), h (B,N,32) -> (B,N,32)."""
+    """Differentiable (w.r.t. h, A, Bm, c) fused TGCN(2) cell step with an incoming state.  x (B,N,Fin,1), h (B,N,Co) -> (B,N,Co),
+    Co = Bm.shape[0] = 32 or 64."""
     return _TgcnCellFn.apply(plan, x, h, A, Bm, c)
 
 

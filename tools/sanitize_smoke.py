@@ -46,7 +46,16 @@ with torch.enable_grad():
     for t in range(3):                                           # TGCN2 training with the state carried: step 0 k_tgcn_attn_bwd,
         h = t2(torch.randn(3, 207, 4, device=dev), ei_t, ew_t, h)   # then k_tgcn_cell_bwd (TMA-staged X, staged Bm) + its reduce
     h.square().mean().backward()
-    for K in (1, 2):                                             # GConvGRU training: stashing forward, k_gru_pack_bwd_weights,
+    for n in (207, 40000):                                       # 64 channels: k_tgcn_wide_attn (Bm staged next to X), k_tgcn_attn_bwd<NQ, 2>,
+        en = torch.randint(0, n, (2, 4 * n), device=dev)         # k_tgcn_wide_cell_bwd + the 64-wide weight-gradient kernels; X staged at
+        a64, t64, h = A3TGCN2(2, 64, 12, 2).to(dev), TGCN2(4, 64, 2).to(dev), None   # 207 nodes, gathered from global memory at 40 000
+        a64(torch.randn(2, n, 2, 12, device=dev), en).square().mean().backward()
+        with torch.no_grad():
+            a64(torch.randn(2, n, 2, 12, device=dev), en, None, torch.randn(2, n, 64, device=dev))
+        for t in range(2):
+            h = t64(torch.randn(2, n, 4, device=dev), en, None, h)
+        h.square().mean().backward()
+    for K in (1, 2):                                           # GConvGRU training: stashing forward, k_gru_pack_bwd_weights,
         gg = GConvGRU(2, 32, K).to(dev)                          # k_gru_bwd_basis, k_gru_bwd_seq (CTA pair), k_dcrnn_wgrad_tc, k_gru_wgrad_reduce
         gg(X[0, 0], ei_t, ew_t, torch.randn(207, 32, device=dev, requires_grad=True)).square().mean().backward()
     ring = torch.arange(301, device=dev)
