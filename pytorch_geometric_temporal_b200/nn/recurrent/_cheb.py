@@ -75,6 +75,17 @@ class ChebPlanMixin:
                                self._lambda_value(lambda_max))
 
 
+def broadcast_states(X: torch.Tensor, states, out_channels: int):
+    """(X, [S, ..]) broadcast to one leading shape, a state None becoming zeros of it: the reference sums conv(X), conv(H) and w_c * C
+    elementwise, so an (N, out) state is shared by every window of a (B, N, F) batch.  The kernels behind the basis buffer walk the
+    rows of X and of every state alike, so each must hold all of them; `broadcast_to` keeps the gradient of a shared state the sum
+    over the batch."""
+    lead = torch.broadcast_shapes(X.shape[:-1], *(S.shape[:-1] for S in states if S is not None))
+    out = [torch.zeros(*lead, out_channels, device=X.device, dtype=X.dtype) if S is None else S.broadcast_to(*lead, out_channels)
+           for S in states]
+    return X.broadcast_to(*lead, X.size(-1)), out
+
+
 def cheb_basis(plan, U: torch.Tensor, K: int):
     """[T_0, .., T_{K-1}](U): T_0=U, T_1=L^U, T_k = 2 L^ T_{k-1} - T_{k-2}."""
     T = [U]

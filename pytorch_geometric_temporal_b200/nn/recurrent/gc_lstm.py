@@ -17,7 +17,7 @@ import torch
 
 from ... import _lib, ops
 from ...plan import _require_cuda
-from ._cheb import ChebParams, ChebPlanMixin, glorot_
+from ._cheb import ChebParams, ChebPlanMixin, broadcast_states, glorot_
 
 
 class GCLSTM(torch.nn.Module, ChebPlanMixin):
@@ -118,10 +118,7 @@ class GCLSTM(torch.nn.Module, ChebPlanMixin):
                 spec, params = self._rows_spec()
                 return ops.lstm_rows_train(plan, _lib.LSTM_GC, K - 1, X, H, C, w, b, None, spec, params)
             return ops.lstm_rows_fwd(plan, _lib.LSTM_GC, K - 1, X, H, C, w, b, None)
-        if H is None:
-            H = torch.zeros(*X.shape[:-1], Co, device=X.device, dtype=X.dtype)
-        if C is None:
-            C = torch.zeros(*X.shape[:-1], Co, device=X.device, dtype=X.dtype)
+        X, (H, C) = broadcast_states(X, (H, C), Co)
         width = Ci + K * Co
         if not needs_grad:
             # the basis is built in place: T_k(H) lands in its column block of S straight from the SpMM kernel

@@ -15,7 +15,7 @@ import torch
 
 from ... import ops
 from ...plan import _require_cuda
-from ._cheb import ChebParams, ChebPlanMixin, cheb_basis
+from ._cheb import ChebParams, ChebPlanMixin, broadcast_states, cheb_basis
 
 
 class GConvGRU(torch.nn.Module, ChebPlanMixin):
@@ -155,6 +155,7 @@ class GConvGRU(torch.nn.Module, ChebPlanMixin):
                 spec, params = self._param_spec(rows=True)
                 return ops.gru_rows_train(plan, K - 1, X, H_given, w, b, spec, params)
             return ops.gru_rows_fwd(plan, K - 1, X, H_given, w, b)
+        X, (H,) = broadcast_states(X, (H,), Co)
         TU = cheb_basis(plan, torch.cat([X, H], dim=-1), K)              # K x (N, Ci+Co)
         S = torch.cat(TU, dim=-1)
         pre = torch.matmul(S, torch.cat([self._gate_weight("z"), self._gate_weight("r")], dim=1))

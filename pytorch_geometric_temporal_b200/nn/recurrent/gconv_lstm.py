@@ -14,7 +14,7 @@ import torch
 
 from ... import _lib, ops
 from ...plan import _require_cuda
-from ._cheb import ChebParams, ChebPlanMixin, cheb_basis, glorot_
+from ._cheb import ChebParams, ChebPlanMixin, broadcast_states, cheb_basis, glorot_
 
 
 def _chunked_tn(A: torch.Tensor, B: torch.Tensor) -> torch.Tensor:
@@ -228,10 +228,7 @@ class GConvLSTM(torch.nn.Module, ChebPlanMixin):
                 spec, params = self._rows_spec()
                 return ops.lstm_rows_train(plan, _lib.LSTM_GCONV, self.K - 1, X, H, C, w, b, peep, spec, params)
             return ops.lstm_rows_fwd(plan, _lib.LSTM_GCONV, self.K - 1, X, H, C, w, b, peep)
-        if H is None:
-            H = torch.zeros(*X.shape[:-1], Co, device=X.device, dtype=X.dtype)
-        if C is None:
-            C = torch.zeros(*X.shape[:-1], Co, device=X.device, dtype=X.dtype)
+        X, (H, C) = broadcast_states(X, (H, C), Co)
         Cw = self.in_channels + Co
         if not needs_grad and Co in (32, 64) and (self.K * Cw) % 4 == 0 and Cw % 4 == 0:
             # large-graph inference: T_k written in place into S = [T_0|T_1|..] by the SpMM kernel, then ONE wgmma

@@ -15,6 +15,14 @@ def _f32c(t: torch.Tensor, name: str) -> torch.Tensor:
     return t.contiguous()
 
 
+def _require_numel(fn: str, n: int, **operands):
+    """Raises unless every operand given (None: absent) holds exactly `n` elements, the count its kernel indexes: the elementwise and
+    epilogue kernels take one row count for all their operands and trust it."""
+    for name, t in operands.items():
+        if t is not None and t.numel() != n:
+            raise RuntimeError(f"{fn}: {name} has {t.numel()} elements, the kernel indexes {n}")
+
+
 def spmm_raw(plan: GraphPlan, op: int, x: torch.Tensor, transposed: bool = False, alpha: float = 1.0,
              z: Optional[torch.Tensor] = None, beta: float = 0.0, att: Optional[torch.Tensor] = None,
              out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -874,9 +882,14 @@ def spmm_attT(plan: GraphPlan, op: int, x: torch.Tensor, attT: torch.Tensor, alp
 
 
 def gemm_lstm(A: torch.Tensor, packed: torch.Tensor, K: int, cout: int, conv_bias, cell, wci, wcf, wco, bi, bf, bc, bo):
-    """(H', C') = peephole-LSTM gates of (A @ W + conv_bias), fused in the GEMM epilogue (stmp_gemm_lstm_f32)."""
-    A, cell = _f32c(A, "A"), _f32c(cell, "C")
+    """(H', C') = peephole-LSTM gates of (A @ W + conv_bias), fused in the GEMM epilogue (stmp_gemm_lstm_f32).  The kernel walks the
+    M = A.numel() / K rows of A, reading and writing one state row per row of A."""
     M = A.numel() // K
+    _require_numel("gemm_lstm", M * K, A=A)
+    _require_numel("gemm_lstm", M * cout, cell=cell)
+    _require_numel("gemm_lstm", 4 * cout, conv_bias=conv_bias)
+    _require_numel("gemm_lstm", cout, wci=wci, wcf=wcf, wco=wco, bi=bi, bf=bf, bc=bc, bo=bo)
+    A, cell = _f32c(A, "A"), _f32c(cell, "C")
     h = torch.empty_like(cell)
     c = torch.empty_like(cell)
     v = [None if t is None else _f32c(t.detach().reshape(-1), "param") for t in (conv_bias, wci, wcf, wco, bi, bf, bc, bo)]
@@ -926,7 +939,8 @@ class PackCache(object):
 
 
 def gru_zr(pz, pr, h):
-    pz, pr, h = _f32c(pz, "pz"), _f32c(pr, "pr"), _f32c(h, "h")
+    _require_numel("gru_zr", pz.numel(), pr=pr, h=h)
+    pz, pr, h =_f32c(pz, "pz"), _f32c(pr, "pr"), _f32c(h, "h")
     z, r, hr = torch.empty_like(pz), torch.empty_like(pz), torch.empty_like(pz)
     with torch.cuda.device(pz.device):
         _lib.check(_lib.lib().stmp_gru_zr(pz.numel(), _lib.ptr(pz), _lib.ptr(pr), _lib.ptr(h), _lib.ptr(z), _lib.ptr(r),
@@ -935,7 +949,8 @@ def gru_zr(pz, pr, h):
 
 
 def gru_out(ph, z, h):
-    ph, z, h = _f32c(ph, "ph"), _f32c(z, "z"), _f32c(h, "h")
+    _require_numel("gru_out", ph.numel(), z=z, h=h)
+    ph, z, h =_f32c(ph, "ph"), _f32c(z, "z"), _f32c(h, "h")
     hn = torch.empty_like(ph)
     with torch.cuda.device(ph.device):
         _lib.check(_lib.lib().stmp_gru_out(ph.numel(), _lib.ptr(ph), _lib.ptr(z), _lib.ptr(h), None, _lib.ptr(hn),
@@ -1326,9 +1341,11 @@ def gru_bwd_zr(cin: int, cout: int, g, hprev, z, r, ht, du2, dpzr):
 
 
 def lstm_ifc(pi, pf, pc, c, wci, wcf, bi, bf, bc):
-    pi, pf, pc, c = (_f32c(t, "gate") for t in (pi, pf, pc, c))
     cout = pi.size(-1)
     rows = pi.numel() // cout
+    _require_numel("lstm_ifc", rows * cout, pf=pf, pc=pc, c=c)
+    _require_numel("lstm_ifc", cout, wci=wci, wcf=wcf, bi=bi, bf=bf, bc=bc)
+    pi, pf, pc, c = (_f32c(t, "gate") for t in (pi, pf, pc, c))
     cn = torch.empty_like(pi)
     v = [_f32c(t.detach().reshape(-1), "param") for t in (wci, wcf, bi, bf, bc)]
     with torch.cuda.device(pi.device):
@@ -1339,9 +1356,11 @@ def lstm_ifc(pi, pf, pc, c, wci, wcf, bi, bf, bc):
 
 
 def lstm_oh(po, cnew, wco, bo):
-    po, cnew = _f32c(po, "po"), _f32c(cnew, "cnew")
     cout = po.size(-1)
     rows = po.numel() // cout
+    _require_numel("lstm_oh", rows * cout, cnew=cnew)
+    _require_numel("lstm_oh", cout, wco=wco, bo=bo)
+    po, cnew = _f32c(po, "po"), _f32c(cnew, "cnew")
     hn = torch.empty_like(po)
     v = [_f32c(t.detach().reshape(-1), "param") for t in (wco, bo)]
     with torch.cuda.device(po.device):
@@ -1352,9 +1371,12 @@ def lstm_oh(po, cnew, wco, bo):
 
 def lstm_gate_bwd(pre, c_old, c_new, gh, gc, wci, wcf, wco, bi, bf, bc, bo):
     """(dpre (rows,4Co), dC_old (rows,Co)) of the peephole-LSTM gate chain (stmp_lstm_gate_bwd); gh / gc may be None."""
-    pre, c_old, c_new = _f32c(pre, "pre"), _f32c(c_old, "c_old"), _f32c(c_new, "c_new")
     cout = c_old.size(-1)
     rows = c_old.numel() // cout
+    _require_numel("lstm_gate_bwd", rows * 4 * cout, pre=pre)
+    _require_numel("lstm_gate_bwd", rows * cout, c_new=c_new, gh=gh, gc=gc)
+    _require_numel("lstm_gate_bwd", cout, wci=wci, wcf=wcf, wco=wco, bi=bi, bf=bf, bc=bc, bo=bo)
+    pre, c_old, c_new = _f32c(pre, "pre"), _f32c(c_old, "c_old"), _f32c(c_new, "c_new")
     dpre = torch.empty_like(pre)
     dco = torch.empty_like(c_old)
     gh = None if gh is None else _f32c(gh, "gh")

@@ -33,7 +33,12 @@ def _install(monkeypatch):
     def gemm_prepack(W):
         return W.clone()                                  # "packed" = the fp32 matrix itself
 
+    def vectors(n, *vs):                                  # per-channel operands: exactly n elements, or absent where the ABI allows it
+        assert all(v is None or v.numel() == n for v in vs), [None if v is None else v.numel() for v in vs]
+
     def gemm(A, packed, K, N, bias=None, out=None):
+        assert A.numel() % K == 0                         # the kernel walks M = A.numel() / K rows
+        vectors(N, bias)
         C = A.reshape(-1, K) @ packed
         if bias is not None:
             C = C + bias
@@ -43,6 +48,10 @@ def _install(monkeypatch):
         return C.reshape(*A.shape[:-1], N)
 
     def gemm_lstm(A, packed, K, cout, cb, cell, wci, wcf, wco, bi, bf, bc, bo):
+        # stmp_gemm_lstm_f32 reads one cell row and writes one H' / C' row per row of A: M = A.numel() / K of each
+        assert A.numel() % K == 0 and cell.numel() == (A.numel() // K) * cout, (tuple(A.shape), K, tuple(cell.shape))
+        vectors(4 * cout, cb)
+        vectors(cout, wci, wcf, wco, bi, bf, bc, bo)
         pre = A @ packed + (0 if cb is None else cb)
         pi, pf, pc, po = (pre[..., j * cout:(j + 1) * cout] for j in range(4))
         I, Fg = torch.sigmoid(pi + wci * cell + bi), torch.sigmoid(pf + wcf * cell + bf)
@@ -51,6 +60,9 @@ def _install(monkeypatch):
 
     def lstm_gate_bwd(pre, c_old, c_new, gh, gc, wci, wcf, wco, bi, bf, bc, bo):
         Co = c_old.size(-1)
+        rows = c_old.numel() // Co                        # stmp_lstm_gate_bwd walks rows x Co elements of every operand
+        assert pre.numel() == rows * 4 * Co and all(t is None or t.numel() == rows * Co for t in (c_new, gh, gc))
+        vectors(Co, wci, wcf, wco, bi, bf, bc, bo)
         pi, pf, pc, po = (pre[:, j * Co:(j + 1) * Co] for j in range(4))
         iv, fv = torch.sigmoid(pi + wci * c_old + bi), torch.sigmoid(pf + wcf * c_old + bf)
         tv, ov, tc = torch.tanh(pc + bc), torch.sigmoid(po + wco * c_new + bo), torch.tanh(c_new)
@@ -119,3 +131,42 @@ def test_lstm_cell_backward_matches_autograd_and_reference(monkeypatch, K, batch
         assert torch.allclose(fx, x.grad, rtol=1e-4, atol=1e-5)
         for k in fp:
             assert torch.allclose(fp[k], p[k].grad, rtol=1e-4, atol=1e-4 * float(p[k].grad.abs().max()) + 1e-6), k
+
+
+@pytest.mark.parametrize("train", [True, False])
+def test_state_shared_across_a_batch_matches_reference(monkeypatch, train):
+    """X (B, N, F) with H, C (N, out): the reference sums conv(X), conv(H) and w_c * C elementwise, so one state serves every window
+    and dH / dC sum over the batch.  Training runs `_LstmCellFn`, a `no_grad` call the fused GEMM + gate epilogue; both must hand the
+    kernels a state row for every row of the basis."""
+    _install(monkeypatch)
+    calls = []
+    gemm_lstm = ops.gemm_lstm
+    monkeypatch.setattr(ops, "gemm_lstm", lambda *a: calls.append(tuple(a[0].shape)) or gemm_lstm(*a))
+    torch.manual_seed(5)
+    n, Ci, Co, K, B = 24, 32, 32, 3, 3
+    ei = torch.stack([torch.randint(0, n, (90,)), torch.randint(0, n, (90,))])
+    ei = torch.unique(ei[:, ei[0] != ei[1]], dim=1)
+    ew = torch.rand(ei.size(1)) + 0.1
+    m = L.GConvLSTM(Ci, Co, K)
+    for p in m.parameters():
+        if p.dim() == 1 or p.size(0) == 1:
+            torch.nn.init.normal_(p, std=0.2)
+    X, H0, C0 = torch.randn(B, n, Ci) * 0.5, torch.randn(n, Co) * 0.5, torch.randn(n, Co) * 0.5
+    wh, wc = torch.randn(B, n, Co), torch.randn(B, n, Co)
+    p = {k: v.detach().clone().requires_grad_(True) for k, v in m.state_dict().items()}
+    leaves = [t.clone().requires_grad_(True) for t in (X, H0, C0)]
+    rh, rc = R.gconv_lstm_cell(p, *leaves[:1], ei, ew, *leaves[1:])
+    assert rh.shape == (B, n, Co)
+    ((rh * wh).sum() + (rc * wc).sum()).backward()
+    got = [t.clone().requires_grad_(train) for t in (X, H0, C0)]
+    with torch.set_grad_enabled(train):
+        h, c = m(got[0], ei, ew, got[1], got[2])
+    assert calls == [(B, n, K * (Ci + Co))], calls                    # one fused GEMM over all B N rows, not the autograd path
+    assert torch.allclose(h, rh, rtol=1e-5, atol=1e-6) and torch.allclose(c, rc, rtol=1e-5, atol=1e-6)
+    if not train:
+        return
+    ((h * wh).sum() + (c * wc).sum()).backward()
+    for name, a, b in zip(("dX", "dH", "dC"), got, leaves):
+        assert a.grad.shape == b.grad.shape and torch.allclose(a.grad, b.grad, rtol=1e-4, atol=1e-5), (name, float((a.grad - b.grad).abs().max()))
+    for k, q in m.named_parameters():
+        assert torch.allclose(q.grad, p[k].grad, rtol=1e-4, atol=1e-4 * float(p[k].grad.abs().max()) + 1e-6), k

@@ -1,7 +1,9 @@
 """Host-side logic of the ChebConv-family modules (weight folding, gate order, shared Chebyshev basis, timestep folding,
 the MSTGCN reshape, autograd through the torch part) checked on the CPU against the committed reference goldens.  The
 two things that need a GPU -- the cached plan and `stmp_spmm` -- are replaced by a dense Laplacian built with the oracle's
-`cheb_norm`; the modules run their autograd (training) code path, which is plain torch around those two calls."""
+`cheb_norm`; the modules run their autograd (training) code path, which is plain torch around those two calls.  For the Chebyshev
+cells' `no_grad` routes the gate kernels (`stmp_gemm_lstm_f32`, `stmp_lstm_ifc` / `_oh`, `stmp_gru_zr` / `_out`) are replaced too, by
+stand-ins that hold every operand to the element count the kernel indexes."""
 import os
 
 import pytest
@@ -35,8 +37,59 @@ def dense_graph_ops(monkeypatch):
         y = alpha * torch.matmul(plan.L, x)
         return y if z is None else y + beta * z
 
+    def spmm_cols(plan, op, buf, src, dst, width, alpha=1.0, z_col=None, beta=0.0, transposed=False):
+        y = alpha * torch.matmul(plan.L, buf[..., src:src + width])
+        buf[..., dst:dst + width] = y if z_col is None else y + beta * buf[..., z_col:z_col + width]
+
+    # The kernels of the `no_grad` routes index flat buffers with one row count for every operand; the stand-ins hold each operand to
+    # exactly the elements the kernel would read or write, and compute on those flat rows.
+    def counts(n, *ts):
+        assert all(t.numel() == n for t in ts), (n, [t.numel() for t in ts])
+
+    def lstm_chain(pre, cell, cout, cb, wci, wcf, wco, bi, bf, bc, bo):
+        v = lambda t: t.reshape(-1)
+        pre = pre if cb is None else pre + v(cb)
+        pi, pf, pc, po = (pre[:, j * cout:(j + 1) * cout] for j in range(4))
+        cn = torch.sigmoid(pf + v(wcf) * cell + v(bf)) * cell + torch.sigmoid(pi + v(wci) * cell + v(bi)) * torch.tanh(pc + v(bc))
+        return torch.sigmoid(po + v(wco) * cn + v(bo)) * torch.tanh(cn), cn
+
+    def gemm_lstm(A, packed, K, cout, cb, cell, wci, wcf, wco, bi, bf, bc, bo):
+        M = A.numel() // K                                          # stmp_gemm_lstm_f32: one cell row per row of A
+        counts(M * K, A)
+        counts(M * cout, cell)
+        counts(cout, wci, wcf, wco, bi, bf, bc, bo)
+        h, c = lstm_chain(A.reshape(M, K) @ packed, cell.reshape(M, cout), cout, cb, wci, wcf, wco, bi, bf, bc, bo)
+        return h.view(cell.shape), c.view(cell.shape)
+
+    def lstm_ifc(pi, pf, pc, c, wci, wcf, bi, bf, bc):
+        cout = pi.size(-1)
+        counts(pi.numel(), pf, pc, c)
+        counts(cout, wci, wcf, bi, bf, bc)
+        flat = [t.reshape(-1, cout) for t in (pi, pf, pc)]
+        pre = torch.cat(flat + [torch.zeros_like(flat[0])], dim=1)
+        zero = torch.zeros(cout)
+        return lstm_chain(pre, c.reshape(-1, cout), cout, None, wci, wcf, zero, bi, bf, bc, zero)[1].view(pi.shape)
+
+    def lstm_oh(po, cnew, wco, bo):
+        cout = po.size(-1)
+        counts(po.numel(), cnew)
+        counts(cout, wco, bo)
+        cn = cnew.reshape(-1, cout)
+        return (torch.sigmoid(po.reshape(-1, cout) + wco.reshape(-1) * cn + bo.reshape(-1)) * torch.tanh(cn)).view(po.shape)
+
+    def gru_zr(pz, pr, h):
+        counts(pz.numel(), pr, h)
+        z, r = torch.sigmoid(pz), torch.sigmoid(pr)
+        return z, r, h.reshape(pz.shape) * r
+
+    def gru_out(ph, z, h):
+        counts(ph.numel(), z, h)
+        return z * h.reshape(ph.shape) + (1 - z) * torch.tanh(ph)
+
     monkeypatch.setattr(cheb_mod.ChebPlanMixin, "_cheb_plan", plan)
-    monkeypatch.setattr(ops, "spmm", spmm)
+    for name, fn in dict(spmm=spmm, spmm_cols=spmm_cols, gemm_prepack=lambda W: W.clone(), gemm_lstm=gemm_lstm, lstm_ifc=lstm_ifc,
+                         lstm_oh=lstm_oh, gru_zr=gru_zr, gru_out=gru_out).items():
+        monkeypatch.setattr(ops, name, fn)
     for m in (gc_mod, gru_mod, lstm_mod):
         monkeypatch.setattr(m, "_require_cuda", lambda *a, **k: None)
     monkeypatch.setattr(GConvGRU, "_fused_ok", lambda self, plan, X, H: False)
@@ -84,6 +137,100 @@ def test_gc_lstm_host_logic_with_gradients(golden_dir, dense_graph_ops):
         for k, p in m.named_parameters():
             _close(p.grad, c["grads"][k], 1e-3, 1e-5)
         _close(x.grad, c["gX"], 1e-3, 1e-5); _close(h.grad, c["gH"], 1e-3, 1e-5); _close(cc.grad, c["gC"], 1e-3, 1e-5)
+
+
+def test_no_grad_routes_host_logic(golden_dir, dense_graph_ops):
+    """The `no_grad` routes of the three cells -- the pointwise gate kernels, and GCLSTM's fused GEMM at 32 channels -- against the same
+    goldens."""
+    with torch.no_grad():
+        g = _load(golden_dir, "gconv_gru_small")
+        for c in g["cases"].values():
+            m = GConvGRU(4, 16, c["K"], normalization=c["normalization"])
+            m.load_state_dict(c["state"])
+            _close(m(c["X"], g["edge_index"], g["edge_weight"], c["H"], c["lambda_max"]), c["out"])
+        g = _load(golden_dir, "gconv_lstm_small")
+        for c in g["cases"].values():
+            m = GConvLSTM(4, 16, c["K"])
+            m.load_state_dict(c["state"])
+            h, cc = m(c["X"], g["edge_index"], g["edge_weight"], c["H"], c["C"])
+            _close(h, c["outH"]); _close(cc, c["outC"])
+        g = _load(golden_dir, "gc_lstm_small")
+        for c in g["cases"].values():                               # (4, 16, K) on the pointwise kernels, (8, 32, 3) on the fused GEMM
+            m = GCLSTM(*c["state"]["W_i"].shape, c["K"], normalization=c["normalization"])
+            m.load_state_dict(c["state"])
+            h, cc = m(c["X"], g["edge_index"], g["edge_weight"], c["H"], c["C"], c["lambda_max"])
+            _close(h, c["outH"]); _close(cc, c["outC"])
+
+
+def _oracle_cell(name, p, X, ei, ew, state):
+    return {"gconv_gru": lambda: [R.gconv_gru_cell(p, X, ei, ew, *state)], "gconv_lstm": lambda: list(R.gconv_lstm_cell(p, X, ei, ew, *state)),
+            "gc_lstm": lambda: list(R.gc_lstm_cell(p, X, ei, ew, *state))}[name]()
+
+
+@pytest.mark.parametrize("train", [False, True])
+@pytest.mark.parametrize("cin,cout,K", [(4, 16, 3), (8, 32, 3)])
+@pytest.mark.parametrize("name", ["gconv_gru", "gconv_lstm", "gc_lstm"])
+def test_state_shared_across_a_batch_matches_reference(dense_graph_ops, name, cin, cout, K, train):
+    """X (B, N, F) with H (and C) of (N, out): the reference broadcasts the state over the batch (its elementwise sums of the convolutions
+    and w_c * C), and its gradient sums over the windows.  `no_grad` runs the fused GEMM + gate epilogue at 32 channels and the pointwise
+    gate kernels at 16; with gradients, the op-for-op path (GConvLSTM's `_LstmCellFn` is pinned in test_gconv_lstm_backward_algebra_cpu)."""
+    B, n = 3, 24
+    torch.manual_seed(cin + cout)
+    ei = torch.stack([torch.randint(0, n, (90,)), torch.randint(0, n, (90,))])
+    ei = torch.unique(ei[:, ei[0] != ei[1]], dim=1)
+    ew = torch.rand(ei.size(1)) + 0.1
+    m = {"gconv_gru": GConvGRU, "gconv_lstm": GConvLSTM, "gc_lstm": GCLSTM}[name](cin, cout, K)
+    m.fused_training = False
+    with torch.no_grad():
+        for k, p in m.named_parameters():
+            if k.endswith("bias") or k.startswith("b_"):
+                p.normal_(0, 0.2)
+    ns = 1 if name == "gconv_gru" else 2
+    X, S = torch.randn(B, n, cin), [0.5 * torch.randn(n, cout) for _ in range(ns)]
+    wgts = [torch.randn(B, n, cout) for _ in range(ns)]
+    p = {k: v.detach().clone().requires_grad_(True) for k, v in m.state_dict().items()}
+    ref_leaves = [t.clone().requires_grad_(True) for t in [X] + S]
+    ref = _oracle_cell(name, p, ref_leaves[0], ei, ew, ref_leaves[1:])
+    assert all(r.shape == (B, n, cout) for r in ref)
+    sum((r * w).sum() for r, w in zip(ref, wgts)).backward()
+    leaves = [t.clone().requires_grad_(train) for t in [X] + S]
+    with torch.set_grad_enabled(train):
+        out = m(leaves[0], ei, ew, *leaves[1:])
+    out = [out] if name == "gconv_gru" else list(out)
+    for o, r in zip(out, ref):
+        _close(o, r.detach(), 1e-5, 1e-6)
+    if not train:
+        return
+    sum((o * w).sum() for o, w in zip(out, wgts)).backward()
+    for label, a, b in zip(["dX", "dH", "dC"], leaves, ref_leaves):
+        assert a.grad.shape == b.grad.shape, label
+        _close(a.grad, b.grad, 1e-4, 1e-5)
+    for k, q in m.named_parameters():
+        _close(q.grad, p[k].grad, 1e-4, 1e-4 * float(p[k].grad.abs().max()) + 1e-6)
+
+
+def test_cell_operand_guards_reject_what_the_kernel_would_overrun():
+    """`ops` checks every operand of the pointwise and epilogue kernels against the rows the kernel walks before it touches the device:
+    a state of N rows beside gates of B N rows is refused, as is a per-channel vector of the wrong width."""
+    rows, Co = 6, 4
+    g, st, v = torch.zeros(rows, Co), torch.zeros(rows // 2, Co), torch.zeros(Co)
+    bad = [lambda: ops.lstm_ifc(g, g, g, st, v, v, v, v, v), lambda: ops.lstm_ifc(g, g, g, g, v, torch.zeros(Co + 1), v, v, v),
+           lambda: ops.lstm_oh(g, st, v, v), lambda: ops.lstm_oh(g, g, v, torch.zeros(1)), lambda: ops.gru_zr(g, g, st),
+           lambda: ops.gru_out(g, st, g), lambda: ops.gru_out(g, g, st),
+           lambda: ops.lstm_gate_bwd(torch.zeros(rows, 4 * Co), g, st, None, None, *[v] * 7),
+           lambda: ops.lstm_gate_bwd(torch.zeros(rows // 2, 4 * Co), g, g, None, None, *[v] * 7),
+           lambda: ops.lstm_gate_bwd(torch.zeros(rows, 4 * Co), g, g, g, st, *[v] * 7),
+           lambda: ops.gemm_lstm(torch.zeros(rows, 8), None, 8, Co, None, st, *[v] * 7),
+           lambda: ops.gemm_lstm(torch.zeros(rows, 8), None, 8, Co, v, g, *[v] * 7),
+           lambda: ops.gemm_lstm(torch.zeros(rows, 8), None, 8, Co, None, g, *[v] * 6, torch.zeros(2 * Co))]
+    for i, call in enumerate(bad):
+        with pytest.raises(RuntimeError, match="elements, the kernel indexes"):
+            call()
+    # operands of the right sizes pass the guard and reach the device check (CPU tensors here)
+    for call in (lambda: ops.lstm_ifc(g, g, g, g, *[v] * 5), lambda: ops.gru_out(g, g, g),
+                 lambda: ops.gemm_lstm(torch.zeros(rows, 8), None, 8, Co, torch.zeros(4 * Co), g, *[v] * 7)):
+        with pytest.raises(RuntimeError, match="CUDA only"):
+            call()
 
 
 def test_stconv_host_logic_with_gradients(golden_dir, dense_graph_ops):

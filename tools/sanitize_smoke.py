@@ -134,6 +134,14 @@ with torch.no_grad():
 x = torch.randn(2, 2000, 64, device=dev, requires_grad=True)
 h, c = lstm(x, eg, wg)
 (h.sum() + c.sum()).backward()                                   # _LstmCellFn backward: k_gemm_split, k_lstm_gate_bwd, transposed SpMM
+# a state of (N, out) shared by a batch of 2 windows (tests/test_gpu_cheb_lstm_envelope.py): the fused GEMM + gate epilogue, the
+# pointwise gates and _LstmCellFn at K = 4, whose adjoint loop runs twice, each with dH / dC summed over the windows
+hs = torch.randn(2000, 32, device=dev, requires_grad=True)
+cs = torch.randn(2000, 32, device=dev, requires_grad=True)
+with torch.no_grad():
+    lstm(torch.randn(2, 2000, 64, device=dev), eg, wg, torch.randn(2000, 64, device=dev), torch.randn(2000, 64, device=dev))
+    GCLSTM(3, 33, 2).to(dev)(torch.randn(2, 2000, 3, device=dev), eg, wg, torch.randn(2000, 33, device=dev), torch.randn(2000, 33, device=dev))
+sum(t.sum() for t in GConvLSTM(32, 32, 4).to(dev)(torch.randn(2, 2000, 32, device=dev, requires_grad=True), eg, wg, hs, cs)).backward()
 # adversarial geometries (tests/test_gpu_graph_geometry.py): a 128-edge row in the second row tile, a backward that reads the global CSR,
 # the FFMA kernel's 7-rows-per-thread mapping
 r129 = torch.arange(129, device=dev)
