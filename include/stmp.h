@@ -53,7 +53,11 @@ enum stmp_flavor {
   STMP_FLAVOR_GCN = 2,
   /* ChebConvAttention.__norm__ (nn/attention/astgcn.py:82-110), propagated on the TRANSPOSED index
    * (:167): dst=row', src=col', E'+2N entries. */
-  STMP_FLAVOR_CHEB_ATT = 3
+  STMP_FLAVOR_CHEB_ATT = 3,
+  /* PyG RGCNConv's mean aggregation (LRGCN, nn/recurrent/lrgcn.py), built by stmp_plan_create_rgcn only: operator k holds the
+   * edges of type rel0 + k in edge order, dst=col, src=row, val = 1/(the destination's count of such edges).  No self loops are
+   * added; duplicates and self loops count as ordinary edges; a node without such an in-edge has an empty row. */
+  STMP_FLAVOR_RGCN = 4
 };
 
 enum stmp_norm { STMP_NORM_NONE = 0, STMP_NORM_SYM = 1, STMP_NORM_RW = 2 };
@@ -83,6 +87,11 @@ int stmp_plan_create(int flavor, int64_t num_nodes, int64_t num_edges, const int
 int stmp_plan_create_pergraph(int flavor, int64_t num_nodes, int64_t num_edges, const int64_t* edge_index,
                               const float* edge_weight, int normalization, const float* lambda_node, uint32_t flags,
                               void* stream, stmp_plan** out);
+/* Relation-masked mean operators (STMP_FLAVOR_RGCN) of relations rel0 .. rel0 + n_rel - 1 (n_rel 1 or 2): edge_type is a device
+ * int64 [E]; a type outside that range matches no operator.  edge_index is validated as stmp_plan_create validates it (STMP_EGRAPH).
+ * More relations take ceil(R / 2) plans.  Setup path: synchronises `stream` once per relation and once to read validation flags. */
+int stmp_plan_create_rgcn(int64_t num_nodes, int64_t num_edges, const int64_t* edge_index, const int64_t* edge_type, int64_t rel0,
+                          int n_rel, void* stream, stmp_plan** out);
 void stmp_plan_destroy(stmp_plan* plan);
 
 /* Introspection (tests, bit-exact index parity): number of operators, nodes, entries of operator `op`. */
@@ -456,6 +465,20 @@ int stmp_lstm_rows_bwd(const stmp_plan* plan, int variant, int n_ops, int64_t ci
 int64_t stmp_lstm_rows_wgrad_workspace_bytes(int variant, int n_ops, int64_t cin);
 int stmp_lstm_rows_wgrad(int variant, int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S, const float* dpre,
                          const float* scratch, void* workspace, float* dw, float* db, float* dpeep, void* stream);
+
+/* ---- the two-operator GConvLSTM basis at 32 channels (LRGCN with two relations, nn/recurrent/lrgcn.py): n_ops = 2 on a plan with two
+ * operators (STMP_FLAVOR_RGCN), basis [X | H | Op0 X | Op0 H | Op1 X | Op1 H], nb = 3 (cin + 32) <= 144.  The two operators are two
+ * independent one-hop products (one per relation), not Chebyshev order 2: ChebConv plans hold one operator, so K = 3 never reaches it.
+ * stmp_lstm_rows_supported answers 1 for (STMP_LSTM_GCONV, n_ops = 2, cin 1..16, cout = 32) on such a plan, 0 at cout = 64.
+ * stmp_lstm_rows_pack_weights, _fwd, _scratch_bytes and _bwd take n_ops = 2 with the layouts above, wx [4][3][32][cin], wh [4][3][32][32]
+ * (block k + 1 = operator k); the backward's gather covers both operators in one launch.  Its weight gradient has its own entry:
+ *   stmp_lstm_rows_wgrad2: dw [128][nb] = dpre^T S and db [128] = 1^T dpre (db nullable; no peepholes) for the basis S (rows, ld),
+ *                          ld = nb rounded up to 8: fp32 FFMA per-CTA partials of the two 64-row halves [dpi | dpf], [dpc | dpo] + a
+ *                          fixed-order sum (two launches); workspace of stmp_lstm_rows_wgrad2_workspace_bytes(cin) bytes, 16-byte aligned
+ *                          S, dpre and workspace.  STMP_EUNSUPPORTED for cin outside 1..16. */
+int64_t stmp_lstm_rows_wgrad2_workspace_bytes(int64_t cin);
+int stmp_lstm_rows_wgrad2(int64_t cin, int64_t rows, int64_t ld, const float* S, const float* dpre, void* workspace, float* dw, float* db,
+                          void* stream);
 
 /* ---- the same cell at 64 hidden channels (lstm_rows.cu, the width-2 instance of its kernels): GConvLSTM / GCLSTM(cin, 64, K <= 2).
  * Envelope: cout = 64, cin 1..16, n_ops 0..1 and at most the plan's operators (stmp_lstm_rows_supported(plan, variant, n_ops, cin, 64)),

@@ -23,12 +23,14 @@ namespace {
 
 using namespace rows;
 
-// per-width constants: out channels, gate rows of the packed weights (i | f | c | o), the widest basis (GConvLSTM, n_ops = 1, cin = 16), the
-// staged weight pitch, basis columns per lane, the backward scratch row (the operator block of dS: Op X columns for GConvLSTM, then Op H)
-// and the peephole sums (w_c_i | w_c_f | w_c_o)
-template <int NC>
+// per-width constants: out channels, gate rows of the packed weights (i | f | c | o), the widest basis (GConvLSTM with NO operators,
+// cin = 16), the staged weight pitch, basis columns per lane, the backward scratch row (the operator blocks of dS: per operator Op X
+// columns for GConvLSTM, then Op H) and the peephole sums (w_c_i | w_c_f | w_c_o).  NO = 2 is the two-operator GConvLSTM basis of LRGCN's
+// two relations, served at 32 channels only (DESIGN §4q).
+template <int NC, int NO = 1>
 struct LWd {
-  static constexpr int CO = 32 * NC, G = 4 * CO, NB = 2 * (kMaxCin + CO), P = NB + 1, NQ = NB / 32, QP = kMaxCin + CO, PEEP = 3 * CO;
+  static constexpr int CO = 32 * NC, G = 4 * CO, NB = (NO + 1) * (kMaxCin + CO), P = NB + 1, NQ = (NB + 31) / 32, QP = NO * (kMaxCin + CO),
+                       PEEP = 3 * CO;
 };
 
 struct LstmFwd {
@@ -41,9 +43,15 @@ struct LstmFwd {
   float* S;                                  // (N, ld) weight-gradient basis, nullable
 };
 
-template <int NC, bool GC, bool HAS_H>
-__global__ void __launch_bounds__(kRowsThreads, 2) k_lstm_rows_fwd(LstmFwd a) {
-  using D = LWd<NC>;
+// the arguments of an NO-operator instance: operator 1's CSR (by destination in the forward, by source in the backward) follows the
+// one-operator arguments, which keep their layout
+struct Op1 { const int* rowptr1; const int2* cv1; };
+template <class A, int NO> struct WithOps : A {};
+template <class A> struct WithOps<A, 2> : A, Op1 {};
+
+template <int NC, bool GC, bool HAS_H, int NO = 1>
+__global__ void __launch_bounds__(kRowsThreads, 2) k_lstm_rows_fwd(WithOps<LstmFwd, NO> a) {
+  using D = LWd<NC, NO>;
   constexpr int CO = D::CO, P = D::P;
   extern __shared__ float ws[];              // [4 CO][P]
   stage_w<P>(ws, a.w, a.nb, 0, D::G);
@@ -63,10 +71,11 @@ __global__ void __launch_bounds__(kRowsThreads, 2) k_lstm_rows_fwd(LstmFwd a) {
     const int t1 = min(t0 + kRowTile, a.n);
     for (int i = t0 + warp; i < t1; i += kRowsWarps) {
       const float xv = lane < cin ? __ldg(a.x + (size_t)i * cin + lane) : 0.f;
-      float hv[NC], lh[NC], lx = 0.f;
+      float hv[NC], lh[NC], lx = 0.f, lh1[NC], lx1 = 0.f;   // lh1, lx1: operator 1 (NO = 2)
 #pragma unroll
-      for (int j = 0; j < NC; ++j) { hv[j] = HAS_H ? __ldg(a.h + (size_t)i * CO + lane + 32 * j) : 0.f; lh[j] = 0.f; }
+      for (int j = 0; j < NC; ++j) { hv[j] = HAS_H ? __ldg(a.h + (size_t)i * CO + lane + 32 * j) : 0.f; lh[j] = 0.f; lh1[j] = 0.f; }
       if (a.nops && (HAS_H || !GC)) gather_rows<NC, HAS_H>(a.rowptr, a.cv, i, a.h, CO, a.x, cin, xo, lane, lh, lx);
+      if constexpr (NO > 1) gather_rows<NC, HAS_H>(a.rowptr1, a.cv1, i, a.h, CO, a.x, cin, xo, lane, lh1, lx1);
       float p[4][NC];                        // pre = b + S W^T, S's columns in basis order
 #pragma unroll
       for (int g = 0; g < 4; ++g)
@@ -97,6 +106,16 @@ __global__ void __launch_bounds__(kRowsThreads, 2) k_lstm_rows_fwd(LstmFwd a) {
           }
         }
       }
+      if constexpr (NO > 1) {                  // operator 1's block [Op1 X | Op1 H] at column 2 C (GConvLSTM basis only)
+        for (int c = 0; c < cin; ++c) col(__shfl_sync(0xffffffffu, lx1, c), 2 * C + c);
+        if (HAS_H) {
+#pragma unroll
+          for (int jo = 0; jo < NC; ++jo) {
+#pragma unroll 8
+            for (int o = 0; o < 32; ++o) col(__shfl_sync(0xffffffffu, lh1[jo], o), 2 * C + cin + 32 * jo + o);
+          }
+        }
+      }
 #pragma unroll
       for (int j = 0; j < NC; ++j) {
         const size_t io = (size_t)i * CO + lane + 32 * j;
@@ -123,6 +142,11 @@ __global__ void __launch_bounds__(kRowsThreads, 2) k_lstm_rows_fwd(LstmFwd a) {
 #pragma unroll
           for (int j = 0; j < NC; ++j) r[C + xo + lane + 32 * j] = lh[j];
         }
+        if constexpr (NO > 1) {
+          if (lane < cin) r[2 * C + lane] = lx1;
+#pragma unroll
+          for (int j = 0; j < NC; ++j) r[2 * C + cin + lane + 32 * j] = lh1[j];
+        }
         if (a.nb + lane < a.ld) r[a.nb + lane] = 0.f;
       }
     }
@@ -141,9 +165,9 @@ struct LstmBwd {
   float* dx; float* dh; float* dc;           // (N, cin), (N, CO), (N, CO), nullable
 };
 
-template <int NC, bool GC>
-__global__ void __launch_bounds__(kRowsThreads, 2) k_lstm_rows_bwd_a(LstmBwd a) {
-  using D = LWd<NC>;
+template <int NC, bool GC, int NO = 1>
+__global__ void __launch_bounds__(kRowsThreads, 2) k_lstm_rows_bwd_a(WithOps<LstmBwd, NO> a) {
+  using D = LWd<NC, NO>;
   constexpr int CO = D::CO, P = D::P, NQ = D::NQ, QP = D::QP, PEEP = D::PEEP;
   extern __shared__ float ws[];              // [4 CO][P], then [kRowsWarps][3 CO] for the peephole sums
   const bool need_ds = a.dx != nullptr || a.dh != nullptr;
@@ -199,7 +223,8 @@ __global__ void __launch_bounds__(kRowsThreads, 2) k_lstm_rows_bwd_a(LstmBwd a) 
           for (int o = 0; o < 32; ++o) {
             const float s = __shfl_sync(0xffffffffu, dp[gt][jo], o);
 #pragma unroll
-            for (int q = 0; q < NQ; ++q) d[q] = fmaf(s, wg[o * P + 32 * q], d[q]);
+            for (int q = 0; q < NQ; ++q)             // a last group past the widest basis (NB % 32 != 0) reads no column beyond it
+              if (32 * (q + 1) <= D::NB || lane + 32 * q < D::NB) d[q] = fmaf(s, wg[o * P + 32 * q], d[q]);
           }
         }
       }
@@ -241,18 +266,28 @@ __global__ void __launch_bounds__(kRowsThreads, 2) k_lstm_rows_bwd_a(LstmBwd a) 
   }
 }
 
-// dH += Op^T Q[:, xo:], and for GConvLSTM dX += Op^T Q[:, :cin]  (either nullable)
-template <int NC, bool GC>
-__global__ void __launch_bounds__(kRowsThreads) k_lstm_rows_bwd_b(LstmBwd a) {
-  constexpr int CO = LWd<NC>::CO, QP = LWd<NC>::QP;
+// dH += Op^T Q[:, xo:], and for GConvLSTM dX += Op^T Q[:, :cin]  (either nullable); with NO = 2 both operators in one pass,
+// dH += Op0^T Q0 + Op1^T Q1 (Q1 at column C of the scratch row)
+template <int NC, bool GC, int NO = 1>
+__global__ void __launch_bounds__(kRowsThreads) k_lstm_rows_bwd_b(WithOps<LstmBwd, NO> a) {
+  constexpr int CO = LWd<NC, NO>::CO, QP = LWd<NC, NO>::QP;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, cin = a.cin, xo = GC ? 0 : cin;
   const int nx = (!GC && a.dx) ? cin : 0;
   for (int t0 = blockIdx.x * kRowTile; t0 < a.n; t0 += gridDim.x * kRowTile) {
     const int t1 = min(t0 + kRowTile, a.n);
     for (int j = t0 + warp; j < t1; j += kRowsWarps) {
-      float th[NC], tx;
-      if (a.dh) gather_rows<NC, true>(a.rowptr, a.cv, j, a.q + xo, QP, a.q, QP, nx, lane, th, tx);
-      else gather_rows<NC, false>(a.rowptr, a.cv, j, a.q + xo, QP, a.q, QP, nx, lane, th, tx);
+      float th[NC], tx, th1[NC], tx1 = 0.f;
+      auto gather = [&](const int* rp, const int2* cv, const float* qk, float (&h)[NC], float& x) {
+        if (a.dh) gather_rows<NC, true>(rp, cv, j, qk + xo, QP, qk, QP, nx, lane, h, x);
+        else gather_rows<NC, false>(rp, cv, j, qk + xo, QP, qk, QP, nx, lane, h, x);
+      };
+      gather(a.rowptr, a.cv, a.q, th, tx);
+      if (NO > 1) {
+        if constexpr (NO > 1) gather(a.rowptr1, a.cv1, a.q + cin + CO, th1, tx1);
+#pragma unroll
+        for (int c = 0; c < NC; ++c) th[c] += th1[c];
+        tx += tx1;
+      }
       if (a.dh)
 #pragma unroll
         for (int c = 0; c < NC; ++c) a.dh[(size_t)j * CO + lane + 32 * c] += th[c];
@@ -262,7 +297,7 @@ __global__ void __launch_bounds__(kRowsThreads) k_lstm_rows_bwd_b(LstmBwd a) {
 }
 
 // w [4 CO][nb]: row gate*CO + o (gates i | f | c | o), column m of the basis; b [4 CO] = (bx + bh) + bg.
-//   GConvLSTM: wx [4][n_ops+1][CO][cin], wh [4][n_ops+1][CO][CO] (gate, Chebyshev order, out, in), bx / bh [4][CO] or NULL
+//   GConvLSTM: wx [4][n_ops+1][CO][cin], wh [4][n_ops+1][CO][CO] (gate, Chebyshev order or operator, out, in), bx / bh [4][CO] or NULL
 //   GCLSTM:    wx [4][cin][CO] (the dense W_g, in x out), wh [4][n_ops+1][CO][CO], bx NULL, bh [4][CO] or NULL
 template <int NC, bool GC>
 __global__ void k_lstm_rows_pack(int nops, int cin, const float* __restrict__ wx, const float* __restrict__ wh, const float* __restrict__ bx,
@@ -331,12 +366,15 @@ static int lstm_nb(int variant, int n_ops, int cin, int cout) {
   return variant == STMP_LSTM_GC ? cin + (n_ops + 1) * cout : (n_ops + 1) * (cin + cout);
 }
 
-static bool lstm_envelope(int variant, int n_ops, int64_t cin) {
-  return (variant == STMP_LSTM_GCONV || variant == STMP_LSTM_GC) && n_ops >= 0 && n_ops <= 1 && cin >= 1 && cin <= kMaxCin;
+// n_ops <= 1 for both bases at 32 and 64 channels; n_ops = 2 (two independent one-hop operators, LRGCN's two relations) for the
+// GConvLSTM basis at 32 channels only: at 64 its 256 staged gate rows would not fit in shared memory
+static bool lstm_envelope(int variant, int n_ops, int64_t cin, int64_t cout) {
+  return (variant == STMP_LSTM_GCONV || variant == STMP_LSTM_GC) && n_ops >= 0 &&
+         (n_ops <= 1 || (n_ops == 2 && variant == STMP_LSTM_GCONV && cout == 32)) && cin >= 1 && cin <= kMaxCin;
 }
 
 static bool lstm_supported(const stmp_plan* plan, int variant, int n_ops, int64_t cin, int64_t cout) {
-  return plan && lstm_envelope(variant, n_ops, cin) && n_ops <= plan->n_ops && (cout == 32 || cout == 64);
+  return plan && (cout == 32 || cout == 64) && lstm_envelope(variant, n_ops, cin, cout) && n_ops <= plan->n_ops;
 }
 
 static int64_t lstm_ld(int variant, int n_ops, int64_t cin, int cout) { return (lstm_nb(variant, n_ops, (int)cin, cout) + 7) / 8 * 8; }
@@ -379,7 +417,8 @@ static int lstm_pack_weights(int variant, int n_ops, int64_t cin, const float* w
   STMP_REQUIRE(wx && wh && bg && w && b, STMP_EINVAL, "%s: NULL tensor", N::pack);
   STMP_REQUIRE(variant == STMP_LSTM_GC ? bx == nullptr : !bx == !bh, STMP_EINVAL,
                "%s: GConvLSTM takes both ChebConv bias stacks or neither, GCLSTM no bx", N::pack);
-  STMP_REQUIRE(lstm_envelope(variant, n_ops, cin), STMP_EUNSUPPORTED, "%s: n_ops <= 1, cin 1..16 only", N::pack);
+  STMP_REQUIRE(lstm_envelope(variant, n_ops, cin, CO), STMP_EUNSUPPORTED, "%s: n_ops <= 1 (2 for GConvLSTM at 32 channels), cin 1..16 only",
+               N::pack);
   const int total = G * lstm_nb(variant, n_ops, (int)cin, CO) + G;
   cudaStream_t st = (cudaStream_t)stream;
   if (variant == STMP_LSTM_GC) k_lstm_rows_pack<NC, true><<<(total + 255) / 256, 256, 0, st>>>(n_ops, (int)cin, wx, wh, bx, bh, bg, w, b);
@@ -388,11 +427,11 @@ static int lstm_pack_weights(int variant, int n_ops, int64_t cin, const float* w
   return STMP_OK;
 }
 
-template <int NC, bool GC, bool HAS_H>
-static int launch_fwd(const LstmFwd& a, int grid, cudaStream_t st) {
-  const int smem = LWd<NC>::G * LWd<NC>::P * 4;
-  STMP_CUDA_OK(cudaFuncSetAttribute(k_lstm_rows_fwd<NC, GC, HAS_H>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  k_lstm_rows_fwd<NC, GC, HAS_H><<<grid, kRowsThreads, smem, st>>>(a);
+template <int NC, bool GC, bool HAS_H, int NO = 1>
+static int launch_fwd(const WithOps<LstmFwd, NO>& a, int grid, cudaStream_t st) {
+  const int smem = LWd<NC, NO>::G * LWd<NC, NO>::P * 4;
+  STMP_CUDA_OK(cudaFuncSetAttribute(k_lstm_rows_fwd<NC, GC, HAS_H, NO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  k_lstm_rows_fwd<NC, GC, HAS_H, NO><<<grid, kRowsThreads, smem, st>>>(a);
   STMP_LAUNCH_OK(LNames<NC>::kfwd);
   return STMP_OK;
 }
@@ -405,38 +444,52 @@ static int lstm_fwd(const stmp_plan* plan, int variant, int n_ops, int64_t cin, 
   STMP_REQUIRE(plan != nullptr, STMP_EINVAL, "%s: plan is NULL", N::fwd);
   STMP_REQUIRE(variant == STMP_LSTM_GCONV || variant == STMP_LSTM_GC, STMP_EINVAL, "%s: unknown variant %d", N::fwd, variant);
   STMP_REQUIRE(lstm_supported(plan, variant, n_ops, cin, CO), STMP_EUNSUPPORTED,
-               "%s: n_ops <= min(1, plan's operators), cin 1..16 only (n_ops=%d, cin=%lld)", N::fwd, n_ops, (long long)cin);
+               "%s: n_ops <= the plan's operators and 1 (2 for GConvLSTM at 32 channels), cin 1..16 only (n_ops=%d, cin=%lld)", N::fwd, n_ops,
+               (long long)cin);
   STMP_REQUIRE(x && w && b && hout && cout, STMP_EINVAL, "%s: NULL tensor", N::fwd);
   STMP_REQUIRE(!S || ld == lstm_ld(variant, n_ops, cin, CO), STMP_ESHAPE, "%s: the basis row pitch must be nb rounded up to 8", N::fwd);
   const void* ps[] = {x, h, c, w, b, peep, hout, cout, stash, S};
   for (const void* p : ps) STMP_REQUIRE(al4(p), STMP_ESHAPE, "%s: misaligned tensor", N::fwd);
   STMP_REQUIRE(((uintptr_t)S & 15u) == 0, STMP_ESHAPE, "%s: S must be 16-byte aligned", N::fwd);
   if (plan->n == 0) return STMP_OK;
-  LstmFwd a;
+  WithOps<LstmFwd, 1> a;
   a.rowptr = plan->fwd[0].rowptr; a.cv = plan->fwd[0].cv;
   a.n = plan->n; a.cin = (int)cin; a.nops = n_ops; a.nb = lstm_nb(variant, n_ops, (int)cin, CO); a.ld = (int)ld;
   a.x = x; a.h = h; a.c = c; a.w = w; a.b = b; a.peep = peep; a.hout = hout; a.cout = cout; a.stash = stash; a.S = S;
   const int grid = rows_grid(plan->n);
   cudaStream_t st = (cudaStream_t)stream;
+  if constexpr (NC == 1) {
+    if (n_ops == 2) {
+      WithOps<LstmFwd, 2> a2;
+      static_cast<LstmFwd&>(a2) = a;
+      a2.rowptr1 = plan->fwd[1].rowptr; a2.cv1 = plan->fwd[1].cv;
+      return h ? launch_fwd<NC, false, true, 2>(a2, grid, st) : launch_fwd<NC, false, false, 2>(a2, grid, st);
+    }
+  }
   if (variant == STMP_LSTM_GC) return h ? launch_fwd<NC, true, true>(a, grid, st) : launch_fwd<NC, true, false>(a, grid, st);
   return h ? launch_fwd<NC, false, true>(a, grid, st) : launch_fwd<NC, false, false>(a, grid, st);
 }
 
-// the backward scratch: N rows of the operator block of dS, then the per-CTA peephole sums
+// the backward scratch row: the operator blocks of dS, one per operator of the widest basis the plan serves (two on a two-operator plan
+// at 32 channels)
+template <int NC>
+static int lstm_qp(int n_ops) { return NC == 1 && n_ops >= 2 ? LWd<1, 2>::QP : LWd<NC>::QP; }
+
+// the backward scratch: N scratch rows, then the per-CTA peephole sums
 template <int NC>
 static int64_t lstm_scratch_bytes(const stmp_plan* plan) {
-  return plan ? ((int64_t)plan->n * LWd<NC>::QP + (int64_t)rows_grid(plan->n) * LWd<NC>::PEEP) * 4 : 0;
+  return plan ? ((int64_t)plan->n * lstm_qp<NC>(plan->n_ops) + (int64_t)rows_grid(plan->n) * LWd<NC>::PEEP) * 4 : 0;
 }
 
-template <int NC, bool GC>
-static int launch_bwd(const LstmBwd& a, int grid, bool gather, cudaStream_t st) {
-  using D = LWd<NC>;
+template <int NC, bool GC, int NO = 1>
+static int launch_bwd(const WithOps<LstmBwd, NO>& a, int grid, bool gather, cudaStream_t st) {
+  using D = LWd<NC, NO>;
   const int smem = (D::G * D::P + kRowsWarps * D::PEEP) * 4;
-  STMP_CUDA_OK(cudaFuncSetAttribute(k_lstm_rows_bwd_a<NC, GC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  k_lstm_rows_bwd_a<NC, GC><<<grid, kRowsThreads, smem, st>>>(a);
+  STMP_CUDA_OK(cudaFuncSetAttribute(k_lstm_rows_bwd_a<NC, GC, NO>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  k_lstm_rows_bwd_a<NC, GC, NO><<<grid, kRowsThreads, smem, st>>>(a);
   STMP_LAUNCH_OK(LNames<NC>::bwd_a);
   if (gather) {
-    k_lstm_rows_bwd_b<NC, GC><<<grid, kRowsThreads, 0, st>>>(a);
+    k_lstm_rows_bwd_b<NC, GC, NO><<<grid, kRowsThreads, 0, st>>>(a);
     STMP_LAUNCH_OK(LNames<NC>::bwd_b);
   }
   return STMP_OK;
@@ -451,29 +504,38 @@ static int lstm_bwd(const stmp_plan* plan, int variant, int n_ops, int64_t cin, 
   STMP_REQUIRE(plan != nullptr, STMP_EINVAL, "%s: plan is NULL", N::bwd);
   STMP_REQUIRE(variant == STMP_LSTM_GCONV || variant == STMP_LSTM_GC, STMP_EINVAL, "%s: unknown variant %d", N::bwd, variant);
   STMP_REQUIRE(lstm_supported(plan, variant, n_ops, cin, CO), STMP_EUNSUPPORTED,
-               "%s: n_ops <= min(1, plan's operators), cin 1..16 only (n_ops=%d, cin=%lld)", N::bwd, n_ops, (long long)cin);
+               "%s: n_ops <= the plan's operators and 1 (2 for GConvLSTM at 32 channels), cin 1..16 only (n_ops=%d, cin=%lld)", N::bwd, n_ops,
+               (long long)cin);
   STMP_REQUIRE(cn && stash && w && scratch && dpre, STMP_EINVAL, "%s: NULL tensor", N::bwd);
   STMP_REQUIRE(c || !dc, STMP_EINVAL, "%s: dc needs c (C = None has no state gradient)", N::bwd);
   const void* ps[] = {gh, gc, c, cn, stash, w, peep, scratch, dx, dh, dc};
   for (const void* p : ps) STMP_REQUIRE(al4(p), STMP_ESHAPE, "%s: misaligned tensor", N::bwd);
   STMP_REQUIRE(((uintptr_t)dpre & 15u) == 0, STMP_ESHAPE, "%s: dpre must be 16-byte aligned", N::bwd);
   if (plan->n == 0) return STMP_OK;
-  LstmBwd a;
+  WithOps<LstmBwd, 1> a;
   a.rowptr = plan->bwd[0].rowptr; a.cv = plan->bwd[0].cv;
   a.n = plan->n; a.cin = (int)cin; a.nops = n_ops; a.nb = lstm_nb(variant, n_ops, (int)cin, CO);
   a.gh = gh; a.gc = gc; a.c = c; a.cn = cn; a.stash = stash; a.w = w; a.peep = peep; a.dpre = dpre;
-  a.q = scratch; a.pp = peep ? scratch + (size_t)plan->n * LWd<NC>::QP : nullptr; a.dx = dx; a.dh = dh; a.dc = dc;
+  a.q = scratch; a.pp = peep ? scratch + (size_t)plan->n * lstm_qp<NC>(n_ops) : nullptr; a.dx = dx; a.dh = dh; a.dc = dc;
   const int grid = rows_grid(plan->n);
   const bool gc_basis = variant == STMP_LSTM_GC;
-  const bool gather = n_ops == 1 && (dh != nullptr || (!gc_basis && dx != nullptr));      // GCLSTM: X is not diffused
+  const bool gather = n_ops >= 1 && (dh != nullptr || (!gc_basis && dx != nullptr));      // GCLSTM: X is not diffused
   cudaStream_t st = (cudaStream_t)stream;
+  if constexpr (NC == 1) {
+    if (n_ops == 2) {
+      WithOps<LstmBwd, 2> a2;
+      static_cast<LstmBwd&>(a2) = a;
+      a2.rowptr1 = plan->bwd[1].rowptr; a2.cv1 = plan->bwd[1].cv;
+      return launch_bwd<NC, false, 2>(a2, grid, gather, st);
+    }
+  }
   return gc_basis ? launch_bwd<NC, true>(a, grid, gather, st) : launch_bwd<NC, false>(a, grid, gather, st);
 }
 
 // the weight-gradient workspace: wgrad_ffma_max_parts() partials of (ld + 1) * 4 CO floats (at 64 wide, one of (ld + 1) * CO per gate)
 template <int NC>
 static int64_t lstm_wgrad_workspace_bytes(int variant, int n_ops, int64_t cin) {
-  if (!lstm_envelope(variant, n_ops, cin)) return 0;
+  if (n_ops > 1 || !lstm_envelope(variant, n_ops, cin, LWd<NC>::CO)) return 0;
   return (int64_t)wgrad_ffma_max_parts() * (lstm_ld(variant, n_ops, cin, LWd<NC>::CO) + 1) * LWd<NC>::G * 4;
 }
 
@@ -488,7 +550,7 @@ static int lstm_wgrad(int variant, int n_ops, int64_t cin, int64_t rows, int64_t
   constexpr int CO = D::CO, G = D::G;
   STMP_REQUIRE(variant == STMP_LSTM_GCONV || variant == STMP_LSTM_GC, STMP_EINVAL, "%s: unknown variant %d", N::wgrad, variant);
   STMP_REQUIRE(S && dpre && workspace && dw && rows >= 0 && (scratch || !dpeep), STMP_EINVAL, "%s: bad argument", N::wgrad);
-  STMP_REQUIRE(lstm_envelope(variant, n_ops, cin), STMP_EUNSUPPORTED, "%s: n_ops <= 1, cin 1..16 only", N::wgrad);
+  STMP_REQUIRE(n_ops <= 1 && lstm_envelope(variant, n_ops, cin, CO), STMP_EUNSUPPORTED, "%s: n_ops <= 1, cin 1..16 only", N::wgrad);
   const int nb = lstm_nb(variant, n_ops, (int)cin, CO);
   STMP_REQUIRE(ld == lstm_ld(variant, n_ops, cin, CO), STMP_ESHAPE, "%s: the basis row pitch must be nb rounded up to 8", N::wgrad);
   STMP_REQUIRE((((uintptr_t)S | (uintptr_t)dpre | (uintptr_t)workspace) & 15u) == 0, STMP_ESHAPE,
@@ -575,4 +637,37 @@ extern "C" int64_t stmp_lstm_wide_rows_wgrad_workspace_bytes(int variant, int n_
 extern "C" int stmp_lstm_wide_rows_wgrad(int variant, int n_ops, int64_t cin, int64_t rows, int64_t ld, const float* S, const float* dpre,
                                          const float* scratch, void* workspace, float* dw, float* db, float* dpeep, void* stream) {
   return lstm_wgrad<2>(variant, n_ops, cin, rows, ld, S, dpre, scratch, workspace, dw, db, dpeep, stream);
+}
+
+// The two-operator GConvLSTM basis at 32 channels (nb = 3 (cin + 32) <= 144): the 64-wide cells' per-gate contraction with the packed rows
+// taken as two 64-row halves, [dpi | dpf] and [dpc | dpo] (k_wide_rows_wgrad<2>, 32-row tiles), then its fixed-order reduce into dw [128][nb]
+// and db [128].  No peepholes (LRGCN has none).
+extern "C" int64_t stmp_lstm_rows_wgrad2_workspace_bytes(int64_t cin) {
+  if (!lstm_envelope(STMP_LSTM_GCONV, 2, cin, kCo)) return 0;
+  return (int64_t)wgrad_ffma_max_parts() * (lstm_ld(STMP_LSTM_GCONV, 2, cin, kCo) + 1) * kG * 4;
+}
+
+extern "C" int stmp_lstm_rows_wgrad2(int64_t cin, int64_t rows, int64_t ld, const float* S, const float* dpre, void* workspace, float* dw,
+                                     float* db, void* stream) {
+  STMP_REQUIRE(S && dpre && workspace && dw && rows >= 0, STMP_EINVAL, "stmp_lstm_rows_wgrad2: bad argument");
+  STMP_REQUIRE(lstm_envelope(STMP_LSTM_GCONV, 2, cin, kCo), STMP_EUNSUPPORTED, "stmp_lstm_rows_wgrad2: cin 1..16 only");
+  const int nb = lstm_nb(STMP_LSTM_GCONV, 2, (int)cin, kCo);
+  STMP_REQUIRE(ld == lstm_ld(STMP_LSTM_GCONV, 2, cin, kCo), STMP_ESHAPE, "stmp_lstm_rows_wgrad2: the basis row pitch must be nb rounded up to 8");
+  STMP_REQUIRE((((uintptr_t)S | (uintptr_t)dpre | (uintptr_t)workspace) & 15u) == 0, STMP_ESHAPE,
+               "stmp_lstm_rows_wgrad2: S, dpre and the workspace must be 16-byte aligned");
+  STMP_REQUIRE(al4(dw) && al4(db), STMP_ESHAPE, "stmp_lstm_rows_wgrad2: misaligned tensor");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rows == 0) {
+    STMP_CUDA_OK(cudaMemsetAsync(dw, 0, (size_t)kG * nb * 4, st));
+    if (db) STMP_CUDA_OK(cudaMemsetAsync(db, 0, (size_t)kG * 4, st));
+    return STMP_OK;
+  }
+  const int parts = wide_wgrad_parts(rows);
+  const WideWgradOps<2> op = {{S, S}, {dpre, dpre + (size_t)rows * 2 * kCo}, {2 * kCo, 2 * kCo}};
+  k_wide_rows_wgrad<2><<<dim3(parts, 2), kWideWgThreads, 0, st>>>(rows, (int)ld, op, reinterpret_cast<float*>(workspace));
+  STMP_LAUNCH_OK("k_lstm_rows_wgrad2");
+  k_wide_rows_wgrad_reduce<2><<<(kG * nb + kG + 31) / 32, 256, 0, st>>>(parts, (int)ld, nb, reinterpret_cast<const float*>(workspace), 0, 0,
+                                                                         nullptr, dw, db, nullptr);
+  STMP_LAUNCH_OK("k_lstm_rows_wgrad2_reduce");
+  return STMP_OK;
 }

@@ -191,6 +191,17 @@ __global__ void k_compact(int e, const int* __restrict__ flag, const int* __rest
   if (i == e - 1) info->count = pos[i] + flag[i];
 }
 
+// ---- RGCN: relation-masked mean operators ------------------------------------------------------------
+__global__ void k_flag_relation(int e, const long long* __restrict__ type, long long rel, int* __restrict__ flag) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < e) flag[i] = type[i] == rel;
+}
+// 1 / cnt_r(dst): every destination that holds an entry has a count >= 1 (the reference's clamp(min=1) never applies to one)
+__global__ void k_mean_vals(int e, const int* __restrict__ dst, const float* __restrict__ cnt, float* __restrict__ val) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < e) val[i] = __frcp_rn(cnt[dst[i]]);
+}
+
 // ---- Laplacian (PyG get_laplacian) -------------------------------------------------------------------
 // entries [0,e2): non-loop edges; [e2, e2+n): loops.  Produces UNSCALED laplacian weights.
 __global__ void k_laplacian_vals(int e2, int n, int normalization, const int* __restrict__ r2,
@@ -398,17 +409,24 @@ struct Builder {
   }
   // remove self loops, keeping order: outputs r2,c2,w2 and the kept count (host sync).
   int compact_nonloops(int e, const int* row, const int* col, const float* w, int** r2, int** c2, float** w2, int* e2) {
+    int* flag = e ? talloc<int>(e) : nullptr;
+    if (e && !flag) return rc;
+    if (e) {
+      k_flag_nonloop<<<blocks_for(e), kThreads, 0, st>>>(e, row, col, flag);
+      STMP_LAUNCH_OK("k_flag_nonloop");
+    }
+    return compact(e, flag, row, col, w, r2, c2, w2, e2);
+  }
+  // keep the edges whose flag is set, in order: outputs r2,c2,w2 and the kept count (host sync).
+  int compact(int e, int* flag, const int* row, const int* col, const float* w, int** r2, int** c2, float** w2, int* e2) {
     *r2 = talloc<int>(e);
     *c2 = talloc<int>(e);
     *w2 = talloc<float>(e);
     if (!*r2 || !*c2 || !*w2) return rc;
     *e2 = 0;
     if (e == 0) return 0;
-    int* flag = talloc<int>(e);
     int* pos = talloc<int>(e);
-    if (!flag || !pos) return rc;
-    k_flag_nonloop<<<blocks_for(e), kThreads, 0, st>>>(e, row, col, flag);
-    STMP_LAUNCH_OK("k_flag_nonloop");
+    if (!pos) return rc;
     size_t tb = 0;
     STMP_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, tb, flag, pos, e, st));
     void* t = talloc<char>(tb);
@@ -592,6 +610,32 @@ int build_gcn(Builder& b, stmp_plan* p, int n, int e, const int* row, const int*
   }
   if ((r = b.both_csr(p, 0, n, nnz, dst, src, val))) return r;
   p->n_ops = 1;
+  return 0;
+}
+
+// PyG RGCNConv (aggr="mean"), relations rel0 .. rel0 + n_rel - 1: operator k holds the edges of type rel0 + k in edge order (the masked
+// edge list the reference propagates), dst = col, src = row, val = 1 / (the destination's count of such edges).  Other types match none.
+int build_rgcn(Builder& b, stmp_plan* p, int n, int e, const int* row, const int* col, const long long* type, long long rel0, int n_rel) {
+  int* flag = b.talloc<int>(e);
+  if (!flag) return b.rc;
+  for (int k = 0; k < n_rel; ++k) {
+    if (e) {
+      k_flag_relation<<<blocks_for(e), kThreads, 0, b.st>>>(e, type, rel0 + k, flag);
+      STMP_LAUNCH_OK("k_flag_relation");
+    }
+    int *src, *dst, ek, r;
+    float *w2, *cnt;
+    if ((r = b.compact(e, flag, row, col, nullptr, &src, &dst, &w2, &ek))) return r;
+    if ((r = b.segment_sum(ek, n, dst, nullptr, &cnt))) return r;    // in-degree per relation: scatter(ones, dst)
+    float* val = b.talloc<float>(ek);
+    if (!val) return b.rc;
+    if (ek) {
+      k_mean_vals<<<blocks_for(ek), kThreads, 0, b.st>>>(ek, dst, cnt, val);
+      STMP_LAUNCH_OK("k_mean_vals");
+    }
+    if ((r = b.both_csr(p, k, n, ek, dst, src, val))) return r;
+  }
+  p->n_ops = n_rel;
   return 0;
 }
 
@@ -881,12 +925,22 @@ using namespace stmp;
 
 static int plan_create_impl(int flavor, int64_t num_nodes, int64_t num_edges, const int64_t* edge_index,
                             const float* edge_weight, int normalization, float lambda_max, const float* lambda_node,
-                            uint32_t flags, void* stream, stmp_plan** out);
+                            uint32_t flags, void* stream, stmp_plan** out, const int64_t* edge_type = nullptr, int64_t rel0 = 0,
+                            int n_rel = 0);
 
 extern "C" int stmp_plan_create(int flavor, int64_t num_nodes, int64_t num_edges, const int64_t* edge_index,
                                 const float* edge_weight, int normalization, float lambda_max, uint32_t flags,
                                 void* stream, stmp_plan** out) {
+  STMP_REQUIRE(flavor != STMP_FLAVOR_RGCN, STMP_EINVAL, "stmp_plan_create: the RGCN flavor is built by stmp_plan_create_rgcn");
   return plan_create_impl(flavor, num_nodes, num_edges, edge_index, edge_weight, normalization, lambda_max, nullptr, flags, stream, out);
+}
+
+extern "C" int stmp_plan_create_rgcn(int64_t num_nodes, int64_t num_edges, const int64_t* edge_index, const int64_t* edge_type,
+                                     int64_t rel0, int n_rel, void* stream, stmp_plan** out) {
+  STMP_REQUIRE(n_rel >= 1 && n_rel <= 2, STMP_EINVAL, "stmp_plan_create_rgcn: a plan holds 1 or 2 relations (got %d)", n_rel);
+  STMP_REQUIRE(edge_type != nullptr || num_edges == 0, STMP_EINVAL, "stmp_plan_create_rgcn: edge_type is NULL");
+  return plan_create_impl(STMP_FLAVOR_RGCN, num_nodes, num_edges, edge_index, nullptr, STMP_NORM_NONE, 0.f, nullptr, 0u, stream, out,
+                          edge_type, rel0, n_rel);
 }
 
 extern "C" int stmp_plan_create_pergraph(int flavor, int64_t num_nodes, int64_t num_edges, const int64_t* edge_index,
@@ -900,10 +954,10 @@ extern "C" int stmp_plan_create_pergraph(int flavor, int64_t num_nodes, int64_t 
 
 static int plan_create_impl(int flavor, int64_t num_nodes, int64_t num_edges, const int64_t* edge_index,
                             const float* edge_weight, int normalization, float lambda_max, const float* lambda_node,
-                            uint32_t flags, void* stream, stmp_plan** out) {
+                            uint32_t flags, void* stream, stmp_plan** out, const int64_t* edge_type, int64_t rel0, int n_rel) {
   STMP_REQUIRE(out != nullptr, STMP_EINVAL, "stmp_plan_create: out is NULL");
   *out = nullptr;
-  STMP_REQUIRE(flavor >= STMP_FLAVOR_DCONV && flavor <= STMP_FLAVOR_CHEB_ATT, STMP_EINVAL, "unknown flavor %d", flavor);
+  STMP_REQUIRE(flavor >= STMP_FLAVOR_DCONV && flavor <= STMP_FLAVOR_RGCN, STMP_EINVAL, "unknown flavor %d", flavor);
   STMP_REQUIRE(normalization >= STMP_NORM_NONE && normalization <= STMP_NORM_RW, STMP_EINVAL,
                "Invalid normalization %d", normalization);
   STMP_REQUIRE(num_nodes > 0 && num_nodes < (1ll << 30), STMP_EINVAL, "num_nodes=%lld out of range", (long long)num_nodes);
@@ -939,6 +993,7 @@ static int plan_create_impl(int flavor, int64_t num_nodes, int64_t num_edges, co
       case STMP_FLAVOR_CHEB: rc = build_cheb(b, p, n, e, row, col, edge_weight, lambda_max, lambda_node); break;
       case STMP_FLAVOR_GCN: rc = build_gcn(b, p, n, e, row, col, edge_weight); break;
       case STMP_FLAVOR_CHEB_ATT: rc = build_cheb_att(b, p, n, e, row, col, edge_weight, lambda_max, lambda_node); break;
+      case STMP_FLAVOR_RGCN: rc = build_rgcn(b, p, n, e, row, col, (const long long*)edge_type, rel0, n_rel); break;
     }
     if (rc) break;
     Info h;

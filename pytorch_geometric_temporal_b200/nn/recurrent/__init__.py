@@ -4,4 +4,5 @@ from .gconv_lstm import GConvLSTM  # noqa: F401
 from .temporalgcn import TGCN, TGCN2  # noqa: F401
 from .attentiontemporalgcn import A3TGCN, A3TGCN2  # noqa: F401
 from .gc_lstm import GCLSTM  # noqa: F401
+from .lrgcn import LRGCN  # noqa: F401
 from ._cheb import ChebConv  # noqa: F401

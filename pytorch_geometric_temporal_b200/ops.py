@@ -527,12 +527,20 @@ def lstm_rows_bwd(plan: GraphPlan, variant: int, n_ops: int, gh, gc, c, cn, stas
 
 def lstm_rows_wgrad(variant: int, n_ops: int, cin: int, S, dpre, scratch, has_peep: bool):
     """(dw (4 cout, nb), dbp (7 cout,)): the packed weights' gradient and, in one vector, the summed biases' gradient dbp[:4 cout] and the
-    peepholes' dbp[4 cout:] (left unwritten without peepholes) of the row-split LSTM cell, two launches; cout = dpre.size(2) / 2."""
+    peepholes' dbp[4 cout:] (left unwritten without peepholes) of the row-split LSTM cell, two launches; cout = dpre.size(2) / 2.  n_ops = 2
+    (the two-operator basis at 32 channels) takes stmp_lstm_rows_wgrad2, which has no peepholes."""
     dev = S.device
     co = dpre.size(2) // 2
-    ws = _wgrad_workspace(dev, _lstm_rows_entry(co, "wgrad_workspace_bytes"), variant, n_ops, cin)
     dw = torch.empty(4 * co, lstm_rows_nb(variant, n_ops, cin, co), device=dev, dtype=torch.float32)
     dbp = torch.empty(7 * co, device=dev, dtype=torch.float32)
+    if n_ops == 2:                     # the two-operator basis (LRGCN, two relations): its own contraction, no peepholes
+        L = _lib.lib()
+        ws = _wgrad_workspace(dev, L.stmp_lstm_rows_wgrad2_workspace_bytes, cin)
+        with torch.cuda.device(dev):
+            _lib.check(L.stmp_lstm_rows_wgrad2(cin, S.size(0), S.size(1), _lib.ptr(S), _lib.ptr(dpre), _lib.ptr(ws), _lib.ptr(dw),
+                                               _lib.ptr(dbp), _lib.stream_ptr()))
+        return dw, dbp
+    ws = _wgrad_workspace(dev, _lstm_rows_entry(co, "wgrad_workspace_bytes"), variant, n_ops, cin)
     dpeep = dbp[4 * co:] if has_peep else None
     with torch.cuda.device(dev):
         _lib.check(_lstm_rows_entry(co, "wgrad")(variant, n_ops, cin, S.size(0), S.size(1), _lib.ptr(S), _lib.ptr(dpre), _lib.ptr(scratch),

@@ -97,6 +97,28 @@ class GraphPlan:
             self._h = None
 
 
+class RgcnPlan(GraphPlan):
+    """The relation-masked mean operators of PyG RGCNConv (STMP_FLAVOR_RGCN) for relations rel0 .. rel0 + n_rel - 1 (n_rel 1 or 2):
+    operator k aggregates the edges whose `rel` (int64, one relation id per edge; anything else matches no operator) is rel0 + k."""
+
+    def __init__(self, edge_index: torch.Tensor, rel: torch.Tensor, num_nodes: int, rel0: int, n_rel: int):
+        _require_cuda(edge_index, "edge_index")
+        if edge_index.dim() != 2 or edge_index.size(0) != 2:
+            raise ValueError(f"edge_index must have shape [2, E], got {tuple(edge_index.shape)}")
+        ei = edge_index.to(torch.int64).contiguous()
+        rel = rel.to(device=ei.device, dtype=torch.int64).contiguous()
+        if rel.numel() != ei.size(1):
+            raise RuntimeError(f"edge_type has {rel.numel()} entries for {ei.size(1)} edges")
+        self.flavor, self.num_nodes, self.num_edges = _lib.FLAVOR_RGCN, int(num_nodes), int(ei.size(1))
+        self.device = ei.device
+        self._h = ctypes.c_void_p()
+        with torch.cuda.device(ei.device):
+            rc = _lib.lib().stmp_plan_create_rgcn(self.num_nodes, self.num_edges, _lib.ptr(ei), _lib.ptr(rel), int(rel0), int(n_rel),
+                                                  _lib.stream_ptr(), ctypes.byref(self._h))
+        _lib.check(rc)
+        self.n_ops = _lib.lib().stmp_plan_num_ops(self._h)
+
+
 class PlanCache:
     """Per-module cache keyed on the identity/version of the graph tensors (no device sync)."""
 

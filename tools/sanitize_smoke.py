@@ -9,7 +9,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from pytorch_geometric_temporal_b200 import _lib, ops                                        # noqa: E402
 from pytorch_geometric_temporal_b200.dataset import synthetic                               # noqa: E402
 from pytorch_geometric_temporal_b200.nn.attention import ASTGCN                              # noqa: E402
-from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, GCLSTM, GConvGRU, GConvLSTM, TGCN2   # noqa: E402
+from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, GCLSTM, GConvGRU, GConvLSTM, LRGCN, TGCN2   # noqa: E402
 
 dev = torch.device("cuda")
 torch.manual_seed(0)
@@ -74,6 +74,12 @@ with torch.enable_grad():
             sum(t.square().mean() for t in gl(xr, e_ring, None)).backward()
             with torch.no_grad():
                 gl(xr, e_ring, None, hc[0].detach(), hc[1].detach())
+    t_ring = torch.arange(e_ring.size(1), device=dev) % 3             # relation 0, 1 and a type that matches neither
+    for co, R in ((32, 2), (64, 1)):                             # LRGCN: the relational plan (k_flag_relation, k_mean_vals) and the two-
+        lr = LRGCN(14, co, R, 2).to(dev)                         # operator cell (k_lstm_rows_*<.., 2>, k_wide_rows_wgrad<2> + reduce)
+        hc = [torch.randn(301, co, device=dev, requires_grad=True) for _ in range(2)]
+        sum(t.square().mean() for t in lr(xr, e_ring, t_ring, *hc)).backward()
+        sum(t.square().mean() for t in lr(xr, e_ring, t_ring)).backward()
     for cin, T in ((2, 3), (4, 1)):                              # 301 nodes: the row-split DCRNN (k_dcrnn_rows_*), T = 1 and T > 1, with and
         dr = BatchedDCRNN(cin, 32, 2).to(dev)                    # without dX (k_dcrnn_rows_bwd_x), k_dcrnn_wgrad_tc + k_dcrnn_wgrad_reduce
         xd = torch.randn(2, T, 301, cin, device=dev)
