@@ -66,18 +66,21 @@ def temporal_attention(p, X):
 
 
 def astgcn_block(p, X, edge_index, normalization, time_strides, lambda_max=None):
-    """ASTGCNBlock.forward (astgcn.py:408-481); static edge_index tensor path.  For
-    normalization != 'sym' the reference computes lambda_max with scipy on every call (:437-438);
-    pass it in (tests use the same value on both sides)."""
+    """ASTGCNBlock.forward (astgcn.py:408-481).  edge_index: one tensor, or a list of one per timestep (:442-450) with
+    `lambda_max` then a list too (or None).  For normalization != 'sym' the reference computes lambda_max with scipy on
+    every call (:437-438); pass it in (tests use the same value on both sides)."""
     B, N, Fi, T = X.shape
     E = temporal_attention(_sub(p, "_temporal_attention."), X)
     Xt = torch.matmul(X.reshape(B, -1, T), E).reshape(B, N, Fi, T)
     S = spatial_attention(_sub(p, "_spatial_attention."), Xt)
-    if normalization != "sym" and lambda_max is None:
-        d = pyg.Data(edge_index=edge_index, edge_attr=None, num_nodes=N)
-        lambda_max = pyg.LaplacianLambdaMax()(d).lambda_max
+    lam = lambda ei: pyg.LaplacianLambdaMax()(pyg.Data(edge_index=ei, edge_attr=None, num_nodes=N)).lambda_max
+    if not isinstance(edge_index, list):
+        eis, lams = [edge_index] * T, [lam(edge_index) if normalization != "sym" and lambda_max is None else lambda_max] * T
+    else:
+        eis = edge_index
+        lams = lambda_max if lambda_max is not None else [lam(ei) if normalization != "sym" else None for ei in eis]
     pc = _sub(p, "_chebconv_attention.")
-    Xh = [cheb_conv_attention(pc, X[:, :, :, t], edge_index, S, normalization, None, lambda_max).unsqueeze(-1)
+    Xh = [cheb_conv_attention(pc, X[:, :, :, t], eis[t], S, normalization, None, lams[t]).unsqueeze(-1)
           for t in range(T)]
     Xh = F.relu(torch.cat(Xh, dim=-1))
     Xh = F.conv2d(Xh.permute(0, 2, 1, 3), p["_time_convolution.weight"], p["_time_convolution.bias"],
@@ -147,7 +150,8 @@ def mstgcn_block(p, X, edge_index, time_strides, lambda_max=None):
     else:                                         # per-timestep graphs (:96-115): a genuine per-slice convolution --
         hats = []                                 # NOT the same function as the tensor path above
         for t in range(T):
-            en = pyg.cheb_norm(edge_index[t], N, None, None, lam(edge_index[t]), X.dtype)
+            lam_t = lambda_max[t] if isinstance(lambda_max, list) else lam(edge_index[t])
+            en = pyg.cheb_norm(edge_index[t], N, None, None, lam_t, X.dtype)
             hats.append(R.cheb_conv(pc, X[:, :, :, t], en, K).unsqueeze(-1))
         Xt = F.relu(torch.cat(hats, dim=-1))
     Xt = F.conv2d(Xt.permute(0, 2, 1, 3), p["_time_conv.weight"], p["_time_conv.bias"], stride=(1, time_strides), padding=(0, 1))
@@ -157,7 +161,7 @@ def mstgcn_block(p, X, edge_index, time_strides, lambda_max=None):
 
 
 def mstgcn(p, X, edge_index, nb_block, time_strides, lambda_max=None):
-    """MSTGCN.forward (mstgcn.py:181-200)."""
+    """MSTGCN.forward (mstgcn.py:181-200).  With a list of per-timestep graphs, `lambda_max` may be a list too (one per graph)."""
     for i in range(nb_block):
         X = mstgcn_block(_sub(p, f"_blocklist.{i}."), X, edge_index, time_strides if i == 0 else 1, lambda_max)
     X = F.conv2d(X.permute(0, 3, 1, 2), p["_final_conv.weight"], p["_final_conv.bias"])

@@ -38,6 +38,8 @@ def spmm_raw(plan: GraphPlan, op: int, x: torch.Tensor, transposed: bool = False
     if z is not None:
         z3 = _f32c(z, "z")
         z3 = z3.unsqueeze(0) if z3.dim() == 2 else z3
+        if z3.shape != x3.shape:                       # the kernel reads z with x's batch and row strides
+            raise RuntimeError(f"z must have the shape of x {tuple(x.shape)}, got {tuple(z.shape)}")
     a3 = None
     if att is not None:
         a3 = _f32c(att, "att")
@@ -68,11 +70,13 @@ class _SpMM(torch.autograd.Function):
         if ctx.has_z and ctx.needs_input_grad[1]:
             gz = gy * ctx.beta
         if ctx.has_att and ctx.needs_input_grad[2]:
-            B, N, F = gy.shape
-            gatt = torch.zeros_like(att)
+            # (N, F) features carry a (1, N, N) attention; the kernel writes gatt row-major whatever att's strides are
+            gy3, x3 = (gy.unsqueeze(0), x.unsqueeze(0)) if gy.dim() == 2 else (gy, x)
+            B, N, F = gy3.shape
+            gatt = torch.zeros(att.shape, dtype=att.dtype, device=att.device)
             with torch.cuda.device(gy.device):
-                rc = _lib.lib().stmp_spmm_att_grad(ctx.plan.handle, ctx.op, B, F, _lib.ptr(gy), F, N * F,
-                                                   _lib.ptr(x.contiguous()), F, N * F, _lib.ptr(gatt), _lib.stream_ptr())
+                rc = _lib.lib().stmp_spmm_att_grad(ctx.plan.handle, ctx.op, B, F, _lib.ptr(gy3), F, N * F,
+                                                   _lib.ptr(x3.contiguous()), F, N * F, _lib.ptr(gatt), _lib.stream_ptr())
             _lib.check(rc)
             if ctx.alpha != 1.0:
                 gatt = gatt * ctx.alpha

@@ -4,6 +4,7 @@ import os
 import sys
 
 import torch
+import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from pytorch_geometric_temporal_b200 import _lib, ops                                        # noqa: E402
@@ -192,5 +193,12 @@ for cls in (GConvLSTM, GCLSTM):
     sum(t.square().mean() for t in l64(xw, e17, None)).backward()
     with torch.no_grad():
         l64(xw, e17, None, hw, hw)
+# an ASTGCN training step (tests/test_gpu_attention_training.py): the attention hop forward, its transposed product and k_att_grad at
+# the first block's F = 12 and the later blocks' F = 768; then ops.spmm on 2-D features and a transposed attention, F = 5 (VEC 1)
+F.l1_loss(ASTGCN(2, 1, 3, 64, 64, 1, 12, 12, 307, normalization="rw").to(dev)(torch.randn(2, 307, 1, 12, device=dev), e4),
+          torch.randn(2, 307, 12, device=dev)).backward()
+p4 = ASTGCN(1, 1, 2, 64, 64, 1, 12, 12, 307)._blocklist[0]._chebconv_attention.to(dev)._plan(e4, None, 307, None)
+s4 = torch.rand(1, 307, 307, device=dev).transpose(1, 2).requires_grad_(True)
+ops.spmm(p4, 0, torch.randn(307, 5, device=dev, requires_grad=True), 0.5, att=s4).square().sum().backward()
 torch.cuda.synchronize()
 print("sanitize_smoke ok:", {k: v for k, v in _lib.path_counters().items() if k.startswith("k_") and v})
