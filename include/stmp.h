@@ -57,8 +57,16 @@ enum stmp_flavor {
   /* PyG RGCNConv's mean aggregation (LRGCN, nn/recurrent/lrgcn.py), built by stmp_plan_create_rgcn only: operator k holds the
    * edges of type rel0 + k in edge order, dst=col, src=row, val = 1/(the destination's count of such edges).  No self loops are
    * added; duplicates and self loops count as ordinary edges; a node without such an in-edge has an empty row. */
-  STMP_FLAVOR_RGCN = 4
+  STMP_FLAVOR_RGCN = 4,
+  /* PyG GatedGraphConv's propagate (DyGrEncoder, nn/recurrent/dygrae.py), built by stmp_plan_create_gated only: one operator over every
+   * edge in edge order, dst=col, src=row, val = w_e for STMP_AGGR_ADD and STMP_AGGR_MAX, w_e / (the destination's count of in-edges) for
+   * STMP_AGGR_MEAN (the count is of edges, not of weights); w_e = 1 without weights.  No self loops are added; duplicates and self loops
+   * are ordinary edges; a node without an in-edge has an empty row. */
+  STMP_FLAVOR_GATED = 5
 };
+
+/* GatedGraphConv's aggregation (stmp_plan_create_gated, stmp_ggc_rows_*). */
+enum stmp_aggr { STMP_AGGR_ADD = 0, STMP_AGGR_MEAN = 1, STMP_AGGR_MAX = 2 };
 
 enum stmp_norm { STMP_NORM_NONE = 0, STMP_NORM_SYM = 1, STMP_NORM_RW = 2 };
 
@@ -92,6 +100,10 @@ int stmp_plan_create_pergraph(int flavor, int64_t num_nodes, int64_t num_edges, 
  * More relations take ceil(R / 2) plans.  Setup path: synchronises `stream` once per relation and once to read validation flags. */
 int stmp_plan_create_rgcn(int64_t num_nodes, int64_t num_edges, const int64_t* edge_index, const int64_t* edge_type, int64_t rel0,
                           int n_rel, void* stream, stmp_plan** out);
+/* GatedGraphConv's aggregation operator (STMP_FLAVOR_GATED) for `aggr` (stmp_aggr): edge_weight is a device float [E] or NULL (ones).
+ * edge_index is validated as stmp_plan_create validates it (STMP_EGRAPH).  Setup path: synchronises `stream` to read validation flags. */
+int stmp_plan_create_gated(int64_t num_nodes, int64_t num_edges, const int64_t* edge_index, const float* edge_weight, int aggr,
+                           void* stream, stmp_plan** out);
 void stmp_plan_destroy(stmp_plan* plan);
 
 /* Introspection (tests, bit-exact index parity): number of operators, nodes, entries of operator `op`. */
@@ -479,6 +491,42 @@ int stmp_lstm_rows_wgrad(int variant, int n_ops, int64_t cin, int64_t rows, int6
 int64_t stmp_lstm_rows_wgrad2_workspace_bytes(int64_t cin);
 int stmp_lstm_rows_wgrad2(int64_t cin, int64_t rows, int64_t ld, const float* S, const float* dpre, void* workspace, float* dw, float* db,
                           void* stream);
+
+/* ---- PyG GatedGraphConv(C, L, aggr, bias=True) -- the convolution of DyGrEncoder (nn/recurrent/dygrae.py) -- on graphs of ANY size, split
+ * over CTAs by destination rows (ggc_rows.cu): x^0 = X padded with zeros to C channels, then for l < L: m = x^l W_l, m = aggr over the
+ * in-edges of w_e m_j, x^{l+1} = GRUCell(m, x^l) with ONE GRU weight set for every layer; the result is x^L.  On a STMP_FLAVOR_GATED plan,
+ * whose aggregation the kernels take from the plan.  add / mean gather a = Op x^l and contract m = a W_l (the aggregation is linear);
+ * max needs the message of every source first, so each launch also writes the next layer's m^{l+1} = x^{l+1} W_{l+1}.  max takes
+ * max_e (w_e m_j) per channel (w_e m_j rounded as the reference's message), 0 for a node without in-edges; its backward splits a
+ * channel's gradient evenly among the messages equal to the maximum, counting the zero-initialised output as one more when the maximum
+ * is exactly 0 (torch's scatter_reduce "amax", include_self=False).  Envelope (stmp_ggc_rows_supported): C 1..32, cin 1..C, L 1..1024, any
+ * number of nodes and edges.  Exact fp32 (separate multiply and add in the gathers, FFMA in the contractions); deterministic (no
+ * atomics, every sum in a fixed order); no host sync and no allocation: scratch and workspace come from the caller, so a call can be
+ * captured.  Weights in PyG's layouts: W (L, C, C) with m = x W_l, W_ih / W_hh (3C, C) in gate order r | z | n, b_ih / b_hh (3C).
+ *   stmp_ggc_rows_fwd:   x (N, cin) -> out (N, C).  L launches for add / mean, L + 1 for max.  Inference passes stash NULL and scratch
+ *                        of stmp_ggc_rows_scratch_bytes(plan, C) bytes; training passes stash (L, 8, N, C): per layer x^l | a^l (add,
+ *                        mean) or m^l (max) | the GRU input | r | z | n | W_hn x^l + b_hn | the max's tie count (scratch may then be
+ *                        NULL).  The output does not depend on which is given.
+ *   stmp_ggc_rows_bwd:   gout = dL/dout (N, C) and the stash -> dG (L, N, 4C) = the GRU pre-activation gradients [dr | dz | dn | r dn] and
+ *                        dM (L, N, C) = the gradient at m (add, mean: per destination) or at the messages m^l (max: per source), the
+ *                        operands of stmp_ggc_rows_wgrad, and dx (N, cin; nullable).  One launch per layer (the transposed gather of
+ *                        layer l + 1 fused with the rowwise GRUCell backward of layer l), plus one when dx is asked for (add, mean)
+ *                        or always (max).  scratch of stmp_ggc_rows_scratch_bytes(plan, C) bytes.
+ *   stmp_ggc_rows_wgrad: dW (L, C, C), dW_ih, dW_hh (3C, C), db_ih, db_hh (3C) from the stash, dG and dM: the GRU's sums run over all
+ *                        L N rows, dW_l's over its layer's N.  fp32 FFMA per-CTA partials + a fixed-order sum (two launches); workspace
+ *                        of stmp_ggc_rows_wgrad_workspace_bytes(L, C) bytes.
+ * STMP_EINVAL for a NULL plan or tensor or a plan of another flavor, STMP_ESHAPE for a misaligned tensor, STMP_EUNSUPPORTED outside the
+ * envelope. */
+int stmp_ggc_rows_supported(const stmp_plan* plan, int64_t num_layers, int64_t cin, int64_t channels);
+int64_t stmp_ggc_rows_scratch_bytes(const stmp_plan* plan, int64_t channels);
+int stmp_ggc_rows_fwd(const stmp_plan* plan, int64_t num_layers, int64_t cin, int64_t channels, const float* x, const float* W,
+                      const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, float* scratch, float* out, float* stash,
+                      void* stream);
+int stmp_ggc_rows_bwd(const stmp_plan* plan, int64_t num_layers, int64_t cin, int64_t channels, const float* gout, const float* stash,
+                      const float* W, const float* w_ih, const float* w_hh, float* scratch, float* dG, float* dM, float* dx, void* stream);
+int64_t stmp_ggc_rows_wgrad_workspace_bytes(int64_t num_layers, int64_t channels);
+int stmp_ggc_rows_wgrad(const stmp_plan* plan, int64_t num_layers, int64_t channels, const float* stash, const float* dG, const float* dM,
+                        void* workspace, float* dW, float* dw_ih, float* dw_hh, float* db_ih, float* db_hh, void* stream);
 
 /* ---- the same cell at 64 hidden channels (lstm_rows.cu, the width-2 instance of its kernels): GConvLSTM / GCLSTM(cin, 64, K <= 2).
  * Envelope: cout = 64, cin 1..16, n_ops 0..1 and at most the plan's operators (stmp_lstm_rows_supported(plan, variant, n_ops, cin, 64)),

@@ -11,7 +11,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("STMP_LIB", os.path.join(_HERE, "lib", "libstmp.so"))   # STMP_LIB: A/B a second build of the library
 
 STMP_OK, STMP_EINVAL, STMP_ESHAPE, STMP_EGRAPH, STMP_ECUDA, STMP_EUNSUPPORTED, STMP_ENOMEM = range(7)
-FLAVOR_DCONV, FLAVOR_CHEB, FLAVOR_GCN, FLAVOR_CHEB_ATT, FLAVOR_RGCN = range(5)
+FLAVOR_DCONV, FLAVOR_CHEB, FLAVOR_GCN, FLAVOR_CHEB_ATT, FLAVOR_RGCN, FLAVOR_GATED = range(6)
+AGGR_CODE = {"add": 0, "mean": 1, "max": 2}        # stmp_aggr: GatedGraphConv's aggregation (STMP_FLAVOR_GATED plans)
 NORM_NONE, NORM_SYM, NORM_RW = range(3)
 GCN_IMPROVED, GCN_NO_SELF_LOOPS, DCONV_ALLOW_DUPLICATES = 1, 2, 4
 NORM_CODE = {None: NORM_NONE, "sym": NORM_SYM, "rw": NORM_RW}
@@ -31,6 +32,7 @@ _SIGNATURES = {
     "stmp_plan_create": (c_int, [c_int, c_int64, c_int64, _P, _P, c_int, c_float, c_uint32, _P, POINTER(c_void_p)]),
     "stmp_plan_create_pergraph": (c_int, [c_int, c_int64, c_int64, _P, _P, c_int, _P, c_uint32, _P, POINTER(c_void_p)]),
     "stmp_plan_create_rgcn": (c_int, [c_int64, c_int64, _P, _P, c_int64, c_int, _P, POINTER(c_void_p)]),
+    "stmp_plan_create_gated": (c_int, [c_int64, c_int64, _P, _P, c_int, _P, POINTER(c_void_p)]),
     "stmp_plan_destroy": (None, [_P]),
     "stmp_plan_num_ops": (c_int, [_P]),
     "stmp_plan_num_nodes": (c_int64, [_P]),
@@ -108,6 +110,12 @@ _SIGNATURES = {
     "stmp_lstm_rows_wgrad_workspace_bytes": (c_int64, [c_int, c_int, c_int64]),
     "stmp_lstm_rows_wgrad": (c_int, [c_int, c_int, c_int64, c_int64, c_int64] + [_P] * 8),
     "stmp_lstm_rows_wgrad2_workspace_bytes": (c_int64, [c_int64]),
+    "stmp_ggc_rows_supported": (c_int, [_P, c_int64, c_int64, c_int64]),
+    "stmp_ggc_rows_scratch_bytes": (c_int64, [_P, c_int64]),
+    "stmp_ggc_rows_fwd": (c_int, [_P, c_int64, c_int64, c_int64] + [_P] * 10),
+    "stmp_ggc_rows_bwd": (c_int, [_P, c_int64, c_int64, c_int64] + [_P] * 10),
+    "stmp_ggc_rows_wgrad_workspace_bytes": (c_int64, [c_int64, c_int64]),
+    "stmp_ggc_rows_wgrad": (c_int, [_P, c_int64, c_int64] + [_P] * 10),
     "stmp_lstm_rows_wgrad2": (c_int, [c_int64, c_int64, c_int64] + [_P] * 6),
     "stmp_lstm_wide_rows_pack_weights": (c_int, [c_int, c_int, c_int64] + [_P] * 8),
     "stmp_lstm_wide_rows_fwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 10 + [c_int64, _P]),

@@ -87,6 +87,7 @@ struct stmp_plan {
   // per (warp, operator, slot).  Its size follows from the number of group rows.
   void* rimg[3] = {nullptr, nullptr, nullptr};
   int rimg_groups[3] = {0, 0, 0};
+  int aggr = 0;                  // STMP_FLAVOR_GATED: the stmp_aggr its operator was built for
 };
 
 namespace stmp {

@@ -202,6 +202,16 @@ __global__ void k_mean_vals(int e, const int* __restrict__ dst, const float* __r
   if (i < e) val[i] = __frcp_rn(cnt[dst[i]]);
 }
 
+// ---- GATED: GatedGraphConv's aggregation operator ----------------------------------------------------
+// add / max: the edge weight (1 without weights); mean: the weight divided by the destination's count of in-edges (>= 1 at every entry)
+__global__ void k_gated_vals(int e, const int* __restrict__ dst, const float* __restrict__ w, const float* __restrict__ cnt,
+                             float* __restrict__ val) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= e) return;
+  const float v = w ? w[i] : 1.0f;
+  val[i] = cnt ? __fdiv_rn(v, cnt[dst[i]]) : v;
+}
+
 // ---- Laplacian (PyG get_laplacian) -------------------------------------------------------------------
 // entries [0,e2): non-loop edges; [e2, e2+n): loops.  Produces UNSCALED laplacian weights.
 __global__ void k_laplacian_vals(int e2, int n, int normalization, const int* __restrict__ r2,
@@ -639,6 +649,24 @@ int build_rgcn(Builder& b, stmp_plan* p, int n, int e, const int* row, const int
   return 0;
 }
 
+// PyG GatedGraphConv's propagate (aggr add / mean / max): one operator over every edge in edge order, dst = col, src = row, val = w_e
+// (add, max) or w_e / cnt(dst) (mean, cnt = the destination's number of in-edges); a missing weight is 1.  No self loops are added.
+int build_gated(Builder& b, stmp_plan* p, int n, int e, const int* row, const int* col, const float* w, int aggr) {
+  float* cnt = nullptr;
+  int r;
+  if (aggr == STMP_AGGR_MEAN && (r = b.segment_sum(e, n, col, nullptr, &cnt))) return r;    // scatter(ones, dst)
+  float* val = b.talloc<float>(e);
+  if (!val) return b.rc;
+  if (e) {
+    k_gated_vals<<<blocks_for(e), kThreads, 0, b.st>>>(e, col, w, cnt, val);
+    STMP_LAUNCH_OK("k_gated_vals");
+  }
+  if ((r = b.both_csr(p, 0, n, e, col, row, val))) return r;
+  p->n_ops = 1;
+  p->aggr = aggr;
+  return 0;
+}
+
 // cost model of the static longest-first deal
 constexpr int kLptHandicap = 24;
 constexpr int kLptA = 2;
@@ -926,12 +954,13 @@ using namespace stmp;
 static int plan_create_impl(int flavor, int64_t num_nodes, int64_t num_edges, const int64_t* edge_index,
                             const float* edge_weight, int normalization, float lambda_max, const float* lambda_node,
                             uint32_t flags, void* stream, stmp_plan** out, const int64_t* edge_type = nullptr, int64_t rel0 = 0,
-                            int n_rel = 0);
+                            int n_rel = 0, int aggr = 0);
 
 extern "C" int stmp_plan_create(int flavor, int64_t num_nodes, int64_t num_edges, const int64_t* edge_index,
                                 const float* edge_weight, int normalization, float lambda_max, uint32_t flags,
                                 void* stream, stmp_plan** out) {
   STMP_REQUIRE(flavor != STMP_FLAVOR_RGCN, STMP_EINVAL, "stmp_plan_create: the RGCN flavor is built by stmp_plan_create_rgcn");
+  STMP_REQUIRE(flavor != STMP_FLAVOR_GATED, STMP_EINVAL, "stmp_plan_create: the GATED flavor is built by stmp_plan_create_gated");
   return plan_create_impl(flavor, num_nodes, num_edges, edge_index, edge_weight, normalization, lambda_max, nullptr, flags, stream, out);
 }
 
@@ -941,6 +970,13 @@ extern "C" int stmp_plan_create_rgcn(int64_t num_nodes, int64_t num_edges, const
   STMP_REQUIRE(edge_type != nullptr || num_edges == 0, STMP_EINVAL, "stmp_plan_create_rgcn: edge_type is NULL");
   return plan_create_impl(STMP_FLAVOR_RGCN, num_nodes, num_edges, edge_index, nullptr, STMP_NORM_NONE, 0.f, nullptr, 0u, stream, out,
                           edge_type, rel0, n_rel);
+}
+
+extern "C" int stmp_plan_create_gated(int64_t num_nodes, int64_t num_edges, const int64_t* edge_index, const float* edge_weight,
+                                      int aggr, void* stream, stmp_plan** out) {
+  STMP_REQUIRE(aggr >= STMP_AGGR_ADD && aggr <= STMP_AGGR_MAX, STMP_EINVAL, "stmp_plan_create_gated: unknown aggregation %d", aggr);
+  return plan_create_impl(STMP_FLAVOR_GATED, num_nodes, num_edges, edge_index, edge_weight, STMP_NORM_NONE, 0.f, nullptr, 0u, stream, out,
+                          nullptr, 0, 0, aggr);
 }
 
 extern "C" int stmp_plan_create_pergraph(int flavor, int64_t num_nodes, int64_t num_edges, const int64_t* edge_index,
@@ -954,10 +990,11 @@ extern "C" int stmp_plan_create_pergraph(int flavor, int64_t num_nodes, int64_t 
 
 static int plan_create_impl(int flavor, int64_t num_nodes, int64_t num_edges, const int64_t* edge_index,
                             const float* edge_weight, int normalization, float lambda_max, const float* lambda_node,
-                            uint32_t flags, void* stream, stmp_plan** out, const int64_t* edge_type, int64_t rel0, int n_rel) {
+                            uint32_t flags, void* stream, stmp_plan** out, const int64_t* edge_type, int64_t rel0, int n_rel,
+                            int aggr) {
   STMP_REQUIRE(out != nullptr, STMP_EINVAL, "stmp_plan_create: out is NULL");
   *out = nullptr;
-  STMP_REQUIRE(flavor >= STMP_FLAVOR_DCONV && flavor <= STMP_FLAVOR_RGCN, STMP_EINVAL, "unknown flavor %d", flavor);
+  STMP_REQUIRE(flavor >= STMP_FLAVOR_DCONV && flavor <= STMP_FLAVOR_GATED, STMP_EINVAL, "unknown flavor %d", flavor);
   STMP_REQUIRE(normalization >= STMP_NORM_NONE && normalization <= STMP_NORM_RW, STMP_EINVAL,
                "Invalid normalization %d", normalization);
   STMP_REQUIRE(num_nodes > 0 && num_nodes < (1ll << 30), STMP_EINVAL, "num_nodes=%lld out of range", (long long)num_nodes);
@@ -994,6 +1031,7 @@ static int plan_create_impl(int flavor, int64_t num_nodes, int64_t num_edges, co
       case STMP_FLAVOR_GCN: rc = build_gcn(b, p, n, e, row, col, edge_weight); break;
       case STMP_FLAVOR_CHEB_ATT: rc = build_cheb_att(b, p, n, e, row, col, edge_weight, lambda_max, lambda_node); break;
       case STMP_FLAVOR_RGCN: rc = build_rgcn(b, p, n, e, row, col, (const long long*)edge_type, rel0, n_rel); break;
+      case STMP_FLAVOR_GATED: rc = build_gated(b, p, n, e, row, col, edge_weight, aggr); break;
     }
     if (rc) break;
     Info h;

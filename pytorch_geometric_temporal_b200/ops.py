@@ -595,6 +595,76 @@ def lstm_rows_train(plan: GraphPlan, variant: int, n_ops: int, x, h, c, w, b, pe
     return _LstmRowsFn.apply(plan, variant, n_ops, x, h, c, w, b, peep, tuple(spec), *params)
 
 
+def ggc_rows_supported(plan: GraphPlan, num_layers: int, cin: int, channels: int) -> bool:
+    return bool(_lib.lib().stmp_ggc_rows_supported(plan.handle, num_layers, cin, channels))
+
+
+def _ggc_scratch(plan: GraphPlan, C: int, device) -> torch.Tensor:
+    return torch.empty(int(_lib.lib().stmp_ggc_rows_scratch_bytes(plan.handle, C)) // 4, device=device, dtype=torch.float32)
+
+
+def ggc_rows_fwd(plan: GraphPlan, x: torch.Tensor, W: torch.Tensor, w_ih, w_hh, b_ih, b_hh, train: bool = False):
+    """GatedGraphConv on a gated plan (stmp_ggc_rows_fwd): x (N, cin) -> x^L (N, C), W (L, C, C), W_ih / W_hh (3C, C), b_ih / b_hh (3C,);
+    L launches (L + 1 for max).  With `train`, returns (out, stash (L, 8, N, C)), the operand of ggc_rows_bwd / ggc_rows_wgrad."""
+    x, W = _f32c(x, "X"), _f32c(W, "weight")
+    w_ih, w_hh, b_ih, b_hh = (_f32c(t, n) for t, n in ((w_ih, "weight_ih"), (w_hh, "weight_hh"), (b_ih, "bias_ih"), (b_hh, "bias_hh")))
+    L, C = W.size(0), W.size(-1)
+    N, cin = x.shape
+    f32 = dict(device=x.device, dtype=torch.float32)
+    out = torch.empty(N, C, **f32)
+    stash = torch.empty(L, 8, N, C, **f32) if train else None
+    scr = None if train else _ggc_scratch(plan, C, x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.lib().stmp_ggc_rows_fwd(plan.handle, L, cin, C, _lib.ptr(x), _lib.ptr(W), _lib.ptr(w_ih), _lib.ptr(w_hh),
+                                                _lib.ptr(b_ih), _lib.ptr(b_hh), _lib.ptr(scr), _lib.ptr(out), _lib.ptr(stash),
+                                                _lib.stream_ptr()))
+    return (out, stash) if train else out
+
+
+class _GgcRowsFn(torch.autograd.Function):
+    """Training form of the row-split GatedGraphConv.  forward = `stmp_ggc_rows_fwd` with the stash (the inference launches, so the output
+    is bit-identical to the `no_grad` one); backward = `stmp_ggc_rows_bwd` + `stmp_ggc_rows_wgrad`: dX (when X requires grad) and the
+    gradients of W, W_ih, W_hh, b_ih and b_hh in their own layouts."""
+
+    @staticmethod
+    def forward(ctx, plan, x, W, w_ih, w_hh, b_ih, b_hh):
+        W, w_ih, w_hh = (_f32c(t.detach(), "weight") for t in (W, w_ih, w_hh))
+        out, stash = ggc_rows_fwd(plan, x.detach(), W, w_ih, w_hh, b_ih.detach(), b_hh.detach(), train=True)
+        ctx.plan, ctx.cin = plan, x.size(1)
+        ctx.save_for_backward(stash, W, w_ih, w_hh)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        stash, W, w_ih, w_hh = ctx.saved_tensors
+        plan, L, C, N = ctx.plan, W.size(0), W.size(-1), stash.size(2)
+        dev = stash.device
+        f32 = dict(device=dev, dtype=torch.float32)
+        gout = _f32c(gout, "gout")
+        dG = torch.empty(L, N, 4 * C, **f32)
+        dM = torch.empty(L, N, C, **f32)
+        dx = torch.empty(N, ctx.cin, **f32) if ctx.needs_input_grad[1] else None
+        L_ = _lib.lib()
+        with torch.cuda.device(dev):
+            _lib.check(L_.stmp_ggc_rows_bwd(plan.handle, L, ctx.cin, C, _lib.ptr(gout), _lib.ptr(stash), _lib.ptr(W), _lib.ptr(w_ih),
+                                            _lib.ptr(w_hh), _lib.ptr(_ggc_scratch(plan, C, dev)), _lib.ptr(dG), _lib.ptr(dM), _lib.ptr(dx),
+                                            _lib.stream_ptr()))
+        grads = [None] * 5
+        if any(ctx.needs_input_grad[2:]):
+            ws = _wgrad_workspace(dev, L_.stmp_ggc_rows_wgrad_workspace_bytes, L, C)
+            grads = [torch.empty(L, C, C, **f32), torch.empty(3 * C, C, **f32), torch.empty(3 * C, C, **f32),
+                     torch.empty(3 * C, **f32), torch.empty(3 * C, **f32)]
+            with torch.cuda.device(dev):
+                _lib.check(L_.stmp_ggc_rows_wgrad(plan.handle, L, C, _lib.ptr(stash), _lib.ptr(dG), _lib.ptr(dM), _lib.ptr(ws),
+                                                  *(_lib.ptr(g) for g in grads), _lib.stream_ptr()))
+        return (None, dx, *grads)
+
+
+def ggc_rows_train(plan: GraphPlan, x, W, w_ih, w_hh, b_ih, b_hh) -> torch.Tensor:
+    """Differentiable (w.r.t. x and the five parameters, see _GgcRowsFn) row-split GatedGraphConv: x (N, cin) -> x^L (N, C)."""
+    return _GgcRowsFn.apply(plan, x, W, w_ih, w_hh, b_ih, b_hh)
+
+
 def _tgcn_entry(co: int, name: str):
     """The library entry `name` of the fused TGCN kernels at hidden width `co`: stmp_tgcn_<name> at 32, stmp_tgcn_wide_<name> at 64."""
     if co not in (32, 64):

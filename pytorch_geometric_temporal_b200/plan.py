@@ -119,6 +119,31 @@ class RgcnPlan(GraphPlan):
         self.n_ops = _lib.lib().stmp_plan_num_ops(self._h)
 
 
+class GatedPlan(GraphPlan):
+    """PyG GatedGraphConv's aggregation operator (STMP_FLAVOR_GATED) for `aggr` ("add", "mean" or "max"): every edge in edge order,
+    value w_e (add, max) or w_e / (the destination's count of in-edges) (mean); edge_weight None means ones."""
+
+    def __init__(self, edge_index: torch.Tensor, edge_weight: Optional[torch.Tensor], num_nodes: int, aggr: str):
+        _require_cuda(edge_index, "edge_index")
+        if edge_index.dim() != 2 or edge_index.size(0) != 2:
+            raise ValueError(f"edge_index must have shape [2, E], got {tuple(edge_index.shape)}")
+        ei = edge_index.to(torch.int64).contiguous()
+        ew = None
+        if edge_weight is not None:
+            _require_cuda(edge_weight, "edge_weight")
+            ew = edge_weight.detach().to(torch.float32).reshape(-1).contiguous()
+            if ew.numel() != ei.size(1):
+                raise RuntimeError(f"edge_weight has {ew.numel()} entries for {ei.size(1)} edges")
+        self.flavor, self.num_nodes, self.num_edges, self.aggr = _lib.FLAVOR_GATED, int(num_nodes), int(ei.size(1)), aggr
+        self.device = ei.device
+        self._h = ctypes.c_void_p()
+        with torch.cuda.device(ei.device):
+            rc = _lib.lib().stmp_plan_create_gated(self.num_nodes, self.num_edges, _lib.ptr(ei), _lib.ptr(ew), _lib.AGGR_CODE[aggr],
+                                                   _lib.stream_ptr(), ctypes.byref(self._h))
+        _lib.check(rc)
+        self.n_ops = _lib.lib().stmp_plan_num_ops(self._h)
+
+
 class PlanCache:
     """Per-module cache keyed on the identity/version of the graph tensors (no device sync)."""
 
