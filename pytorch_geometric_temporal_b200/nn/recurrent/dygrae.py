@@ -3,11 +3,12 @@ conv_aggr, lstm_out_channels, lstm_num_layers)`, `forward(X, edge_index, edge_we
 `conv_layer` (PyG GatedGraphConv's parameters `weight`, `rnn.*`) and `recurrent_layer` (a torch.nn.LSTM), so the state_dict keys and a
 seeded initialisation equal the reference's.
 
-GatedGraphConv runs on the row-split kernels (stmp_ggc_rows_*, DESIGN §4r) for 2-D float32 X with in_channels <= C <= 32, any number of
-layers, any aggregation and edge_weight None or a constant float32 (E,) vector: one launch per layer (one more for max), with a
-hand-written backward.  The LSTM on top of it is the row-split LSTM cell on the basis [x | H] (stmp_lstm_rows_*, n_ops = 0) when C <= 16,
-lstm_out_channels is 32 or 64 and lstm_num_layers is 1; otherwise the convolution's output goes to the module's own torch.nn.LSTM.
-Everything else -- wider or non-float32 inputs, batched X, or `fused_training = False` for a training call -- runs op for op on the GPU
+GatedGraphConv runs on the row-split kernels (stmp_ggc_rows_*, DESIGN §4r) for 2-D float32 X with in_channels <= C <= 32, as many
+layers as the library supports (1 024; _conv_route asks ops.ggc_rows_supported), any aggregation and edge_weight None or a constant
+float32 (E,) vector: one launch per layer (one more for max), with a hand-written backward.  The LSTM on top of it is the row-split LSTM
+cell on the basis [x | H] (stmp_lstm_rows_*, n_ops = 0) when C <= 16, lstm_out_channels is 32 or 64 and lstm_num_layers is 1; otherwise
+the convolution's output goes to the module's own torch.nn.LSTM.  Everything else -- wider or non-float32 inputs, more layers, batched
+X, or `fused_training = False` for a training call -- runs op for op on the GPU
 (ops.spmm for add and mean in float32, index_select + scatter_reduce "amax" for max and index_add for other dtypes, then the GRUCell and
 the LSTM modules)."""
 import math
@@ -64,8 +65,8 @@ class DyGrEncoder(torch.nn.Module):
         return plan
 
     def _conv_ok(self, X, edge_weight, training):
-        """The row-split GatedGraphConv: 2-D float32 X with 1 <= in_channels <= C <= 32, float32 parameters, edge_weight None or a float32
-        (E,) vector that needs no gradient; training calls also need `fused_training`."""
+        """The module's own conditions for the row-split GatedGraphConv: 2-D float32 X with 1 <= in_channels <= C <= 32, float32
+        parameters, edge_weight None or a float32 (E,) vector that needs no gradient; training calls also need `fused_training`."""
         C = self.conv_out_channels
         if X.dim() != 2 or X.dtype != torch.float32 or not 1 <= X.size(1) <= C <= 32 or X.size(0) < 1:
             return False
@@ -74,6 +75,13 @@ class DyGrEncoder(torch.nn.Module):
         if edge_weight is not None and (edge_weight.dtype != torch.float32 or edge_weight.dim() != 1 or edge_weight.requires_grad):
             return False
         return not (training and not self.fused_training)
+
+    def _conv_route(self, plan, X, edge_weight, training):
+        """Whether the convolution runs on the row-split kernels: the module's conditions (_conv_ok), then the library's envelope for this
+        plan, layer count and width (ops.ggc_rows_supported: 1 024 layers at most), which is asked and never restated here."""
+        if not self._conv_ok(X, edge_weight, training):
+            return False
+        return ops.ggc_rows_supported(plan, self.conv_num_layers, X.size(1), self.conv_out_channels)
 
     def _lstm_ok(self, plan, N, H, C):
         """The row-split LSTM stage after a row-split convolution: C <= 16, lstm_out_channels 32 or 64, one LSTM layer, float32 LSTM
@@ -144,7 +152,7 @@ class DyGrEncoder(torch.nn.Module):
         params = list(self.parameters())
         needs_grad = torch.is_grad_enabled() and (any(p.requires_grad for p in params) or X.requires_grad
                                                   or (H is not None and H.requires_grad) or (C is not None and C.requires_grad))
-        if not self._conv_ok(X, edge_weight, needs_grad):
+        if not self._conv_route(plan, X, edge_weight, needs_grad):
             Ht = self._conv_op_for_op(plan, X, edge_index, edge_weight)
         else:
             g = self.conv_layer

@@ -160,6 +160,27 @@ def test_conv_routing_predicate(F, C, dtype, ew, training, fused, want):
     assert m._conv_ok(X.unsqueeze(0), None, training) is False
 
 
+@pytest.mark.parametrize("F,C,Lg,training,fused,want", [
+    (4, 4, 1, False, True, True), (4, 4, 1024, False, True, True), (4, 4, 1025, False, True, False), (4, 4, 1025, True, True, False),
+    (1, 32, 2, True, True, True), (5, 4, 2, False, True, False), (4, 4, 2, True, False, False)])
+def test_conv_route_asks_the_library(monkeypatch, F, C, Lg, training, fused, want):
+    """_conv_route: the module's own conditions (_conv_ok), then the library's envelope, asked through ops.ggc_rows_supported and
+    restated here (1 024 layers at most) so the route runs without the library.  The library is asked exactly when the module's
+    conditions hold, with the plan, L_g, in_channels and C."""
+    asked = []
+
+    def supported(plan, num_layers, cin, channels):
+        asked.append((plan, num_layers, cin, channels))
+        return 1 <= num_layers <= 1024 and 1 <= cin <= channels <= 32
+    monkeypatch.setattr(ops, "ggc_rows_supported", supported)
+    m = DyGrEncoder(C, Lg, "add", 32, 1)
+    m.fused_training = fused
+    X = torch.zeros(20, F)
+    plan = _Plan()
+    assert m._conv_route(plan, X, None, training) is want
+    assert asked == ([(plan, Lg, F, C)] if m._conv_ok(X, None, training) else [])
+
+
 @pytest.mark.parametrize("C,Ho,Ll,shape,dtype,want", [
     (4, 32, 1, None, torch.float32, True), (16, 64, 1, (20, 64), torch.float32, True), (17, 32, 1, None, torch.float32, False),
     (4, 48, 1, None, torch.float32, False), (4, 32, 2, None, torch.float32, False), (4, 32, 1, (32,), torch.float32, False),
