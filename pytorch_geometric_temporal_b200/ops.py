@@ -148,6 +148,7 @@ def dcrnn_seq_fwd(plan: GraphPlan, x: torch.Tensor, wz, wr, wh, bz, br, bh, K: i
     if B == 0 or T == 0:   # nothing to launch (empty tensors have NULL data pointers)
         return (out, st) if stash else out
     h0c = None if h0 is None else _f32c(h0, "H")
+    _require_numel("dcrnn_seq_fwd", B * N * cout, h0=h0c)                # every window reads its own (N, cout) state
     args = [_f32c(w.detach(), "weight") for w in (wz, wr, wh)]
     bs = [None if b is None else _f32c(b.detach(), "bias") for b in (bz, br, bh)]
     with torch.cuda.device(x.device):
@@ -184,6 +185,7 @@ def gru_seq_fwd(plan: GraphPlan, n_ops: int, x: torch.Tensor, wcat: torch.Tensor
     if h0 is not None:
         h0c = _f32c(h0, "H")
         hs = 0 if h0_shared else N * 32
+        _require_numel("gru_seq_fwd", N * 32 if h0_shared else B * N * 32, h0=h0c)   # the kernel reads h0 at batch stride hs
     with torch.cuda.device(x.device):
         rc = _lib.lib().stmp_gru_seq_fwd(plan.handle, n_ops, B, T, cin, _lib.ptr(x), None, T * N * cin, N * cin, _lib.ptr(wcat),
                                          _lib.ptr(bcat), _lib.ptr(h0c), hs, _lib.ptr(out), _lib.ptr(st), _lib.ptr(wimage),

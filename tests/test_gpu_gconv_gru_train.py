@@ -124,14 +124,17 @@ def test_fused_vs_autograd(cin, K, norm):
                         _close_grad(a, b)
 
 
-def _restated(plan, n_ops, x, h0, wcat, bcat):
-    """The recurrence of stmp_gru_seq_fwd chained op for op from differentiable SpMMs and torch ops."""
+def _restated(plan, n_ops, x, h0, wcat, bcat, spmm=None, stash=None):
+    """The recurrence of stmp_gru_seq_fwd chained op for op from differentiable SpMMs and torch ops.  `spmm(k, t)` applies operator k
+    (default: the plan's, `ops.spmm`); h0 (B, N, 32), or one (N, 32) state shared by every window.  A `stash` list receives the
+    kernel's stash of every step, (Z, R, H~)."""
     B, T, N, Ci = x.shape
-    H = x.new_zeros(B, N, 32) if h0 is None else h0
+    H = x.new_zeros(B, N, 32) if h0 is None else h0.expand(B, N, 32)
+    spmm = spmm or (lambda k, t: ops.spmm(plan, k, t))
 
     def A(X, Hp):
-        cols = [Hp] + [ops.spmm(plan, k, Hp) for k in range(n_ops)] + [Hp.new_zeros(B, N, 32)] * (2 - n_ops)
-        xs = [X] + [ops.spmm(plan, k, X) for k in range(n_ops)] + [X.new_zeros(B, N, Ci)] * (2 - n_ops)
+        cols = [Hp] + [spmm(k, Hp) for k in range(n_ops)] + [Hp.new_zeros(B, N, 32)] * (2 - n_ops)
+        xs = [X] + [spmm(k, X) for k in range(n_ops)] + [X.new_zeros(B, N, Ci)] * (2 - n_ops)
         pad = [X.new_zeros(B, N, 4 - Ci)] * 3
         xcols = [t for pair in zip(xs, pad) for t in pair]
         return torch.cat(cols + xcols + [X.new_zeros(B, N, 4)], dim=-1)
@@ -140,6 +143,8 @@ def _restated(plan, n_ops, x, h0, wcat, bcat):
         pre = A(x[:, t], H) @ wcat.t() + bcat
         Z, R = torch.sigmoid(pre[..., :32]), torch.sigmoid(pre[..., 32:64])
         Ht = torch.tanh((A(x[:, t], H * R) @ wcat.t() + bcat)[..., 64:])
+        if stash is not None:
+            stash.append((Z, R, Ht))
         H = Z * H + (1 - Z) * Ht
         outs.append(H)
     return torch.stack(outs, dim=1)

@@ -59,6 +59,15 @@ with torch.enable_grad():
     for K in (1, 2):                                           # GConvGRU training: stashing forward, k_gru_pack_bwd_weights,
         gg = GConvGRU(2, 32, K).to(dev)                          # k_gru_bwd_basis, k_gru_bwd_seq (CTA pair), k_dcrnn_wgrad_tc, k_gru_wgrad_reduce
         gg(X[0, 0], ei_t, ew_t, torch.randn(207, 32, device=dev, requires_grad=True)).square().mean().backward()
+    # the generic graph-GRU envelope (tests/test_gpu_gru_seq_envelope.py): K = 1 (n_ops = 0) with H = None and dX; the one-CTA backward
+    # at one operator, SMs / 2 + 1 windows; a forward from one h0 shared by every window
+    GConvGRU(2, 32, 1).to(dev)(X[0, 0].clone().requires_grad_(True), ei_t, ew_t).square().mean().backward()
+    nb = torch.cuda.get_device_properties(dev).multi_processor_count // 2 + 1
+    pg, (wg_, bg, ig), (sg, prm) = gg._cheb_plan(ei_t, ew_t, 207, "sym", None), gg._packed(), gg._param_spec()
+    xb = torch.randn(nb, 2, 207, 2, device=dev, requires_grad=True)
+    ops.gru_seq_train(pg, 1, xb, torch.randn(nb, 207, 32, device=dev, requires_grad=True), wg_, bg, ig, sg, prm).square().mean().backward()
+    with torch.no_grad():
+        ops.gru_seq_fwd(pg, 1, xb.detach(), wg_, bg, h0=torch.randn(207, 32, device=dev), h0_shared=True, wimage=ig)
     ring = torch.arange(301, device=dev)
     e_ring = torch.cat([torch.stack([ring, (ring + 1) % 301]), torch.stack([(ring + 5) % 301, ring])], dim=1)
     gr = GConvGRU(14, 32, 2).to(dev)                             # 301 nodes: the row-split cell kernels (k_gru_rows_*), H given and None,
