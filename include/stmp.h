@@ -127,6 +127,11 @@ int64_t stmp_plan_graph_image(const stmp_plan* plan, int n_ops, void* dst, int64
  * capacity >= that size, the image is written to dst (host memory).  Needs no GPU. */
 int64_t stmp_row_image_build(int64_t num_nodes, int n_ops, const int32_t* rowptr0, const int32_t* col0, const float* val0,
                              const int32_t* rowptr1, const int32_t* col1, const float* val1, void* dst, int64_t capacity);
+/* The same image with the nodes sorted by operator 0's group count, then operator 1's: the image a plan gives the kernel whenever it
+ * fits (stmp_row_image_build's nodes are sorted by the sum of both, which decides whether a plan has an image at all).  Arguments
+ * and return value as stmp_row_image_build. */
+int64_t stmp_row_image_build_by_operator(int64_t num_nodes, int n_ops, const int32_t* rowptr0, const int32_t* col0, const float* val0,
+                                         const int32_t* rowptr1, const int32_t* col1, const float* val1, void* dst, int64_t capacity);
 
 /* ---- K1/K3: gather -> weighted scatter-add (SpMM) with fused Chebyshev axpby -------------------
  * y[b,i,:] = alpha * sum_k val_k * x[b, col_k, :] + beta * z[b,i,:]        (z may be NULL)

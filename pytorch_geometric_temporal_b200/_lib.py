@@ -40,6 +40,7 @@ _SIGNATURES = {
     "stmp_plan_export": (c_int, [_P, c_int, c_int, _P, _P, _P, _P, _P]),
     "stmp_plan_graph_image": (c_int64, [_P, c_int, _P, c_int64]),
     "stmp_row_image_build": (c_int64, [c_int64, c_int, _P, _P, _P, _P, _P, _P, _P, c_int64]),
+    "stmp_row_image_build_by_operator": (c_int64, [c_int64, c_int, _P, _P, _P, _P, _P, _P, _P, c_int64]),
     "stmp_spmm": (c_int, [_P, c_int, c_int, c_int64, c_int64, _P, c_int64, c_int64, _P, c_int64, c_int64, c_float,
                           _P, c_int64, c_int64, c_float, _P, _P]),
     "stmp_spmm_att_t": (c_int, [_P, c_int, c_int64, c_int64, _P, c_int64, c_int64, _P, c_int64, c_int64, c_float, _P, c_int64, c_int64,

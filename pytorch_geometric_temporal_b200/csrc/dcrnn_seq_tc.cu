@@ -630,6 +630,13 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_tc(const TcParams p) {
 // the outputs are bit-identical to it.
 constexpr int RF_UBUF = kRiPos * 32;   // floats per gather buffer
 
+// Measurement only, never set in a shipped build: -DSTMP_RF_OMIT=1 compiles the per-step gathers of k_dcrnn_seq_rf out (the
+// diffusion fragments are zero), -DSTMP_RF_OMIT=2 its wgmmas (the gates read zero accumulators).  The results are wrong; the launch
+// times of the two builds against the full one give the step's phase breakdown (DESIGN §4).
+#ifndef STMP_RF_OMIT
+#define STMP_RF_OMIT 0
+#endif
+
 // 8 floats of a row in fragment order (v[2jj + x] = channel 8jj + 2q + x) <-> the two 16-byte chunks 2q, 2q+1 of the row; `par`
 // (quad parity) selects which chunk is touched first
 __device__ __forceinline__ void rf_ld_row(const float* row, int q, int par, float (&v)[8]) {
@@ -764,10 +771,17 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_rf(const TcParams p) {
   // Accumulators: GEMM 1 z in [0, 16), r in [16, 32); GEMM 2 the candidate.  Value of fragment row e, channel 8jj + 2q + x at
   // 4jj + 2e + x (+16 for r).
   float acc1[32], acc2[16];
+  if (STMP_RF_OMIT == 2) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc1[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc2[i] = 0.f;
+  }
   // A fragments, [k-step of the block][register]: H | H*R (k-steps 0, 1), P_o (2, 3), P_i (4, 5); X (k-step 6)
   uint32_t aH_hi[2][4], aH_lo[2][4], aO_hi[2][4], aO_lo[2][4], aI_hi[2][4], aI_lo[2][4], aX_hi[4], aX_lo[4];
 
   auto mma = [&](int gm, int ks, int pass, const uint32_t (&a)[4]) {
+    if (STMP_RF_OMIT == 2) return;
     const uint32_t bb = pass == 1 ? b_lo_s : b_hi_s;
     const uint32_t bk = bb + (ks >> 2) * TC_PANEL_B + (ks & 3) * 32;
     const bool first = ks == 0 && pass == 0;   // overwrites the accumulator
@@ -809,7 +823,7 @@ __global__ void __launch_bounds__(512, 1) k_dcrnn_seq_rf(const TcParams p) {
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
       float v[8];
-      if (p.n_ops > op) {
+      if (STMP_RF_OMIT != 1 && p.n_ops > op) {
         rf_gather(Ub, s_idx, s_val, s_gstart[ri_list(warp, op, e)], s_gcount[ri_list(warp, op, e)], quad, q, par, v);
       } else {
 #pragma unroll

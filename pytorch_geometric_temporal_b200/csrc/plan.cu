@@ -834,10 +834,14 @@ int build_graph_images(Builder& b, stmp_plan* p) {
   const int* cls[2] = {cl[0].data(), cl[1].data()};
   const float* vls[2] = {vl[0].data(), vl[1].data()};
   for (int n_ops = 1; n_ops <= p->n_ops; ++n_ops) {
-    const int64_t bytes = build_row_image(N, n_ops, rps, cls, vls, nullptr, 0);
+    // which graphs get an image is decided by the by-total image, as it always was; the kernel gets the by-operator one when that fits
+    int64_t bytes = build_row_image(N, n_ops, rps, cls, vls, ROW_ORDER_BY_TOTAL, nullptr, 0);
     if (bytes <= 0 || bytes > tc_row_image_budget()) continue;
+    RowOrder order = ROW_ORDER_BY_OPERATOR;
+    const int64_t by_op = build_row_image(N, n_ops, rps, cls, vls, order, nullptr, 0);
+    if (by_op <= tc_row_image_budget()) bytes = by_op; else order = ROW_ORDER_BY_TOTAL;
     std::vector<unsigned char> img((size_t)bytes);
-    build_row_image(N, n_ops, rps, cls, vls, img.data(), bytes);
+    build_row_image(N, n_ops, rps, cls, vls, order, img.data(), bytes);
     STMP_CUDA_OK(cudaMalloc(&p->rimg[n_ops], (size_t)bytes));
     STMP_CUDA_OK(cudaMemcpy(p->rimg[n_ops], img.data(), (size_t)bytes, cudaMemcpyHostToDevice));
     p->rimg_groups[n_ops] = reinterpret_cast<const int*>(img.data())[0];
@@ -855,8 +859,8 @@ void free_csr(Csr& c) {
 }  // namespace
 
 // ---- row image for the one-CTA wgmma kernel (row_image.cuh) -------------------------------------------------------------
-int64_t build_row_image(int N, int n_ops, const int* const rowptr[2], const int* const col[2], const float* const val[2], void* dst,
-                        int64_t capacity) {
+int64_t build_row_image(int N, int n_ops, const int* const rowptr[2], const int* const col[2], const float* const val[2], RowOrder order_by,
+                        void* dst, int64_t capacity) {
   if (N < 1 || N > kRiMaxN || n_ops < 1 || n_ops > 2) return 0;
   std::vector<int> ng(2 * N, 0);   // groups of 4 entries per (operator, row)
   for (int op = 0; op < n_ops; ++op)
@@ -867,10 +871,14 @@ int64_t build_row_image(int N, int n_ops, const int* const rowptr[2], const int*
         if (col[op][k] < 0 || col[op][k] >= N) return 0;
       ng[op * N + i] = (end - beg + 3) / 4;
     }
-  // nodes by descending group count over both operators (ties: node id), then the empty positions
+  // nodes by descending group count -- of both operators together, or of operator 0 and then operator 1 (ties: node id) -- then the
+  // empty positions
   std::vector<int> order(N);
   std::iota(order.begin(), order.end(), 0);
-  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return ng[a] + ng[N + a] > ng[b] + ng[N + b]; });
+  if (order_by == ROW_ORDER_BY_OPERATOR)
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return ng[a] != ng[b] ? ng[a] > ng[b] : ng[N + a] > ng[N + b]; });
+  else
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return ng[a] + ng[N + a] > ng[b] + ng[N + b]; });
   order.resize(kRiPos, -1);
   // bins of 8 consecutive nodes (one row per quad of a (warp, slot)); a bin's gather runs as long as its longest row per operator
   constexpr int kBins = kRiPos / 8;
@@ -1110,7 +1118,17 @@ extern "C" int64_t stmp_row_image_build(int64_t num_nodes, int n_ops, const int3
   const int* rp[2] = {rowptr0, rowptr1};
   const int* cl[2] = {col0, col1};
   const float* vl[2] = {val0, val1};
-  return build_row_image((int)num_nodes, n_ops, rp, cl, vl, dst, capacity);
+  return build_row_image((int)num_nodes, n_ops, rp, cl, vl, ROW_ORDER_BY_TOTAL, dst, capacity);
+}
+
+extern "C" int64_t stmp_row_image_build_by_operator(int64_t num_nodes, int n_ops, const int32_t* rowptr0, const int32_t* col0,
+                                                    const float* val0, const int32_t* rowptr1, const int32_t* col1, const float* val1,
+                                                    void* dst, int64_t capacity) {
+  if (num_nodes < 1 || num_nodes > kRiMaxN || n_ops < 1 || n_ops > 2 || !rowptr0 || (n_ops > 1 && !rowptr1)) return 0;
+  const int* rp[2] = {rowptr0, rowptr1};
+  const int* cl[2] = {col0, col1};
+  const float* vl[2] = {val0, val1};
+  return build_row_image((int)num_nodes, n_ops, rp, cl, vl, ROW_ORDER_BY_OPERATOR, dst, capacity);
 }
 
 /* Test hook: select, at run time, the implementation or launch shape a test cross-checks against the default (common.cuh). */
