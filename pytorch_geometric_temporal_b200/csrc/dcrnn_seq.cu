@@ -387,6 +387,13 @@ int launch(const Layout& L, int grid, cudaStream_t st) {
   STMP_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
   kern<<<grid, NW * 32, L.smem_bytes, st>>>(L.p);
   STMP_LAUNCH_OK("k_dcrnn_seq");
+  // per-instance launch counter ("k_dcrnn_seq[<OUT,RT,NW>]"), so callers and tests can see which row mapping served a call
+  static const int slot = [] {
+    static char name[40];
+    snprintf(name, sizeof(name), "k_dcrnn_seq[<%d,%d,%d>]", OUT, RT, NW);
+    return path_slot(name);
+  }();
+  count_path(slot);
   return STMP_OK;
 }
 
@@ -476,8 +483,9 @@ extern "C" int stmp_dcrnn_seq_fwd(const stmp_plan* plan, int64_t B, int64_t T, i
   STMP_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   int grid = (int)(B < sms ? B : sms);
   cudaStream_t st = (cudaStream_t)stream;
-  if (cout == 16) return launch_rt<16>(L, grid, st);
-  return launch_rt<32>(L, grid, st);
+  const int rc = cout == 16 ? launch_rt<16>(L, grid, st) : launch_rt<32>(L, grid, st);
+  if (rc == STMP_OK && !p.use_tma) { static const int slotp = path_slot("k_dcrnn_seq[x-plain]"); count_path(slotp); }
+  return rc;
 }
 
 extern "C" int stmp_gru_seq_supported(const stmp_plan* plan, int n_ops, int64_t cin, int64_t cout) {
