@@ -533,6 +533,42 @@ int64_t stmp_ggc_rows_wgrad_workspace_bytes(int64_t num_layers, int64_t channels
 int stmp_ggc_rows_wgrad(const stmp_plan* plan, int64_t num_layers, int64_t channels, const float* stash, const float* dG, const float* dM,
                         void* workspace, float* dW, float* dw_ih, float* dw_hh, float* db_ih, float* db_hh, void* stream);
 
+/* ---- EvolveGCN-O and EvolveGCN-H (nn/recurrent/evolvegcno.py, evolvegcnh.py) on graphs of ANY size, split over CTAs by destination rows
+ * (evolvegcn_rows.cu).  One call replaces the reference's step: the torch GRU over the C rows of the weight (evolvegcno.py:186-189,
+ * evolvegcnh.py:97-100), TopKPooling for -H (evolvegcnh.py:95-96: PyG SelectTopK's score, stable sort and gather) and
+ * GCNConv_Fixed_W (evolvegcno.py:86-97, :190: gcn_norm, matmul and propagate).  The plan holds Op: STMP_FLAVOR_GCN (normalize=True, with
+ * STMP_GCN_IMPROVED / STMP_GCN_NO_SELF_LOOPS) or STMP_FLAVOR_GATED with STMP_AGGR_ADD (normalize=False: the raw edge weights, no self
+ * loops).  Envelope (stmp_evolvegcn_rows_supported): C 1..32, any number of nodes and edges; -H needs N >= C.  Exact fp32 (separate
+ * multiply and add in the gathers, FFMA in the contractions); deterministic (no atomics, every sum in a fixed order); no host sync and no
+ * allocation, so a call can be captured.  Weights in torch.nn.GRU's layouts: W_ih / W_hh (3C, C) in gate order r | z | n, b_ih / b_hh
+ * (3C); the evolving weight W (C, C), row r = batch entry r of the GRU; p (C) = TopKPooling's select.weight.
+ *   stmp_evolvegcn_rows_fwd:   x (N, C), w_prev = W_{t-1} -> w_new = W_t, out = Op x W_t (N, C).  p NULL: -O, W_t = GRU(W_{t-1},
+ *                              W_{t-1}), one launch.  p given: -H, two launches: s = tanh((x p) / |p|), perm = the C nodes of highest s
+ *                              (the lower index first on equal scores), W_t = GRU(x[perm] s[perm], W_{t-1}); perm (int32, C) and
+ *                              score = s[perm] (C) are written, and scratch of stmp_evolvegcn_rows_scratch_bytes(plan, C) bytes is used.
+ *                              Training passes stash (N, C) = Op x, the operand of the backward (NULL for inference); the outputs do not
+ *                              depend on it.
+ *   stmp_evolvegcn_rows_bwd:   gout = dL/dout (N, C) and the stash -> dx = Op^T gout W_t^T (N, C; nullable) and per-CTA partials of
+ *                              (Op x)^T gout in the workspace (stmp_evolvegcn_rows_workspace_bytes(plan, C) bytes).  One launch.
+ *   stmp_evolvegcn_rows_wgrad: one launch of one CTA after stmp_evolvegcn_rows_bwd on the same workspace: dL/dW_t = the fixed-order sum of
+ *                              the partials + g_wnew (dL/dW_t from later calls; NULL for none), then the GRU backward over the C rows ->
+ *                              dw_prev (-O: the input's and the hidden state's gradients added), dw_ih, dw_hh, db_ih, db_hh; -H (p given,
+ *                              with x, perm and score of the forward): dp and, when dx is given, the TopK term added to dx's rows perm.
+ * STMP_EINVAL for a NULL plan or tensor or a plan of another flavor, STMP_ESHAPE for a misaligned tensor, STMP_EUNSUPPORTED outside the
+ * envelope (C outside 1..32, a GatedGraphConv plan that is not add, -H on fewer than C nodes). */
+int stmp_evolvegcn_rows_supported(const stmp_plan* plan, int64_t channels);
+int64_t stmp_evolvegcn_rows_scratch_bytes(const stmp_plan* plan, int64_t channels);
+int stmp_evolvegcn_rows_fwd(const stmp_plan* plan, int64_t channels, const float* x, const float* w_prev, const float* w_ih, const float* w_hh,
+                            const float* b_ih, const float* b_hh, const float* p, void* scratch, float* out, float* w_new, int32_t* perm,
+                            float* score, float* stash, void* stream);
+int64_t stmp_evolvegcn_rows_workspace_bytes(const stmp_plan* plan, int64_t channels);
+int stmp_evolvegcn_rows_bwd(const stmp_plan* plan, int64_t channels, const float* gout, const float* stash, const float* w_new,
+                            void* workspace, float* dx, void* stream);
+int stmp_evolvegcn_rows_wgrad(const stmp_plan* plan, int64_t channels, void* workspace, const float* g_wnew, const float* x,
+                              const float* w_prev, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* p,
+                              const int32_t* perm, const float* score, float* dw_prev, float* dw_ih, float* dw_hh, float* db_ih,
+                              float* db_hh, float* dp, float* dx, void* stream);
+
 /* ---- the same cell at 64 hidden channels (lstm_rows.cu, the width-2 instance of its kernels): GConvLSTM / GCLSTM(cin, 64, K <= 2).
  * Envelope: cout = 64, cin 1..16, n_ops 0..1 and at most the plan's operators (stmp_lstm_rows_supported(plan, variant, n_ops, cin, 64)),
  * any number of nodes and any degree.  Same argument lists, launch chain and guarantees as the stmp_lstm_rows_* entries, with 32 -> 64

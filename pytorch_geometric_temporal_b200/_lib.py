@@ -118,6 +118,12 @@ _SIGNATURES = {
     "stmp_ggc_rows_wgrad_workspace_bytes": (c_int64, [c_int64, c_int64]),
     "stmp_ggc_rows_wgrad": (c_int, [_P, c_int64, c_int64] + [_P] * 10),
     "stmp_lstm_rows_wgrad2": (c_int, [c_int64, c_int64, c_int64] + [_P] * 6),
+    "stmp_evolvegcn_rows_supported": (c_int, [_P, c_int64]),
+    "stmp_evolvegcn_rows_scratch_bytes": (c_int64, [_P, c_int64]),
+    "stmp_evolvegcn_rows_fwd": (c_int, [_P, c_int64] + [_P] * 14),
+    "stmp_evolvegcn_rows_workspace_bytes": (c_int64, [_P, c_int64]),
+    "stmp_evolvegcn_rows_bwd": (c_int, [_P, c_int64] + [_P] * 6),
+    "stmp_evolvegcn_rows_wgrad": (c_int, [_P, c_int64] + [_P] * 19),
     "stmp_lstm_wide_rows_pack_weights": (c_int, [c_int, c_int, c_int64] + [_P] * 8),
     "stmp_lstm_wide_rows_fwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 10 + [c_int64, _P]),
     "stmp_lstm_wide_rows_scratch_bytes": (c_int64, [_P]),

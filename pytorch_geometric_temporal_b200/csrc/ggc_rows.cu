@@ -21,8 +21,8 @@ namespace {
 
 using namespace rows;
 
-constexpr int kGgcMaxC = 32;
-constexpr int kGP = kGgcMaxC + 1;            // staged pitch: lane-indexed rows and lane-indexed columns are both conflict-free
+constexpr int kGgcMaxC = kGruMaxC;
+constexpr int kGP = kGruPitch;               // the staged pitch of the GRUCell and row products (rows.cuh)
 constexpr int kGgcMaxLayers = 1024;         // the weight-gradient grid holds one row of CTAs per layer
 constexpr int kSlots = 8;                    // stash slots per layer
 enum Slot { kX = 0, kPre = 1, kIn = 2, kR = 3, kZ = 4, kN = 5, kHn = 6, kCnt = 7 };
@@ -56,20 +56,6 @@ __device__ __forceinline__ void stage(GgcSmem& s, const float* __restrict__ Wl, 
       }
   }
   __syncthreads();
-}
-
-// y[c] = sum_{k < K} v[k] W[k][c]: lane c, W staged at pitch kGP
-__device__ __forceinline__ float row_times_w(const float* __restrict__ w, float v, int K, int lc) {
-  float y = 0.f;
-  for (int k = 0; k < K; ++k) y = fmaf(__shfl_sync(0xffffffffu, v, k), w[k * kGP + lc], y);
-  return y;
-}
-
-// y[k] = sum_{c < C} v[c] W[k][c] (v W^T): lane k
-__device__ __forceinline__ float row_times_wt(const float* __restrict__ w, float v, int C, int lc) {
-  float y = 0.f;
-  for (int c = 0; c < C; ++c) y = fmaf(__shfl_sync(0xffffffffu, v, c), w[lc * kGP + c], y);
-  return y;
 }
 
 struct GgcFwd {
@@ -178,19 +164,8 @@ __global__ void __launch_bounds__(kRowsThreads) k_ggc_rows_fwd(GgcFwd a, int l) 
         gather_row<false>(a.rowptr, a.cv, i, nullptr, 0, xl, kin, kin, lane, unused, pre);
         gin = row_times_w(s.w, pre, kin, lc);
       }
-      float gr = bir, gz = biz, gn = bin, hr = bhr, hz = bhz, hn = bhn;
-      for (int k = 0; k < C; ++k) {
-        const float u = __shfl_sync(0xffffffffu, gin, k), v = __shfl_sync(0xffffffffu, hv, k);
-        gr = fmaf(u, s.ih[lc * kGP + k], gr);
-        gz = fmaf(u, s.ih[(C + lc) * kGP + k], gz);
-        gn = fmaf(u, s.ih[(2 * C + lc) * kGP + k], gn);
-        hr = fmaf(v, s.hh[lc * kGP + k], hr);
-        hz = fmaf(v, s.hh[(C + lc) * kGP + k], hz);
-        hn = fmaf(v, s.hh[(2 * C + lc) * kGP + k], hn);
-      }
-      const float r = sigmoidf_acc(gr + hr), z = sigmoidf_acc(gz + hz);
-      const float nn = tanhf(gn + r * hn);
-      const float h1 = (1.f - z) * nn + z * hv;
+      const GruFwd g = gru_cell_fwd(s.ih, s.hh, gin, hv, bir, biz, bin, bhr, bhz, bhn, C, lc);
+      const float r = g.r, z = g.z, nn = g.n, hn = g.hn, h1 = g.h;
       if (mo) {
         const float y = row_times_w(s.w, h1, C, lc);
         if (lane < C) mo[(size_t)i * C + lane] = y;
@@ -275,26 +250,13 @@ __global__ void __launch_bounds__(kRowsThreads) k_ggc_rows_bwd(GgcBwd a, int l) 
       if (lane < C) {
         r = sl[kR * NC + jo]; z = sl[kZ * NC + jo]; nn = sl[kN * NC + jo]; hn = sl[kHn * NC + jo]; hv = sl[kX * NC + jo];
       }
-      const float dn = dx * (1.f - z);
-      const float dzp = dx * (hv - nn) * z * (1.f - z);
-      const float dnp = dn * (1.f - nn * nn);
-      const float dhn = dnp * r;
-      const float drp = dnp * hn * r * (1.f - r);
+      const GruGrad gg = gru_cell_bwd_gates(dx, r, z, nn, hn, hv);
       if (lane < C) {
         float* g = a.dG + ((size_t)l * n + j) * 4 * C;
-        g[lane] = drp; g[C + lane] = dzp; g[2 * C + lane] = dnp; g[3 * C + lane] = dhn;
+        g[lane] = gg.dr; g[C + lane] = gg.dz; g[2 * C + lane] = gg.dn; g[3 * C + lane] = gg.dhn;
       }
       float din = 0.f, dh = dx * z;              // the gradients at the GRU input and (direct) at x^l
-      for (int c = 0; c < C; ++c) {
-        const float ur = __shfl_sync(0xffffffffu, drp, c), uz = __shfl_sync(0xffffffffu, dzp, c);
-        const float un = __shfl_sync(0xffffffffu, dnp, c), uh = __shfl_sync(0xffffffffu, dhn, c);
-        din = fmaf(ur, s.ih[c * kGP + lc], din);
-        din = fmaf(uz, s.ih[(C + c) * kGP + lc], din);
-        din = fmaf(un, s.ih[(2 * C + c) * kGP + lc], din);
-        dh = fmaf(ur, s.hh[c * kGP + lc], dh);
-        dh = fmaf(uz, s.hh[(C + c) * kGP + lc], dh);
-        dh = fmaf(uh, s.hh[(2 * C + c) * kGP + lc], dh);
-      }
+      gru_cell_bwd_inputs(s.ih, s.hh, gg, C, lc, din, dh);
       float opv = din;                           // max: dagg is the operand; add / mean: dm is dW_l's, da = dm W_l^T the operand
       if (!MAX) {
         opv = row_times_wt(s.w, din, C, lc);

@@ -1,6 +1,6 @@
 // rows.cuh -- the pieces shared by the row-split recurrent cells (gru_rows.cu, lstm_rows.cu): one warp per destination row, lane = output
 // channel (lane + 32 j for j < NC in the 64-wide instances), CTAs owning grid-strided tiles of kRowTile rows, weights staged once per CTA at pitch kWPitch, and the entry-order CSR gather.
-// Also the weight-gradient pieces of train.cu, gru_rows.cu and lstm_rows.cu: the FFMA contraction's launch, the part count of every
+// Also the lane-level torch GRUCell and C x C row products of ggc_rows.cu and evolvegcn_rows.cu, and the weight-gradient pieces of train.cu, gru_rows.cu and lstm_rows.cu: the FFMA contraction's launch, the part count of every
 // weight-gradient contraction, the fixed-order sum every reduce kernel adds the partials with, and the per-gate contraction and reduce of
 // the 64-wide cells.
 #pragma once
@@ -85,6 +85,76 @@ inline int rows_grid(int n) {
 }
 
 inline bool al4(const void* p) { return ((uintptr_t)p & 3u) == 0; }
+
+// ---- the lane-level torch GRUCell of ggc_rows.cu and evolvegcn_rows.cu: one warp per row, lane = channel (C <= 32), weights staged in
+// shared memory at pitch kGruPitch, W_ih / W_hh rows in gate order r | z | n ------------------------------------------------------------
+constexpr int kGruMaxC = 32;
+constexpr int kGruPitch = kGruMaxC + 1;     // staged pitch: lane-indexed rows and lane-indexed columns are both conflict-free
+
+// y[c] = sum_{k < K} v[k] W[k][c]: lane c, W staged at pitch kGruPitch
+__device__ __forceinline__ float row_times_w(const float* __restrict__ w, float v, int K, int lc) {
+  float y = 0.f;
+  for (int k = 0; k < K; ++k) y = fmaf(__shfl_sync(0xffffffffu, v, k), w[k * kGruPitch + lc], y);
+  return y;
+}
+
+// y[k] = sum_{c < C} v[c] W[k][c] (v W^T): lane k
+__device__ __forceinline__ float row_times_wt(const float* __restrict__ w, float v, int C, int lc) {
+  float y = 0.f;
+  for (int c = 0; c < C; ++c) y = fmaf(__shfl_sync(0xffffffffu, v, c), w[lc * kGruPitch + c], y);
+  return y;
+}
+
+struct GruFwd {
+  float r, z, n, hn, h;                      // the gates, W_hn h + b_hn, and the new state
+};
+
+// h' = GRUCell(x, h) of one row: lane c holds x[c] (gin) and h[c] (hv), bi* / bh* its channel's biases
+__device__ __forceinline__ GruFwd gru_cell_fwd(const float* __restrict__ ih, const float* __restrict__ hh, float gin, float hv, float bir,
+                                               float biz, float bin, float bhr, float bhz, float bhn, int C, int lc) {
+  float gr = bir, gz = biz, gn = bin, hr = bhr, hz = bhz, hn = bhn;
+  for (int k = 0; k < C; ++k) {
+    const float u = __shfl_sync(0xffffffffu, gin, k), v = __shfl_sync(0xffffffffu, hv, k);
+    gr = fmaf(u, ih[lc * kGruPitch + k], gr);
+    gz = fmaf(u, ih[(C + lc) * kGruPitch + k], gz);
+    gn = fmaf(u, ih[(2 * C + lc) * kGruPitch + k], gn);
+    hr = fmaf(v, hh[lc * kGruPitch + k], hr);
+    hz = fmaf(v, hh[(C + lc) * kGruPitch + k], hz);
+    hn = fmaf(v, hh[(2 * C + lc) * kGruPitch + k], hn);
+  }
+  const float r = sigmoidf_acc(gr + hr), z = sigmoidf_acc(gz + hz);
+  const float nn = tanhf(gn + r * hn);
+  return {r, z, nn, hn, (1.f - z) * nn + z * hv};
+}
+
+struct GruGrad {
+  float dr, dz, dn, dhn;                     // pre-activation gradients of r, z and n, and dhn = r dn (W_hn's)
+};
+
+// the pre-activation gradients of one row from dL/dh' (dh1) and the forward's gates
+__device__ __forceinline__ GruGrad gru_cell_bwd_gates(float dh1, float r, float z, float nn, float hn, float hv) {
+  const float dn = dh1 * (1.f - z);
+  const float dzp = dh1 * (hv - nn) * z * (1.f - z);
+  const float dnp = dn * (1.f - nn * nn);
+  const float dhn = dnp * r;
+  const float drp = dnp * hn * r * (1.f - r);
+  return {drp, dzp, dnp, dhn};
+}
+
+// din += [dr dz dn] W_ih (the gradient at the GRU input), dh += [dr dz dhn] W_hh (at h; enters as its direct part dh' z)
+__device__ __forceinline__ void gru_cell_bwd_inputs(const float* __restrict__ ih, const float* __restrict__ hh, const GruGrad& g, int C,
+                                                    int lc, float& din, float& dh) {
+  for (int c = 0; c < C; ++c) {
+    const float ur = __shfl_sync(0xffffffffu, g.dr, c), uz = __shfl_sync(0xffffffffu, g.dz, c);
+    const float un = __shfl_sync(0xffffffffu, g.dn, c), uh = __shfl_sync(0xffffffffu, g.dhn, c);
+    din = fmaf(ur, ih[c * kGruPitch + lc], din);
+    din = fmaf(uz, ih[(C + c) * kGruPitch + lc], din);
+    din = fmaf(un, ih[(2 * C + c) * kGruPitch + lc], din);
+    dh = fmaf(ur, hh[c * kGruPitch + lc], dh);
+    dh = fmaf(uz, hh[(C + c) * kGruPitch + lc], dh);
+    dh = fmaf(uh, hh[(2 * C + c) * kGruPitch + lc], dh);
+  }
+}
 
 }  // namespace rows
 

@@ -6,4 +6,5 @@ from .attentiontemporalgcn import A3TGCN, A3TGCN2  # noqa: F401
 from .gc_lstm import GCLSTM  # noqa: F401
 from .lrgcn import LRGCN  # noqa: F401
 from .dygrae import DyGrEncoder  # noqa: F401
+from .evolvegcn import EvolveGCNH, EvolveGCNO  # noqa: F401
 from ._cheb import ChebConv  # noqa: F401

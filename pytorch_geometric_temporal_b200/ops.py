@@ -667,6 +667,80 @@ def ggc_rows_train(plan: GraphPlan, x, W, w_ih, w_hh, b_ih, b_hh) -> torch.Tenso
     return _GgcRowsFn.apply(plan, x, W, w_ih, w_hh, b_ih, b_hh)
 
 
+def evolvegcn_rows_supported(plan: GraphPlan, channels: int) -> bool:
+    return bool(_lib.lib().stmp_evolvegcn_rows_supported(plan.handle, channels))
+
+
+def evolvegcn_rows_fwd(plan: GraphPlan, x: torch.Tensor, w_prev: torch.Tensor, w_ih, w_hh, b_ih, b_hh, p=None, train: bool = False):
+    """One EvolveGCN step (stmp_evolvegcn_rows_fwd): x (N, C), w_prev (C, C), the GRU's W_ih / W_hh (3C, C) and b_ih / b_hh (3C,), p (C,)
+    for -H or None for -O -> (out (N, C), w_new (C, C), perm (C,) int32 or None, score (C,) or None, stash (N, C) with `train`, else None).
+    One launch for -O, two for -H."""
+    x, w_prev = _f32c(x, "X"), _f32c(w_prev, "weight")
+    w_ih, w_hh, b_ih, b_hh = (_f32c(t, n) for t, n in ((w_ih, "weight_ih"), (w_hh, "weight_hh"), (b_ih, "bias_ih"), (b_hh, "bias_hh")))
+    N, C = x.shape
+    f32 = dict(device=x.device, dtype=torch.float32)
+    out, w_new = torch.empty(N, C, **f32), torch.empty(C, C, **f32)
+    stash = torch.empty(N, C, **f32) if train else None
+    perm = score = scr = None
+    if p is not None:
+        p = _f32c(p, "pooling weight")
+        perm, score = torch.empty(C, device=x.device, dtype=torch.int32), torch.empty(C, **f32)
+        scr = torch.empty(int(_lib.lib().stmp_evolvegcn_rows_scratch_bytes(plan.handle, C)), device=x.device, dtype=torch.uint8)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.lib().stmp_evolvegcn_rows_fwd(plan.handle, C, *(_lib.ptr(t) for t in (x, w_prev, w_ih, w_hh, b_ih, b_hh, p, scr, out,
+                                                                                              w_new, perm, score, stash)),
+                                                      _lib.stream_ptr()))
+    return out, w_new, perm, score, stash
+
+
+class _EvolveGCNRowsFn(torch.autograd.Function):
+    """Training form of one EvolveGCN step -> (out, w_new).  forward = `stmp_evolvegcn_rows_fwd` with the stash Op x, kept in ctx (the
+    inference launches, so the outputs are bit-identical to the `no_grad` ones); backward = `stmp_evolvegcn_rows_bwd` +
+    `stmp_evolvegcn_rows_wgrad`: dX (when X requires grad) and the gradients of w_prev, the four GRU tensors and p.  Either output's
+    gradient may be None; dL/dw_new enters the GRU backward with the convolution's."""
+
+    @staticmethod
+    def forward(ctx, plan, x, w_prev, w_ih, w_hh, b_ih, b_hh, p):
+        ctx.set_materialize_grads(False)
+        ts = [None if t is None else t.detach() for t in (x, w_prev, w_ih, w_hh, b_ih, b_hh, p)]
+        ts = [None if t is None else _f32c(t, "operand") for t in ts]
+        out, w_new, perm, score, stash = evolvegcn_rows_fwd(plan, *ts, train=True)
+        ctx.plan = plan
+        ctx.save_for_backward(*ts, perm, score, stash, w_new)
+        return out, w_new
+
+    @staticmethod
+    def backward(ctx, gout, gw):
+        x, w_prev, w_ih, w_hh, b_ih, b_hh, p, perm, score, stash, w_new = ctx.saved_tensors
+        if gout is None and gw is None:
+            return (None,) * 8
+        plan, dev = ctx.plan, x.device
+        N, C = x.shape
+        f32 = dict(device=dev, dtype=torch.float32)
+        gout = torch.zeros(N, C, **f32) if gout is None else _f32c(gout, "gout")
+        gw = None if gw is None else _f32c(gw, "gout")
+        dx = torch.empty(N, C, **f32) if ctx.needs_input_grad[1] else None
+        grads = [torch.empty(C, C, **f32), torch.empty(3 * C, C, **f32), torch.empty(3 * C, C, **f32), torch.empty(3 * C, **f32),
+                 torch.empty(3 * C, **f32)]
+        dp = torch.empty(C, **f32) if p is not None else None
+        L_ = _lib.lib()
+        ws = torch.empty(int(L_.stmp_evolvegcn_rows_workspace_bytes(plan.handle, C)), device=dev, dtype=torch.uint8)
+        with torch.cuda.device(dev):
+            _lib.check(L_.stmp_evolvegcn_rows_bwd(plan.handle, C, _lib.ptr(gout), _lib.ptr(stash), _lib.ptr(w_new), _lib.ptr(ws),
+                                                  _lib.ptr(dx), _lib.stream_ptr()))
+            _lib.check(L_.stmp_evolvegcn_rows_wgrad(plan.handle, C, _lib.ptr(ws), *(_lib.ptr(t) for t in (gw, x, w_prev, w_ih, w_hh, b_ih,
+                                                                                                          b_hh, p, perm, score, *grads, dp,
+                                                                                                          dx)),
+                                                    _lib.stream_ptr()))
+        want = ctx.needs_input_grad
+        return (None, dx, *(g if want[2 + i] else None for i, g in enumerate(grads)), dp if p is not None and want[7] else None)
+
+
+def evolvegcn_rows_train(plan: GraphPlan, x, w_prev, w_ih, w_hh, b_ih, b_hh, p=None):
+    """Differentiable (w.r.t. x, w_prev, the GRU's four tensors and p, see _EvolveGCNRowsFn) EvolveGCN step -> (out (N, C), w_new (C, C))."""
+    return _EvolveGCNRowsFn.apply(plan, x, w_prev, w_ih, w_hh, b_ih, b_hh, p)
+
+
 def _tgcn_entry(co: int, name: str):
     """The library entry `name` of the fused TGCN kernels at hidden width `co`: stmp_tgcn_<name> at 32, stmp_tgcn_wide_<name> at 64."""
     if co not in (32, 64):

@@ -168,12 +168,22 @@ class PlanCache:
             else:
                 lam = float(lambda_max)  # scalar lambda_max (host value or 0-d tensor; a sync only if it is a tensor)
         key = (flavor, self._tkey(edge_index), self._tkey(edge_weight), int(num_nodes), normalization, lam, flags) + extra
+        return self._lookup(key, lambda: GraphPlan(flavor, edge_index, edge_weight, num_nodes, normalization, lam, flags,
+                                                   lambda_node=lam_node),
+                            (edge_index, edge_weight, lambda_max if extra else None, batch if extra else None))
+
+    def get_gated(self, edge_index, edge_weight, num_nodes, aggr) -> GatedPlan:
+        """The GatedPlan of `aggr` ("add", "mean" or "max") for this graph."""
+        key = (_lib.FLAVOR_GATED, self._tkey(edge_index), self._tkey(edge_weight), int(num_nodes), aggr)
+        return self._lookup(key, lambda: GatedPlan(edge_index, edge_weight, num_nodes, aggr), (edge_index, edge_weight))
+
+    def _lookup(self, key, make, keep):
         hit = self._entries.get(key)
         if hit is not None:
             return hit[0]
-        plan = GraphPlan(flavor, edge_index, edge_weight, num_nodes, normalization, lam, flags, lambda_node=lam_node)
+        plan = make()
         if len(self._entries) >= self._max:
             self._entries.pop(next(iter(self._entries)))
         # keep the keyed tensors alive so their addresses cannot be recycled while the entry exists
-        self._entries[key] = (plan, edge_index, edge_weight, lambda_max if extra else None, batch if extra else None)
+        self._entries[key] = (plan, *keep)
         return plan

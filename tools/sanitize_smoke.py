@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from pytorch_geometric_temporal_b200 import _lib, ops                                        # noqa: E402
 from pytorch_geometric_temporal_b200.dataset import synthetic                               # noqa: E402
 from pytorch_geometric_temporal_b200.nn.attention import ASTGCN                              # noqa: E402
-from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, DyGrEncoder, GCLSTM, GConvGRU, GConvLSTM, LRGCN, TGCN2   # noqa: E402
+from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, DyGrEncoder, EvolveGCNH, EvolveGCNO, GCLSTM, GConvGRU, GConvLSTM, LRGCN, TGCN2   # noqa: E402
 
 dev = torch.device("cuda")
 torch.manual_seed(0)
@@ -95,6 +95,11 @@ with torch.enable_grad():
         dy = DyGrEncoder(C, Lg, aggr, 32, 1).to(dev)            # _fwd / _bwd (with dX) / _wgrad + reduce, and the LSTM cell with n_ops = 0
         xg = xr[:, :C].detach().clone().requires_grad_(True)    # (C = 16) or the cuDNN LSTM (C = 32)
         sum(t.square().mean() for t in dy(xg, e_ring, w_ring)).backward()
+    for eg in (EvolveGCNO(14).to(dev), EvolveGCNH(301, 14).to(dev)):    # EvolveGCN: k_egcn_fwd / k_egcn_score + k_egcn_fwd_topk,
+        xe = xr.detach().clone().requires_grad_(True)                 # k_egcn_bwd_rows (with dX) and k_egcn_wgrad(_topk), two calls chained
+        (eg(xe, e_ring, w_ring).square().mean() + eg(xe, e_ring, w_ring).mean()).backward()
+        with torch.no_grad():
+            eg(xr, e_ring, None)
     for cin, T in ((2, 3), (4, 1)):                              # 301 nodes: the row-split DCRNN (k_dcrnn_rows_*), T = 1 and T > 1, with and
         dr = BatchedDCRNN(cin, 32, 2).to(dev)                    # without dX (k_dcrnn_rows_bwd_x), k_dcrnn_wgrad_tc + k_dcrnn_wgrad_reduce
         xd = torch.randn(2, T, 301, cin, device=dev)
