@@ -569,6 +569,52 @@ int stmp_evolvegcn_rows_wgrad(const stmp_plan* plan, int64_t channels, void* wor
                               const int32_t* perm, const float* score, float* dw_prev, float* dw_ih, float* dw_hh, float* db_ih,
                               float* db_hh, float* dp, float* dx, void* stream);
 
+/* ---- MPNN-LSTM (nn/recurrent/mpnn_lstm.py) on graphs of ANY size, split over CTAs by destination rows (mpnn_rows.cu).  One call replaces
+ * the reference's forward (mpnn_lstm.py:60-105): gcn_norm and two GCNConvs (shared: the plan's operator 0), ReLU, BatchNorm1d and
+ * dropout after each, the concatenation and transposes, and two cuDNN LSTMs over `window` steps.  The plan is STMP_FLAVOR_GCN with flags 0
+ * (remaining self loops of fill 1, as GCNConv's defaults) built on all R = B * window * num_nodes rows of x.  Envelope
+ * (stmp_mpnn_rows_supported): hidden = 32, cin 1..64, window >= 1 dividing R; any number of nodes and edges.  Exact fp32 (separate
+ * multiply and add in the gathers, FFMA in the contractions); deterministic (no atomics; BatchNorm's batch statistics are per-CTA
+ * Welford partials merged with Chan's formula in one fixed order by every CTA of the next launch); no host sync and no allocation, so a
+ * call can be captured.  Weights in the reference's layouts: w1 (32, cin), w2 (32, 32), b1 / b2 (32); BatchNorm weight / bias / running
+ * mean / running var (32) and num_batches_tracked (int64, 8-byte aligned); LSTM w_ih1 (128, 64), w_hh1 / w_ih2 / w_hh2 (128, 32), biases
+ * (128), gate order i | f | g | o.
+ *   stmp_mpnn_rows_fwd: x (R, cin) -> out (B num_nodes, 64 + cin + window - 1) = [h1 | h2 | S], S = every feature of step 0 and the last
+ *                       feature of steps 1 .. window-1.  training != 0: BatchNorm normalises with the batch mean and biased variance and
+ *                       updates the running statistics (unbiased variance) and num_batches_tracked in place; a negative momentum means
+ *                       None (1 / num_batches_tracked).  training = 0: the running statistics.  u (2, R, 32) or NULL: the dropout
+ *                       uniforms of both layers, kept where u >= p and scaled by 1 / (1 - p) (0 < p < 1; BatchNorm's mode aside).  Scratch of
+ *                       stmp_mpnn_rows_scratch_bytes(plan, cin, 32, window) bytes.  Three launches.
+ *                       Training passes stash (stmp_mpnn_rows_stash_bytes, 16-byte aligned): the convolutions' gathers, the LSTMs'
+ *                       gates and cell states, z2 and BatchNorm's statistics; NULL for inference.  The outputs do not depend on it.
+ *   stmp_mpnn_rows_bwd: after a training forward, with its scratch and stash (both kept) and gout = dL/dout: dx (R, cin; nullable) and
+ *                       dbn (4, 32) = dbeta1 | dgamma1 | dbeta2 | dgamma2; the other gradients' operands go to the workspace
+ *                       (stmp_mpnn_rows_workspace_bytes, 16-byte aligned).  training and p are the forward's (p = 0: it had no
+ *                       dropout).  Four launches, five with dx.
+ *   stmp_mpnn_rows_wgrad: after stmp_mpnn_rows_bwd on the same workspace: dw (320, 96) and db (320): rows 0..127 LSTM-1 ([dW_ih | dW_hh]
+ *                       in columns 0..95; db = db_ih = db_hh), rows 128..255 LSTM-2 (dW_ih columns 0..31, dW_hh 32..63), rows
+ *                       256..287 dW1 (columns 0..cin-1) and db1, rows 288..319 dW2 (columns ld1 .. ld1 + 31, ld1 = cin rounded up to 8)
+ *                       and db2.  Two launches; every sum in a fixed order.
+ * STMP_EINVAL for a NULL plan or tensor, a plan of another flavor, uniforms with p outside (0, 1), or one row in training mode; STMP_ESHAPE for a misaligned tensor or R not a multiple of window * num_nodes; STMP_EUNSUPPORTED outside the envelope (a GCN
+ * plan with flags included). */
+int stmp_mpnn_rows_supported(const stmp_plan* plan, int64_t cin, int64_t hidden, int64_t window);
+int64_t stmp_mpnn_rows_scratch_bytes(const stmp_plan* plan, int64_t cin, int64_t hidden, int64_t window);
+int stmp_mpnn_rows_fwd(const stmp_plan* plan, int64_t cin, int64_t hidden, int64_t window, int64_t num_nodes, const float* x, const float* w1,
+                       const float* b1, const float* w2, const float* b2, const float* bn1_weight, const float* bn1_bias, float* bn1_mean,
+                       float* bn1_var, int64_t* bn1_count, float bn1_eps, float bn1_momentum, const float* bn2_weight,
+                       const float* bn2_bias, float* bn2_mean, float* bn2_var, int64_t* bn2_count, float bn2_eps, float bn2_momentum,
+                       const float* w_ih1, const float* w_hh1, const float* b_ih1, const float* b_hh1, const float* w_ih2,
+                       const float* w_hh2, const float* b_ih2, const float* b_hh2, int training, float p, const float* u,
+                       void* scratch, void* stash, float* out, void* stream);
+int64_t stmp_mpnn_rows_stash_bytes(const stmp_plan* plan, int64_t cin, int64_t hidden, int64_t window);
+int64_t stmp_mpnn_rows_workspace_bytes(const stmp_plan* plan, int64_t cin, int64_t hidden, int64_t window);
+int stmp_mpnn_rows_bwd(const stmp_plan* plan, int64_t cin, int64_t hidden, int64_t window, int64_t num_nodes, const float* gout,
+                       const float* w1, const float* w2, const float* bn1_weight, const float* bn2_weight, const float* w_ih1,
+                       const float* w_hh1, const float* w_ih2, const float* w_hh2, int training, float p, void* scratch, void* stash,
+                       void* workspace, float* dx, float* dbn, void* stream);
+int stmp_mpnn_rows_wgrad(const stmp_plan* plan, int64_t cin, int64_t hidden, int64_t window, void* stash, void* workspace, float* dw,
+                         float* db, void* stream);
+
 /* ---- the same cell at 64 hidden channels (lstm_rows.cu, the width-2 instance of its kernels): GConvLSTM / GCLSTM(cin, 64, K <= 2).
  * Envelope: cout = 64, cin 1..16, n_ops 0..1 and at most the plan's operators (stmp_lstm_rows_supported(plan, variant, n_ops, cin, 64)),
  * any number of nodes and any degree.  Same argument lists, launch chain and guarantees as the stmp_lstm_rows_* entries, with 32 -> 64

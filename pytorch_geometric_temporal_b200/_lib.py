@@ -124,6 +124,14 @@ _SIGNATURES = {
     "stmp_evolvegcn_rows_workspace_bytes": (c_int64, [_P, c_int64]),
     "stmp_evolvegcn_rows_bwd": (c_int, [_P, c_int64] + [_P] * 6),
     "stmp_evolvegcn_rows_wgrad": (c_int, [_P, c_int64] + [_P] * 19),
+    "stmp_mpnn_rows_supported": (c_int, [_P, c_int64, c_int64, c_int64]),
+    "stmp_mpnn_rows_scratch_bytes": (c_int64, [_P, c_int64, c_int64, c_int64]),
+    "stmp_mpnn_rows_fwd": (c_int, [_P, c_int64, c_int64, c_int64, c_int64] + [_P] * 10 + [c_float, c_float] + [_P] * 5 + [c_float, c_float]
+                           + [_P] * 8 + [c_int, c_float] + [_P] * 5),
+    "stmp_mpnn_rows_stash_bytes": (c_int64, [_P, c_int64, c_int64, c_int64]),
+    "stmp_mpnn_rows_workspace_bytes": (c_int64, [_P, c_int64, c_int64, c_int64]),
+    "stmp_mpnn_rows_bwd": (c_int, [_P, c_int64, c_int64, c_int64, c_int64] + [_P] * 9 + [c_int, c_float] + [_P] * 6),
+    "stmp_mpnn_rows_wgrad": (c_int, [_P, c_int64, c_int64, c_int64] + [_P] * 5),
     "stmp_lstm_wide_rows_pack_weights": (c_int, [c_int, c_int, c_int64] + [_P] * 8),
     "stmp_lstm_wide_rows_fwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 10 + [c_int64, _P]),
     "stmp_lstm_wide_rows_scratch_bytes": (c_int64, [_P]),

@@ -7,4 +7,5 @@ from .gc_lstm import GCLSTM  # noqa: F401
 from .lrgcn import LRGCN  # noqa: F401
 from .dygrae import DyGrEncoder  # noqa: F401
 from .evolvegcn import EvolveGCNH, EvolveGCNO  # noqa: F401
+from .mpnn_lstm import MPNNLSTM  # noqa: F401
 from ._cheb import ChebConv  # noqa: F401

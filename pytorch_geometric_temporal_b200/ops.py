@@ -741,6 +741,96 @@ def evolvegcn_rows_train(plan: GraphPlan, x, w_prev, w_ih, w_hh, b_ih, b_hh, p=N
     return _EvolveGCNRowsFn.apply(plan, x, w_prev, w_ih, w_hh, b_ih, b_hh, p)
 
 
+def mpnn_rows_supported(plan: GraphPlan, cin: int, hidden: int, window: int) -> bool:
+    return bool(_lib.lib().stmp_mpnn_rows_supported(plan.handle, cin, hidden, window))
+
+
+def _mpnn_params(conv1, conv2, bn1, bn2, lstm1, lstm2):
+    """The 17 tensors one MPNN-LSTM call reads, in the order of _MpnnRowsFn's inputs."""
+    return (conv1.lin.weight, conv1.bias, conv2.lin.weight, conv2.bias, bn1.weight, bn1.bias, bn2.weight, bn2.bias,
+            *(getattr(m, k) for m in (lstm1, lstm2) for k in ("weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0")))
+
+
+def mpnn_rows_fwd(plan: GraphPlan, x: torch.Tensor, num_nodes: int, window: int, conv1, conv2, bn1, bn2, lstm1, lstm2, training: bool,
+                  p: float, u: Optional[torch.Tensor], params=None, train: bool = False):
+    """The MPNN-LSTM forward (stmp_mpnn_rows_fwd, three launches): x (R, cin) with R = B * window * num_nodes -> (B num_nodes,
+    64 + cin + window - 1) = [h1 | h2 | S].  conv1 / conv2 hold GCNConv's `lin.weight` (32, K) and `bias` (32); bn1 / bn2 are
+    BatchNorm1d(32) modules (affine, running statistics tracked; updated in place when `training`, BatchNorm's mode); lstm1 / lstm2
+    torch.nn.LSTM(64, 32) and (32, 32).  u (2, R, 32) holds the dropout uniforms (kept where u >= p) or None for no dropout.  `params`
+    overrides the 16 tensors of _mpnn_params.  Returns out, or (out, scratch, stash) with `train` (the backward's operands).  No
+    autograd."""
+    x = _f32c(x, "X")
+    R, cin = x.shape
+    ts = [_f32c(t.detach(), "MPNN-LSTM parameter") for t in (params or _mpnn_params(conv1, conv2, bn1, bn2, lstm1, lstm2))]
+    bns = []
+    for bn, (w, b) in ((bn1, ts[4:6]), (bn2, ts[6:8])):
+        mom = -1.0 if bn.momentum is None else float(bn.momentum)
+        bns.append(([_lib.ptr(w), _lib.ptr(b), _lib.ptr(bn.running_mean), _lib.ptr(bn.running_var), _lib.ptr(bn.num_batches_tracked)],
+                    float(bn.eps), mom))
+    if u is not None:
+        u = _f32c(u, "dropout uniforms")
+        _require_numel("mpnn_rows_fwd", 2 * R * 32, u=u)
+    out = torch.empty(R // window, 64 + cin + window - 1, device=x.device, dtype=torch.float32)
+    L_ = _lib.lib()
+    byt = lambda n: torch.empty(int(n), device=x.device, dtype=torch.uint8)
+    scr = byt(L_.stmp_mpnn_rows_scratch_bytes(plan.handle, cin, 32, window))
+    stash = byt(L_.stmp_mpnn_rows_stash_bytes(plan.handle, cin, 32, window)) if train else None
+    with torch.cuda.device(x.device):
+        _lib.check(L_.stmp_mpnn_rows_fwd(plan.handle, cin, 32, window, num_nodes, _lib.ptr(x), *(_lib.ptr(t) for t in ts[:4]), *bns[0][0],
+                                         bns[0][1], bns[0][2], *bns[1][0], bns[1][1], bns[1][2], *(_lib.ptr(t) for t in ts[8:]),
+                                         int(training), float(p), _lib.ptr(u), _lib.ptr(scr), _lib.ptr(stash), _lib.ptr(out),
+                                         _lib.stream_ptr()))
+    return (out, scr, stash) if train else out
+
+
+class _MpnnRowsFn(torch.autograd.Function):
+    """Training form of one MPNN-LSTM call.  forward = stmp_mpnn_rows_fwd with the stash (the inference launches: the outputs are
+    bit-identical to the no_grad ones for the same mode and masks), scratch and stash kept in ctx; backward = stmp_mpnn_rows_bwd +
+    stmp_mpnn_rows_wgrad: dX (when X requires grad) and the gradients of the 16 parameters."""
+
+    @staticmethod
+    def forward(ctx, plan, meta, x, *params):
+        num_nodes, window, mods, training, p, u = meta
+        out, scr, stash = mpnn_rows_fwd(plan, x.detach(), num_nodes, window, *mods, training, p, u, params=params, train=True)
+        ctx.plan, ctx.meta, ctx.scr, ctx.stash = plan, (num_nodes, window, training, p if u is not None else 0.0), scr, stash
+        ctx.save_for_backward(*(t.detach() for t in params))
+        ctx.shape = x.shape
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        ps = [_f32c(t, "MPNN-LSTM parameter") for t in ctx.saved_tensors]
+        num_nodes, window, training, p = ctx.meta
+        R, cin = ctx.shape
+        dev = gout.device
+        gout = _f32c(gout, "gout")
+        f32 = dict(device=dev, dtype=torch.float32)
+        dx = torch.empty(R, cin, **f32) if ctx.needs_input_grad[2] else None
+        dbn, dw, db = torch.empty(4, 32, **f32), torch.empty(320, 96, **f32), torch.empty(320, **f32)
+        L_, h = _lib.lib(), ctx.plan.handle
+        ws = torch.empty(int(L_.stmp_mpnn_rows_workspace_bytes(h, cin, 32, window)), device=dev, dtype=torch.uint8)
+        with torch.cuda.device(dev):
+            _lib.check(L_.stmp_mpnn_rows_bwd(h, cin, 32, window, num_nodes, _lib.ptr(gout), *(_lib.ptr(ps[i]) for i in (0, 2, 4, 6, 8, 9, 12,
+                                                                                                                      13)),
+                                             int(training), float(p), _lib.ptr(ctx.scr), _lib.ptr(ctx.stash), _lib.ptr(ws), _lib.ptr(dx),
+                                             _lib.ptr(dbn), _lib.stream_ptr()))
+            _lib.check(L_.stmp_mpnn_rows_wgrad(h, cin, 32, window, _lib.ptr(ctx.stash), _lib.ptr(ws), _lib.ptr(dw), _lib.ptr(db),
+                                               _lib.stream_ptr()))
+        ld1 = (cin + 7) // 8 * 8
+        grads = (dw[256:288, :cin], db[256:288], dw[288:320, ld1:ld1 + 32], db[288:320], dbn[1], dbn[0], dbn[3], dbn[2],
+                 dw[0:128, :64], dw[0:128, 64:96], db[0:128], db[0:128].clone(), dw[128:256, :32], dw[128:256, 32:64], db[128:256],
+                 db[128:256].clone())
+        want = ctx.needs_input_grad
+        return (None, None, dx, *(g if want[3 + i] else None for i, g in enumerate(grads)))
+
+
+def mpnn_rows_train(plan: GraphPlan, x, num_nodes: int, window: int, conv1, conv2, bn1, bn2, lstm1, lstm2, training: bool, p: float,
+                    u: Optional[torch.Tensor]) -> torch.Tensor:
+    """Differentiable (w.r.t. x and the 16 parameters of _mpnn_params, see _MpnnRowsFn) MPNN-LSTM call; arguments as mpnn_rows_fwd."""
+    mods = (conv1, conv2, bn1, bn2, lstm1, lstm2)
+    return _MpnnRowsFn.apply(plan, (num_nodes, window, mods, training, p, u), x, *_mpnn_params(*mods))
+
+
 def _tgcn_entry(co: int, name: str):
     """The library entry `name` of the fused TGCN kernels at hidden width `co`: stmp_tgcn_<name> at 32, stmp_tgcn_wide_<name> at 64."""
     if co not in (32, 64):

@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from pytorch_geometric_temporal_b200 import _lib, ops                                        # noqa: E402
 from pytorch_geometric_temporal_b200.dataset import synthetic                               # noqa: E402
 from pytorch_geometric_temporal_b200.nn.attention import ASTGCN                              # noqa: E402
-from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, DyGrEncoder, EvolveGCNH, EvolveGCNO, GCLSTM, GConvGRU, GConvLSTM, LRGCN, TGCN2   # noqa: E402
+from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, DyGrEncoder, EvolveGCNH, EvolveGCNO, GCLSTM, GConvGRU, GConvLSTM, LRGCN, MPNNLSTM, TGCN2   # noqa: E402
 
 dev = torch.device("cuda")
 torch.manual_seed(0)
@@ -100,6 +100,11 @@ with torch.enable_grad():
         (eg(xe, e_ring, w_ring).square().mean() + eg(xe, e_ring, w_ring).mean()).backward()
         with torch.no_grad():
             eg(xr, e_ring, None)
+    mp = MPNNLSTM(14, 32, 301, 1, 0.5).to(dev)                  # MPNN-LSTM: k_mpnn_conv1 / _conv2 / _lstm in training mode (dropout
+    with torch.no_grad():                                        # bits, running statistics) and eval mode, and the backward with dX
+        mp(xr, e_ring, w_ring)
+        mp.eval()(xr, e_ring, None)
+    mp.train()(xr, e_ring, w_ring).square().mean().backward()
     for cin, T in ((2, 3), (4, 1)):                              # 301 nodes: the row-split DCRNN (k_dcrnn_rows_*), T = 1 and T > 1, with and
         dr = BatchedDCRNN(cin, 32, 2).to(dev)                    # without dX (k_dcrnn_rows_bwd_x), k_dcrnn_wgrad_tc + k_dcrnn_wgrad_reduce
         xd = torch.randn(2, T, 301, cin, device=dev)
