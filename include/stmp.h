@@ -615,6 +615,37 @@ int stmp_mpnn_rows_bwd(const stmp_plan* plan, int64_t cin, int64_t hidden, int64
 int stmp_mpnn_rows_wgrad(const stmp_plan* plan, int64_t cin, int64_t hidden, int64_t window, void* stash, void* workspace, float* dw,
                          float* db, void* stream);
 
+/* ---- AGCRN (nn/recurrent/agcrn.py), the adaptive graph convolutional recurrent cell (agcrn.cu).  One call replaces the reference's
+ * AGCRN.forward with its two AVWGCNs (agcrn.py:40-56, 118-127): S = softmax(relu(E E^T)) and its Chebyshev supports, the node weights
+ * E weights_pool and biases E bias_pool of both AVWGCNs, the support products, the per-node contractions and the GRU gates (Z gates the
+ * state inside the candidate, R is the update gate; at K = 1 the single weight block multiplies Y + S Y, as the reference's einsum
+ * broadcast does).  No graph plan: the operator is learned from E.  Envelope (stmp_agcrn_supported): 1 <= N <= 4096, in >= 1,
+ * 1 <= out <= 64, in + out <= 128, 1 <= K <= 3, 1 <= d <= 64, 0 <= B <= 8388607 (B = 0: no launch).  Exact fp32 (FFMA products, one
+ * fixed order per sum), deterministic (no atomics); no host sync and no allocation, so a call can be captured.  Tensors contiguous
+ * float32: x (B, N, in), e (N, d), h (B, N, out) or NULL (zeros), weights_pool (d, K, in + out, Co), bias_pool (d, Co), Co = 2 out for
+ * the gate and out for the update.
+ *   stmp_agcrn_fwd: -> hout (B, N, out).  Scratch of stmp_agcrn_scratch_bytes(B, N, in, out, K) bytes (the supports, both AVWGCNs' node
+ *                   weights, the support products and the gates).  Training passes stash (stmp_agcrn_stash_bytes); NULL for inference.
+ *                   Six launches, seven at K = 3.
+ *   stmp_agcrn_bwd: after a training forward, with its scratch and stash (both kept) and gh = dL/dhout: dx, dh (only with h), de and the
+ *                   pools' gradients dwp_* (d, K, in + out, Co) and dbp_* (d, Co), each nullable; workspace of stmp_agcrn_workspace_bytes.
+ *                   Every sum over the batch or the nodes runs in one fixed order; long dT / dE products are split over k in chunks
+ *                   that depend on the shapes alone, summed in chunk order.  Eight to fifteen launches (B = 0: none, the requested
+ *                   gradients zeroed).
+ * STMP_EINVAL for a NULL required tensor or B < 0; STMP_ESHAPE for a misaligned tensor; STMP_EUNSUPPORTED outside the envelope
+ * (B > 8388607 included). */
+int stmp_agcrn_supported(int64_t b, int64_t n, int64_t in, int64_t out, int64_t K, int64_t d);
+int64_t stmp_agcrn_scratch_bytes(int64_t b, int64_t n, int64_t in, int64_t out, int64_t K);
+int64_t stmp_agcrn_stash_bytes(int64_t b, int64_t n, int64_t in, int64_t out, int64_t K);
+int64_t stmp_agcrn_workspace_bytes(int64_t b, int64_t n, int64_t in, int64_t out, int64_t K);
+int stmp_agcrn_fwd(int64_t b, int64_t n, int64_t in, int64_t out, int64_t K, int64_t d, const float* x, const float* e, const float* h,
+                   const float* wp_gate, const float* bp_gate, const float* wp_update, const float* bp_update, void* scratch, void* stash,
+                   float* hout, void* stream);
+int stmp_agcrn_bwd(int64_t b, int64_t n, int64_t in, int64_t out, int64_t K, int64_t d, const float* x, const float* e, const float* h,
+                   const float* wp_gate, const float* bp_gate, const float* wp_update, const float* bp_update, void* scratch, void* stash,
+                   const float* gh, void* workspace, float* dx, float* dh, float* de, float* dwp_gate, float* dbp_gate,
+                   float* dwp_update, float* dbp_update, void* stream);
+
 /* ---- the same cell at 64 hidden channels (lstm_rows.cu, the width-2 instance of its kernels): GConvLSTM / GCLSTM(cin, 64, K <= 2).
  * Envelope: cout = 64, cin 1..16, n_ops 0..1 and at most the plan's operators (stmp_lstm_rows_supported(plan, variant, n_ops, cin, 64)),
  * any number of nodes and any degree.  Same argument lists, launch chain and guarantees as the stmp_lstm_rows_* entries, with 32 -> 64

@@ -132,6 +132,12 @@ _SIGNATURES = {
     "stmp_mpnn_rows_workspace_bytes": (c_int64, [_P, c_int64, c_int64, c_int64]),
     "stmp_mpnn_rows_bwd": (c_int, [_P, c_int64, c_int64, c_int64, c_int64] + [_P] * 9 + [c_int, c_float] + [_P] * 6),
     "stmp_mpnn_rows_wgrad": (c_int, [_P, c_int64, c_int64, c_int64] + [_P] * 5),
+    "stmp_agcrn_supported": (c_int, [c_int64] * 6),
+    "stmp_agcrn_scratch_bytes": (c_int64, [c_int64] * 5),
+    "stmp_agcrn_stash_bytes": (c_int64, [c_int64] * 5),
+    "stmp_agcrn_workspace_bytes": (c_int64, [c_int64] * 5),
+    "stmp_agcrn_fwd": (c_int, [c_int64] * 6 + [_P] * 11),
+    "stmp_agcrn_bwd": (c_int, [c_int64] * 6 + [_P] * 19),
     "stmp_lstm_wide_rows_pack_weights": (c_int, [c_int, c_int, c_int64] + [_P] * 8),
     "stmp_lstm_wide_rows_fwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 10 + [c_int64, _P]),
     "stmp_lstm_wide_rows_scratch_bytes": (c_int64, [_P]),

@@ -8,4 +8,5 @@ from .lrgcn import LRGCN  # noqa: F401
 from .dygrae import DyGrEncoder  # noqa: F401
 from .evolvegcn import EvolveGCNH, EvolveGCNO  # noqa: F401
 from .mpnn_lstm import MPNNLSTM  # noqa: F401
+from .agcrn import AGCRN, AVWGCN  # noqa: F401
 from ._cheb import ChebConv  # noqa: F401

@@ -831,6 +831,76 @@ def mpnn_rows_train(plan: GraphPlan, x, num_nodes: int, window: int, conv1, conv
     return _MpnnRowsFn.apply(plan, (num_nodes, window, mods, training, p, u), x, *_mpnn_params(*mods))
 
 
+def agcrn_supported(batch: int, num_nodes: int, in_channels: int, out_channels: int, K: int, embedding_dimensions: int) -> bool:
+    return bool(_lib.lib().stmp_agcrn_supported(batch, num_nodes, in_channels, out_channels, K, embedding_dimensions))
+
+
+def _agcrn_dims(x, e, h, wp_gate, bp_gate, wp_update, bp_update):
+    """(B, N, in, out, K, d) of one AGCRN call; raises on operands whose shapes disagree (the kernels trust them)."""
+    B, N, cin = x.shape
+    d, K, ci, out = wp_update.shape
+    want = dict(e=(N, d), wp_gate=(d, K, ci, 2 * out), bp_gate=(d, 2 * out), bp_update=(d, out))
+    got = dict(e=tuple(e.shape), wp_gate=tuple(wp_gate.shape), bp_gate=tuple(bp_gate.shape), bp_update=tuple(bp_update.shape))
+    if h is not None:
+        want["h"], got["h"] = (B, N, out), tuple(h.shape)
+    if ci != cin + out or got != want:
+        raise RuntimeError(f"agcrn: operand shapes {got} with X {tuple(x.shape)} and weights_pool {tuple(wp_update.shape)}, want {want}")
+    return B, N, cin, out, K, d
+
+
+def agcrn_fwd(x, e, h, wp_gate, bp_gate, wp_update, bp_update, train: bool = False):
+    """One AGCRN call (stmp_agcrn_fwd, six launches, seven at K = 3): x (B, N, in), e (N, d), h (B, N, out) or None (zeros), the
+    gate's pools (d, K, in + out, 2 out), (d, 2 out) and the update's (d, K, in + out, out), (d, out) -> H' (B, N, out).  Returns H',
+    or (H', scratch, stash) with `train` (the backward's operands).  No autograd."""
+    x, e, wp_gate, bp_gate, wp_update, bp_update = (_f32c(t.detach(), n) for t, n in (
+        (x, "X"), (e, "E"), (wp_gate, "weights_pool"), (bp_gate, "bias_pool"), (wp_update, "weights_pool"), (bp_update, "bias_pool")))
+    h = None if h is None else _f32c(h.detach(), "H")
+    B, N, cin, out, K, d = _agcrn_dims(x, e, h, wp_gate, bp_gate, wp_update, bp_update)
+    hout = torch.empty(B, N, out, device=x.device, dtype=torch.float32)
+    L_ = _lib.lib()
+    byt = lambda n: torch.empty(int(n), device=x.device, dtype=torch.uint8)
+    scr = byt(L_.stmp_agcrn_scratch_bytes(B, N, cin, out, K))
+    stash = byt(L_.stmp_agcrn_stash_bytes(B, N, cin, out, K)) if train else None
+    with torch.cuda.device(x.device):
+        _lib.check(L_.stmp_agcrn_fwd(B, N, cin, out, K, d, *(_lib.ptr(t) for t in (x, e, h, wp_gate, bp_gate, wp_update, bp_update, scr,
+                                                                                  stash, hout)), _lib.stream_ptr()))
+    return (hout, scr, stash) if train else hout
+
+
+class _AgcrnFn(torch.autograd.Function):
+    """Training form of one AGCRN call.  forward = stmp_agcrn_fwd with the stash (the inference launches, so H' is bit-identical to the
+    no_grad call), scratch and stash kept in ctx; backward = stmp_agcrn_bwd: the gradients of X, E, H and both AVWGCNs' pools that
+    autograd asks for."""
+
+    @staticmethod
+    def forward(ctx, x, e, h, wp_gate, bp_gate, wp_update, bp_update):
+        ops_in = (x, e, h, wp_gate, bp_gate, wp_update, bp_update)
+        hout, ctx.scr, ctx.stash = agcrn_fwd(*ops_in, train=True)
+        ctx.save_for_backward(*(None if t is None else t.detach() for t in ops_in))
+        return hout
+
+    @staticmethod
+    def backward(ctx, gout):
+        x, e, h, wp_gate, bp_gate, wp_update, bp_update = (None if t is None else t.contiguous() for t in ctx.saved_tensors)
+        B, N, cin, out, K, d = _agcrn_dims(x, e, h, wp_gate, bp_gate, wp_update, bp_update)
+        gout = _f32c(gout, "gout")
+        want = ctx.needs_input_grad
+        new = lambda t, i: torch.empty_like(t) if want[i] and t is not None else None
+        dx, de, dh, *dpools = (new(t, i) for i, t in enumerate((x, e, h, wp_gate, bp_gate, wp_update, bp_update)))
+        L_ = _lib.lib()
+        ws = torch.empty(int(L_.stmp_agcrn_workspace_bytes(B, N, cin, out, K)), device=x.device, dtype=torch.uint8)
+        with torch.cuda.device(x.device):
+            _lib.check(L_.stmp_agcrn_bwd(B, N, cin, out, K, d, *(_lib.ptr(t) for t in (x, e, h, wp_gate, bp_gate, wp_update, bp_update,
+                                                                                      ctx.scr, ctx.stash, gout, ws, dx, dh, de, *dpools)),
+                                         _lib.stream_ptr()))
+        return (dx, de, dh, *dpools)
+
+
+def agcrn_train(x, e, h, wp_gate, bp_gate, wp_update, bp_update) -> torch.Tensor:
+    """Differentiable (w.r.t. x, e, h and the four pools, see _AgcrnFn) AGCRN call; arguments as agcrn_fwd."""
+    return _AgcrnFn.apply(x, e, h, wp_gate, bp_gate, wp_update, bp_update)
+
+
 def _tgcn_entry(co: int, name: str):
     """The library entry `name` of the fused TGCN kernels at hidden width `co`: stmp_tgcn_<name> at 32, stmp_tgcn_wide_<name> at 64."""
     if co not in (32, 64):

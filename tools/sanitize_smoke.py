@@ -11,6 +11,7 @@ from pytorch_geometric_temporal_b200 import _lib, ops                           
 from pytorch_geometric_temporal_b200.dataset import synthetic                               # noqa: E402
 from pytorch_geometric_temporal_b200.nn.attention import ASTGCN                              # noqa: E402
 from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, DyGrEncoder, EvolveGCNH, EvolveGCNO, GCLSTM, GConvGRU, GConvLSTM, LRGCN, MPNNLSTM, TGCN2   # noqa: E402
+from pytorch_geometric_temporal_b200.nn.recurrent import AGCRN                                # noqa: E402
 
 dev = torch.device("cuda")
 torch.manual_seed(0)
@@ -105,6 +106,13 @@ with torch.enable_grad():
         mp(xr, e_ring, w_ring)
         mp.eval()(xr, e_ring, None)
     mp.train()(xr, e_ring, w_ring).square().mean().backward()
+    for K in (1, 3):                                             # AGCRN: every k_agcrn_* kernel, partial tiles (N = 67, B = 3), with and
+        ag = AGCRN(67, 5, 7, K, 6).to(dev)                       # without H, the backward with every gradient
+        xa, ea = torch.randn(3, 67, 5, device=dev), torch.randn(67, 6, device=dev, requires_grad=True)
+        ha = ag(xa.requires_grad_(True), ea)
+        ag(xa, ea, ha).square().mean().backward()
+        with torch.no_grad():
+            ag(xa, ea)
     for cin, T in ((2, 3), (4, 1)):                              # 301 nodes: the row-split DCRNN (k_dcrnn_rows_*), T = 1 and T > 1, with and
         dr = BatchedDCRNN(cin, 32, 2).to(dev)                    # without dX (k_dcrnn_rows_bwd_x), k_dcrnn_wgrad_tc + k_dcrnn_wgrad_reduce
         xd = torch.randn(2, T, 301, cin, device=dev)
