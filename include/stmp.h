@@ -641,6 +641,37 @@ int64_t stmp_agcrn_workspace_bytes(int64_t b, int64_t n, int64_t in, int64_t out
 int stmp_agcrn_fwd(int64_t b, int64_t n, int64_t in, int64_t out, int64_t K, int64_t d, const float* x, const float* e, const float* h,
                    const float* wp_gate, const float* bp_gate, const float* wp_update, const float* bp_update, void* scratch, void* stash,
                    float* hout, void* stream);
+/* ---- HeteroGCLSTM (nn/hetero/heterogclstm.py), the heterogeneous graph LSTM (hetero_rows.cu): every destination node type of one call in
+ * ONE launch.  Per type t with incoming edge types e_1 .. e_R (sources s_r): pre = S w^T + b on the basis
+ * S = [X_t | H_t | mean_{e_1}(H_{s_1}) | ... | mean_{e_R}(H_{s_R})], packed weight w (4 out, nb), nb = in + out (1 + R), per gate the rows
+ * [W_g^T | sum_r lin_r^{g,e_r} | lin_l^{g,e_1} | ...] and b = b_g + sum_r lin_l^{g,e_r}.bias; then I, F, O sigmoids, T tanh,
+ * C' = F C + I T, H' = O tanh(C') (no peepholes).  mean_e is an STMP_FLAVOR_RGCN plan of one relation over at least N_t nodes whose
+ * columns index the source type's rows (the caller checks them against N_s when it makes the plan).  Exact fp32, deterministic, no host
+ * sync and no allocation, so a call can be captured.
+ * Envelope (stmp_hetero_lstm_supported, per type): 1 <= in <= 32 and out 32 with 1 <= R <= 4, or out 64 with R = 1; at most
+ * STMP_HETERO_MAX_TYPES destination types per call, each with 1 <= N.
+ *   stmp_hetero_lstm_fwd: desc holds num_types rows of STMP_HETERO_DESC int64 fields: N, in, R, then device pointers x (N, in),
+ *                         h (N, out) or 0, c (N, out) or 0 (zeros), w (4 out, nb), b (4 out), hout (N, out), cout (N, out), then
+ *                         STMP_HETERO_MAX_REL plan handles and STMP_HETERO_MAX_REL source states H_{s_r} (N_{s_r}, out) (entries past R
+ *                         ignored), fields 18.. below.  has_h = 0 means H = 0 for every type: no H loads and no gathers.  One launch.
+ * STMP_EINVAL for a NULL required pointer or a plan of another flavor or too few rows; STMP_ESHAPE for a misaligned tensor;
+ * STMP_EUNSUPPORTED outside the envelope.
+ * Training: fields 18 stash (4 planes of N x out: I, F, T, O) and 19 S (N x nb, the basis rows) make the forward write both (the same
+ * launch and arithmetic, so H' and C' equal the inference call's bit for bit); NULL for inference.
+ *   stmp_hetero_lstm_bwd: after a training forward, with fields 20 gh, 21 gc (dL/dH', dL/dC', each nullable), 22 dpre (N x 4 out,
+ *                         scratch), 23 dx, 25 dc (nullable), 24 dh and 26.. Q_r (N x out, scratch) when want_dh, 30.. the table index of
+ *                         each incoming edge type's source type, 34.. its rank in metadata order, 38 dw ((4 out) x (nb + 1): [dw | db],
+ *                         nullable for no weight gradient) and workspace of stmp_hetero_lstm_workspace_bytes.  Launches: the rowwise
+ *                         backward (dpre, dC, dX, the own-row dH and Q_r = dpre lin_l^{e_r}); with want_dh one transposed gather over
+ *                         every source type (own term, then its outgoing edge types in metadata order, then CSR entries); with dw the
+ *                         contraction dpre^T [S | 1] over fixed row chunks and its chunk-order reduce: at most four, whatever the number
+ *                         of types.  At most 8 outgoing edge types per source type (STMP_EUNSUPPORTED beyond). */
+enum { STMP_HETERO_MAX_TYPES = 8, STMP_HETERO_MAX_REL = 4, STMP_HETERO_DESC = 39 };
+int stmp_hetero_lstm_supported(int64_t out, int64_t in, int64_t num_rel);
+int stmp_hetero_lstm_fwd(int64_t out, int64_t num_types, const int64_t* desc, int has_h, void* stream);
+int64_t stmp_hetero_lstm_workspace_bytes(int64_t out, int64_t num_types, const int64_t* desc);
+int stmp_hetero_lstm_bwd(int64_t out, int64_t num_types, const int64_t* desc, int want_dh, void* workspace, void* stream);
+
 int stmp_agcrn_bwd(int64_t b, int64_t n, int64_t in, int64_t out, int64_t K, int64_t d, const float* x, const float* e, const float* h,
                    const float* wp_gate, const float* bp_gate, const float* wp_update, const float* bp_update, void* scratch, void* stash,
                    const float* gh, void* workspace, float* dx, float* dh, float* de, float* dwp_gate, float* dbp_gate,

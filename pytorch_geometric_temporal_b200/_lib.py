@@ -17,6 +17,8 @@ NORM_NONE, NORM_SYM, NORM_RW = range(3)
 GCN_IMPROVED, GCN_NO_SELF_LOOPS, DCONV_ALLOW_DUPLICATES = 1, 2, 4
 NORM_CODE = {None: NORM_NONE, "sym": NORM_SYM, "rw": NORM_RW}
 LSTM_GCONV, LSTM_GC = range(2)                     # stmp_lstm_basis: the row-split LSTM cell's basis (GConvLSTM / GCLSTM)
+HETERO_MAX_TYPES, HETERO_MAX_REL = 8, 4           # STMP_HETERO_*: node types per stmp_hetero_lstm_fwd call, plan slots per type
+HETERO_DESC = 39                                  # int64 fields per type row of stmp_hetero_lstm_fwd / _bwd's desc
 
 
 class StmpError(RuntimeError):
@@ -138,6 +140,10 @@ _SIGNATURES = {
     "stmp_agcrn_workspace_bytes": (c_int64, [c_int64] * 5),
     "stmp_agcrn_fwd": (c_int, [c_int64] * 6 + [_P] * 11),
     "stmp_agcrn_bwd": (c_int, [c_int64] * 6 + [_P] * 19),
+    "stmp_hetero_lstm_supported": (c_int, [c_int64] * 3),
+    "stmp_hetero_lstm_fwd": (c_int, [c_int64, c_int64, _P, c_int, _P]),
+    "stmp_hetero_lstm_workspace_bytes": (c_int64, [c_int64, c_int64, _P]),
+    "stmp_hetero_lstm_bwd": (c_int, [c_int64, c_int64, _P, c_int, _P, _P]),
     "stmp_lstm_wide_rows_pack_weights": (c_int, [c_int, c_int, c_int64] + [_P] * 8),
     "stmp_lstm_wide_rows_fwd": (c_int, [_P, c_int, c_int, c_int64] + [_P] * 10 + [c_int64, _P]),
     "stmp_lstm_wide_rows_scratch_bytes": (c_int64, [_P]),

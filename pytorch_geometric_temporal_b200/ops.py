@@ -1720,3 +1720,155 @@ def window_gather(series: torch.Tensor, start: torch.Tensor, horizon: int, with_
         _lib.check(_lib.lib().stmp_window_gather(_lib.ptr(series), series.size(0), row, _lib.ptr(start), B, horizon,
                                                  _lib.ptr(x), _lib.ptr(y), _lib.stream_ptr()))
     return (x, y) if with_target else x
+
+
+def hetero_lstm_supported(out_channels: int, in_channels: int, num_rel: int) -> bool:
+    return bool(_lib.lib().stmp_hetero_lstm_supported(out_channels, in_channels, num_rel))
+
+
+def _hetero_desc(types):
+    """stmp_hetero_lstm_fwd / _bwd's desc of `types` (see hetero_lstm_fwd) and the contiguous float32 operands it points at."""
+    desc = (ctypes.c_int64 * (_lib.HETERO_DESC * len(types)))()
+    ops_ = []
+    for t, (x, h, c, w, b, plans, sources, src_idx, ranks) in enumerate(types):
+        x, w, b = _f32c(x.detach(), "X"), _f32c(w, "w"), _f32c(b, "b")
+        h = None if h is None else _f32c(h.detach(), "H")
+        c = None if c is None else _f32c(c.detach(), "C")
+        srcs = [None if s is None else _f32c(s.detach(), "H") for s in sources]
+        R, pad = len(plans), [0] * (_lib.HETERO_MAX_REL - len(plans))
+        row = [x.size(0), x.size(1), R] + [_addr(v) for v in (x, h, c, w, b)] + [0, 0]
+        row += [p.handle.value for p in plans] + pad + [_addr(v) for v in srcs] + pad + [0] * (_lib.HETERO_DESC - 18)
+        row[30:30 + R], row[34:34 + R] = list(src_idx), list(ranks)
+        desc[t * _lib.HETERO_DESC:(t + 1) * _lib.HETERO_DESC] = row
+        ops_.append(dict(x=x, h=h, c=c, w=w, srcs=srcs, n=x.size(0), cin=x.size(1), R=R))
+    return desc, ops_
+
+
+def _addr(v):
+    return 0 if v is None else v.data_ptr()
+
+
+def _set(desc, t, field, v):
+    desc[t * _lib.HETERO_DESC + field] = _addr(v)
+
+
+def hetero_lstm_fwd(out_channels: int, types, has_h: bool, train: bool = False):
+    """One HeteroGCLSTM step for every destination type in one launch (stmp_hetero_lstm_fwd).  `types`: per type a tuple
+    (x (N, in), h (N, out) or None, c (N, out) or None, w (4 out, nb), b (4 out), plans, sources, src_idx, ranks) with `plans` the
+    BipartitePlans of its incoming edge types, `sources` their source states (N_s, out) (None without H), `src_idx` the position of each
+    source type in `types` and `ranks` each edge type's position in the metadata (both read by the backward only).  Returns
+    [(H', C')] in `types` order; with `train`, also (desc, operands) for hetero_lstm_bwd, the stash and basis rows included.  No
+    autograd."""
+    desc, ops_ = _hetero_desc(types)
+    dev = types[0][0].device
+    outs = []
+    for t, o in enumerate(ops_):
+        hout = torch.empty(o["n"], out_channels, device=dev, dtype=torch.float32)
+        cout = torch.empty_like(hout)
+        _set(desc, t, 8, hout)
+        _set(desc, t, 9, cout)
+        outs.append((hout, cout))
+        o["cout"] = cout
+        if train:
+            o["stash"] = torch.empty(4, o["n"], out_channels, device=dev, dtype=torch.float32)
+            o["S"] = torch.empty(o["n"], o["cin"] + out_channels * (1 + o["R"]), device=dev, dtype=torch.float32)
+            _set(desc, t, 18, o["stash"])
+            _set(desc, t, 19, o["S"])
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().stmp_hetero_lstm_fwd(out_channels, len(types), desc, int(has_h), _lib.stream_ptr()))
+    return (outs, desc, ops_) if train else outs
+
+
+def hetero_lstm_bwd(out_channels: int, desc, ops_, gh, gc, want_dx, want_dh: bool, want_dc, want_dw: bool):
+    """The backward of a training hetero_lstm_fwd (stmp_hetero_lstm_bwd, at most four launches): gh / gc per type (None: zero), want_dx /
+    want_dc per type.  Returns per type (dx, dh, dc, dw (4 out, nb), db (4 out)), each None when not asked for."""
+    dev = ops_[0]["x"].device
+    res, keep = [], []
+    for t, o in enumerate(ops_):
+        g = [None if v is None else _f32c(v, "grad") for v in (gh[t], gc[t])]
+        new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
+        n, R = o["n"], o["R"]
+        nb = o["cin"] + out_channels * (1 + R)
+        r = dict(dpre=new(n, 4 * out_channels), dx=new(n, o["cin"]) if want_dx[t] else None, dh=new(n, out_channels) if want_dh else None,
+                 dc=new(n, out_channels) if want_dc[t] else None, q=[new(n, out_channels) for _ in range(R)] if want_dh else [],
+                 dw=new(4 * out_channels, nb + 1) if want_dw else None)
+        for f, v in ((20, g[0]), (21, g[1]), (22, r["dpre"]), (23, r["dx"]), (24, r["dh"]), (25, r["dc"]), (38, r["dw"])):
+            _set(desc, t, f, v)
+        for k, q in enumerate(r["q"]):
+            _set(desc, t, 26 + k, q)
+        keep += g
+        res.append(r)
+    L_ = _lib.lib()
+    ws = torch.empty(int(L_.stmp_hetero_lstm_workspace_bytes(out_channels, len(ops_), desc)) if want_dw else 0, device=dev,
+                     dtype=torch.uint8)
+    with torch.cuda.device(dev):
+        _lib.check(L_.stmp_hetero_lstm_bwd(out_channels, len(ops_), desc, int(want_dh), _lib.ptr(ws) if want_dw else None,
+                                           _lib.stream_ptr()))
+    out = []
+    for o, r in zip(ops_, res):
+        nb = r["dw"].size(1) - 1 if want_dw else 0
+        out.append((r["dx"], r["dh"], r["dc"], r["dw"][:, :nb] if want_dw else None, r["dw"][:, nb] if want_dw else None))
+    return out
+
+
+class _HeteroLstmFn(torch.autograd.Function):
+    """Training form of hetero_lstm_fwd for T node types.  forward = the inference launch with the stash and the basis rows (so H', C'
+    are bit-identical to the no_grad call), kept in ctx with the desc; backward = hetero_lstm_bwd: dX, dH, dC where asked for, and each
+    type's packed weight / bias gradient handed to `params` as blocks described by its spec (see _spec_grads).  Inputs: X (T), H (T),
+    C (T), then every type's parameters; outputs: H' (T), C' (T)."""
+
+    @staticmethod
+    def forward(ctx, out_channels, layout, specs, *flat):
+        ctx.set_materialize_grads(False)
+        T = len(layout)
+        xs, hs, cs, params = flat[:T], flat[T:2 * T], flat[2 * T:3 * T], flat[3 * T:]
+        types = [(xs[t], hs[t], cs[t]) + tuple(layout[t]) for t in range(T)]
+        outs, ctx.desc, ctx.ops = hetero_lstm_fwd(out_channels, types, hs[0] is not None, train=True)
+        ctx.out, ctx.T, ctx.specs, ctx.shapes = out_channels, T, specs, [p.shape for p in params]
+        ctx.has_h, ctx.has_c = hs[0] is not None, cs[0] is not None
+        return (*[o[0] for o in outs], *[o[1] for o in outs])
+
+    @staticmethod
+    def backward(ctx, *grads):
+        T, need = ctx.T, ctx.needs_input_grad
+        if all(g is None for g in grads):
+            return (None,) * len(need)
+        want_dx = [need[3 + t] for t in range(T)]
+        want_dh = ctx.has_h and any(need[3 + T + t] for t in range(T))
+        want_dc = [ctx.has_c and need[3 + 2 * T + t] for t in range(T)]
+        want_dw = any(need[3 + 3 * T:])
+        res = hetero_lstm_bwd(ctx.out, ctx.desc, ctx.ops, grads[:T], grads[T:], want_dx, want_dh, want_dc, want_dw)
+        pgrads = []
+        for t, (dx, dh, dc, dw, db) in enumerate(res):
+            if want_dw:
+                pgrads += _spec_grads(ctx.specs[t], dw, db)
+            else:
+                pgrads += [None] * len(ctx.specs[t])
+        pgrads = [None if g is None else g.reshape(s) for g, s in zip(pgrads, ctx.shapes)]
+        return (None, None, None, *[r[0] for r in res], *[r[1] if want_dh else None for r in res],
+                *[r[2] for r in res], *pgrads)
+
+
+def hetero_lstm_train(out_channels: int, types, params, specs):
+    """Differentiable hetero_lstm_fwd: `types` as there; `params` the flat list of every type's parameters and `specs` per type the
+    packed blocks they receive.  Returns [(H', C')]."""
+    layout = [tuple(t[3:]) for t in types]
+    flat = [t[0] for t in types] + [t[1] for t in types] + [t[2] for t in types]
+    outs = _HeteroLstmFn.apply(out_channels, layout, specs, *flat, *params)
+    T = len(types)
+    return [(outs[t], outs[T + t]) for t in range(T)]
+
+
+def bipartite_mean(plan, edge_index: torch.Tensor, h_src: torch.Tensor) -> torch.Tensor:
+    """SAGEConv's mean of the source rows h_src (N_src, F) onto the plan's N_dst destination rows (0 for a row without edges): float32
+    through spmm on the BipartitePlan (autograd through its source CSR), other dtypes by index_add over edge_index."""
+    if h_src.size(0) != plan.num_src:
+        raise RuntimeError(f"source state has {h_src.size(0)} rows, the edge type's plan {plan.num_src}")
+    if h_src.dtype == torch.float32:
+        pad = plan.num_nodes - h_src.size(0)
+        x = torch.cat([h_src, h_src.new_zeros(pad, h_src.size(1))]) if pad else h_src
+        return spmm(plan, 0, x)[:plan.num_dst]
+    src, dst = edge_index[0], edge_index[1]
+    agg = h_src.new_zeros(plan.num_dst, h_src.size(1)).index_add(0, dst, h_src[src])
+    cnt = torch.zeros(plan.num_dst, dtype=h_src.dtype, device=h_src.device).index_add_(0, dst, torch.ones_like(dst, dtype=h_src.dtype))
+    return agg / cnt.clamp(min=1).unsqueeze(1)

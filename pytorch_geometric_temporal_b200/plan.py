@@ -119,6 +119,23 @@ class RgcnPlan(GraphPlan):
         self.n_ops = _lib.lib().stmp_plan_num_ops(self._h)
 
 
+class BipartitePlan(RgcnPlan):
+    """PyG SAGEConv's mean aggregation from `num_src` source rows onto `num_dst` destination rows (one edge type of a heterogeneous
+    graph): an STMP_FLAVOR_RGCN plan of one relation holding every edge, built on max(num_src, num_dst) nodes, so its rows < num_dst are
+    the destinations and its columns are < num_src.  Sources are checked against num_src and destinations against num_dst here (one host
+    sync, a setup path); anything out of range raises RuntimeError."""
+
+    def __init__(self, edge_index: torch.Tensor, num_src: int, num_dst: int):
+        _require_cuda(edge_index, "edge_index")
+        if edge_index.dim() != 2 or edge_index.size(0) != 2:
+            raise ValueError(f"edge_index must have shape [2, E], got {tuple(edge_index.shape)}")
+        ei = edge_index.to(torch.int64)
+        if ei.size(1) and bool(((ei < 0).any(1) | (ei.max(1).values >= torch.tensor([num_src, num_dst], device=ei.device))).any()):
+            raise RuntimeError(f"edge_index out of range for {num_src} source and {num_dst} destination nodes")
+        super().__init__(ei, torch.zeros(ei.size(1), dtype=torch.int64, device=ei.device), max(int(num_src), int(num_dst), 1), 0, 1)
+        self.num_src, self.num_dst = int(num_src), int(num_dst)
+
+
 class GatedPlan(GraphPlan):
     """PyG GatedGraphConv's aggregation operator (STMP_FLAVOR_GATED) for `aggr` ("add", "mean" or "max"): every edge in edge order,
     value w_e (add, max) or w_e / (the destination's count of in-edges) (mean); edge_weight None means ones."""
@@ -176,6 +193,11 @@ class PlanCache:
         """The GatedPlan of `aggr` ("add", "mean" or "max") for this graph."""
         key = (_lib.FLAVOR_GATED, self._tkey(edge_index), self._tkey(edge_weight), int(num_nodes), aggr)
         return self._lookup(key, lambda: GatedPlan(edge_index, edge_weight, num_nodes, aggr), (edge_index, edge_weight))
+
+    def get_bipartite(self, edge_index, num_src, num_dst) -> BipartitePlan:
+        """The BipartitePlan of one edge type of a heterogeneous graph."""
+        key = ("bipartite", self._tkey(edge_index), int(num_src), int(num_dst))
+        return self._lookup(key, lambda: BipartitePlan(edge_index, num_src, num_dst), (edge_index,))
 
     def _lookup(self, key, make, keep):
         hit = self._entries.get(key)

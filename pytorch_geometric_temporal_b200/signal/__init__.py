@@ -5,3 +5,4 @@ from .dynamic_graph_signal import (DynamicGraphTemporalSignal, DynamicGraphStati
                                    DynamicGraphTemporalSignalBatch, DynamicGraphStaticSignalBatch)
 from .train_test_split import temporal_signal_split  # noqa: F401
 from .index_dataset import IndexDataset, IndexBatchLoader, DevicePrefetcher, shard_indices, index_splits  # noqa: F401
+from .static_hetero_graph_temporal_signal import StaticHeteroGraphTemporalSignal, HeteroData  # noqa: F401

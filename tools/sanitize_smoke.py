@@ -12,6 +12,7 @@ from pytorch_geometric_temporal_b200.dataset import synthetic                   
 from pytorch_geometric_temporal_b200.nn.attention import ASTGCN                              # noqa: E402
 from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, DyGrEncoder, EvolveGCNH, EvolveGCNO, GCLSTM, GConvGRU, GConvLSTM, LRGCN, MPNNLSTM, TGCN2   # noqa: E402
 from pytorch_geometric_temporal_b200.nn.recurrent import AGCRN                                # noqa: E402
+from pytorch_geometric_temporal_b200.nn.hetero import HeteroGCLSTM                          # noqa: E402
 
 dev = torch.device("cuda")
 torch.manual_seed(0)
@@ -113,6 +114,16 @@ with torch.enable_grad():
         ag(xa, ea, ha).square().mean().backward()
         with torch.no_grad():
             ag(xa, ea)
+    for out, rel in ((32, 4), (64, 1)):                          # HeteroGCLSTM: k_hetero_lstm_fwd at both widths, H None and carried,
+        ht = {"a": (301, 5), "b": (17, 32)}                      # partial tiles and a type change inside a CTA's tiles
+        eh = {("a", "r", "b"): torch.stack([torch.arange(60) % 301, torch.arange(60) % 17]).to(dev),
+              ("b", "r", "a"): torch.stack([torch.arange(400) % 17, torch.arange(400) % 301]).to(dev)}
+        for k in range(1, rel):
+            eh[("b", f"s{k}", "b")] = torch.stack([torch.arange(30) % 17, (torch.arange(30) * 7) % 17]).to(dev)
+        hg = HeteroGCLSTM({t: c for t, (_, c) in ht.items()}, out, (list(ht), list(eh))).to(dev)
+        xh = {t: torch.randn(n, c, device=dev) for t, (n, c) in ht.items()}
+        with torch.no_grad():
+            hg(xh, eh, *hg(xh, eh))
     for cin, T in ((2, 3), (4, 1)):                              # 301 nodes: the row-split DCRNN (k_dcrnn_rows_*), T = 1 and T > 1, with and
         dr = BatchedDCRNN(cin, 32, 2).to(dev)                    # without dX (k_dcrnn_rows_bwd_x), k_dcrnn_wgrad_tc + k_dcrnn_wgrad_reduce
         xd = torch.randn(2, T, 301, cin, device=dev)
