@@ -677,6 +677,34 @@ int stmp_agcrn_bwd(int64_t b, int64_t n, int64_t in, int64_t out, int64_t K, int
                    const float* gh, void* workspace, float* dx, float* dh, float* de, float* dwp_gate, float* dbp_gate,
                    float* dwp_update, float* dbp_update, void* stream);
 
+/* ---- GMAN's multi-head attention (nn/attention/gman.py), gman_attention.cu.  One call replaces the attention core of the reference's
+ * SpatialAttention, TemporalAttention or TransformAttention.forward (gman.py:235-242, 297-319, 463-474: the split into heads, Q K^T,
+ * the division by sqrt(d), the optional tril mask, softmax, the product with V and the concatenation of the heads), read and written
+ * in place in the channels-last activations.  A call serves p0 x p1 problems of `heads` heads of width `width`; element (i0, i1, row r,
+ * head h, channel c) of tensor t sits at t + i0 s0 + i1 s1 + r sl + h width + c, with strides[12] = host array of (s0, s1, sl) for Q,
+ * K, V and O in that order (elements).  The backward's dQ, dK, dV take Q's, K's and V's strides and dO takes O's.
+ *   S = scale Q K^T; with mask, S[i][j] = -32767 for j > i, still inside the softmax sum (the reference's torch.where); O = softmax(S) V.
+ *   long_kernel = 1: any Lq, Lk, no mask (the spatial attention): online softmax over key tiles, one launch; backward two launches
+ *                    (dQ and D = rowsum(dO . O) over query rows, then dK and dV over key rows), workspace of
+ *                    stmp_gman_attn_workspace_bytes (D).
+ *   long_kernel = 0: Lq, Lk <= 64, a mask needs Lq == Lk (temporal and transform): one warp per (problem, head), exact two-pass
+ *                    softmax; backward one launch.
+ *   stmp_gman_attn_fwd: -> O.  stash (stmp_gman_attn_stash_bytes: the per-row log-sum-exp, (p0, p1, heads, Lq) floats) for a
+ *                       training call, NULL for inference.
+ *   stmp_gman_attn_bwd: after a training forward, with its O and stash and dout = dL/dO: dq, dk, dv, each nullable (none: no launch).
+ * Envelope (stmp_gman_attn_supported): 1 <= width <= 16, Lq, Lk >= 1, heads >= 1, p0, p1 >= 0 (p0 p1 = 0: no launch) and every grid
+ * below 2^31 CTAs.  Exact fp32 (FFMA, every sum in one fixed order), deterministic (no atomics), no host sync and no allocation.
+ * STMP_EINVAL for a NULL required tensor or a negative count; STMP_EUNSUPPORTED outside the envelope. */
+int stmp_gman_attn_supported(int64_t p0, int64_t p1, int64_t heads, int64_t width, int64_t lq, int64_t lk, int mask, int long_kernel);
+int64_t stmp_gman_attn_stash_bytes(int64_t p0, int64_t p1, int64_t heads, int64_t lq);
+int64_t stmp_gman_attn_workspace_bytes(int64_t p0, int64_t p1, int64_t heads, int64_t lq, int long_kernel);
+int stmp_gman_attn_fwd(int64_t p0, int64_t p1, int64_t heads, int64_t width, int64_t lq, int64_t lk, int mask, int long_kernel,
+                       float scale, const int64_t* strides, const float* q, const float* k, const float* v, float* o, float* stash,
+                       void* stream);
+int stmp_gman_attn_bwd(int64_t p0, int64_t p1, int64_t heads, int64_t width, int64_t lq, int64_t lk, int mask, int long_kernel,
+                       float scale, const int64_t* strides, const float* q, const float* k, const float* v, const float* o,
+                       const float* stash, const float* dout, void* workspace, float* dq, float* dk, float* dv, void* stream);
+
 /* ---- the same cell at 64 hidden channels (lstm_rows.cu, the width-2 instance of its kernels): GConvLSTM / GCLSTM(cin, 64, K <= 2).
  * Envelope: cout = 64, cin 1..16, n_ops 0..1 and at most the plan's operators (stmp_lstm_rows_supported(plan, variant, n_ops, cin, 64)),
  * any number of nodes and any degree.  Same argument lists, launch chain and guarantees as the stmp_lstm_rows_* entries, with 32 -> 64

@@ -140,6 +140,11 @@ _SIGNATURES = {
     "stmp_agcrn_workspace_bytes": (c_int64, [c_int64] * 5),
     "stmp_agcrn_fwd": (c_int, [c_int64] * 6 + [_P] * 11),
     "stmp_agcrn_bwd": (c_int, [c_int64] * 6 + [_P] * 19),
+    "stmp_gman_attn_supported": (c_int, [c_int64] * 6 + [c_int, c_int]),
+    "stmp_gman_attn_stash_bytes": (c_int64, [c_int64] * 4),
+    "stmp_gman_attn_workspace_bytes": (c_int64, [c_int64] * 4 + [c_int]),
+    "stmp_gman_attn_fwd": (c_int, [c_int64] * 6 + [c_int, c_int, c_float] + [_P] * 7),
+    "stmp_gman_attn_bwd": (c_int, [c_int64] * 6 + [c_int, c_int, c_float] + [_P] * 12),
     "stmp_hetero_lstm_supported": (c_int, [c_int64] * 3),
     "stmp_hetero_lstm_fwd": (c_int, [c_int64, c_int64, _P, c_int, _P]),
     "stmp_hetero_lstm_workspace_bytes": (c_int64, [c_int64, c_int64, _P]),

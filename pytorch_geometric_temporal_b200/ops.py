@@ -901,6 +901,85 @@ def agcrn_train(x, e, h, wp_gate, bp_gate, wp_update, bp_update) -> torch.Tensor
     return _AgcrnFn.apply(x, e, h, wp_gate, bp_gate, wp_update, bp_update)
 
 
+def gman_attn_supported(batch: int, other: int, heads: int, width: int, Lq: int, Lk: int, spatial: bool, mask: bool) -> bool:
+    """stmp_gman_attn_supported for one GMAN attention call: spatial (B, T = other, N = Lq = Lk) on the long kernel, else (B, Lq / Lk
+    steps, N = other) on the short one."""
+    return bool(_lib.lib().stmp_gman_attn_supported(batch, other, heads, width, Lq, Lk, int(mask), int(spatial)))
+
+
+def _gman_problem(t: torch.Tensor, spatial: bool):
+    """(p0, p1, sequence length) and the (s0, s1, sl) strides of a channels-last (B, T, N, D) operand: problems (b, t) over the nodes
+    for the spatial attention, (b, n) over the steps otherwise."""
+    if spatial:
+        return (t.shape[0], t.shape[1], t.shape[2]), (t.stride(0), t.stride(1), t.stride(2))
+    return (t.shape[0], t.shape[2], t.shape[1]), (t.stride(0), t.stride(2), t.stride(1))
+
+
+def _gman_call(q, k, v, heads: int, width: int, spatial: bool, mask: bool):
+    """The arguments every stmp_gman_attn_* call shares, with O's (B, Lq, N, D) layout; raises on operands whose shapes disagree."""
+    if q.dim() != 4 or k.shape != v.shape or k.dim() != 4 or q.shape[-1] != heads * width or k.shape[-1] != heads * width or \
+            q.shape[0] != k.shape[0] or (q.shape[2] != k.shape[2] if not spatial else q.shape[:3] != k.shape[:3]):
+        raise RuntimeError(f"gman_attention: Q {tuple(q.shape)}, K {tuple(k.shape)}, V {tuple(v.shape)} with {heads} heads of width "
+                           f"{width}")
+    (p0, p1, lq), sq = _gman_problem(q, spatial)
+    (_, _, lk), sk = _gman_problem(k, spatial)
+    _, sv = _gman_problem(v, spatial)
+    _, so = _gman_problem(torch.empty(q.shape, device="meta"), spatial)
+    strides = (ctypes.c_int64 * 12)(*sq, *sk, *sv, *so)
+    return (p0, p1, heads, width, lq, lk, int(mask), int(spatial)), strides
+
+
+def gman_attn_fwd(q, k, v, heads: int, width: int, scale: float, spatial: bool, mask: bool, train: bool = False):
+    """One GMAN attention (stmp_gman_attn_fwd, one launch): q (B, Lq, N, D), k and v (B, Lk, N, D), D = heads width, head h in channels
+    [h width, (h + 1) width); spatial attends over the nodes (Lq = Lk), otherwise over the steps (mask: the reference's tril mask).
+    Returns O (B, Lq, N, D), or (O, stash) with `train`.  No autograd."""
+    q, k, v = (_f32c(t.detach(), n) for t, n in ((q, "Q"), (k, "K"), (v, "V")))
+    dims, strides = _gman_call(q, k, v, heads, width, spatial, mask)
+    o = torch.empty(q.shape, device=q.device, dtype=torch.float32)
+    L_ = _lib.lib()
+    stash = torch.empty(int(L_.stmp_gman_attn_stash_bytes(*dims[:3], dims[4])) // 4, device=q.device, dtype=torch.float32) \
+        if train else None
+    with torch.cuda.device(q.device):
+        _lib.check(L_.stmp_gman_attn_fwd(*dims, scale, strides, *(_lib.ptr(t) for t in (q, k, v, o, stash)), _lib.stream_ptr()))
+    return (o, stash) if train else o
+
+
+class _GmanAttnFn(torch.autograd.Function):
+    """Training form of one GMAN attention.  forward = stmp_gman_attn_fwd with the log-sum-exp stash (the inference launch, so O is
+    bit-identical to the no_grad call), the stash kept in ctx; backward = stmp_gman_attn_bwd: the gradients of Q, K and V that autograd
+    asks for, P recomputed from the stash."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, heads, width, scale, spatial, mask):
+        o, ctx.stash = gman_attn_fwd(q, k, v, heads, width, scale, spatial, mask, train=True)
+        ctx.meta = (heads, width, scale, spatial, mask)
+        ctx.save_for_backward(q.detach(), k.detach(), v.detach(), o)
+        return o
+
+    @staticmethod
+    def backward(ctx, gout):
+        q, k, v, o = (t.contiguous() for t in ctx.saved_tensors)
+        heads, width, scale, spatial, mask = ctx.meta
+        gout = _f32c(gout, "gout")
+        dims, strides = _gman_call(q, k, v, heads, width, spatial, mask)
+        want = ctx.needs_input_grad
+        dq, dk, dv = (torch.empty_like(t) if want[i] else None for i, t in enumerate((q, k, v)))
+        L_ = _lib.lib()
+        ws = torch.empty(int(L_.stmp_gman_attn_workspace_bytes(*dims[:3], dims[4], dims[7])), device=q.device, dtype=torch.uint8)
+        with torch.cuda.device(q.device):
+            _lib.check(L_.stmp_gman_attn_bwd(*dims, scale, strides, *(_lib.ptr(t) for t in (q, k, v, o, ctx.stash, gout, ws, dq, dk, dv)),
+                                             _lib.stream_ptr()))
+        return dq, dk, dv, None, None, None, None, None
+
+
+def gman_attention(q, k, v, heads: int, width: int, scale: float, spatial: bool, mask: bool, train: bool):
+    """One GMAN attention on the fused kernels, differentiable w.r.t. q, k, v with `train` (see _GmanAttnFn); arguments as
+    gman_attn_fwd."""
+    if train:
+        return _GmanAttnFn.apply(q, k, v, heads, width, scale, spatial, mask)
+    return gman_attn_fwd(q, k, v, heads, width, scale, spatial, mask)
+
+
 def _tgcn_entry(co: int, name: str):
     """The library entry `name` of the fused TGCN kernels at hidden width `co`: stmp_tgcn_<name> at 32, stmp_tgcn_wide_<name> at 64."""
     if co not in (32, 64):

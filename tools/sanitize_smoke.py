@@ -12,6 +12,7 @@ from pytorch_geometric_temporal_b200.dataset import synthetic                   
 from pytorch_geometric_temporal_b200.nn.attention import ASTGCN                              # noqa: E402
 from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, DyGrEncoder, EvolveGCNH, EvolveGCNO, GCLSTM, GConvGRU, GConvLSTM, LRGCN, MPNNLSTM, TGCN2   # noqa: E402
 from pytorch_geometric_temporal_b200.nn.recurrent import AGCRN                                # noqa: E402
+from pytorch_geometric_temporal_b200.nn.attention import GMAN                                 # noqa: E402
 from pytorch_geometric_temporal_b200.nn.hetero import HeteroGCLSTM                          # noqa: E402
 
 dev = torch.device("cuda")
@@ -114,6 +115,13 @@ with torch.enable_grad():
         ag(xa, ea, ha).square().mean().backward()
         with torch.no_grad():
             ag(xa, ea)
+    for K, d, N, mask in ((8, 8, 131, True), (13, 2, 5, False)):  # GMAN: every k_gman_attn_* kernel at widths 8 and 16 (13 padded), a
+        gm = GMAN(1, K, d, 5, 0.1, 12, True, mask).to(dev)        # partial query / key tile (N = 131), the masked short kernels and
+        xg, se = torch.rand(2, 5, N, device=dev), torch.randn(N, K * d, device=dev)   # their backwards
+        te = torch.randint(0, 12, (2, 9, 2), device=dev).float()
+        gm(xg, se, te).square().mean().backward()
+        with torch.no_grad():
+            gm.eval()(xg, se, te)
     for out, rel in ((32, 4), (64, 1)):                          # HeteroGCLSTM: k_hetero_lstm_fwd at both widths, H None and carried,
         ht = {"a": (301, 5), "b": (17, 32)}                      # partial tiles and a type change inside a CTA's tiles
         eh = {("a", "r", "b"): torch.stack([torch.arange(60) % 301, torch.arange(60) % 17]).to(dev),
