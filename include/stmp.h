@@ -705,6 +705,40 @@ int stmp_gman_attn_bwd(int64_t p0, int64_t p1, int64_t heads, int64_t width, int
                        float scale, const int64_t* strides, const float* q, const float* k, const float* v, const float* o,
                        const float* stash, const float* dout, void* workspace, float* dq, float* dk, float* dv, void* stream);
 
+/* ---- MTGNN's graph work (nn/attention/mtgnn.py), mtgnn.cu: the top-k graph of GraphConstructor and the mix-hop propagation of the two
+ * MixProps of a layer (operators (A + I) / rowsum and (A^T + I) / rowsum), with their backward.  A graph of N nodes and row width W
+ * (W = k for a learned graph, the widest row for a predefined one) lives in three caller-owned buffers:
+ *   pattern int32 [N W | N | N + 1 | N W | N W]: col1, cnt1 (the entries of each row of A), ptr2, row2 (the rows of each column of A,
+ *           ascending) and pos2 (where each column entry sits in the row arrays);
+ *   state   fp32  [N W | N | N]: the raw entries a of A, d1 = 1 + row sums, d2 = 1 + column sums;
+ *   values  fp32  [N W | N W | N | N]: v1 = a / d1[row], v2 = a / d2[column] (both at the row position of entry (i, j)), diag1 = 1 / d1,
+ *           diag2 = 1 / d2.  Unused row slots hold zero values.
+ *   stmp_mtgnn_graph_fwd:   m1, m2 (N, dim) -> A = relu(tanh(alpha (m1 m2^T - m2 m1^T))) keeping the k largest entries of each row
+ *                           (equal values: the lower column first; zero entries dropped); workspace: stmp_mtgnn_graph_workspace_bytes.
+ *   stmp_mtgnn_graph_dense: the same structures from the nonzeros of a dense (N, N) A, W >= its widest row (a wider row keeps its
+ *                           first W nonzeros: nothing is written past a row's slots).
+ *   stmp_mtgnn_graph_bwd:   dvals (the values' layout) -> dm1, dm2 through both normalisations, the mask, relu and tanh;
+ *                           workspace: stmp_mtgnn_graph_bwd_workspace_bytes.
+ *   stmp_mtgnn_prop_fwd:    x (B, C, N, T) contiguous -> hops (B, 2 depth C, N, T): channel block o depth + k - 1 = hop k of operator o,
+ *                           H_k = alpha x + (1 - alpha) S_o H_{k-1}, H_0 = x.  2 depth launches.
+ *   stmp_mtgnn_prop_bwd:    dhops = dL/dhops (overwritten), dx = the direct gradient of x (accumulated in place) -> dx, and dvals
+ *                           (nullable) the gradient of the values.  2 depth + 1 launches.
+ * Envelope (stmp_mtgnn_supported returns STMP_OK or STMP_EUNSUPPORTED): 1 <= N <= 4096, 1 <= k <= min(N, 64), 1 <= dim <= 64,
+ * 1 <= C <= 64, 1 <= depth <= 4, B >= 0 (B = 0: no launch), T >= 1, every grid below 2^31 CTAs.  Exact fp32 (FFMA, every sum in one
+ * fixed order), deterministic (no atomics), no host sync and no allocation. */
+int stmp_mtgnn_supported(int64_t n, int64_t k, int64_t dim, int64_t channels, int64_t depth, int64_t batch, int64_t steps);
+int64_t stmp_mtgnn_graph_workspace_bytes(int64_t n);
+int stmp_mtgnn_graph_fwd(int64_t n, int64_t k, int64_t dim, float alpha, const float* m1, const float* m2, void* workspace, int* pattern,
+                         float* state, float* vals, void* stream);
+int stmp_mtgnn_graph_dense(int64_t n, int64_t w, const float* A, void* workspace, int* pattern, float* state, float* vals, void* stream);
+int64_t stmp_mtgnn_graph_bwd_workspace_bytes(int64_t n);
+int stmp_mtgnn_graph_bwd(int64_t n, int64_t k, int64_t dim, float alpha, const float* m1, const float* m2, const int* pattern,
+                         const float* state, const float* vals, const float* dvals, void* workspace, float* dm1, float* dm2, void* stream);
+int stmp_mtgnn_prop_fwd(int64_t B, int64_t C, int64_t N, int64_t T, int64_t W, int64_t depth, float alpha, const float* x,
+                        const int* pattern, const float* vals, float* hops, void* stream);
+int stmp_mtgnn_prop_bwd(int64_t B, int64_t C, int64_t N, int64_t T, int64_t W, int64_t depth, float alpha, const float* x,
+                        const int* pattern, const float* vals, const float* hops, float* dhops, float* dx, float* dvals, void* stream);
+
 /* ---- the same cell at 64 hidden channels (lstm_rows.cu, the width-2 instance of its kernels): GConvLSTM / GCLSTM(cin, 64, K <= 2).
  * Envelope: cout = 64, cin 1..16, n_ops 0..1 and at most the plan's operators (stmp_lstm_rows_supported(plan, variant, n_ops, cin, 64)),
  * any number of nodes and any degree.  Same argument lists, launch chain and guarantees as the stmp_lstm_rows_* entries, with 32 -> 64

@@ -145,6 +145,14 @@ _SIGNATURES = {
     "stmp_gman_attn_workspace_bytes": (c_int64, [c_int64] * 4 + [c_int]),
     "stmp_gman_attn_fwd": (c_int, [c_int64] * 6 + [c_int, c_int, c_float] + [_P] * 7),
     "stmp_gman_attn_bwd": (c_int, [c_int64] * 6 + [c_int, c_int, c_float] + [_P] * 12),
+    "stmp_mtgnn_supported": (c_int, [c_int64] * 7),
+    "stmp_mtgnn_graph_workspace_bytes": (c_int64, [c_int64]),
+    "stmp_mtgnn_graph_fwd": (c_int, [c_int64] * 3 + [c_float] + [_P] * 7),
+    "stmp_mtgnn_graph_dense": (c_int, [c_int64] * 2 + [_P] * 6),
+    "stmp_mtgnn_graph_bwd_workspace_bytes": (c_int64, [c_int64]),
+    "stmp_mtgnn_graph_bwd": (c_int, [c_int64] * 3 + [c_float] + [_P] * 10),
+    "stmp_mtgnn_prop_fwd": (c_int, [c_int64] * 6 + [c_float] + [_P] * 5),
+    "stmp_mtgnn_prop_bwd": (c_int, [c_int64] * 6 + [c_float] + [_P] * 8),
     "stmp_hetero_lstm_supported": (c_int, [c_int64] * 3),
     "stmp_hetero_lstm_fwd": (c_int, [c_int64, c_int64, _P, c_int, _P]),
     "stmp_hetero_lstm_workspace_bytes": (c_int64, [c_int64, c_int64, _P]),

@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libstmp.so")
-SOURCES = ["plan.cu", "spmm.cu", "dcrnn_seq.cu", "dcrnn_seq_tc.cu", "gemm_tc.cu", "cells.cu", "dcrnn_bwd.cu", "dcrnn_narrow.cu", "tgcn_attn.cu", "gemm_blocks.cu", "spatial_attention_tiled.cu", "astgcn_factors.cu", "train.cu", "wgrad_tc.cu", "gru_rows.cu", "lstm_rows.cu", "dcrnn_rows.cu", "dcrnn_narrow_rows.cu", "dcrnn_wide_rows.cu", "ggc_rows.cu", "evolvegcn_rows.cu", "mpnn_rows.cu", "agcrn.cu", "hetero_rows.cu", "gman_attention.cu"]
+SOURCES = ["plan.cu", "spmm.cu", "dcrnn_seq.cu", "dcrnn_seq_tc.cu", "gemm_tc.cu", "cells.cu", "dcrnn_bwd.cu", "dcrnn_narrow.cu", "tgcn_attn.cu", "gemm_blocks.cu", "spatial_attention_tiled.cu", "astgcn_factors.cu", "train.cu", "wgrad_tc.cu", "gru_rows.cu", "lstm_rows.cu", "dcrnn_rows.cu", "dcrnn_narrow_rows.cu", "dcrnn_wide_rows.cu", "ggc_rows.cu", "evolvegcn_rows.cu", "mpnn_rows.cu", "agcrn.cu", "hetero_rows.cu", "gman_attention.cu", "mtgnn.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v",

@@ -980,6 +980,175 @@ def gman_attention(q, k, v, heads: int, width: int, scale: float, spatial: bool,
     return gman_attn_fwd(q, k, v, heads, width, scale, spatial, mask)
 
 
+def mtgnn_supported(n: int, k: int, dim: int, channels: int, depth: int, batch: int, steps: int) -> bool:
+    """stmp_mtgnn_supported: whether MTGNN's graph build and propagation kernels take a graph of n nodes with k entries per row (or
+    the widest row of a predefined A), embeddings of width dim, and (batch, channels, n, steps) activations at gcn_depth `depth`."""
+    return _lib.lib().stmp_mtgnn_supported(n, k, dim, channels, depth, batch, steps) == _lib.STMP_OK
+
+
+def _mtgnn_sizes(n: int, w: int):
+    """Element counts of the pattern (int32), state and values (fp32) buffers of an N-node graph of row width w (include/stmp.h)."""
+    return 3 * n * w + 2 * n + 1, n * w + 2 * n, 2 * n * w + 2 * n
+
+
+def _mtgnn_require_graph(fn: str, n: int, w: int, pattern, vals, state=None):
+    """Raises unless the graph buffers hold the counts the kernels index for n nodes of row width w: they trust (n, w)."""
+    if pattern.dim() != 1:
+        raise RuntimeError(f"{fn}: the pattern must be flat, got {pattern.dim()} dimensions")
+    np_, ns, nv = _mtgnn_sizes(n, w)
+    _require_numel(fn, np_, pattern=pattern)
+    _require_numel(fn, nv, values=vals)
+    _require_numel(fn, ns, state=state)
+    if pattern.dtype != torch.int32:
+        raise RuntimeError(f"{fn}: the pattern must be int32, got {pattern.dtype}")
+
+
+def _mtgnn_buffers(n: int, w: int, device):
+    np_, ns, nv = _mtgnn_sizes(n, w)
+    return (torch.empty(np_, device=device, dtype=torch.int32), torch.empty(ns, device=device, dtype=torch.float32),
+            torch.empty(nv, device=device, dtype=torch.float32))
+
+
+def mtgnn_graph_fwd(m1: torch.Tensor, m2: torch.Tensor, k: int, alpha: float):
+    """GraphConstructor's top-k graph from its node vectors m1, m2 (N, dim) (stmp_mtgnn_graph_fwd, four launches):
+    -> (pattern, state, values), see include/stmp.h.  No autograd."""
+    m1, m2 = _f32c(m1.detach(), "M1"), _f32c(m2.detach(), "M2")
+    n, dim = m1.shape
+    if k > n:
+        raise RuntimeError("selected index k out of range")
+    pattern, state, vals = _mtgnn_buffers(n, k, m1.device)
+    L_ = _lib.lib()
+    ws = torch.empty(int(L_.stmp_mtgnn_graph_workspace_bytes(n)), device=m1.device, dtype=torch.uint8)
+    with torch.cuda.device(m1.device):
+        _lib.check(L_.stmp_mtgnn_graph_fwd(n, k, dim, alpha, *(_lib.ptr(t) for t in (m1, m2, ws, pattern, state, vals)), _lib.stream_ptr()))
+    return pattern, state, vals
+
+
+def mtgnn_graph_dense(A: torch.Tensor):
+    """The same structures from the nonzeros of a predefined dense (N, N) A (stmp_mtgnn_graph_dense): -> (pattern, state, values, w)
+    with w the widest row.  A setup path: sizing it reads one number back to the host."""
+    A = _f32c(A.detach(), "A_tilde")
+    n = A.shape[0]
+    w = max(1, int((A != 0).sum(1).max().item()))
+    pattern, state, vals = _mtgnn_buffers(n, w, A.device)
+    L_ = _lib.lib()
+    ws = torch.empty(int(L_.stmp_mtgnn_graph_workspace_bytes(n)), device=A.device, dtype=torch.uint8)
+    with torch.cuda.device(A.device):
+        _lib.check(L_.stmp_mtgnn_graph_dense(n, w, *(_lib.ptr(t) for t in (A, ws, pattern, state, vals)), _lib.stream_ptr()))
+    return pattern, state, vals, w
+
+
+class _MtgnnGraphFn(torch.autograd.Function):
+    """(M1, M2) -> the operator values on the top-k pattern; the pattern is a non-differentiable second output.  backward =
+    stmp_mtgnn_graph_bwd: both normalisations, the mask, relu and tanh, then dM1 = (dz - dz^T) M2, dM2 = (dz^T - dz) M1."""
+
+    @staticmethod
+    def forward(ctx, m1, m2, k, alpha):
+        pattern, state, vals = mtgnn_graph_fwd(m1, m2, k, alpha)
+        ctx.meta = (k, alpha)
+        ctx.save_for_backward(m1.detach().contiguous(), m2.detach().contiguous(), pattern, state, vals)
+        ctx.mark_non_differentiable(pattern)
+        return vals, pattern
+
+    @staticmethod
+    def backward(ctx, dvals, _dpattern):
+        m1, m2, pattern, state, vals = ctx.saved_tensors
+        k, alpha = ctx.meta
+        n, dim = m1.shape
+        _mtgnn_require_graph("mtgnn_graph_bwd", n, k, pattern, dvals, state)
+        dvals = _f32c(dvals, "dvals")
+        dm1, dm2 = torch.empty_like(m1), torch.empty_like(m2)
+        L_ = _lib.lib()
+        ws = torch.empty(int(L_.stmp_mtgnn_graph_bwd_workspace_bytes(n)), device=m1.device, dtype=torch.uint8)
+        with torch.cuda.device(m1.device):
+            _lib.check(L_.stmp_mtgnn_graph_bwd(n, k, dim, alpha, *(_lib.ptr(t) for t in (m1, m2, pattern, state, vals, dvals, ws, dm1, dm2)),
+                                               _lib.stream_ptr()))
+        return dm1, dm2, None, None
+
+
+def mtgnn_graph(m1: torch.Tensor, m2: torch.Tensor, k: int, alpha: float, train: bool):
+    """The learned graph's (values, pattern); with `train` the values are differentiable w.r.t. m1 and m2 (_MtgnnGraphFn)."""
+    if train:
+        return _MtgnnGraphFn.apply(m1, m2, k, alpha)
+    pattern, _, vals = mtgnn_graph_fwd(m1, m2, k, alpha)
+    return vals, pattern
+
+
+def mtgnn_prop_fwd(x: torch.Tensor, pattern: torch.Tensor, vals: torch.Tensor, w: int, depth: int, alpha: float) -> torch.Tensor:
+    """Both MixProps' hop chains (stmp_mtgnn_prop_fwd, 2 depth launches): x (B, C, N, T) -> hops (B, 2 depth C, N, T)."""
+    _mtgnn_require_graph("mtgnn_prop_fwd", x.shape[2], w, pattern, vals)
+    x = _f32c(x.detach(), "X")
+    B, C, N, T = x.shape
+    hops = torch.empty(B, 2 * depth * C, N, T, device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.lib().stmp_mtgnn_prop_fwd(B, C, N, T, w, depth, alpha, *(_lib.ptr(t) for t in (x, pattern, vals.detach(), hops)),
+                                                  _lib.stream_ptr()))
+    return hops
+
+
+def _mixprop_weights(w1, w2, C: int):
+    """The two MixProp MLPs as one: the X block's weights summed (both MLPs read H_0 = X), then operator 1's hops, operator 2's."""
+    w1, w2 = w1.view(w1.shape[0], -1), w2.view(w2.shape[0], -1)
+    return w1[:, :C] + w2[:, :C], torch.cat((w1[:, C:], w2[:, C:]), dim=1)
+
+
+def _mixprop_out(x, hops, w1, b1, w2, b2):
+    B, C, N, T = x.shape
+    wx, wh = _mixprop_weights(w1, w2, C)
+    y = torch.matmul(wh, hops.view(B, hops.shape[1], N * T))
+    y += torch.matmul(wx, x.reshape(B, C, N * T))
+    y += (b1 + b2).view(1, -1, 1)
+    return y.view(B, wx.shape[0], N, T)
+
+
+class _MtgnnMixPropFn(torch.autograd.Function):
+    """mixprop1(X, A) + mixprop2(X, A^T) of one MTGNN layer: (X, values, MLP weights) -> output (B, C_out, N, T).  forward =
+    stmp_mtgnn_prop_fwd and the MLPs as fp32 GEMMs; backward = the GEMMs' transposes, then stmp_mtgnn_prop_bwd (the adjoint hop chains
+    into dX and, when asked for, the values' gradient)."""
+
+    @staticmethod
+    def forward(ctx, x, vals, w1, b1, w2, b2, pattern, w, depth, alpha):
+        x = _f32c(x.detach(), "X")
+        hops = mtgnn_prop_fwd(x, pattern, vals, w, depth, alpha)
+        ctx.meta = (w, depth, alpha)
+        ctx.save_for_backward(x, vals.detach(), w1.detach(), w2.detach(), hops, pattern)
+        return _mixprop_out(x, hops, w1.detach(), b1.detach(), w2.detach(), b2.detach())
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, vals, w1, w2, hops, pattern = ctx.saved_tensors
+        w, depth, alpha = ctx.meta
+        B, C, N, T = x.shape
+        gy = _f32c(gy, "gout").view(B, w1.shape[0], N * T)
+        wx, wh = _mixprop_weights(w1, w2, C)
+        want = ctx.needs_input_grad
+        dx = torch.matmul(wx.t(), gy)
+        dhops = torch.matmul(wh.t(), gy)
+        dvals = torch.empty_like(vals) if want[1] else None
+        with torch.cuda.device(x.device):
+            _lib.check(_lib.lib().stmp_mtgnn_prop_bwd(B, C, N, T, w, depth, alpha,
+                                                      *(_lib.ptr(t) for t in (x, pattern, vals, hops, dhops, dx, dvals)), _lib.stream_ptr()))
+        dw1 = dw2 = db = None
+        if want[2] or want[4]:
+            dwx = torch.matmul(gy, x.view(B, C, N * T).transpose(1, 2)).sum(0)
+            dwh = torch.matmul(gy, hops.view(B, hops.shape[1], N * T).transpose(1, 2)).sum(0)
+            gC = depth * C
+            dw1 = torch.cat((dwx, dwh[:, :gC]), dim=1).view_as(w1)
+            dw2 = torch.cat((dwx, dwh[:, gC:]), dim=1).view_as(w2)
+        if want[3] or want[5]:
+            db = gy.sum((0, 2))
+        return (dx.view(B, C, N, T) if want[0] else None, dvals, dw1, db, dw2, db, None, None, None, None)
+
+
+def mtgnn_mixprop(x, vals, pattern, w: int, depth: int, alpha: float, w1, b1, w2, b2, train: bool) -> torch.Tensor:
+    """One MTGNN layer's two MixProps over the graph (vals, pattern) of row width w, x (B, C, N, T): differentiable w.r.t. x, vals and
+    the MLP weights with `train` (_MtgnnMixPropFn)."""
+    if train:
+        return _MtgnnMixPropFn.apply(x, vals, w1, b1, w2, b2, pattern, w, depth, alpha)
+    x = _f32c(x.detach(), "X")
+    return _mixprop_out(x, mtgnn_prop_fwd(x, pattern, vals, w, depth, alpha), w1.detach(), b1.detach(), w2.detach(), b2.detach())
+
+
 def _tgcn_entry(co: int, name: str):
     """The library entry `name` of the fused TGCN kernels at hidden width `co`: stmp_tgcn_<name> at 32, stmp_tgcn_wide_<name> at 64."""
     if co not in (32, 64):

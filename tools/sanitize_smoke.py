@@ -12,7 +12,7 @@ from pytorch_geometric_temporal_b200.dataset import synthetic                   
 from pytorch_geometric_temporal_b200.nn.attention import ASTGCN                              # noqa: E402
 from pytorch_geometric_temporal_b200.nn.recurrent import A3TGCN2, BatchedDCRNN, DyGrEncoder, EvolveGCNH, EvolveGCNO, GCLSTM, GConvGRU, GConvLSTM, LRGCN, MPNNLSTM, TGCN2   # noqa: E402
 from pytorch_geometric_temporal_b200.nn.recurrent import AGCRN                                # noqa: E402
-from pytorch_geometric_temporal_b200.nn.attention import GMAN                                 # noqa: E402
+from pytorch_geometric_temporal_b200.nn.attention import GMAN, MTGNN                          # noqa: E402
 from pytorch_geometric_temporal_b200.nn.hetero import HeteroGCLSTM                          # noqa: E402
 
 dev = torch.device("cuda")
@@ -122,6 +122,13 @@ with torch.enable_grad():
         gm(xg, se, te).square().mean().backward()
         with torch.no_grad():
             gm.eval()(xg, se, te)
+    for n, k, depth, T in ((37, 5, 2, 13), (70, 64, 1, 40)):    # MTGNN: every k_mtgnn_* kernel; a partial bitmap word column (37, 70
+        mt = MTGNN(True, True, depth, n, [2, 3], 3, 0.0, k, 6, 1, 4, 5, 6, 8, T, 2, 3, 2, 0.05, 3.0, True).to(dev)   # nodes), T below
+        xm = torch.rand(2, 2, n, T, device=dev)                  # and above a warp, the graph backward; then a predefined A
+        mt(xm).square().mean().backward()
+        with torch.no_grad():
+            MTGNN(True, False, depth, n, [2, 3], 3, 0.0, k, 6, 1, 4, 5, 6, 8, T, 2, 3, 2, 0.05, 3.0, True).to(dev)(
+                xm, (torch.rand(n, n, device=dev) < 0.2).float())
     for out, rel in ((32, 4), (64, 1)):                          # HeteroGCLSTM: k_hetero_lstm_fwd at both widths, H None and carried,
         ht = {"a": (301, 5), "b": (17, 32)}                      # partial tiles and a type change inside a CTA's tiles
         eh = {("a", "r", "b"): torch.stack([torch.arange(60) % 301, torch.arange(60) % 17]).to(dev),
